@@ -272,8 +272,7 @@ struct ScopedFree {
 // multiples of 512 KB); src may be anything.
 inline void stream_copy(void* dst, const void* src, size_t n) {
 #if defined(__x86_64__) && defined(__SSE2__)
-  static const bool temporal = std::getenv("CB_STAGE_TEMPORAL") != nullptr;  // diagnostic: ordinary stores
-  if (((uintptr_t)dst & 15u) == 0 && !temporal) {
+  if (((uintptr_t)dst & 15u) == 0) {
     char* d = (char*)dst;
     const char* s2 = (const char*)src;
     size_t i = 0;
@@ -314,7 +313,6 @@ class WorkerPool {
   WorkerPool() {
     unsigned hw = std::thread::hardware_concurrency();
     int n = (int)std::min<unsigned>(hw > 2 ? hw - 1 : 1, 12u);
-    if (const char* e = std::getenv("CB_STAGE_THREADS")) n = std::max(1, std::atoi(e));
     for (int i = 0; i < n; ++i) {
       threads_.emplace_back([this] {
         for (;;) {
@@ -429,12 +427,18 @@ int dalloc(T** p, size_t n) {
 
 }  // namespace
 
+// One captured LM trial (ensure_graph), keyed by everything that is baked into the captured launches.  A failure to build
+// it is remembered for its key, so that later solves go straight to the fallback.
 struct TrialGraph {
+  struct Key {
+    void *nccl, *peer; int rank, world;
+    bool operator==(const Key& o) const { return nccl == o.nccl && peer == o.peer && rank == o.rank && world == o.world; }
+  };
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
-  cudaEvent_t ev_a = nullptr, ev_b = nullptr;  // bracket the point pass inside the graph
-  cudaEvent_t ev_c = nullptr, ev_d = nullptr;  // bracket the Schur product
-  int n_kernels = 0;
+  Key key = {};
+  bool valid = false, failed = false;
+  int n_kernels = 0;  // kernels of one trial
 };
 
 struct CbBaProblem {
@@ -488,25 +492,11 @@ struct CbBaProblem {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev_state[2] = {nullptr, nullptr};
   cudaEvent_t ev_pp[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};  // point-pass / Schur brackets (direct mode)
   cudaStream_t cap_stream = nullptr;
-  // trial graphs, keyed by everything that is baked into the captured launches
-  struct GraphKey {
-    void *nccl, *peer; int rank, world;
-    bool operator==(const GraphKey& o) const { return nccl == o.nccl && peer == o.peer && rank == o.rank && world == o.world; }
-  };
-  long long n_solves = 0;
-  bool graph_valid = false;
-  GraphKey graph_key = {};
-  TrialGraph tg[2];
-  // device-loop mode: ONE graph whose body (a WHILE conditional node) is the LM trial; the loop ends on the device
-  cudaGraph_t loop_graph = nullptr;
-  cudaGraphExec_t loop_exec = nullptr;
-  bool loop_valid = false, loop_failed = false;
-  GraphKey loop_key = {};
-  int loop_kernels = 0;
+  TrialGraph trial_graph;  // sharded solves: one graph launch per trial
+  TrialGraph loop_graph;   // one GPU: ONE graph whose body (a WHILE conditional node) is the LM trial
   // pcg launch configuration
-  int pcg_cs = 1, pcg_rows = 0, pcg_mode = 0, pcg_cl = 1, pcg_npa = 0;
-  bool fuse_small = true;      // direct_solve: prep + solve + camera step in one kernel (CB_FUSE_SMALL=0 keeps them apart)
-  bool direct_solve = false;  // n_camera_params <= DIRECT_MAX_N: dense LDL^T in one CTA instead of the cluster PCG
+  int pcg_cs = 1, pcg_rows = 0, pcg_mode = 2, pcg_cl = 1, pcg_npa = 0;
+  bool direct_solve = false;  // n_camera_params <= DIRECT_MAX_N: prep, dense LDL^T and camera step in one CTA (small_rig_step_kernel)
   size_t direct_smem = 0;
   size_t pcg_smem = 0;
   // rigid-distance constraints (optional)
@@ -552,16 +542,10 @@ int bits_for(unsigned long long v) {
   return b;
 }
 
-void destroy_graphs(CbBaProblem* p) {
-  for (auto& g : p->tg) {
-    if (g.exec) cudaGraphExecDestroy(g.exec);
-    if (g.graph) cudaGraphDestroy(g.graph);
-    g.exec = nullptr; g.graph = nullptr; g.n_kernels = 0;
-  }
-  p->graph_valid = false;
-  if (p->loop_exec) cudaGraphExecDestroy(p->loop_exec);
-  if (p->loop_graph) cudaGraphDestroy(p->loop_graph);
-  p->loop_exec = nullptr; p->loop_graph = nullptr; p->loop_valid = false;
+void destroy_graph(TrialGraph& g) {
+  if (g.exec) cudaGraphExecDestroy(g.exec);
+  if (g.graph) cudaGraphDestroy(g.graph);
+  g.exec = nullptr; g.graph = nullptr; g.valid = false; g.n_kernels = 0;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -603,9 +587,7 @@ int choose_camera_order(CbBaProblem* p, const int* cam_order, cudaStream_t st) {
   } else {
     const int cams_per_tile = std::max(1, cb::SY_TILE / p->P);
     const double avg = (double)p->n_obs / std::max(p->n_pts, 1);
-    int want = (p->n_blk >= 3 && avg <= nc / 3.0) ? 1 : 0;
-    if (const char* e = std::getenv("CB_CAM_ORDER")) want = std::atoi(e);
-    if (want) {
+    if (p->n_blk >= 3 && avg <= nc / 3.0) {
       p->order_auto = true;
       const int stride = std::max(1, p->n_pts / 8192), ns = cdiv(p->n_pts, stride);
       unsigned int* d_W;
@@ -749,8 +731,7 @@ int build_indices(CbBaProblem* p, const int* d_obs_cam, const int* d_obs_pt, con
   }
   p->n_dups = bad[1];
   std::vector<int> cc, cbeg, cend, ccs(p->n_cams + 1);
-  int chunk = cb::RJ_CHUNK;
-  if (const char* e = std::getenv("CB_RJ_CHUNK")) chunk = std::max(cb::RJ_THREADS, std::atoi(e));
+  const int chunk = cb::RJ_CHUNK;
   for (int c = 0; c < p->n_cams; ++c) {
     ccs[c] = (int)cc.size();
     for (int b = cam_start[c]; b < cam_start[c + 1]; b += chunk) {
@@ -820,7 +801,7 @@ void launch_pt_backsub(CbBaProblem* p, double* dp_out, cudaStream_t st) {
 
 using PcgFn = void (*)(const cb::LmState*, const double*, const double*, const double*, int, int, int, double, int,
                        double*, double*);
-// mode 0: slab in shared memory, 1: slab from global, 2: slab in registers with cl columns per lane
+// mode 1: slab streamed from L2, 2: slab in registers with cl columns per lane
 PcgFn pcg_fn(int mode, int P, int cl) {
   if (mode == 2) {
     if (P == 6)
@@ -829,16 +810,10 @@ PcgFn pcg_fn(int mode, int P, int cl) {
     return cl == 2 ? cb::pcg_cluster_kernel<2, 9, 2> : cl == 6 ? cb::pcg_cluster_kernel<2, 9, 6>
          : cl == 12 ? cb::pcg_cluster_kernel<2, 9, 12> : cb::pcg_cluster_kernel<2, 9, 18>;
   }
-  if (P == 6) return mode == 0 ? cb::pcg_cluster_kernel<0, 6, 1> : cb::pcg_cluster_kernel<1, 6, 1>;
-  return mode == 0 ? cb::pcg_cluster_kernel<0, 9, 1> : cb::pcg_cluster_kernel<1, 9, 1>;
+  return P == 6 ? cb::pcg_cluster_kernel<1, 6, 1> : cb::pcg_cluster_kernel<1, 9, 1>;
 }
 
 int launch_pcg(CbBaProblem* p, const cb::LmState* st_dev, double tol2, int max_iter, cudaStream_t st) {
-  if (p->direct_solve) {
-    CB_LAUNCH(cb::dense_ldlt_kernel, 1, cb::DIRECT_THREADS, p->direct_smem, st, st_dev, (const double*)p->d_red,
-              (const double*)(p->d_red + (size_t)p->nP * p->nP), p->nP, p->d_dc, p->d_sc);
-    return CB_OK;
-  }
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(p->pcg_cs);
   cfg.blockDim = dim3(cb::PCG_THREADS);
@@ -876,20 +851,21 @@ int camera_pass(CbBaProblem* p, int flip, int mode, cudaStream_t st) {
 }
 
 // damped system at the current point: point pass, Schur product, reduced system (+ all-reduce), head-of-iteration tests
+// (the last at the head of small_rig_step_kernel on small rigs, see solve_step).  ev: nullptr, or four events that
+// bracket the point pass (0, 1) and the Schur product (2, 3)
 template <int P>
-int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, cudaEvent_t ev_a, cudaEvent_t ev_b,
-                 cudaEvent_t ev_c = nullptr, cudaEvent_t ev_d = nullptr, bool fuse_small = false) {
-  if (ev_a) CB_CUDA(cudaEventRecord(ev_a, st));
+int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const cudaEvent_t* ev = nullptr) {
+  if (ev) CB_CUDA(cudaEventRecord(ev[0], st));
   launch_pt_pass<P>(p, st);
-  if (ev_b) CB_CUDA(cudaEventRecord(ev_b, st));
+  if (ev) CB_CUDA(cudaEventRecord(ev[1], st));
   if (p->n_c)
     CB_LAUNCH((cb::comp_build_kernel<P>), p->n_comp, cb::CC_THREADS, p->comp_build_smem, st, (const cb::LmState*)p->d_state,
               p->ct, p->d_pt_start, p->d_pm_cam, p->d_V6, p->d_gp, p->d_Dp2, p->d_gpt, p->c_crs(), p->c_cdirw(), p->n_cams,
               p->d_compL, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax);
-  if (ev_c) CB_CUDA(cudaEventRecord(ev_c, st));
+  if (ev) CB_CUDA(cudaEventRecord(ev[2], st));
   CB_LAUNCH(cb::schur_syrk_kernel, p->n_items, cb::SY_THREADS, sizeof(cb::SyrkSmem), st, (const cb::LmState*)p->d_state,
             p->d_Zt, (size_t)p->LD, p->d_tvec, p->d_items, (const int*)p->d_klist, p->d_part, p->d_tpart);
-  if (ev_d) CB_CUDA(cudaEventRecord(ev_d, st));
+  if (ev) CB_CUDA(cudaEventRecord(ev[3], st));
   const size_t nfin = (size_t)p->nP * p->nP + p->nP + 1;
   // gradient inf-norm over points: one slot per rank so a SUM all-reduce carries the max
   const int rank = sharded(opt) ? std::min(std::max(opt->rank, 0), p->red_slots - 1) : 0;
@@ -915,16 +891,16 @@ int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, cudaEv
               p->d_red);
     if (sharded(opt)) CB_TRY(do_allreduce(opt, p->d_red, (long long)p->red_len(), st));
   }
-  if (!(fuse_small && p->direct_solve))  // small rigs: prep runs at the head of small_rig_step_kernel (solve_step)
+  if (!p->direct_solve)
     CB_LAUNCH((cb::reduced_prep_kernel<P>), 1, 256, 0, st, p->d_state, p->nP, p->n_cams, p->red_slots, p->d_red, p->d_Dc2,
               p->d_active, p->d_Minv, p->d_gmax, p->d_sc);
   return CB_OK;
 }
 
 template <int P>
-int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st, bool fuse_small = false) {
+int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st) {
   const size_t nn = (size_t)p->nP * p->nP;
-  if (fuse_small && p->direct_solve) {
+  if (p->direct_solve) {
     CB_LAUNCH((cb::small_rig_step_kernel<P>), 1, cb::DIRECT_THREADS, p->direct_smem, st, p->d_state, p->nP, p->n_cams,
               p->red_slots, p->d_red, p->d_Dc2, p->d_active, p->d_gmax, p->d_sc, p->m_xc(), p->d_dc, p->d_lo, p->d_hi,
               p->d_cam_flags, p->d_cam_const, p->m_camtab());
@@ -944,9 +920,9 @@ int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st, bool fuse_small 
 
 // one whole LM trial: the same launches every time, all decisions on the device
 template <int P>
-int enqueue_trial(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, cudaEvent_t* ev) {
-  CB_TRY(build_system<P>(p, opt, st, ev[0], ev[1], ev[2], ev[3], p->fuse_small));
-  CB_TRY(solve_step<P>(p, nullptr, st, p->fuse_small));
+int enqueue_trial(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const cudaEvent_t* ev = nullptr) {
+  CB_TRY(build_system<P>(p, opt, st, ev));
+  CB_TRY(solve_step<P>(p, nullptr, st));
   const bool multi = sharded(opt);
   CB_TRY(camera_pass<P>(p, 1, multi ? 2 : 1, st));
   if (multi) {
@@ -1024,83 +1000,55 @@ int init_state(CbBaProblem* p, const CbBaOptions* opt, double lam, long long max
   return CB_OK;
 }
 
-// capture one LM trial into a graph (two instances, so that the event pair of trial t can be read while trial t+1 runs)
+// Capture one LM trial into g.  loop = false: the trial is the whole graph, launched once per trial.  loop = true: the
+// trial is the body of a WHILE conditional node (CUDA 12.4+) whose last kernel sets the loop condition from
+// LmState::done, so the whole solve is ONE graph launch and ONE host synchronisation, and no predicated-off trial is
+// ever queued.
 template <int P>
-int ensure_graphs(CbBaProblem* p, const CbBaOptions* opt) {
-  CbBaProblem::GraphKey key{opt->nccl_comm, opt->peer_group, opt->rank, opt->world_size};
-  if (p->graph_valid && p->graph_key == key) return CB_OK;
-  destroy_graphs(p);
-  if (!p->cap_stream) CB_CUDA(cudaStreamCreateWithFlags(&p->cap_stream, cudaStreamNonBlocking));
-  for (int k = 0; k < 2; ++k) {
-    TrialGraph& g = p->tg[k];
-    if (!g.ev_a) {
-      CB_CUDA(cudaEventCreate(&g.ev_a)); CB_CUDA(cudaEventCreate(&g.ev_b));
-      CB_CUDA(cudaEventCreate(&g.ev_c)); CB_CUDA(cudaEventCreate(&g.ev_d));
-    }
-    cudaEvent_t evs[4] = {g.ev_a, g.ev_b, g.ev_c, g.ev_d};
-    const long long l0 = g_launches.load();
-    CB_CUDA(cudaStreamBeginCapture(p->cap_stream, cudaStreamCaptureModeThreadLocal));
-    int rc = enqueue_trial<P>(p, opt, p->cap_stream, evs);
-    cudaError_t e = cudaStreamEndCapture(p->cap_stream, &g.graph);
-    g_launches.store(l0);  // capture launches nothing
-    if (rc != CB_OK) { if (g.graph) { cudaGraphDestroy(g.graph); g.graph = nullptr; } return rc; }
-    if (e != cudaSuccess) {
-      g_last_error = std::string("cudaStreamEndCapture: ") + cudaGetErrorString(e);
-      cudaGetLastError();
-      return CB_E_CUDA;
-    }
-    size_t nn = 0;
-    cudaGraphGetNodes(g.graph, nullptr, &nn);
-    g.n_kernels = (int)nn - 4;  // minus the four event-record nodes
-    CB_CUDA(cudaGraphInstantiate(&g.exec, g.graph, 0));
-  }
-  p->graph_key = key;
-  p->graph_valid = true;
-  return CB_OK;
-}
-
-// Device-loop mode: a graph with one WHILE conditional node (CUDA 12.4+) whose body is the trial; the last body node sets
-// the loop condition from LmState::done, so the whole solve is ONE graph launch and ONE host synchronisation, and no
-// predicated-off trial is ever queued.  Any failure to build it is remembered and the per-trial graphs are used instead.
-template <int P>
-int ensure_loop_graph(CbBaProblem* p, const CbBaOptions* opt) {
-  CbBaProblem::GraphKey key{opt->nccl_comm, opt->peer_group, opt->rank, opt->world_size};
-  if (p->loop_valid && p->loop_key == key) return CB_OK;
-  if (p->loop_failed) return CB_E_UNSUPPORTED;
-  if (p->loop_exec) { cudaGraphExecDestroy(p->loop_exec); p->loop_exec = nullptr; }
-  if (p->loop_graph) { cudaGraphDestroy(p->loop_graph); p->loop_graph = nullptr; }
-  p->loop_valid = false;
-  if (!p->cap_stream && cudaStreamCreateWithFlags(&p->cap_stream, cudaStreamNonBlocking) != cudaSuccess) { cudaGetLastError(); p->loop_failed = true; return CB_E_UNSUPPORTED; }
+int ensure_graph(CbBaProblem* p, const CbBaOptions* opt, bool loop) {
+  TrialGraph& g = loop ? p->loop_graph : p->trial_graph;
+  const TrialGraph::Key key{opt->nccl_comm, opt->peer_group, opt->rank, opt->world_size};
+  if (g.key == key && (g.valid || g.failed)) return g.valid ? CB_OK : CB_E_UNSUPPORTED;
+  destroy_graph(g);
+  g.key = key;
+  g.failed = false;
   auto fail = [&](const char* what) {
-    g_last_error = std::string("device-loop graph: ") + what + ": " + cudaGetErrorString(cudaGetLastError());
-    if (p->loop_graph) { cudaGraphDestroy(p->loop_graph); p->loop_graph = nullptr; }
-    p->loop_failed = true;
+    g_last_error = std::string(loop ? "device-loop graph: " : "trial graph: ") + what + ": " +
+                   cudaGetErrorString(cudaGetLastError());
+    destroy_graph(g);
+    g.failed = true;
     return CB_E_UNSUPPORTED;
   };
-  if (cudaGraphCreate(&p->loop_graph, 0) != cudaSuccess) return fail("cudaGraphCreate");
-  cudaGraphConditionalHandle h;
-  if (cudaGraphConditionalHandleCreate(&h, p->loop_graph, 1, cudaGraphCondAssignDefault) != cudaSuccess) return fail("cudaGraphConditionalHandleCreate");
-  cudaGraphNodeParams np = {};
-  np.type = cudaGraphNodeTypeConditional;
-  np.conditional.handle = h;
-  np.conditional.type = cudaGraphCondTypeWhile;
-  np.conditional.size = 1;
-  cudaGraphNode_t node;
-  if (cudaGraphAddNode(&node, p->loop_graph, nullptr, 0, &np) != cudaSuccess) return fail("cudaGraphAddNode(conditional)");
-  cudaGraph_t body = np.conditional.phGraph_out[0];
-  if (cudaStreamBeginCaptureToGraph(p->cap_stream, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal) != cudaSuccess)
-    return fail("cudaStreamBeginCaptureToGraph");
+  if (!p->cap_stream && cudaStreamCreateWithFlags(&p->cap_stream, cudaStreamNonBlocking) != cudaSuccess)
+    return fail("cudaStreamCreateWithFlags");
+  cudaGraphConditionalHandle h = {};
+  cudaError_t e;
+  if (loop) {
+    if (cudaGraphCreate(&g.graph, 0) != cudaSuccess) return fail("cudaGraphCreate");
+    if (cudaGraphConditionalHandleCreate(&h, g.graph, 1, cudaGraphCondAssignDefault) != cudaSuccess)
+      return fail("cudaGraphConditionalHandleCreate");
+    cudaGraphNodeParams np = {};
+    np.type = cudaGraphNodeTypeConditional;
+    np.conditional.handle = h;
+    np.conditional.type = cudaGraphCondTypeWhile;
+    np.conditional.size = 1;
+    cudaGraphNode_t node;
+    if (cudaGraphAddNode(&node, g.graph, nullptr, 0, &np) != cudaSuccess) return fail("cudaGraphAddNode(conditional)");
+    e = cudaStreamBeginCaptureToGraph(p->cap_stream, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                      cudaStreamCaptureModeThreadLocal);
+  } else {
+    e = cudaStreamBeginCapture(p->cap_stream, cudaStreamCaptureModeThreadLocal);
+  }
+  if (e != cudaSuccess) return fail("begin capture");
   const long long l0 = g_launches.load();
-  cudaEvent_t none[4] = {nullptr, nullptr, nullptr, nullptr};
-  int rc = enqueue_trial<P>(p, opt, p->cap_stream, none);
-  if (rc == CB_OK) CB_LAUNCH(cb::lm_loop_cond_kernel, 1, 1, 0, p->cap_stream, (const cb::LmState*)p->d_state, h);
-  p->loop_kernels = (int)(g_launches.load() - l0);
-  g_launches.store(l0);
-  cudaError_t e = cudaStreamEndCapture(p->cap_stream, nullptr);
+  int rc = enqueue_trial<P>(p, opt, p->cap_stream);
+  if (loop && rc == CB_OK) CB_LAUNCH(cb::lm_loop_cond_kernel, 1, 1, 0, p->cap_stream, (const cb::LmState*)p->d_state, h);
+  g.n_kernels = (int)(g_launches.load() - l0);
+  g_launches.store(l0);  // capture launches nothing
+  e = loop ? cudaStreamEndCapture(p->cap_stream, nullptr) : cudaStreamEndCapture(p->cap_stream, &g.graph);
   if (rc != CB_OK || e != cudaSuccess) return fail("capture of the trial");
-  if (cudaGraphInstantiate(&p->loop_exec, p->loop_graph, 0) != cudaSuccess) return fail("cudaGraphInstantiate");
-  p->loop_key = key;
-  p->loop_valid = true;
+  if (cudaGraphInstantiate(&g.exec, g.graph, 0) != cudaSuccess) return fail("cudaGraphInstantiate");
+  g.valid = true;
   return CB_OK;
 }
 
@@ -1117,25 +1065,15 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
   std::memset(res, 0, sizeof(*res));
 
   // The trials are replayed from CUDA graphs: one GPU -> device loop (ONE graph launch per solve: a WHILE node around the
-  // trial); sharded -> one graph per trial (the host keeps one trial ahead).  Capture + instantiation cost less than the
-  // launch gaps and host round trips of even one 3-iteration solve.  Direct launches: a host callback carries the
-  // all-reduce (cannot be captured), verbose >= 2, opt->time_kernels, or graph construction failed.
-  // CB_LM_GRAPH = 0: direct launches, 1 (default): as above, 2: per-trial graphs always, 3: device loop always.
-  int graph_mode = 1;
-  if (const char* e = std::getenv("CB_LM_GRAPH")) graph_mode = std::atoi(e);
-  if (opt->time_kernels) graph_mode = 0;
-  ++p->n_solves;
-  bool use_loop = opt->allreduce == nullptr && (graph_mode == 3 || (graph_mode == 1 && !sharded(opt))) && opt->verbose < 2;
-  if (use_loop && ensure_loop_graph<P>(p, opt) != CB_OK) { cudaGetLastError(); use_loop = false; }
-  bool use_graph = !use_loop && opt->allreduce == nullptr && graph_mode >= 1 && opt->verbose < 2;
-  if (use_graph) {
-    int rc = ensure_graphs<P>(p, opt);
-    if (rc != CB_OK) {
-      if (std::getenv("CB_LM_GRAPH_STRICT")) return rc;
-      cudaGetLastError();
-      use_graph = false;  // capture unsupported for this configuration: direct launches
-    }
-  }
+  // trial); sharded over NCCL or peer memory -> one graph per trial (the host keeps one trial ahead).  Capture +
+  // instantiation cost less than the launch gaps and host round trips of even one 3-iteration solve.  Direct launches:
+  // a host callback carries the all-reduce (cannot be captured), or opt->time_kernels (CUDA events recorded during a
+  // capture cannot be read back).  A graph that cannot be built falls back: device loop -> per-trial graph -> direct.
+  const bool direct = opt->allreduce != nullptr || opt->time_kernels;
+  bool use_loop = !direct && !sharded(opt);
+  if (use_loop && ensure_graph<P>(p, opt, true) != CB_OK) { cudaGetLastError(); use_loop = false; }
+  bool use_graph = !direct && !use_loop;
+  if (use_graph && ensure_graph<P>(p, opt, false) != CB_OK) { cudaGetLastError(); use_graph = false; }
 
   CB_TRY(set_bounds(p, opt->use_bounds != 0, st));
   CB_TRY(init_state(p, opt, opt->lambda0 > 0 ? opt->lambda0 : 1e-4, max_nfev, st));
@@ -1148,14 +1086,12 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
   long long pp_launches = 0, trials = 0;
   double sy_ms_total = 0.0;
   long long sy_launches = 0;
-  auto read_pp = [&](long long t) {
+  auto read_pp = [&](long long t) {  // direct launches: the event brackets of trial t
     float ms = 0.f;
-    const TrialGraph& g = p->tg[t & 1];
-    cudaEvent_t a = use_graph ? g.ev_a : p->ev_pp[t & 1][0], b = use_graph ? g.ev_b : p->ev_pp[t & 1][1];
-    cudaEvent_t c = use_graph ? g.ev_c : p->ev_pp[t & 1][2], d = use_graph ? g.ev_d : p->ev_pp[t & 1][3];
-    if (cudaEventElapsedTime(&ms, a, b) == cudaSuccess) { pp_ms_total += ms; ++pp_launches; }
+    const cudaEvent_t* ev = p->ev_pp[t & 1];
+    if (cudaEventElapsedTime(&ms, ev[0], ev[1]) == cudaSuccess) { pp_ms_total += ms; ++pp_launches; }
     else cudaGetLastError();
-    if (cudaEventElapsedTime(&ms, c, d) == cudaSuccess) { sy_ms_total += ms; ++sy_launches; }
+    if (cudaEventElapsedTime(&ms, ev[2], ev[3]) == cudaSuccess) { sy_ms_total += ms; ++sy_launches; }
     else cudaGetLastError();
   };
   bool done = false;
@@ -1163,12 +1099,12 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
   int rc = CB_OK;
   if (use_loop) {
     // the whole LM loop is one graph launch; the state comes back once
-    cudaError_t e = cudaGraphLaunch(p->loop_exec, st);
+    cudaError_t e = cudaGraphLaunch(p->loop_graph.exec, st);
     if (e != cudaSuccess) {
       // nothing of the loop ran: remember that this configuration cannot be launched and run the trials directly
       cudaGetLastError();
-      p->loop_failed = true;
-      p->loop_valid = false;
+      p->loop_graph.failed = true;
+      p->loop_graph.valid = false;
       use_loop = false;
     } else {
       cudaMemcpyAsync(&p->h_state[1], p->d_state, sizeof(cb::LmState), cudaMemcpyDeviceToHost, st);
@@ -1178,9 +1114,9 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
   }
   while (!done) {
     if (use_graph) {
-      cudaError_t e = cudaGraphLaunch(p->tg[t & 1].exec, st);
+      cudaError_t e = cudaGraphLaunch(p->trial_graph.exec, st);
       if (e != cudaSuccess) { g_last_error = std::string("cudaGraphLaunch: ") + cudaGetErrorString(e); rc = CB_E_CUDA; break; }
-      g_launches.fetch_add(p->tg[t & 1].n_kernels);
+      g_launches.fetch_add(p->trial_graph.n_kernels);
     } else {
       NvtxRange nvtx_trial("lm_trial (direct launches)");
       rc = enqueue_trial<P>(p, opt, st, p->ev_pp[t & 1]);
@@ -1193,7 +1129,7 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
       // trial t is queued; now look at the outcome of trial t-1
       cudaError_t e = cudaEventSynchronize(p->ev_state[(t - 1) & 1]);
       if (e != cudaSuccess) { g_last_error = std::string("LM trial: ") + cudaGetErrorString(e); rc = CB_E_CUDA; break; }
-      read_pp(t - 1);
+      if (!use_graph) read_pp(t - 1);
       if (p->h_state[(t - 1) & 1].done) done = true;
     }
     ++t;
@@ -1249,7 +1185,7 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
   res->syrk_launches = sy_launches;
   if (use_loop) {
     trials = fin.nfev - 1 + ((fin.status == 1 || fin.err) ? 1 : 0);
-    g_launches.fetch_add((long long)p->loop_kernels * trials);
+    g_launches.fetch_add((long long)p->loop_graph.n_kernels * trials);
     res->kernel_launches = g_launches.load() - launches0;
   }
   res->trials_queued = trials;
@@ -1274,7 +1210,7 @@ int choose_pcg_config(CbBaProblem* p) {
   auto try_config = [&](int mode, int cs, int cl) -> bool {
     const int rows = (nP + cs - 1) / cs;
     const int npa = std::max((nP + 7) & ~7, mode == 2 ? cl * 32 : 0);
-    const size_t smem = (9 * (size_t)npa + 2 * nw + 2 * 16 * nw + minv + (mode == 0 ? (size_t)rows * nP : 0)) * sizeof(double);
+    const size_t smem = (9 * (size_t)npa + 2 * nw + 2 * 16 * nw + minv) * sizeof(double);
     if (smem > budget) return false;
     if (mode == 2 && rows > 3 * nw) return false;
     const void* fn = (const void*)pcg_fn(mode, P, cl);
@@ -1300,35 +1236,26 @@ int choose_pcg_config(CbBaProblem* p) {
     p->pcg_cs = cs; p->pcg_rows = rows; p->pcg_mode = mode; p->pcg_cl = cl; p->pcg_npa = npa; p->pcg_smem = smem;
     return true;
   };
-  int force_mode = -1;
-  if (const char* ev = std::getenv("CB_PCG_MODE")) force_mode = std::atoi(ev);
-  // (0) small rigs: direct LDL^T in one CTA (force_mode 3, or automatically when it fits)
+  // (0) small rigs: prep, direct LDL^T and camera step in one CTA (small_rig_step_kernel) when it fits
   p->direct_solve = false;
-  if (nP <= cb::DIRECT_MAX_N && (force_mode < 0 || force_mode == 3)) {
+  if (nP <= cb::DIRECT_MAX_N) {
     const size_t smem = ((size_t)(nP + 1) * (nP | 1) + nP) * sizeof(double);
-    if (smem <= budget &&
-        cudaFuncSetAttribute(cb::dense_ldlt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess) {
+    const void* fn = P == 6 ? (const void*)cb::small_rig_step_kernel<6> : (const void*)cb::small_rig_step_kernel<9>;
+    if (smem <= budget && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess) {
       p->direct_solve = true;
       p->direct_smem = smem;
-      if (const char* ev = std::getenv("CB_FUSE_SMALL")) p->fuse_small = std::atoi(ev) != 0;
-      if (p->P == 6) cudaFuncSetAttribute(cb::small_rig_step_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      else cudaFuncSetAttribute(cb::small_rig_step_kernel<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     } else {
       cudaGetLastError();
     }
   }
   // (1) slab in registers: 3 rows x (32 cl) columns per warp; up to 384 reduced parameters in one portable cluster (<= 8
   //     CTAs), up to 576 (64 cameras with free intrinsics) in a 12-CTA cluster (non-portable size, allowed up to 16)
-  if (nP <= 576 && (force_mode < 0 || force_mode == 2)) {
+  if (nP <= 576) {
     const int cl = nP <= 64 ? 2 : nP <= 192 ? 6 : nP <= 384 ? 12 : 18;
     const int cs = (nP + 3 * nw - 1) / (3 * nw);
     if (cs <= 16 && try_config(2, cs, cl)) return CB_OK;
   }
-  // (2) slab in shared memory, smallest cluster that fits
-  if (force_mode < 0 || force_mode == 0)
-    for (int cs : {1, 2, 4, 8, 16})
-      if (try_config(0, cs, 1)) return CB_OK;
-  // (3) slab streamed from L2
+  // (2) larger systems, or a register-mode cluster the device refuses: slab streamed from L2
   if (try_config(1, 8, 1)) return CB_OK;
   g_last_error = "no feasible PCG cluster configuration for n_camera_params = " + std::to_string(nP);
   return CB_E_UNSUPPORTED;
@@ -1501,11 +1428,8 @@ int cb_nccl_comm_destroy(void* comm) {
 int cb_ba_problem_destroy(CbBaProblem* p) {
   if (!p) return CB_OK;
   cudaSetDevice(p->device);
-  destroy_graphs(p);
-  for (auto& g : p->tg) {
-    for (cudaEvent_t e : {g.ev_a, g.ev_b, g.ev_c, g.ev_d})
-      if (e) cudaEventDestroy(e);
-  }
+  destroy_graph(p->trial_graph);
+  destroy_graph(p->loop_graph);
   if (p->cap_stream) cudaStreamDestroy(p->cap_stream);
   for (void* a : p->allocs) cached_free(a);
   cached_free_host(p->h_state);
@@ -1540,8 +1464,7 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
   int nt = 0;
   for (int I = 0; I < nb; ++I)
     for (int J = I; J < nb; ++J) tof[(size_t)I * nb + J] = nt++;
-  double w_pair = 1.55;  // measured cost of a diagonal-pair CTA per k chunk relative to an off-diagonal one
-  if (const char* ev = std::getenv("CB_SY_PAIR_W")) w_pair = std::atof(ev);
+  const double w_pair = 1.55;  // measured cost of a diagonal-pair CTA per k chunk relative to an off-diagonal one
   const double w_single = 0.75;
 
   // per-pair row lists, if sparse: offset of each tile pair's list in d_klist (-1: no common point) and its point count
@@ -1779,7 +1702,6 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   // (8 lanes keep every lane busy for any group size that is not tiny against 8; a whole warp per point only pays when
   // points carry hundreds of rows -- static objects seen in every frame)
   p->pt_lanes = ((double)p->n_obs / std::max(p->n_pts, 1) <= 96.0) ? 8 : 32;
-  if (const char* ev = std::getenv("CB_PT_LANES")) p->pt_lanes = std::atoi(ev) == 8 ? 8 : 32;
   {
     const int per_block = cb::PT_WARPS * (32 / p->pt_lanes);
     p->pt_grid = std::max(1, std::min(cdiv(std::max(p->n_pts, 1), per_block), 2 * p->num_sms));
@@ -2078,11 +2000,12 @@ int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss, double
   CB_TRY(upload_x(p, x, st));
   CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
   CB_TRY(camera_pass<P>(p, 0, 0, st));
-  CB_TRY(build_system<P>(p, &opt, st, nullptr, nullptr));
+  CB_TRY(build_system<P>(p, &opt, st));
+  CB_TRY(solve_step<P>(p, p->d_dp, st));
+  // after solve_step: small rigs apply the damping in small_rig_step_kernel; nothing in solve_step writes d_red otherwise
   const size_t nn = (size_t)p->nP * p->nP;
   std::vector<double> hS(nn + 3 * (size_t)p->nP + 1);
   CB_CUDA(cudaMemcpyAsync(hS.data(), p->d_red, sizeof(double) * hS.size(), cudaMemcpyDeviceToHost, st));
-  CB_TRY(solve_step<P>(p, p->d_dp, st));
   std::vector<double> hU((size_t)p->n_cams * RT::NU), hV(6 * (size_t)std::max(p->n_pts, 1));
   CB_CUDA(cudaMemcpyAsync(hU.data(), p->d_Upk[0], sizeof(double) * hU.size(), cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(hV.data(), p->d_V6, sizeof(double) * hV.size(), cudaMemcpyDeviceToHost, st));
@@ -2143,6 +2066,7 @@ int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32
 // cb_ba_normal_equations call, forcing exactly max_iter iterations (tolerance 0).
 int cb_ba_debug_pcg_time(CbBaProblem* p, int max_iter, int reps, double* ms_per_launch, void* stream) {
   if (!p || !ms_per_launch || reps <= 0) { g_last_error = "cb_ba_debug_pcg_time: bad argument"; return CB_E_INVALID; }
+  if (p->direct_solve) { g_last_error = "cb_ba_debug_pcg_time: this problem is solved directly, not by PCG"; return CB_E_UNSUPPORTED; }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
   CB_TRY(launch_pcg(p, nullptr, 0.0, max_iter, st));
@@ -2395,7 +2319,9 @@ int cb_ba_problem_set_constraints(CbBaProblem* p, int64_t n_c, const int32_t* gr
   CB_TRY(palloc(p, &p->d_camcost, (size_t)p->n_cams + p->n_cblk));
   CB_TRY(palloc(p, &p->d_partial, (size_t)std::max(p->n_chunks, 1) * NACC + p->n_cblk));
   CB_TRY(palloc(p, &p->d_bpart, 3 * ((size_t)p->pt_grid + ncomp)));
-  destroy_graphs(p);  // captured launches hold the old buffer addresses
+  // captured launches hold the old buffer addresses
+  destroy_graph(p->trial_graph);
+  destroy_graph(p->loop_graph);
   CB_CUDA(cudaStreamSynchronize(st));
   p->ct.n_c = nc; p->ct.n_comp = ncomp; p->ct.n_dim_max = ndmax;
   p->ct.c_nu = d_nu; p->ct.c_gidx = d_g; p->ct.c_lidx = d_l; p->ct.c_coef = d_coef; p->ct.c_dist = d_dist; p->ct.c_w = d_w;

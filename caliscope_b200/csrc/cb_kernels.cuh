@@ -11,7 +11,8 @@
 //   schur_finalize_kernel  S = U - Z Z^T, b = g_c - Z t into the all-reduce buffer
 //   reduced_prep_kernel (cb_lm.cuh) Marquardt scaling (running max of diag U, scipy x_scale='jac' analogue,
 //                       site-packages/scipy/optimize/_lsq/common.py:598-610), damping, block-Jacobi inverses
-//   pcg_cluster_kernel  block-Jacobi PCG on the dense reduced system
+//   pcg_cluster_kernel  block-Jacobi PCG on the dense reduced system (small rigs: small_rig_step_kernel, cb_lm.cuh,
+//                       runs damping, a direct LDL^T solve and the camera step in one CTA instead)
 //   cam_step_kernel / pt_backsub_kernel (cb_lm.cuh)   step, bounds clamp, predicted reduction
 #pragma once
 #include <cooperative_groups.h>
@@ -629,7 +630,7 @@ __global__ void schur_finalize_kernel(const LmState* __restrict__ st, int nP, in
 
 // ---------------------------------------------------------------------------------------------
 // PCG on the dense reduced camera system S x = -b, one thread-block cluster.  Each CTA owns a slab
-// of rows of S (resident in shared memory when it fits), computes its slice of w = S u and writes
+// of rows of S, computes its slice of w = S u and writes
 // it into every CTA's w buffer through distributed shared memory; all vector updates and dot
 // products are replicated in every CTA, so the only cluster-wide exchange is that slice.
 // Chronopoulos-Gear single-reduction recurrence: one fused (r.u, w.u) reduction and one cluster
@@ -637,9 +638,9 @@ __global__ void schur_finalize_kernel(const LmState* __restrict__ st, int nP, in
 //   u = M^-1 r, w = S u, g = r.u, d = w.u, beta = g/g_old, alpha = g / (d - beta g / alpha_old)
 //   p = u + beta p, q = w + beta q (= S p), x += alpha p, r -= alpha q
 // ---------------------------------------------------------------------------------------------
-// MODE 0: S slab in shared memory, 1: slab streamed from global/L2, 2: slab in REGISTERS
-// (3 rows x CL columns-per-lane per warp; n_camera_params <= 32*CL, rows_per <= 48) -- the matvec then
-// touches shared memory only for the vector u, instead of re-reading 147 KB of slab per iteration.
+// MODE 1: slab streamed from global/L2 (any size), 2: slab in REGISTERS (3 rows x CL columns-per-lane
+// per warp; n_camera_params <= 32*CL, rows_per <= 48) -- the matvec then touches shared memory only for
+// the vector u.
 //
 // Per iteration: [A] replicated vector update + block-Jacobi solve (each thread recomputes the P residual
 // entries of its camera block, so no barrier is needed between the two), __syncthreads, [B] slab matvec,
@@ -651,7 +652,6 @@ __global__ void __launch_bounds__(PCG_THREADS, 1)
 pcg_cluster_kernel(const LmState* __restrict__ st, const double* __restrict__ S, const double* __restrict__ bvec,
                    const double* __restrict__ Minv, int nP, int nPa, int rows_per, double tol2, int max_iter,
                    double* __restrict__ xout, double* __restrict__ sc) {
-  constexpr bool SLAB_SMEM = (MODE == 0);
   if (st != nullptr) {
     if (st->done) return;  // uniform over the cluster, before any cluster operation
     tol2 = st->pcg_tol2;
@@ -663,7 +663,7 @@ pcg_cluster_kernel(const LmState* __restrict__ st, const double* __restrict__ S,
   cg::cluster_group cluster = cg::this_cluster();
   const int rank = (int)cluster.block_rank(), csize = (int)cluster.num_blocks();
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  // layout: x u p | r[2] q[2] w[2] (nPa each) | gslot[2][NW] | dslot[2][MAXC*NW] | Minv | slab
+  // layout: x u p | r[2] q[2] w[2] (nPa each) | gslot[2][NW] | dslot[2][MAXC*NW] | Minv
   double* vx = psm;
   double* vu = vx + nPa;
   double* vp = vu + nPa;
@@ -673,14 +673,11 @@ pcg_cluster_kernel(const LmState* __restrict__ st, const double* __restrict__ S,
   double* gslot = vw + 2 * nPa;
   double* dslot = gslot + 2 * NW;
   double* Mi = dslot + 2 * MAXC * NW;
-  double* slab = Mi + (((size_t)(nP / P) * P * P + 7) & ~(size_t)7);
   const int row0 = rank * rows_per;
   const int nrows = max(0, min(rows_per, nP - row0));
   const int n_cams = nP / P;
 
   for (int i = tid; i < n_cams * P * P; i += PCG_THREADS) Mi[i] = Minv[i];
-  if (SLAB_SMEM)
-    for (size_t i = tid; i < (size_t)nrows * nP; i += PCG_THREADS) slab[i] = S[(size_t)row0 * nP + i];
   double sreg[MODE == 2 ? 3 : 1][MODE == 2 ? CL : 1];
   if constexpr (MODE == 2) {
 #pragma unroll
@@ -763,7 +760,7 @@ pcg_cluster_kernel(const LmState* __restrict__ st, const double* __restrict__ S,
         }
         s0 = e0 + o0; s1 = e1 + o1; s2 = e2 + o2;
       } else {
-        const double* a0 = SLAB_SMEM ? slab + (size_t)r0 * nP : S + (size_t)(row0 + r0) * nP;
+        const double* a0 = S + (size_t)(row0 + r0) * nP;
         const double* a1 = a0 + (h1 ? nP : 0);
         const double* a2 = a0 + (h2 ? 2 * nP : 0);
         double t0[4] = {0, 0, 0, 0}, t1[4] = {0, 0, 0, 0}, t2[4] = {0, 0, 0, 0};
@@ -772,16 +769,16 @@ pcg_cluster_kernel(const LmState* __restrict__ st, const double* __restrict__ S,
 #pragma unroll
           for (int j = 0; j < 4; ++j) {
             const double uk = vu[k + 32 * j];
-            t0[j] = fma(SLAB_SMEM ? a0[k + 32 * j] : __ldg(a0 + k + 32 * j), uk, t0[j]);
-            t1[j] = fma(SLAB_SMEM ? a1[k + 32 * j] : __ldg(a1 + k + 32 * j), uk, t1[j]);
-            t2[j] = fma(SLAB_SMEM ? a2[k + 32 * j] : __ldg(a2 + k + 32 * j), uk, t2[j]);
+            t0[j] = fma(__ldg(a0 + k + 32 * j), uk, t0[j]);
+            t1[j] = fma(__ldg(a1 + k + 32 * j), uk, t1[j]);
+            t2[j] = fma(__ldg(a2 + k + 32 * j), uk, t2[j]);
           }
         }
         for (; k < nP; k += 32) {
           const double uk = vu[k];
-          t0[0] = fma(SLAB_SMEM ? a0[k] : __ldg(a0 + k), uk, t0[0]);
-          t1[0] = fma(SLAB_SMEM ? a1[k] : __ldg(a1 + k), uk, t1[0]);
-          t2[0] = fma(SLAB_SMEM ? a2[k] : __ldg(a2 + k), uk, t2[0]);
+          t0[0] = fma(__ldg(a0 + k), uk, t0[0]);
+          t1[0] = fma(__ldg(a1 + k), uk, t1[0]);
+          t2[0] = fma(__ldg(a2 + k), uk, t2[0]);
         }
         s0 = (t0[0] + t0[1]) + (t0[2] + t0[3]);
         s1 = (t1[0] + t1[1]) + (t1[2] + t1[3]);
@@ -877,7 +874,8 @@ pcg_cluster_kernel(const LmState* __restrict__ st, const double* __restrict__ S,
 //           a_ij -= a_ik a_jk / d_k  (k < j <= i <= n): one block barrier per step; row n comes out as z = L^-1 (-b)
 //   back substitution L^T x = D^-1 z by warp 0 alone (register-resident, shuffles, no block barrier).
 // Same contract as pcg_cluster_kernel: x solves S x = -b; SC_PCG_FLAG = 1 on a non-positive pivot, 2 on NaN.
-// A small PCG needs ~20 cluster-synchronised iterations per trial; this is one pass of one CTA.
+// A small PCG needs ~20 cluster-synchronised iterations per trial; this is one pass of one CTA, run inside
+// small_rig_step_kernel (cb_lm.cuh).
 // ---------------------------------------------------------------------------------------------
 constexpr int DIRECT_MAX_N = 96;
 constexpr int DIRECT_THREADS = 256;
@@ -942,13 +940,6 @@ __device__ __forceinline__ void dense_ldlt_body(double* __restrict__ dsm, const 
     sc[SC_PCG_REL] = 0.0;
     sc[SC_PCG_FLAG] = (double)flag;
   }
-}
-__global__ void __launch_bounds__(DIRECT_THREADS, 1)
-dense_ldlt_kernel(const LmState* __restrict__ st, const double* __restrict__ S, const double* __restrict__ bvec, int n,
-                  double* __restrict__ xout, double* __restrict__ sc) {
-  extern __shared__ __align__(16) double dsm[];
-  if (st != nullptr && st->done) return;
-  dense_ldlt_body(dsm, S, bvec, n, xout, sc);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -12,6 +12,7 @@
 //   reduced_prep_kernel   damping, gradient norm, gtol / max_nfev tests, block-Jacobi inverses
 //   pcg_cluster_kernel    reduced camera solve
 //   cam_step_kernel       camera step, bounds clamp, predicted reduction, camera table of the trial point
+//                         (n_camera_params <= 96: these three are small_rig_step_kernel, with a direct LDL^T solve)
 //   pt_backsub_kernel     dX = -L^-T (t + L sum Jp^T (Jc dc)), again recomputed from the observation list
 //   resjac_kernel<P,5>    camera-major pass at the TRIAL point: cost, U_c, g_c (these are the next linearisation's
 //                         camera blocks if the step is accepted)

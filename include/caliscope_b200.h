@@ -114,8 +114,8 @@ typedef struct {
   int32_t rank;       /* informational (verbose output only on rank 0) */
   int32_t world_size; /* 1 if allreduce is NULL */
   int32_t time_kernels; /* diagnostic: launch every trial directly with CUDA events around the point pass and the Schur
-                           product (CbBaResult.rj_ms / syrk_ms); 0 (default): the loop is replayed from CUDA graphs, where
-                           events cannot be read back */
+                           product (CbBaResult.rj_ms / syrk_ms); 0 (default): the trials are replayed from CUDA graphs
+                           (see used_graph), where events cannot be read back */
   int32_t pad_;
 } CbBaOptions;
 
@@ -138,7 +138,9 @@ typedef struct {
   double syrk_ms;  /* total device time spent in the Schur product kernel */
   int64_t syrk_launches;
   int64_t trials_queued; /* LM trials handed to the device (the last one runs predicated-off) */
-  int32_t used_graph;    /* 0: trials launched directly, 1: one CUDA graph per trial, 2: device loop (one WHILE-conditional graph per solve) */
+  int32_t used_graph;    /* how the trials ran: 2 device loop, one WHILE-conditional graph per solve (one GPU); 1 one CUDA
+                            graph per trial (sharded over nccl_comm or peer_group); 0 launched directly (allreduce callback,
+                            time_kernels, or a graph that could not be built) */
   int32_t pad_;
 } CbBaResult;
 
@@ -214,7 +216,8 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
                int64_t* n_kept, uint8_t* keep_mask, void* stream);
 
 /* Diagnostic: mean milliseconds of one PCG-kernel launch forced to run exactly max_iter iterations on the
- * system left by the last cb_ba_normal_equations call. */
+ * system left by the last cb_ba_normal_equations call.  CB_E_UNSUPPORTED on problems of at most 96 camera parameters,
+ * which are solved directly (small_rig_step_kernel), not by PCG. */
 int cb_ba_debug_pcg_time(CbBaProblem* p, int max_iter, int reps, double* ms_per_launch, void* stream);
 
 /* Measured fp64 throughput of the device (TFLOP/s): `mma.sync.m8n8k4.f64` (DMMA, the tensor path the Schur product

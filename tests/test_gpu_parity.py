@@ -380,7 +380,8 @@ def test_solve_filter_resolve_loop_matches_scipy_stage_by_stage():
 # ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize(
     "n_cams,refine",
-    [(5, False), (17, False), (33, False), (40, True), (64, False)],  # 30, 102, 198, 360, 384 reduced parameters
+    # 30, 102, 198, 360, 384 reduced parameters; 600 takes the PCG with the slab streamed from L2, over 7 column tiles
+    [(5, False), (17, False), (33, False), (40, True), (64, False), (100, False)],
 )
 def test_schur_system_all_tile_shapes(n_cams, refine):
     from caliscope_b200 import synthetic
