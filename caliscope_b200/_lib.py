@@ -127,6 +127,10 @@ SYMBOLS = {
         C.c_int,
         [_P, _P, C.c_double, C.c_int32, C.c_double, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P],
     ),
+    "cb_ba_covariance": (
+        C.c_int,
+        [_P, _P, C.c_int32, C.c_double, C.c_int32, _P, C.c_double, _P, _P, _P, _P, _P, _P],
+    ),
     "cb_ba_error_order_stats": (C.c_int, [_P, _P, C.c_double, _P, _P, _P, _P, _P]),
     "cb_ba_rmse_px": (C.c_int, [_P, _P, _P, _P, _P]),
     "cb_ba_cull": (C.c_int, [_P, _P, _P, C.c_int32, C.POINTER(_P), _P, _P, _P]),

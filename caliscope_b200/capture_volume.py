@@ -9,6 +9,8 @@ Mirrors /root/reference/src/caliscope/core/capture_volume.py:
                                 same errors (``CalibrationError`` iff ``strict`` and not converged).
   * ``reprojection_report``  == ``CaptureVolume.reprojection_report`` (:150-235): pixel errors from the engine,
                                 per-camera / per-point RMSE by ``np.bincount`` instead of one boolean mask per key.
+  * ``pose_uncertainty``     (no reference counterpart) per-camera position / orientation uncertainty at the current
+                                state, from the arrays optimize() builds (DESIGN.md 4.6).
 
 Everything except the solve itself is the reference's own classes (imported from ``caliscope`` at call
 time); the solve goes to the CUDA engine through ``caliscope_b200.solver.solve_arrays``.
@@ -72,21 +74,18 @@ def ba_arrays(self):
     return camera_indices, image_coords, self.img_to_obj_map[mask], mask
 
 
-def optimize(self, ftol: float = 1e-8, max_nfev: int | None = None, verbose: int = 0, strict: bool = True,
-             use_constraints: bool = True, pixel_sigma: float = 1.0, *, refine_intrinsics: bool = False,
-             loss: str = "linear", f_scale: float = 1.0):  # fmt: skip
-    """Bundle adjustment via pixel-space residuals on the GPU (drop-in for CaptureVolume.optimize)."""
+def _problem_arrays(self, use_constraints: bool, pixel_sigma: float, refine_intrinsics: bool):
+    """The arrays optimize() hands to the solver (capture_volume.py:346-399): (parameterization, its camera array copy,
+    cam_flags, cam_const, camera_indices, image_to_world_indices, image_coords, x0, constraints or None, f_median)."""
     from caliscope.core.bundle_parameterization import BundleParameterization
-    from caliscope.core.capture_volume import _SCIPY_STATUS_REASONS, CaptureVolume, OptimizationStatus
-    from caliscope.core.point_data import WorldPoints
 
     constraints = None
+    focal = [cam.matrix[0, 0] for cam in self.camera_array.posed_cameras.values() if cam.matrix is not None]
+    f_median = float(np.median(focal)) if focal else float("nan")
     if use_constraints and self.constraints is not None:
         arrays = self._build_constraint_arrays()
         if arrays is not None:  # capture_volume.py:373-383
             groups_a, groups_b, distances, sigmas = arrays
-            focal = [cam.matrix[0, 0] for cam in self.camera_array.posed_cameras.values() if cam.matrix is not None]
-            f_median = float(np.median(focal))
             constraints = (groups_a, groups_b, distances, (pixel_sigma / f_median) / sigmas)
             logger.info(f"Adding {len(groups_a)} constraint rows (f_median={f_median:.0f}, pixel_sigma={pixel_sigma})")
     camera_indices, image_coords, image_to_world_indices, _ = ba_arrays(self)
@@ -96,6 +95,19 @@ def optimize(self, ftol: float = 1e-8, max_nfev: int | None = None, verbose: int
     )
     x0 = parameterization.pack(new_camera_array, self.world_points.points)
     flags, const = blocks_to_arrays(parameterization.blocks)
+    return (parameterization, new_camera_array, flags, const, camera_indices, image_to_world_indices, image_coords, x0,
+            constraints, f_median)  # fmt: skip
+
+
+def optimize(self, ftol: float = 1e-8, max_nfev: int | None = None, verbose: int = 0, strict: bool = True,
+             use_constraints: bool = True, pixel_sigma: float = 1.0, *, refine_intrinsics: bool = False,
+             loss: str = "linear", f_scale: float = 1.0):  # fmt: skip
+    """Bundle adjustment via pixel-space residuals on the GPU (drop-in for CaptureVolume.optimize)."""
+    from caliscope.core.capture_volume import _SCIPY_STATUS_REASONS, CaptureVolume, OptimizationStatus
+    from caliscope.core.point_data import WorldPoints
+
+    (parameterization, new_camera_array, flags, const, camera_indices, image_to_world_indices, image_coords, x0,
+     constraints, _) = _problem_arrays(self, use_constraints, pixel_sigma, refine_intrinsics)  # fmt: skip
     logger.info(f"Beginning bundle adjustment on {len(image_coords)} observations")
     result = solver.solve_arrays(
         flags, const, parameterization.n_points, camera_indices, image_to_world_indices, image_coords, x0,
@@ -128,6 +140,25 @@ def optimize(self, ftol: float = 1e-8, max_nfev: int | None = None, verbose: int
         constraints=self.constraints,
         _optimization_status=status,
     )
+
+
+def pose_uncertainty(self, *, refine_intrinsics: bool = False, use_constraints: bool = True, pixel_sigma: float = 1.0):
+    """How well each posed camera is determined by this capture volume's observations, at its current state (normally
+    the result of optimize()): {cam_id: uncertainty.PoseUncertainty, or None for a camera without observations}.
+    Built from the same arrays as optimize(); the covariance is scaled for ``pixel_sigma`` px of image noise,
+    s2 = (pixel_sigma / f_median)^2, and is relative to uncertainty.default_gauge (the first observed camera shows 0)."""
+    from . import uncertainty
+    from .problem import BAProblem
+
+    (_, _, flags, const, camera_indices, image_to_world_indices, image_coords, x0, constraints,
+     f_median) = _problem_arrays(self, use_constraints, pixel_sigma, refine_intrinsics)  # fmt: skip
+    n_points = len(self.world_points.points)
+    with BAProblem(flags, const, n_points, camera_indices, image_to_world_indices, image_coords,
+                   constraints=constraints) as p:  # fmt: skip
+        cov = p.covariance(x0, variance_factor=(pixel_sigma / f_median) ** 2, points=False)
+        offsets = p.cam_offsets
+    poses = uncertainty.camera_poses(x0, offsets, cov.cameras)
+    return {cam_id: poses[i] for cam_id, i in self.camera_array.posed_cam_id_to_index.items()}
 
 
 def _errors_px(camera_array, camera_indices, image_coords, world_coords) -> np.ndarray:

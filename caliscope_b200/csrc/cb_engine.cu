@@ -509,6 +509,14 @@ struct CbBaProblem {
   std::vector<double> h_cdist, h_cw;
   int red_slots = 64;
   CbPeerGroup* peer = nullptr;  // set for the duration of a solve that uses the peer transport
+  // cb_ba_covariance scratch, allocated on its first call: sweep matrix (cov_n^2), column panel, pivot inverse, S_F^-1,
+  // diag of the sweep matrix, pseudo-inverse roots and ranks of V, point covariances, free mask, failure indices
+  int cov_n = 0;
+  double *d_covA = nullptr, *d_covC = nullptr, *d_covD = nullptr, *d_covS = nullptr, *d_covDiag = nullptr,
+         *d_covR = nullptr, *d_covPt = nullptr;
+  int *d_covRank = nullptr, *d_covFail = nullptr;
+  unsigned char* d_covFree = nullptr;
+  float cov_ms[3] = {0.f, 0.f, 0.f};  // last call: linearisation + Schur, dense inverse, point marginals
   size_t red_len() const { return (size_t)nP * nP + 3 * (size_t)nP + 1 + red_slots; }
   cb::CPtr2 c_camtab() const { return {{d_camtab[0], d_camtab[1]}}; }
   cb::Ptr2 m_camtab() const { return {{d_camtab[0], d_camtab[1]}}; }
@@ -774,12 +782,14 @@ void launch_resjac(CbBaProblem* p, const cb::LmState* st_dev, int flip, int loss
             fscale, p->d_partial, out2);
 }
 
-template <int P>
+// COV: the covariance variant (pseudo-inverse root of V into d_covR, rank into d_covRank)
+template <int P, bool COV = false>
 void launch_pt_pass(CbBaProblem* p, cudaStream_t st) {
 #define CB_PT_PASS(LANES, DUPS, SM)                                                                                   \
-  CB_LAUNCH((cb::pt_pass_kernel<P, LANES, DUPS, SM>), p->pt_grid, cb::PT_WARPS * 32, p->pt_smem, st, p->d_state,      \
+  CB_LAUNCH((cb::pt_pass_kernel<P, LANES, DUPS, SM, COV>), p->pt_grid, cb::PT_WARPS * 32, p->pt_smem, st, p->d_state, \
             p->d_pt_start, p->d_pm_cam, p->d_pm_xy, p->d_pt_comp, p->n_pts, p->n_cams, p->c_camtab(), p->c_xp(),       \
-            p->d_V6, p->d_gp, p->d_Dp2, p->d_Linv6, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax)
+            p->d_V6, p->d_gp, p->d_Dp2, COV ? p->d_covR : p->d_Linv6, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax,    \
+            COV ? p->d_covRank : nullptr)
 #define CB_PT_PASS2(LANES, DUPS) do { if (p->cam_in_smem) CB_PT_PASS(LANES, DUPS, true); else CB_PT_PASS(LANES, DUPS, false); } while (0)
   if (p->pt_lanes == 8) { if (p->n_dups) CB_PT_PASS2(8, true); else CB_PT_PASS2(8, false); }
   else { if (p->n_dups) CB_PT_PASS2(32, true); else CB_PT_PASS2(32, false); }
@@ -852,11 +862,13 @@ int camera_pass(CbBaProblem* p, int flip, int mode, cudaStream_t st) {
 
 // damped system at the current point: point pass, Schur product, reduced system (+ all-reduce), head-of-iteration tests
 // (the last at the head of small_rig_step_kernel on small rigs, see solve_step).  ev: nullptr, or four events that
-// bracket the point pass (0, 1) and the Schur product (2, 3)
+// bracket the point pass (0, 1) and the Schur product (2, 3).  cov: the undamped covariance linearisation (point pass with
+// the pseudo-inverse root of V, no reduced_prep_kernel), single rank only
 template <int P>
-int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const cudaEvent_t* ev = nullptr) {
+int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const cudaEvent_t* ev = nullptr, bool cov = false) {
   if (ev) CB_CUDA(cudaEventRecord(ev[0], st));
-  launch_pt_pass<P>(p, st);
+  if (cov) launch_pt_pass<P, true>(p, st);
+  else launch_pt_pass<P>(p, st);
   if (ev) CB_CUDA(cudaEventRecord(ev[1], st));
   if (p->n_c)
     CB_LAUNCH((cb::comp_build_kernel<P>), p->n_comp, cb::CC_THREADS, p->comp_build_smem, st, (const cb::LmState*)p->d_state,
@@ -891,7 +903,7 @@ int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const 
               p->d_red);
     if (sharded(opt)) CB_TRY(do_allreduce(opt, p->d_red, (long long)p->red_len(), st));
   }
-  if (!p->direct_solve)
+  if (!p->direct_solve && !cov)
     CB_LAUNCH((cb::reduced_prep_kernel<P>), 1, 256, 0, st, p->d_state, p->nP, p->n_cams, p->red_slots, p->d_red, p->d_Dc2,
               p->d_active, p->d_Minv, p->d_gmax, p->d_sc);
   return CB_OK;
@@ -1450,6 +1462,7 @@ double cb_ba_problem_stat(const CbBaProblem* p, int what) {
     case 1: return p->schur_flop_issued;
     case 2: return p->direct_solve ? 1.0 : 0.0;
     case 3: return (double)p->n_items;
+    case 4: case 5: case 6: return (double)p->cov_ms[what - 4];
     default: return -1.0;
   }
 }
@@ -1850,6 +1863,10 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
       cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a);   \
       cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
       cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a);  \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
       cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);     \
       cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);    \
       cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);    \
@@ -2060,6 +2077,163 @@ int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32
   cudaStream_t st = (cudaStream_t)stream;
   return p->P == 6 ? normal_eq_impl<6>(p, x, lambda, loss, f_scale, cost, U, gc, V, gp, S, b, dc, dp, st)
                    : normal_eq_impl<9>(p, x, lambda, loss, f_scale, cost, U, gc, V, gp, S, b, dc, dp, st);
+}
+
+}  // extern "C"
+namespace {
+template <int P>
+int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs, int n_fixed, const int32_t* fixed, double vf,
+                    double* cam_cov, double* pt_cov, double* s2_out, int64_t* dof_out, int32_t* pt_rank, cudaStream_t st) {
+  const int nP = p->nP, nc = p->n_cams, npts = std::max(p->n_pts, 1);
+  const size_t nn = (size_t)nP * nP;
+  // free mask (internal slot order): the camera's own slots, camera observed, not fixed
+  std::vector<int> cs(nc + 1);
+  CB_CUDA(cudaMemcpyAsync(cs.data(), p->d_cam_start, sizeof(int) * (nc + 1), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  std::vector<char> is_fixed((size_t)p->ncp, 0);
+  for (int i = 0; i < n_fixed; ++i) is_fixed[fixed[i]] = 1;
+  std::vector<unsigned char> fr((size_t)nP, 0);
+  std::vector<int> xidx((size_t)nP, -1);  // caller x index of each internal slot (-1: padding)
+  long long n_masked = 0, n_fix = 0;
+  for (int i = 0; i < nc; ++i) {
+    const int c = p->h_perm[i], w = p->h_cam_off[c + 1] - p->h_cam_off[c];
+    const bool observed = cs[i + 1] > cs[i];
+    for (int a = 0; a < w; ++a) {
+      const int xi = p->h_cam_off[c] + a;
+      xidx[(size_t)i * P + a] = xi;
+      if (!observed) ++n_masked;
+      else if (is_fixed[xi]) ++n_fix;
+      else fr[(size_t)i * P + a] = 1;
+    }
+  }
+  if (!p->d_covA) {
+    const int n = (int)cdiv(nP, cb::CV_B) * cb::CV_B;
+    CB_TRY(palloc(p, &p->d_covA, (size_t)n * n));
+    CB_TRY(palloc(p, &p->d_covC, (size_t)n * cb::CV_B));
+    CB_TRY(palloc(p, &p->d_covD, (size_t)cb::CV_B * cb::CV_B));
+    CB_TRY(palloc(p, &p->d_covDiag, (size_t)n));
+    CB_TRY(palloc(p, &p->d_covS, nn));
+    CB_TRY(palloc(p, &p->d_covR, 9 * (size_t)npts));
+    CB_TRY(palloc(p, &p->d_covPt, 9 * (size_t)npts));
+    CB_TRY(palloc(p, &p->d_covRank, (size_t)npts));
+    CB_TRY(palloc(p, &p->d_covFail, 2));
+    CB_TRY(palloc(p, &p->d_covFree, (size_t)nP));
+    p->cov_n = n;
+  }
+  const int n = p->cov_n;
+  CbBaOptions opt;
+  cb_ba_default_options(&opt);
+  opt.loss = loss; opt.f_scale = fs;
+  opt.ftol = opt.xtol = opt.gtol = 0.0;
+  CB_CUDA(cudaEventRecord(p->ev0, st));
+  CB_TRY(init_state(p, &opt, 0.0, 1ll << 40, st));
+  CB_CUDA(cudaMemsetAsync(p->d_covRank, 0, sizeof(int) * npts, st));
+  const int big[2] = {INT32_MAX, INT32_MAX};
+  CB_CUDA(cudaMemcpyAsync(p->d_covFail, big, sizeof(big), cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(p->d_covFree, fr.data(), nP, cudaMemcpyHostToDevice, st));
+  CB_TRY(upload_x(p, x, st));
+  CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
+  CB_TRY(camera_pass<P>(p, 0, 0, st));
+  CB_TRY(build_system<P>(p, &opt, st, nullptr, true));
+  if (p->n_c) CB_LAUNCH(cb::comp_failed_kernel, cdiv(p->n_comp, 128), 128, 0, st, p->ct, (const double*)p->d_compL, p->d_covFail + 1);
+  CB_CUDA(cudaEventRecord(p->ev1, st));
+  // dense inverse of the gauge-fixed reduced system
+  CB_LAUNCH(cb::cov_prep_kernel, cdiv((long long)n * n, 256), 256, 0, st, (const double*)p->d_red, nP,
+            (const unsigned char*)p->d_covFree, n, p->d_covA, p->d_covDiag);
+  for (int kb = 0; kb < n; kb += cb::CV_B) {
+    CB_LAUNCH(cb::cov_sweep_pivot_kernel, 1, cb::CV_B * cb::CV_B, 0, st, (const double*)p->d_covA, n, kb,
+              (const double*)p->d_covDiag, CB_COV_PIVOT_RTOL, p->d_covD, p->d_covC, p->d_covFail);
+    CB_LAUNCH(cb::cov_sweep_update_kernel, dim3(n / cb::CV_B, n / cb::CV_B), cb::CV_B * cb::CV_B, 0, st, p->d_covA, n, kb,
+              (const double*)p->d_covD, (const double*)p->d_covC);
+  }
+  CB_LAUNCH(cb::cov_finish_kernel, cdiv((long long)nn, 256), 256, 0, st, (const double*)p->d_covA, n, nP,
+            (const unsigned char*)p->d_covFree, p->d_covS);
+  CB_CUDA(cudaEventRecord(p->ev2, st));
+  double cost = 0.0;
+  int fail[2];
+  std::vector<int> rank((size_t)npts);
+  CB_CUDA(cudaMemcpyAsync(&cost, p->d_red + nn + 3 * (size_t)nP, sizeof(double), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(fail, p->d_covFail, sizeof(fail), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rank.data(), p->d_covRank, sizeof(int) * npts, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  char msg[256];
+  if (fail[1] != INT32_MAX) {
+    std::snprintf(msg, sizeof msg, "cb_ba_covariance: constraint component %d is not positive definite at lambda = 0", fail[1]);
+    g_last_error = msg;
+    return CB_E_INVALID;
+  }
+  if (fail[0] != INT32_MAX) {
+    const int slot = fail[0] / P, a = fail[0] % P;
+    std::snprintf(msg, sizeof msg,
+                  "cb_ba_covariance: the gauge-fixed reduced camera system is singular: the pivot of camera %d parameter %d "
+                  "(x index %d) collapsed below %.0e of its diagonal; fix more parameters (see default_gauge)",
+                  p->h_perm[slot], a, xidx[fail[0]], CB_COV_PIVOT_RTOL);
+    g_last_error = msg;
+    return CB_E_INVALID;
+  }
+  long long null_pts = 0;
+  for (int j = 0; j < p->n_pts; ++j)
+    if (rank[j] >= 0) null_pts += 3 - rank[j];
+  const long long m = 2ll * p->n_obs + p->n_c;
+  const long long rk = (long long)p->n_params - n_fix - n_masked - null_pts;
+  const long long dof = m - rk;
+  const double s2 = vf > 0.0 ? vf : (dof > 0 ? 2.0 * cost / (double)dof : std::nan(""));
+  if (s2_out) *s2_out = s2;
+  if (dof_out) *dof_out = dof;
+  if (pt_rank) std::memcpy(pt_rank, rank.data(), sizeof(int) * p->n_pts);
+  if (pt_cov && p->n_pts > 0) {
+    CB_LAUNCH((cb::cov_point_kernel<P>), 4 * p->num_sms, 256, 0, st, (const int*)p->d_pt_start, (const int*)p->d_pm_cam,
+              p->n_pts, (const double*)p->d_Zt, (size_t)p->LD, (const double*)p->d_covS, nP, (const double*)p->d_covR,
+              (const int*)p->d_covRank, s2, p->d_covPt);
+  }
+  CB_CUDA(cudaEventRecord(p->ev3, st));
+  if (pt_cov && p->n_pts > 0)
+    CB_CUDA(cudaMemcpyAsync(pt_cov, p->d_covPt, sizeof(double) * 9 * p->n_pts, cudaMemcpyDeviceToHost, st));
+  std::vector<double> hS;
+  if (cam_cov) {
+    hS.resize(nn);
+    CB_CUDA(cudaMemcpyAsync(hS.data(), p->d_covS, sizeof(double) * nn, cudaMemcpyDeviceToHost, st));
+  }
+  CB_CUDA(cudaStreamSynchronize(st));
+  CB_CUDA(cudaEventElapsedTime(&p->cov_ms[0], p->ev0, p->ev1));
+  CB_CUDA(cudaEventElapsedTime(&p->cov_ms[1], p->ev1, p->ev2));
+  CB_CUDA(cudaEventElapsedTime(&p->cov_ms[2], p->ev2, p->ev3));
+  if (cam_cov) {
+    // caller layout: NaN rows / columns for the cameras without observations, zero for the fixed parameters
+    const size_t ncp = (size_t)p->ncp;
+    std::vector<double> rowv(ncp);
+    for (int i = 0; i < nc; ++i) {
+      const bool observed = cs[i + 1] > cs[i];
+      const int c = p->h_perm[i];
+      for (int a = p->h_cam_off[c]; a < p->h_cam_off[c + 1]; ++a) rowv[a] = observed ? 0.0 : std::nan("");
+    }
+    for (size_t i = 0; i < ncp; ++i)
+      for (size_t j = 0; j < ncp; ++j) cam_cov[i * ncp + j] = std::isnan(rowv[i]) ? rowv[i] : rowv[j];
+    for (int i = 0; i < nP; ++i) {
+      if (!fr[i]) continue;
+      for (int j = 0; j < nP; ++j)
+        if (fr[j]) cam_cov[(size_t)xidx[i] * ncp + xidx[j]] = s2 * hS[(size_t)i * nP + j];
+    }
+  }
+  return CB_OK;
+}
+}  // namespace
+extern "C" {
+
+int cb_ba_covariance(CbBaProblem* p, const double* x, int32_t loss, double f_scale, int32_t n_fixed, const int32_t* fixed,
+                     double variance_factor, double* cam_cov, double* pt_cov, double* s2_out, int64_t* dof_out,
+                     int32_t* pt_rank, void* stream) {
+  if (!p || !x || (n_fixed > 0 && !fixed) || n_fixed < 0) { g_last_error = "cb_ba_covariance: null argument"; return CB_E_INVALID; }
+  if (loss < CB_LOSS_LINEAR || loss > CB_LOSS_ARCTAN) { g_last_error = "cb_ba_covariance: unknown loss"; return CB_E_INVALID; }
+  for (int i = 0; i < n_fixed; ++i)
+    if (fixed[i] < 0 || fixed[i] >= p->ncp) {
+      g_last_error = "cb_ba_covariance: fixed index " + std::to_string(fixed[i]) + " is outside the camera section of x";
+      return CB_E_INVALID;
+    }
+  CB_CUDA(cudaSetDevice(p->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  return p->P == 6 ? covariance_impl<6>(p, x, loss, f_scale, n_fixed, fixed, variance_factor, cam_cov, pt_cov, s2_out, dof_out, pt_rank, st)
+                   : covariance_impl<9>(p, x, loss, f_scale, n_fixed, fixed, variance_factor, cam_cov, pt_cov, s2_out, dof_out, pt_rank, st);
 }
 
 // Diagnostic: time `reps` launches of the PCG kernel on the system left by the last

@@ -22,7 +22,7 @@
 // The decision follows scipy's TRF bookkeeping (site-packages/scipy/optimize/_lsq/trf.py:465-560,
 // common.py:705-717): nfev / njev / nit count the same events, termination statuses 0..4 are scipy's.
 #pragma once
-#include "cb_kernels.cuh"
+#include "cb_covariance.cuh"
 
 namespace cb {
 
@@ -51,13 +51,34 @@ __device__ __forceinline__ double group_sum(double v) {
 // CAMSM: the camera table is staged in shared memory (it fits: <= 64 KB).  A template parameter, not a run-time pointer
 // select: with a pointer that may be shared or global the compiler emits GENERIC loads (LD.E) for the ~36 table reads per
 // observation, which wait on the long scoreboard like global loads (ncu: 55 % of the stalls of the first version).
-template <int P, int LANES, bool DUPS, bool CAMSM>
+//
+// COV: the covariance linearisation (cb_covariance.cuh).  The damping is ignored and the factor is the pseudo-inverse root R
+// of V (V^+ = R^T R, 9 values per point into Linv6, rank(V) into pt_rank, -1 for component points); Z = (Jc^T Jp) R^T,
+// t = 0, and neither Dp2 nor the gradient norm is touched.
+template <bool COV>
+__device__ __forceinline__ void pt_factor_rows(const double* JX, const double* Li, double& q00, double& q01, double& q02,
+                                               double& q10, double& q11, double& q12) {
+  if constexpr (COV) {
+    q00 = JX[0] * Li[0] + JX[1] * Li[1] + JX[2] * Li[2];
+    q01 = JX[0] * Li[3] + JX[1] * Li[4] + JX[2] * Li[5];
+    q02 = JX[0] * Li[6] + JX[1] * Li[7] + JX[2] * Li[8];
+    q10 = JX[3] * Li[0] + JX[4] * Li[1] + JX[5] * Li[2];
+    q11 = JX[3] * Li[3] + JX[4] * Li[4] + JX[5] * Li[5];
+    q12 = JX[3] * Li[6] + JX[4] * Li[7] + JX[5] * Li[8];
+  } else {
+    q00 = JX[0] * Li[0]; q01 = JX[0] * Li[1] + JX[1] * Li[2]; q02 = JX[0] * Li[3] + JX[1] * Li[4] + JX[2] * Li[5];
+    q10 = JX[3] * Li[0]; q11 = JX[3] * Li[1] + JX[4] * Li[2]; q12 = JX[3] * Li[3] + JX[4] * Li[4] + JX[5] * Li[5];
+  }
+}
+
+template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false>
 __global__ void __launch_bounds__(PT_WARPS * 32, 2)
 pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start, const int* __restrict__ pm_cam,
                const double2* __restrict__ pm_xy, const int* __restrict__ pt_comp, int n_pts, int n_cams,
                CPtr2 camtab2, CPtr2 xp2, double* __restrict__ V6, double* __restrict__ gp,
                double* __restrict__ Dp2, double* __restrict__ Linv6, double* __restrict__ tvec,
-               double* __restrict__ Zt, size_t LD, unsigned long long* __restrict__ gmax_bits) {
+               double* __restrict__ Zt, size_t LD, unsigned long long* __restrict__ gmax_bits,
+               int* __restrict__ pt_rank = nullptr) {
   extern __shared__ __align__(16) double pt_sm[];
   __shared__ double wmax[PT_WARPS];
   if (st->done) return;
@@ -118,10 +139,32 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
       const double* d = Dp2 + (size_t)j * 3;
       D[0] = fmax(d[0], v[0]); D[1] = fmax(d[1], v[3]); D[2] = fmax(d[2], v[5]);
     }
-    double Li[6];
-    if (in_comp) { Li[0] = 1.0; Li[1] = 0.0; Li[2] = 1.0; Li[3] = 0.0; Li[4] = 0.0; Li[5] = 1.0; }
-    else chol3_inv(v, D, lam, Li);
-    if (valid && gl == 0) {
+    constexpr int NL = COV ? 9 : 6;
+    double Li[NL];
+    int rank = -1;
+    if (in_comp) {
+#pragma unroll
+      for (int k = 0; k < NL; ++k) Li[k] = 0.0;
+      if constexpr (COV) Li[0] = Li[4] = Li[8] = 1.0;
+      else Li[0] = Li[2] = Li[5] = 1.0;
+    } else {
+      if constexpr (COV) pinv_root3(v, Li, rank);
+      else chol3_inv(v, D, lam, Li);
+    }
+    if constexpr (COV) {
+      if (valid && gl == 0) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) V6[(size_t)j * 6 + k] = v[k];
+#pragma unroll
+        for (int k = 0; k < 9; ++k) Linv6[(size_t)j * 9 + k] = Li[k];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) gp[(size_t)j * 3 + k] = v[6 + k];
+        if (!in_comp)
+#pragma unroll
+          for (int k = 0; k < 3; ++k) tvec[3 * (size_t)j + k] = 0.0;
+        pt_rank[j] = rank;
+      }
+    } else if (valid && gl == 0) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) V6[(size_t)j * 6 + k] = v[k];
 #pragma unroll
@@ -146,8 +189,8 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
         const double2 xy = xy_n;
         if (pos + LANES < e) { cam_n = pm_cam[pos + LANES]; xy_n = pm_xy[pos + LANES]; }
         obs_jac<P>(cam_entry(cam), X0, X1, X2, xy.x, xy.y, loss, fscale, f, JX, Jc);
-        const double q00 = JX[0] * Li[0], q01 = JX[0] * Li[1] + JX[1] * Li[2], q02 = JX[0] * Li[3] + JX[1] * Li[4] + JX[2] * Li[5];
-        const double q10 = JX[3] * Li[0], q11 = JX[3] * Li[1] + JX[4] * Li[2], q12 = JX[3] * Li[3] + JX[4] * Li[4] + JX[5] * Li[5];
+        double q00, q01, q02, q10, q11, q12;
+        pt_factor_rows<COV>(JX, Li, q00, q01, q02, q10, q11, q12);
 #pragma unroll
         for (int p = 0; p < P; ++p) {
           z[0][p] = fma(Jc[p], q00, Jc[P + p] * q10);
@@ -165,8 +208,8 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
         do {
           const double2 xy = pm_xy[r];
           obs_jac<P>(cam_entry(cam), X0, X1, X2, xy.x, xy.y, loss, fscale, f, JX, Jc);
-          const double q00 = JX[0] * Li[0], q01 = JX[0] * Li[1] + JX[1] * Li[2], q02 = JX[0] * Li[3] + JX[1] * Li[4] + JX[2] * Li[5];
-          const double q10 = JX[3] * Li[0], q11 = JX[3] * Li[1] + JX[4] * Li[2], q12 = JX[3] * Li[3] + JX[4] * Li[4] + JX[5] * Li[5];
+          double q00, q01, q02, q10, q11, q12;
+          pt_factor_rows<COV>(JX, Li, q00, q01, q02, q10, q11, q12);
 #pragma unroll
           for (int p = 0; p < P; ++p) {
             z[0][p] = fma(Jc[p], q00, fma(Jc[P + p], q10, z[0][p]));

@@ -34,6 +34,23 @@ def blocks_to_arrays(blocks) -> tuple[np.ndarray, np.ndarray]:
 
 
 @dataclass
+class Covariance:
+    """``BAProblem.covariance``: parameter covariance at x, relative to the gauge ``fixed`` (DESIGN.md section 4.6).
+
+    ``cameras``: (n_camera_params, n_camera_params) in x's camera layout; rows and columns of fixed parameters are 0,
+    those of cameras without observations NaN.  ``points``: (n_pts, 3, 3), NaN where ``point_rank`` is not 3 (points
+    seen by one camera, unobserved points, points of rigid-constraint components, rank -1).  ``variance_factor``: the s2
+    the inverse was scaled by; ``dof``: m - rank of the gauge-fixed Jacobian."""
+
+    cameras: np.ndarray
+    points: np.ndarray | None
+    point_rank: np.ndarray
+    variance_factor: float
+    dof: int
+    fixed: np.ndarray
+
+
+@dataclass
 class SolveResult:
     """Fields of scipy's OptimizeResult that the reference reads (capture_volume.py:413-433) plus counters."""
 
@@ -269,6 +286,37 @@ class BAProblem:
         )  # fmt: skip
         out["cost"] = cost.value
         return out
+
+    def covariance(self, x, *, loss: str = "linear", f_scale: float = 1.0, fixed=None, variance_factor=None,
+                   points: bool = True, stream: int = 0) -> Covariance:
+        """Covariance of the parameters at x (normally a solution of the same loss), ``cb_ba_covariance``.
+        ``fixed``: indices into x's camera section held fixed to remove the gauge; None: ``uncertainty.default_gauge``.
+        ``variance_factor``: s2 (e.g. ``(pixel_sigma / fx) ** 2``); None: 2 cost / dof.  The problem must hold every
+        observation (not one rank's shard)."""
+        from . import uncertainty
+
+        if loss not in L.LOSS_IDS:
+            raise ValueError(f"`loss` must be one of {list(L.LOSS_IDS)}")
+        x = self._x(x)
+        if fixed is None:
+            observed = self.error_order_stats(x, 50.0, stream, want_err=False)[3] > 0
+            fixed = uncertainty.default_gauge(x, self.cam_offsets, observed, self.n_constraints > 0)
+        fixed = np.ascontiguousarray(fixed, dtype=np.int32).ravel()
+        cam = np.empty((self.n_camera_params, self.n_camera_params))
+        pts = np.empty((self.n_pts, 3, 3)) if points else None
+        rank = np.empty(self.n_pts, np.int32)
+        s2 = C.c_double()
+        dof = C.c_int64()
+        L.check(
+            self._lib.cb_ba_covariance(
+                self._h, _ptr(x), L.LOSS_IDS[loss], float(f_scale), len(fixed), _ptr(fixed) if len(fixed) else None,
+                float(variance_factor) if variance_factor is not None else 0.0, _ptr(cam), _ptr(pts) if points else None,
+                C.addressof(s2), C.addressof(dof), _ptr(rank), C.c_void_p(stream),
+            ),
+            "covariance",
+        )  # fmt: skip
+        return Covariance(cameras=cam, points=pts, point_rank=rank, variance_factor=s2.value, dof=int(dof.value),
+                          fixed=fixed)  # fmt: skip
 
     def error_order_stats(self, x, q_percent: float, stream: int = 0, want_err: bool = True):
         x = self._x(x)

@@ -195,6 +195,29 @@ int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32
                            double* cost, double* U, double* gc, double* V, double* gp, double* S, double* b,
                            double* dc, double* dp, void* stream);
 
+/* Covariance of the parameters at x (normally a solution), DESIGN.md section 4.6.  With J the engine's residual Jacobian
+ * (pixels / fx_initial, then the constraint rows) after the robust row rescaling at x:
+ *   Sigma = s2 * (J_F^T J_F)^-1,  F = parameters neither fixed nor masked,
+ * through the Schur complement at lambda = 0 with the pseudo-inverse of every 3x3 point block V_j (a point seen by one
+ * camera has rank(V_j) = 2, an unobserved point 0: their null directions are not parameters of F).
+ *   fixed: n_fixed indices into x's camera section (caller layout), the gauge (caliscope_b200.uncertainty.default_gauge);
+ *          their rows and columns of cam_cov are 0.
+ *   masked: every parameter of a camera without observations; NaN rows and columns of cam_cov.
+ *   variance_factor > 0: s2 as given (e.g. (pixel_sigma / fx)^2); <= 0: s2 = 2 cost / dof with dof = m - rank,
+ *          m = 2 n_obs + n_c, rank = n_params - |fixed| - |masked| - sum_j (3 - rank V_j) over unconstrained points.
+ *   cam_cov (nullable): n_camera_params^2, caller layout.  pt_cov (nullable): n_pts*9, NaN for points with a rank
+ *          deficient V_j and for points of rigid-constraint components.  pt_rank (nullable): n_pts, rank of V_j, -1 for
+ *          component points.  s2_out / dof_out nullable.
+ * Fails with CB_E_INVALID when the gauge-fixed reduced system S_F is not positive definite (a Cholesky pivot at or below
+ * CB_COV_PIVOT_RTOL times the parameter's diagonal of S_F; cb_ba_last_error() names the camera and parameter), or when a
+ * constraint component's block is not positive definite at lambda = 0.  The problem must hold every observation: a
+ * per-rank shard of a sharded problem holds only part of the information.  cb_ba_problem_stat(p, 4 / 5 / 6) give the
+ * last call's milliseconds (CUDA events) in linearisation + Schur product, dense inverse, and point marginals. */
+#define CB_COV_PIVOT_RTOL 1e-10
+int cb_ba_covariance(CbBaProblem* p, const double* x, int32_t loss, double f_scale, int32_t n_fixed, const int32_t* fixed,
+                     double variance_factor, double* cam_cov, double* pt_cov, double* s2_out, int64_t* dof_out,
+                     int32_t* pt_rank, void* stream);
+
 /* Per-camera order statistics of the pixel error norm for the percentile filter
  * (capture_volume.py:709-753): for camera c with n_c observations, lo[c] / hi[c] are the
  * floor / ceil order statistics of rank (n_c - 1) * q / 100 (numpy's linear interpolation
