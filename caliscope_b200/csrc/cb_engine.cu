@@ -1463,6 +1463,13 @@ double cb_ba_problem_stat(const CbBaProblem* p, int what) {
     case 2: return p->direct_solve ? 1.0 : 0.0;
     case 3: return (double)p->n_items;
     case 4: case 5: case 6: return (double)p->cov_ms[what - 4];
+    case 7: return (double)p->pt_lanes;
+    case 8: return p->n_dups ? 1.0 : 0.0;
+    case 9: return (double)p->cam_in_smem;
+    case 10: return p->direct_solve ? 0.0 : (double)p->pcg_mode;
+    case 11: return (double)p->pcg_cs;
+    case 12: return p->pcg_mode == 2 ? (double)p->pcg_cl : 0.0;
+    case 13: return p->order_identity ? 0.0 : 1.0;
     default: return -1.0;
   }
 }

@@ -15,6 +15,28 @@ def _ptr(a: np.ndarray) -> int:
     return a.ctypes.data
 
 
+def _check_device_obs(obs_cam, obs_pt, obs_xy, device: int) -> int:
+    """Validate a device-resident observation list, which the engine reads in place: CUDA tensors on ``device``,
+    contiguous, equal lengths; obs_cam int32 or int16, obs_pt int32, obs_xy float64 (n, 2).  Returns obs_cam's width in
+    bits.  Nothing is converted: a conversion would be a copy the caller did not ask for."""
+    dtypes = {"obs_cam": ("torch.int32", "torch.int16"), "obs_pt": ("torch.int32",), "obs_xy": ("torch.float64",)}
+    arrays = {"obs_cam": obs_cam, "obs_pt": obs_pt, "obs_xy": obs_xy}
+    for name, a in arrays.items():
+        dev = getattr(a, "device", None)
+        if getattr(dev, "type", None) != "cuda" or dev.index != device:
+            raise ValueError(f"{name} must be a CUDA tensor on cuda:{device}, got device {dev}")
+        if str(getattr(a, "dtype", None)) not in dtypes[name]:
+            raise ValueError(f"{name} must have dtype {' or '.join(dtypes[name])}, got {getattr(a, 'dtype', None)}")
+        if not a.is_contiguous():
+            raise ValueError(f"{name} must be contiguous")
+    n = int(obs_cam.shape[0])
+    if tuple(obs_cam.shape) != (n,) or tuple(obs_pt.shape) != (n,):
+        raise ValueError(f"obs_cam and obs_pt must be 1-D of the same length, got {tuple(obs_cam.shape)}, {tuple(obs_pt.shape)}")
+    if tuple(obs_xy.shape) != (n, 2):
+        raise ValueError(f"obs_xy must have shape ({n}, 2), got {tuple(obs_xy.shape)}")
+    return 16 if str(obs_cam.dtype) == "torch.int16" else 32
+
+
 def blocks_to_arrays(blocks) -> tuple[np.ndarray, np.ndarray]:
     """``BundleParameterization.blocks`` (bundle_parameterization.py:36-51) -> (cam_flags, cam_const)."""
     flags = np.zeros(len(blocks), np.int32)
@@ -93,8 +115,9 @@ class SolveResult:
 class BAProblem:
     """One observation list + camera table on one GPU.
 
-    ``obs_*`` may be NumPy arrays (copied host->device inside the constructor) or CUDA tensors /
-    objects exposing ``data_ptr()`` on ``device`` (used in place, no copy).
+    ``obs_*`` may be NumPy arrays (copied host->device inside the constructor) or contiguous CUDA tensors on ``device``
+    (used in place, no copy): obs_cam int32 or int16, obs_pt int32, obs_xy float64 of shape (n, 2).  Tensors of any
+    other dtype, device, layout or length raise ValueError.
     """
 
     def __init__(self, cam_flags, cam_const, n_pts, obs_cam, obs_pt, obs_xy, *, constraints=None, device: int = 0,
@@ -112,6 +135,7 @@ class BAProblem:
         on_dev = hasattr(obs_cam, "data_ptr")
         cam_bits = 32
         if on_dev:
+            cam_bits = _check_device_obs(obs_cam, obs_pt, obs_xy, self.device)
             keep = (obs_cam, obs_pt, obs_xy)
             n_obs = int(obs_cam.shape[0])
             ptrs = (obs_cam.data_ptr(), obs_pt.data_ptr(), obs_xy.data_ptr())
@@ -182,7 +206,11 @@ class BAProblem:
         self.close()
 
     def stat(self, what: int) -> float:
-        """``cb_ba_problem_stat``: 0 sparse Schur lists in use, 1 flops per Schur-product launch, 2 direct reduced solve, 3 Schur CTAs."""
+        """``cb_ba_problem_stat``: 0 sparse Schur lists in use, 1 flops per Schur-product launch, 2 direct reduced solve,
+        3 Schur CTAs, 4-6 stage milliseconds of the last ``covariance`` call, 7 lanes per point (8 or 32), 8 repeated
+        (camera, point) rows, 9 camera table in shared memory, 10 reduced solve (0 direct, 1 L2-streamed PCG, 2 register
+        PCG), 11 PCG cluster CTAs, 12 register-PCG columns per lane (0 otherwise), 13 internal camera order differs from
+        the caller's numbering.  -1 for an unknown key."""
         return float(self._lib.cb_ba_problem_stat(self._h, int(what)))
 
     def _x(self, x) -> np.ndarray:

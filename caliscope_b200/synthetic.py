@@ -85,6 +85,28 @@ def _ring_cameras(n_cams: int):
     return np.array(rv), np.array(tv)
 
 
+def _dome_cameras(n_cams: int):
+    """Cameras spread evenly (golden-angle spiral, equal area) over a spherical cap of radius 3 m between 10 and 60
+    degrees of elevation around the centre of the point cylinder, each looking at that centre: every camera sees nearly
+    every point, so the camera count can grow without cameras that see nothing."""
+    centre = np.array([0.0, 0.0, 0.6])
+    lo, hi = np.sin(np.radians(10.0)), np.sin(np.radians(60.0))
+    rv, tv = [], []
+    for i in range(n_cams):
+        sz = lo + (hi - lo) * (i + 0.5) / n_cams
+        az = i * np.pi * (3.0 - np.sqrt(5.0))
+        pos = centre + 3.0 * np.array([np.sqrt(1.0 - sz * sz) * np.cos(az), np.sqrt(1.0 - sz * sz) * np.sin(az), sz])
+        fwd = centre - pos
+        fwd /= np.linalg.norm(fwd)
+        right = np.cross(fwd, [0.0, 0.0, 1.0])
+        right /= np.linalg.norm(right)
+        down = np.cross(fwd, right)
+        R = np.stack([right, down, fwd])  # world -> camera
+        rv.append(_rodrigues_vec(R))
+        tv.append(-R @ pos)
+    return np.array(rv), np.array(tv)
+
+
 def _project_pinhole(X, rvec, tvec, fx, fy, cx, cy, dist):
     k1, k2, p1, p2, k3 = dist
     Xc = X @ _rot(rvec).T + tvec
@@ -108,12 +130,17 @@ def make_rig(
     outlier_px: float = 50.0,
     name: str = "",
     cams_per_point: int | None = None,
+    layout: str = "ring",
 ) -> SyntheticRig:
-    """``cams_per_point``: local visibility -- every point faces a random azimuth and is seen only by the
+    """``layout``: "ring" -- rings of 16 inward-facing cameras stacked upward (above the fifth ring the cameras see
+    almost no points); "dome" -- cameras over a spherical cap, each seeing nearly every point (``_dome_cameras``).
+    ``cams_per_point``: local visibility -- every point faces a random azimuth and is seen only by the
     ``cams_per_point`` in-frame cameras nearest to that direction (a marker on a subject inside a ring rig: the
     realistic Caliscope shape, 2-8 cameras per point), instead of by a uniform random subset of all cameras."""
+    if layout not in ("ring", "dome"):
+        raise ValueError(f"layout must be 'ring' or 'dome', got {layout!r}")
     rng = np.random.default_rng(seed)
-    rvec, tvec = _ring_cameras(n_cams)
+    rvec, tvec = _ring_cameras(n_cams) if layout == "ring" else _dome_cameras(n_cams)
     w, h = WEBCAM_SIZE
     cx, cy = w / 2.0, h / 2.0
 

@@ -155,7 +155,12 @@ int cb_ba_problem_destroy(CbBaProblem* p);
 int64_t cb_ba_problem_n_params(const CbBaProblem* p);
 /* Facts about how the engine laid the problem out (measurement / diagnostics): what = 0: 1 if the Schur product walks
  * compacted row lists (sparse visibility), 1: floating-point operations one Schur-product launch issues, 2: 1 if the reduced
- * system is solved directly (<= 96 camera parameters), 3: CTAs of the Schur product.  -1 for an unknown key. */
+ * system is solved directly (<= 96 camera parameters), 3: CTAs of the Schur product, 4 / 5 / 6: see cb_ba_covariance,
+ * 7: lanes per point in the point kernels (8, or 32 when points average more than 96 rows), 8: 1 if some (camera, point)
+ * pair has repeated rows, 9: 1 if the point kernels stage the camera table in shared memory, 10: reduced solve (0 direct,
+ * 1 PCG with the slab streamed from L2, 2 PCG with the slab in registers), 11: CTAs of the PCG cluster, 12: matrix
+ * columns per lane of the register PCG (0 otherwise), 13: 1 if the internal camera order is not the caller's numbering.
+ * -1 for an unknown key. */
 double cb_ba_problem_stat(const CbBaProblem* p, int what);
 
 /* Rigid-distance constraint rows (reprojection.py:112-117 and :207-226): groups_a / groups_b are n_c x 4 world-point

@@ -83,7 +83,10 @@ def schur_system(lin: Linearization, rig: O.Rig, lam: float, Dc2: np.ndarray, Dp
     Wd = np.zeros((rig.n_pts, n_cams, P, 3))
     np.add.at(Wd, (rig.obs_pt, rig.obs_cam), W)
     Y = np.einsum("jcpa,jab->jcpb", Wd, Einv)
-    S4 = -np.einsum("jcpa,jdqa->cpdq", Y, Wd)
+    # sum over points j and point coordinates a as one (n_cams P) x (n_pts 3) matrix product
+    Y2 = Y.transpose(1, 2, 0, 3).reshape(n_cams * P, -1)
+    W2 = Wd.transpose(1, 2, 0, 3).reshape(n_cams * P, -1)
+    S4 = -(Y2 @ W2.T).reshape(n_cams, P, n_cams, P)
     b = lin.gc - np.einsum("jcpa,ja->cp", Y, lin.gp)
     for c in range(n_cams):
         S4[c, :, c, :] += lin.U[c] + lam * np.diag(Dc2[c])

@@ -8,6 +8,7 @@ import pytest
 from oracle import ba_oracle as O
 from oracle import covariance as OC
 from tests import _covariance_cases as CC
+from tests import _engine_cases as EC
 
 pytestmark = pytest.mark.gpu
 
@@ -56,21 +57,24 @@ def test_covariance_with_single_view_and_unobserved_points_and_cameras():
     assert (cov.cameras[np.ix_(cov.fixed, cov.fixed)] == 0).all()
 
 
-@pytest.mark.parametrize("n_cams,refine", [(5, False), (17, False), (33, False), (40, True), (64, False), (100, False)])
-def test_covariance_all_tile_shapes(n_cams, refine):
+@pytest.mark.parametrize("case", EC.COVARIANCE_CASES)
+def test_covariance_all_tile_shapes(case):
     """The rigs of test_schur_system_all_tile_shapes (30 .. 600 reduced parameters: every Schur tile shape, direct and
-    PCG-sized systems, 1 .. 19 pivot blocks of the sweep).  Cameras with fewer than 20 observations lose them all: on the
+    PCG-sized systems, 1 .. 19 pivot blocks of the sweep), plus the rigs whose points carry more than 96 rows (the
+    32-lane variant of the covariance point pass, with and without repeated rows) and the 240-camera dome (camera table
+    in global memory, 1440 reduced parameters).  Cameras with fewer than 20 observations lose them all: on the
     100-camera ring, cameras 80..99 see at most a handful of points, which leaves their poses undetermined (the call would
     rightly refuse the singular system); unobserved, they are masked and the reduced system keeps its 600 parameters."""
-    from caliscope_b200 import synthetic
-
-    r = synthetic.make_rig(n_cams, 700, 9000, seed=n_cams, refine_intrinsics=refine)
-    keep = np.bincount(r.obs_cam, minlength=n_cams)[r.obs_cam] >= 20
-    rig = O.Rig(r.cam_flags, r.cam_const, r.n_pts, r.obs_cam[keep], r.obs_pt[keep], r.obs_xy[keep])
+    c = EC.CASES[case]
+    r = c.make()
+    keep = np.bincount(r.obs_cam, minlength=c.n_cams)[r.obs_cam] >= 20
+    rig = EC.oracle_rig(r, keep)
     with make_problem(rig) as p:
+        if c.stats:
+            EC.check_stats(p, c)
         cov = p.covariance(r.x0)
     ref = OC.schur_covariance(r.x0, rig, cov.fixed)
-    _check(cov, ref, 1e-8, f"{n_cams} cameras")
+    _check(cov, ref, 1e-8, case)
 
 
 def test_covariance_without_scale_gauge_names_the_singular_parameter():
