@@ -1497,6 +1497,9 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
     CB_TRY(dalloc(&d_mask, (size_t)p->n_pts));
     ScopedFree sf; sf.dev.push_back(d_mask);
     CB_LAUNCH(cb::pt_tile_mask_kernel, cdiv(p->n_pts, 256), 256, 0, st, p->d_pt_start, p->d_pm_cam, p->n_pts, p->P, d_mask);
+    if (p->n_comp)  // rebuilt by cb_ba_problem_set_constraints: the lists must see the components' fill-in
+      CB_LAUNCH(cb::comp_tile_mask_kernel, cdiv(p->n_comp, 256), 256, 0, st, p->ct.comp_pt_start, p->ct.comp_pts, p->n_comp,
+                d_mask);
     // incidence counts per tile pair (dense rigs stop here: no mask download, no host pass over the points)
     unsigned long long* d_cnt;
     CB_TRY(dalloc(&d_cnt, (size_t)nt));
@@ -1669,6 +1672,27 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
   if (!sflat.empty())
     CB_CUDA(cudaMemcpyAsync(p->d_tile_slots, sflat.data(), sizeof(int) * sflat.size(), cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaStreamSynchronize(st));  // the host vectors above go out of scope
+  return CB_OK;
+}
+
+// Constraint components arrive after problem creation and fill in the Zt rows of their points (comp_tile_mask_kernel).
+// Row lists built without them would leave those rows out of the tile pairs they reach, so the work items are built
+// again: the dense / list decision, the lists and the CTA split.  The partial-tile buffers follow the new slot count.
+static int rebuild_schur_items(CbBaProblem* p, cudaStream_t st) {
+  CB_CUDA(cudaStreamSynchronize(st));
+  for (void** a : {(void**)&p->d_klist, (void**)&p->d_items, (void**)&p->d_tile_of, (void**)&p->d_tile_slot_start,
+                   (void**)&p->d_tile_slots, (void**)&p->d_part, (void**)&p->d_tpart}) {
+    if (!*a) continue;
+    p->allocs.erase(std::remove(p->allocs.begin(), p->allocs.end(), *a), p->allocs.end());
+    cached_free(*a);
+    *a = nullptr;
+  }
+  CB_TRY(build_schur_items(p, st));
+  CB_TRY(palloc(p, &p->d_part, (size_t)p->n_slots * cb::SY_TILE * cb::SY_TILE));
+  CB_TRY(palloc(p, &p->d_tpart, (size_t)p->n_slots * cb::SY_TILE));
+  CB_CUDA(cudaMemsetAsync(p->d_tpart, 0, sizeof(double) * (size_t)p->n_slots * cb::SY_TILE, st));
+  CB_CUDA(cudaMemsetAsync(p->d_part, 0, sizeof(double) * (size_t)p->n_slots * cb::SY_TILE * cb::SY_TILE, st));
+  CB_CUDA(cudaStreamSynchronize(st));
   return CB_OK;
 }
 
@@ -2517,6 +2541,8 @@ int cb_ba_problem_set_constraints(CbBaProblem* p, int64_t n_c, const int32_t* gr
   else
     CB_CUDA(cudaFuncSetAttribute(cb::comp_build_kernel<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_build_smem));
   CB_CUDA(cudaFuncSetAttribute(cb::comp_backsub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_back_smem));
+  // merging the components' tile masks only adds incidences, so problems on the dense product stay on it unchanged
+  if (p->schur_sparse) CB_TRY(rebuild_schur_items(p, st));
   p->h_ga.assign(groups_a, groups_a + 4 * (size_t)nc); p->h_gb.assign(groups_b, groups_b + 4 * (size_t)nc);
   p->h_cdist.assign(distances, distances + nc); p->h_cw.assign(weights, weights + nc);
   return CB_OK;

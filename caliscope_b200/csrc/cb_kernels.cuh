@@ -1026,6 +1026,18 @@ __global__ void pt_tile_mask_kernel(const int* __restrict__ pt_start, const int*
   }
   mask[j] = m;
 }
+// per rigid-constraint component: every point gets the union of its component's tile masks.  comp_build_kernel writes a
+// component point's Zt rows in the columns of every camera that sees ANY point of the component, so a point seen only
+// from tile A still has non-zero rows in tile B when another point of its component is seen from B.  Components are
+// disjoint, so one thread per component reads and writes its own points only.
+__global__ void comp_tile_mask_kernel(const int* __restrict__ comp_pt_start, const int* __restrict__ comp_pts, int n_comp,
+                                      unsigned long long* __restrict__ mask) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_comp) return;
+  unsigned long long m = 0ull;
+  for (int i = comp_pt_start[c]; i < comp_pt_start[c + 1]; ++i) m |= mask[comp_pts[i]];
+  for (int i = comp_pt_start[c]; i < comp_pt_start[c + 1]; ++i) mask[comp_pts[i]] = m;
+}
 // cnt[tile(I,J)] = number of points whose mask has bits I and J (I <= J; tile(I,J) = I*nb - I(I-1)/2 + J-I): what the host
 // needs to choose between the dense and the k-list Schur product, without downloading the masks.  Lanes holding the same
 // mask (the usual case: neighbouring points are seen by the same cameras) are counted once per warp.

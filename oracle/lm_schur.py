@@ -93,6 +93,100 @@ def schur_system(lin: Linearization, rig: O.Rig, lam: float, Dc2: np.ndarray, Dp
     return S4.reshape(n_cams * P, n_cams * P), b.reshape(-1), Einv, Wd
 
 
+def constraint_components(rig: O.Rig) -> list[np.ndarray]:
+    """Point sets linked by rigid-distance rows (connected components of the constraint graph), each ascending."""
+    from scipy.sparse import coo_matrix
+    from scipy.sparse.csgraph import connected_components
+
+    if not rig.n_constraints:
+        return []
+    members = np.concatenate([np.asarray(rig.groups_a), np.asarray(rig.groups_b)], axis=1).astype(np.int64)
+    rows = np.repeat(members[:, :1], members.shape[1], axis=1).ravel()
+    G = coo_matrix((np.ones(len(rows)), (rows, members.ravel())), shape=(rig.n_pts, rig.n_pts))
+    _, label = connected_components(G, directed=False)
+    used = np.unique(members)
+    return [used[label[used] == k] for k in np.unique(label[used])]
+
+
+@dataclass
+class ComponentSchur:
+    """The reduced camera system with rigid-distance rows, laid out at the engine's camera stride P."""
+
+    cost: float
+    S: np.ndarray  # (n_cams P, n_cams P)
+    b: np.ndarray  # (n_cams P,)
+    dc: np.ndarray  # (n_cams, P): dense solve of S dc = -b
+    Hcp: object  # sparse (n_camera_params, 3 n_pts), damped
+    Einv: object  # sparse block-diagonal inverse of the damped point block
+    gp: np.ndarray  # (3 n_pts,) total point gradient, constraint rows included
+    slot: np.ndarray  # camera-parameter index -> index in the P-stride layout
+
+    def backsub(self, dc: np.ndarray) -> np.ndarray:
+        """dp = -E^-1 (g_p + W^T dc), (n_pts, 3), for a camera step dc given at stride P."""
+        d = np.asarray(dc).reshape(-1)[self.slot]
+        return -(self.Einv @ (self.gp + self.Hcp.T @ d)).reshape(-1, 3)
+
+
+def component_schur(x: np.ndarray, rig: O.Rig, lam: float, loss: str = "linear", f_scale: float = 1.0,
+                    P: int | None = None) -> ComponentSchur:  # fmt: skip
+    """The engine's damped reduced system when points are tied by rigid-distance rows, from the sparse H = Js^T Js of
+    ``ba_oracle.jacobian`` (constraint rows included, robust row scales applied).  D = diag(H), entries <= 0 replaced by
+    1 (the Marquardt scale at a first linearisation).  Free points are eliminated as 3 x 3 blocks and each constraint
+    component as one dense block; nothing of size n_params squared is formed, so rigs of tens of thousands of parameters
+    fit.  Without constraint rows this is ``schur_system`` (padding slots of 6-parameter cameras at P = 9 hold lam)."""
+    from scipy.sparse import coo_matrix, diags
+
+    P = cam_stride(rig) if P is None else P
+    x = np.asarray(x, dtype=np.float64)
+    f = O.residuals(x, rig)
+    js, fs = O.robust_row_scales(f, loss, f_scale)
+    Js = (diags(js) @ O.jacobian(x, rig)).tocsr()
+    H = (Js.T @ Js).tocsr()
+    g = Js.T @ fs
+    D = H.diagonal().copy()
+    D[D <= 0] = 1.0
+    A = (H + lam * diags(D)).tocsr()
+    ncp, n_pts = rig.n_camera_params, rig.n_pts
+    Hcc = A[:ncp, :ncp].toarray()
+    Hcp = A[:ncp, ncp:].tocsr()
+    App = A[ncp:, ncp:].tocoo()
+    # 3 x 3 diagonal blocks of every point; components overwrite theirs with one dense inverse
+    same = App.row // 3 == App.col // 3
+    blk = np.zeros((n_pts, 3, 3))
+    np.add.at(blk, (App.row[same] // 3, App.row[same] % 3, App.col[same] % 3), App.data[same])
+    comps = constraint_components(rig)
+    free = np.ones(n_pts, bool)
+    for c in comps:
+        free[c] = False
+    fi = np.nonzero(free)[0]
+    inv3 = np.linalg.inv(blk[fi])
+    r3 = (3 * fi[:, None, None] + np.arange(3)[None, :, None]) + np.zeros((1, 1, 3), np.int64)
+    rows, cols, vals = [r3.ravel()], [r3.transpose(0, 2, 1).ravel()], [inv3.ravel()]
+    Appr = App.tocsr()
+    for c in comps:
+        idx = (3 * c[:, None] + np.arange(3)[None]).ravel()
+        Ei = np.linalg.inv(Appr[idx][:, idx].toarray())
+        rows.append(np.repeat(idx, len(idx)))
+        cols.append(np.tile(idx, len(idx)))
+        vals.append(Ei.ravel())
+    Einv = coo_matrix((np.concatenate(vals), (np.concatenate(rows), np.concatenate(cols))), shape=(3 * n_pts, 3 * n_pts)).tocsr()
+    gc, gp = g[:ncp], g[ncp:]
+    Y = (Hcp @ Einv).tocsr()
+    S_small = Hcc - (Y @ Hcp.T).toarray()
+    b_small = gc - Y @ gp
+    # stride-P layout
+    slot = np.concatenate([c * P + np.arange(rig.cam_offsets[c + 1] - rig.cam_offsets[c]) for c in range(rig.n_cams)])
+    n = rig.n_cams * P
+    S = np.zeros((n, n))
+    S[np.ix_(slot, slot)] = S_small
+    pad = np.setdiff1d(np.arange(n), slot)
+    S[pad, pad] = lam
+    b = np.zeros(n)
+    b[slot] = b_small
+    dc = np.linalg.solve(S, -b).reshape(rig.n_cams, P)
+    return ComponentSchur(O.robust_cost(f, loss, f_scale), S, b, dc, Hcp, Einv, gp, slot)
+
+
 def block_jacobi_pcg(S: np.ndarray, rhs: np.ndarray, P: int, tol: float, maxit: int):
     """Preconditioned CG on the dense reduced camera system, P x P diagonal blocks as
     the preconditioner; stops on sqrt(r^T M^-1 r) <= tol * its initial value."""

@@ -25,13 +25,14 @@ class Case:
     layout: str = "ring"
     seed: int | None = None  # None: n_cams
     stats: dict = field(default_factory=dict)  # stat key -> value the problem must report
+    cams_per_point: int | None = None  # local visibility (synthetic.make_rig)
 
     def make(self):
         from caliscope_b200 import synthetic
 
         seed = self.n_cams if self.seed is None else self.seed
         return synthetic.make_rig(self.n_cams, self.n_pts, self.n_obs, seed=seed, refine_intrinsics=self.refine,
-                                  layout=self.layout)  # fmt: skip
+                                  layout=self.layout, cams_per_point=self.cams_per_point)  # fmt: skip
 
 
 def _s(lanes, dups, smem, solve, ctas, cl, reordered=0):
