@@ -40,6 +40,11 @@ class ProblemDesc(C.Structure):
         ("obs_on_device", C.c_int32),
         ("obs_cam_bits", C.c_int32),
         ("cam_order", C.c_void_p),
+        ("n_constraints", C.c_int64),
+        ("groups_a", C.c_void_p),
+        ("groups_b", C.c_void_p),
+        ("distances", C.c_void_p),
+        ("weights", C.c_void_p),
     ]
 
 
@@ -115,8 +120,6 @@ SYMBOLS = {
     "cb_ba_problem_destroy": (C.c_int, [_P]),
     "cb_ba_problem_n_params": (C.c_int64, [_P]),
     "cb_ba_problem_stat": (C.c_double, [_P, C.c_int]),
-    "cb_ba_problem_set_constraints": (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P]),
-    "cb_ba_problem_n_constraints": (C.c_int64, [_P]),
     "cb_ba_constraint_rows": (C.c_int, [_P, _P, _P, _P, _P]),
     "cb_ba_solve": (C.c_int, [_P, C.POINTER(Options), _P, C.POINTER(Result), _P]),
     "cb_ba_residuals": (C.c_int, [_P, _P, _P, _P]),

@@ -456,7 +456,6 @@ struct CbBaProblem {
   int *d_cam_xoff = nullptr, *d_cam_slot = nullptr, *d_klist = nullptr;
   bool schur_sparse = false;
   double schur_flop_issued = 0.0;  // flops one schur_syrk_kernel launch issues (dense tiles or compacted lists)
-  double schur_rows_dense = 0.0, schur_rows_listed = 0.0;  // weighted k rows the Schur product streams: all vs listed
   std::vector<void*> allocs;
   // problem tables
   int* d_cam_flags = nullptr;
@@ -1497,7 +1496,7 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
     CB_TRY(dalloc(&d_mask, (size_t)p->n_pts));
     ScopedFree sf; sf.dev.push_back(d_mask);
     CB_LAUNCH(cb::pt_tile_mask_kernel, cdiv(p->n_pts, 256), 256, 0, st, p->d_pt_start, p->d_pm_cam, p->n_pts, p->P, d_mask);
-    if (p->n_comp)  // rebuilt by cb_ba_problem_set_constraints: the lists must see the components' fill-in
+    if (p->n_comp)  // comp_build_kernel fills a component point's Zt rows in every column its component's cameras reach
       CB_LAUNCH(cb::comp_tile_mask_kernel, cdiv(p->n_comp, 256), 256, 0, st, p->ct.comp_pt_start, p->ct.comp_pts, p->n_comp,
                 d_mask);
     // incidence counts per tile pair (dense rigs stop here: no mask download, no host pass over the points)
@@ -1517,7 +1516,6 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
         listed += w * (double)cnt[tof[(size_t)I * nb + J]];
         dense += w * (double)p->n_pts;
       }
-    p->schur_rows_dense = 3.0 * dense; p->schur_rows_listed = 3.0 * listed;
     sparse = want_sparse == 1 || listed < 0.7 * dense;
     if (sparse) {
       // the row lists are built on the device (inc_count .. klist_expand in cb_kernels.cuh); the host only lays out where each
@@ -1675,24 +1673,118 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
   return CB_OK;
 }
 
-// Constraint components arrive after problem creation and fill in the Zt rows of their points (comp_tile_mask_kernel).
-// Row lists built without them would leave those rows out of the tile pairs they reach, so the work items are built
-// again: the dense / list decision, the lists and the CTA split.  The partial-tile buffers follow the new slot count.
-static int rebuild_schur_items(CbBaProblem* p, cudaStream_t st) {
-  CB_CUDA(cudaStreamSynchronize(st));
-  for (void** a : {(void**)&p->d_klist, (void**)&p->d_items, (void**)&p->d_tile_of, (void**)&p->d_tile_slot_start,
-                   (void**)&p->d_tile_slots, (void**)&p->d_part, (void**)&p->d_tpart}) {
-    if (!*a) continue;
-    p->allocs.erase(std::remove(p->allocs.begin(), p->allocs.end(), *a), p->allocs.end());
-    cached_free(*a);
-    *a = nullptr;
+// Rigid-distance constraint rows (reprojection.py:112-117, 207-226; arrays as built by
+// CaptureVolume._build_constraint_arrays, capture_volume.py:446-516, with
+// weights = (pixel_sigma / f_median) / sigma, :377-381): the connected components of the constraint graph and the
+// device tables of ConstraintTables.  Runs before build_schur_items, whose row lists must see the components' fill-in.
+static int build_components(CbBaProblem* p, const CbBaProblemDesc* d, cudaStream_t st) {
+  if (d->n_constraints == 0) return CB_OK;
+  const int32_t *groups_a = d->groups_a, *groups_b = d->groups_b;
+  const double *distances = d->distances, *weights = d->weights;
+  const int nc = (int)d->n_constraints, npts = p->n_pts;
+  for (long long i = 0; i < 4ll * nc; ++i)
+    if (groups_a[i] < 0 || groups_a[i] >= npts || groups_b[i] < 0 || groups_b[i] >= npts) {
+      g_last_error = "constraint group index out of range";
+      return CB_E_INVALID;
+    }
+  // connected components of the constraint graph (union-find over points)
+  std::vector<int> parent(npts);
+  for (int i = 0; i < npts; ++i) parent[i] = i;
+  auto find = [&](int a) { while (parent[a] != a) { parent[a] = parent[parent[a]]; a = parent[a]; } return a; };
+  std::vector<char> used(npts, 0);
+  for (int k = 0; k < nc; ++k) {
+    const int r0 = find(groups_a[4 * k]);
+    used[groups_a[4 * k]] = 1;
+    for (int q = 0; q < 4; ++q) {
+      used[groups_a[4 * k + q]] = 1; used[groups_b[4 * k + q]] = 1;
+      parent[find(groups_a[4 * k + q])] = r0;
+      parent[find(groups_b[4 * k + q])] = r0;
+    }
   }
-  CB_TRY(build_schur_items(p, st));
-  CB_TRY(palloc(p, &p->d_part, (size_t)p->n_slots * cb::SY_TILE * cb::SY_TILE));
-  CB_TRY(palloc(p, &p->d_tpart, (size_t)p->n_slots * cb::SY_TILE));
-  CB_CUDA(cudaMemsetAsync(p->d_tpart, 0, sizeof(double) * (size_t)p->n_slots * cb::SY_TILE, st));
-  CB_CUDA(cudaMemsetAsync(p->d_part, 0, sizeof(double) * (size_t)p->n_slots * cb::SY_TILE * cb::SY_TILE, st));
+  std::vector<int> comp_of_root(npts, -1), pt_comp(npts, -1), pt_lidx(npts, -1);
+  std::vector<std::vector<int>> comp_pts;
+  for (int j = 0; j < npts; ++j) {
+    if (!used[j]) continue;
+    const int r = find(j);
+    if (comp_of_root[r] < 0) { comp_of_root[r] = (int)comp_pts.size(); comp_pts.emplace_back(); }
+    const int c = comp_of_root[r];
+    pt_comp[j] = c;
+    pt_lidx[j] = (int)comp_pts[c].size();
+    comp_pts[c].push_back(j);
+  }
+  const int ncomp = (int)comp_pts.size();
+  std::vector<int> cps(ncomp + 1, 0), cpts, ccs(ncomp + 1, 0), ccons(nc);
+  std::vector<long long> loff(ncomp);
+  long long ltot = 0;
+  int ndmax = 0;
+  for (int c = 0; c < ncomp; ++c) {
+    cps[c] = (int)cpts.size();
+    cpts.insert(cpts.end(), comp_pts[c].begin(), comp_pts[c].end());
+    const long long n = 3ll * comp_pts[c].size();
+    loff[c] = ltot;
+    ltot += n * n;
+    ndmax = std::max(ndmax, (int)n);
+  }
+  cps[ncomp] = (int)cpts.size();
+  if (ndmax > 1200) {
+    g_last_error = "a rigid component couples more than 400 points; not supported by this build";
+    return CB_E_UNSUPPORTED;
+  }
+  std::vector<int> cnu(nc), cg((size_t)nc * 8, -1), cl((size_t)nc * 8, 0), ccomp(nc);
+  std::vector<double> ccoef((size_t)nc * 8, 0.0);
+  for (int k = 0; k < nc; ++k) {
+    int nu = 0;
+    for (int side = 0; side < 2; ++side)
+      for (int q = 0; q < 4; ++q) {
+        const int pt = side == 0 ? groups_a[4 * k + q] : groups_b[4 * k + q];
+        int u = 0;
+        for (; u < nu; ++u)
+          if (cg[(size_t)k * 8 + u] == pt) break;
+        if (u == nu) { cg[(size_t)k * 8 + u] = pt; cl[(size_t)k * 8 + u] = pt_lidx[pt]; ++nu; }
+        ccoef[(size_t)k * 8 + u] += side == 0 ? 0.25 : -0.25;
+      }
+    cnu[k] = nu;
+    ccomp[k] = pt_comp[groups_a[4 * k]];
+    ccs[ccomp[k] + 1]++;
+  }
+  for (int c = 0; c < ncomp; ++c) ccs[c + 1] += ccs[c];
+  {
+    std::vector<int> cur(ccs.begin(), ccs.end() - 1);
+    for (int k = 0; k < nc; ++k) ccons[cur[ccomp[k]]++] = k;  // ascending constraint id within a component
+  }
+  // upload
+  int *d_nu, *d_g, *d_l, *d_cps, *d_cpts, *d_ccs, *d_ccons;
+  double *d_coef, *d_dist, *d_w;
+  long long* d_loff;
+  CB_TRY(palloc(p, &d_nu, nc)); CB_TRY(palloc(p, &d_g, (size_t)nc * 8)); CB_TRY(palloc(p, &d_l, (size_t)nc * 8));
+  CB_TRY(palloc(p, &d_coef, (size_t)nc * 8)); CB_TRY(palloc(p, &d_dist, nc)); CB_TRY(palloc(p, &d_w, nc));
+  CB_TRY(palloc(p, &d_cps, ncomp + 1)); CB_TRY(palloc(p, &d_cpts, cpts.size())); CB_TRY(palloc(p, &d_ccs, ncomp + 1));
+  CB_TRY(palloc(p, &d_ccons, nc)); CB_TRY(palloc(p, &d_loff, ncomp)); CB_TRY(palloc(p, &p->d_pt_comp, npts));
+  for (int k = 0; k < 2; ++k) { CB_TRY(palloc(p, &p->d_c_rs[k], nc)); CB_TRY(palloc(p, &p->d_c_dirw[k], 3 * (size_t)nc)); }
+  CB_TRY(palloc(p, &p->d_compL, (size_t)ltot));
+#define CB_UP(dst, vec) CB_CUDA(cudaMemcpyAsync(dst, (vec).data(), sizeof((vec)[0]) * (vec).size(), cudaMemcpyHostToDevice, st))
+  CB_UP(d_nu, cnu); CB_UP(d_g, cg); CB_UP(d_l, cl); CB_UP(d_coef, ccoef); CB_UP(d_cps, cps); CB_UP(d_cpts, cpts);
+  CB_UP(d_ccs, ccs); CB_UP(d_ccons, ccons); CB_UP(d_loff, loff); CB_UP(p->d_pt_comp, pt_comp);
+#undef CB_UP
+  CB_CUDA(cudaMemcpyAsync(d_dist, distances, sizeof(double) * nc, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(d_w, weights, sizeof(double) * nc, cudaMemcpyHostToDevice, st));
+  p->n_cblk = cdiv(nc, cb::CC_THREADS);
   CB_CUDA(cudaStreamSynchronize(st));
+  p->ct.n_c = nc; p->ct.n_comp = ncomp; p->ct.n_dim_max = ndmax;
+  p->ct.c_nu = d_nu; p->ct.c_gidx = d_g; p->ct.c_lidx = d_l; p->ct.c_coef = d_coef; p->ct.c_dist = d_dist; p->ct.c_w = d_w;
+  p->ct.comp_pt_start = d_cps; p->ct.comp_pts = d_cpts; p->ct.comp_c_start = d_ccs; p->ct.comp_cons = d_ccons;
+  p->ct.comp_L_off = d_loff; p->ct.pt_comp = p->d_pt_comp;
+  p->n_c = nc; p->n_comp = ncomp; p->n_dim_max = ndmax;
+  const int esm = std::min(ndmax, cb::CC_SMEM_DIM);
+  p->comp_build_smem = sizeof(double) * ((size_t)ndmax * (1 + p->P) + (size_t)esm * esm) + 4 * ((size_t)(p->n_cams + 31) / 32 + 4);
+  p->comp_back_smem = sizeof(double) * ((size_t)p->nP + ndmax);
+  if (p->P == 6)
+    CB_CUDA(cudaFuncSetAttribute(cb::comp_build_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_build_smem));
+  else
+    CB_CUDA(cudaFuncSetAttribute(cb::comp_build_kernel<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_build_smem));
+  CB_CUDA(cudaFuncSetAttribute(cb::comp_backsub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_back_smem));
+  p->h_ga.assign(groups_a, groups_a + 4 * (size_t)nc); p->h_gb.assign(groups_b, groups_b + 4 * (size_t)nc);
+  p->h_cdist.assign(distances, distances + nc); p->h_cw.assign(weights, weights + nc);
   return CB_OK;
 }
 
@@ -1832,6 +1924,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   }
 
   lap("index build + camera tables");
+  CB_TRY(build_components(p, d, st));
   CB_TRY(build_schur_items(p, st));
   lap("schur work items");
   std::vector<unsigned char> act((size_t)p->nP, 0);
@@ -1852,8 +1945,9 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
     CB_TRY(palloc(p, &p->d_Upk[k], (size_t)p->n_cams * NU)); CB_TRY(palloc(p, &p->d_gc[k], p->nP));
     CB_TRY(palloc(p, &p->d_costsum[k], 4));
   }
-  CB_TRY(palloc(p, &p->d_partial, (size_t)std::max(p->n_chunks, 1) * NACC));
-  CB_TRY(palloc(p, &p->d_camcost, p->n_cams));
+  // the cost / step partial-sum arrays grow by the constraint blocks / components (by nothing without constraints)
+  CB_TRY(palloc(p, &p->d_partial, (size_t)std::max(p->n_chunks, 1) * NACC + p->n_cblk));
+  CB_TRY(palloc(p, &p->d_camcost, (size_t)p->n_cams + p->n_cblk));
   CB_TRY(palloc(p, &p->d_gpt, 3 * npts));
   CB_TRY(palloc(p, &p->d_V6, 6 * npts)); CB_TRY(palloc(p, &p->d_gp, 3 * npts)); CB_TRY(palloc(p, &p->d_Dp2, 3 * npts));
   CB_TRY(palloc(p, &p->d_Dc2, p->nP)); CB_TRY(palloc(p, &p->d_Linv6, 6 * npts));
@@ -1865,7 +1959,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   CB_TRY(palloc(p, &p->d_red, p->red_len()));
   CB_TRY(palloc(p, &p->d_Minv, (size_t)p->n_cams * p->P * p->P));
   CB_TRY(palloc(p, &p->d_dc, p->nP)); CB_TRY(palloc(p, &p->d_dp, 3 * npts));
-  CB_TRY(palloc(p, &p->d_bpart, 3 * (size_t)p->pt_grid));
+  CB_TRY(palloc(p, &p->d_bpart, 3 * ((size_t)p->pt_grid + p->n_comp)));
   CB_TRY(palloc(p, &p->d_sc, cb::SC_COUNT)); CB_TRY(palloc(p, &p->d_red2, 8));
   CB_TRY(palloc(p, &p->d_gmax, 2));
   CB_TRY(palloc(p, &p->d_counter, 4));
@@ -1925,7 +2019,8 @@ int cb_ba_problem_create(const CbBaProblemDesc* d, int device, void* stream, CbB
     return CB_E_INVALID;
   }
   if (!d || !out || d->n_cams <= 0 || d->n_pts <= 0 || d->n_obs < 0 || d->n_obs > (1ll << 30) || !d->cam_flags ||
-      !d->cam_const || (d->n_obs > 0 && (!d->obs_cam || !d->obs_pt || !d->obs_xy))) {
+      !d->cam_const || (d->n_obs > 0 && (!d->obs_cam || !d->obs_pt || !d->obs_xy)) || d->n_constraints < 0 ||
+      (d->n_constraints > 0 && (!d->groups_a || !d->groups_b || !d->distances || !d->weights))) {
     g_last_error = "cb_ba_problem_create: bad descriptor";
     return CB_E_INVALID;
   }
@@ -2418,138 +2513,6 @@ int cb_ba_error_order_stats(CbBaProblem* p, const double* x, double q_percent, d
   return CB_OK;
 }
 
-// Rigid-distance constraint rows (reprojection.py:112-117, 207-226; arrays as built by
-// CaptureVolume._build_constraint_arrays, capture_volume.py:446-516, with
-// weights = (pixel_sigma / f_median) / sigma, :377-381).  Host arrays; call once after problem_create.
-int cb_ba_problem_set_constraints(CbBaProblem* p, int64_t n_c, const int32_t* groups_a, const int32_t* groups_b,
-                                  const double* distances, const double* weights, void* stream) {
-  if (!p || n_c < 0 || (n_c > 0 && (!groups_a || !groups_b || !distances || !weights))) {
-    g_last_error = "cb_ba_problem_set_constraints: bad argument";
-    return CB_E_INVALID;
-  }
-  if (p->n_c) { g_last_error = "constraints already set on this problem"; return CB_E_INVALID; }
-  if (n_c == 0) return CB_OK;
-  CB_CUDA(cudaSetDevice(p->device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int nc = (int)n_c, npts = p->n_pts;
-  for (long long i = 0; i < 4ll * nc; ++i)
-    if (groups_a[i] < 0 || groups_a[i] >= npts || groups_b[i] < 0 || groups_b[i] >= npts) {
-      g_last_error = "constraint group index out of range";
-      return CB_E_INVALID;
-    }
-  // connected components of the constraint graph (union-find over points)
-  std::vector<int> parent(npts);
-  for (int i = 0; i < npts; ++i) parent[i] = i;
-  auto find = [&](int a) { while (parent[a] != a) { parent[a] = parent[parent[a]]; a = parent[a]; } return a; };
-  std::vector<char> used(npts, 0);
-  for (int k = 0; k < nc; ++k) {
-    const int r0 = find(groups_a[4 * k]);
-    used[groups_a[4 * k]] = 1;
-    for (int q = 0; q < 4; ++q) {
-      used[groups_a[4 * k + q]] = 1; used[groups_b[4 * k + q]] = 1;
-      parent[find(groups_a[4 * k + q])] = r0;
-      parent[find(groups_b[4 * k + q])] = r0;
-    }
-  }
-  std::vector<int> comp_of_root(npts, -1), pt_comp(npts, -1), pt_lidx(npts, -1);
-  std::vector<std::vector<int>> comp_pts;
-  for (int j = 0; j < npts; ++j) {
-    if (!used[j]) continue;
-    const int r = find(j);
-    if (comp_of_root[r] < 0) { comp_of_root[r] = (int)comp_pts.size(); comp_pts.emplace_back(); }
-    const int c = comp_of_root[r];
-    pt_comp[j] = c;
-    pt_lidx[j] = (int)comp_pts[c].size();
-    comp_pts[c].push_back(j);
-  }
-  const int ncomp = (int)comp_pts.size();
-  std::vector<int> cps(ncomp + 1, 0), cpts, ccs(ncomp + 1, 0), ccons(nc);
-  std::vector<long long> loff(ncomp);
-  long long ltot = 0;
-  int ndmax = 0;
-  for (int c = 0; c < ncomp; ++c) {
-    cps[c] = (int)cpts.size();
-    cpts.insert(cpts.end(), comp_pts[c].begin(), comp_pts[c].end());
-    const long long n = 3ll * comp_pts[c].size();
-    loff[c] = ltot;
-    ltot += n * n;
-    ndmax = std::max(ndmax, (int)n);
-  }
-  cps[ncomp] = (int)cpts.size();
-  if (ndmax > 1200) {
-    g_last_error = "a rigid component couples more than 400 points; not supported by this build";
-    return CB_E_UNSUPPORTED;
-  }
-  std::vector<int> cnu(nc), cg((size_t)nc * 8, -1), cl((size_t)nc * 8, 0), ccomp(nc);
-  std::vector<double> ccoef((size_t)nc * 8, 0.0);
-  for (int k = 0; k < nc; ++k) {
-    int nu = 0;
-    for (int side = 0; side < 2; ++side)
-      for (int q = 0; q < 4; ++q) {
-        const int pt = side == 0 ? groups_a[4 * k + q] : groups_b[4 * k + q];
-        int u = 0;
-        for (; u < nu; ++u)
-          if (cg[(size_t)k * 8 + u] == pt) break;
-        if (u == nu) { cg[(size_t)k * 8 + u] = pt; cl[(size_t)k * 8 + u] = pt_lidx[pt]; ++nu; }
-        ccoef[(size_t)k * 8 + u] += side == 0 ? 0.25 : -0.25;
-      }
-    cnu[k] = nu;
-    ccomp[k] = pt_comp[groups_a[4 * k]];
-    ccs[ccomp[k] + 1]++;
-  }
-  for (int c = 0; c < ncomp; ++c) ccs[c + 1] += ccs[c];
-  {
-    std::vector<int> cur(ccs.begin(), ccs.end() - 1);
-    for (int k = 0; k < nc; ++k) ccons[cur[ccomp[k]]++] = k;  // ascending constraint id within a component
-  }
-  // upload
-  int *d_nu, *d_g, *d_l, *d_cps, *d_cpts, *d_ccs, *d_ccons;
-  double *d_coef, *d_dist, *d_w;
-  long long* d_loff;
-  CB_TRY(palloc(p, &d_nu, nc)); CB_TRY(palloc(p, &d_g, (size_t)nc * 8)); CB_TRY(palloc(p, &d_l, (size_t)nc * 8));
-  CB_TRY(palloc(p, &d_coef, (size_t)nc * 8)); CB_TRY(palloc(p, &d_dist, nc)); CB_TRY(palloc(p, &d_w, nc));
-  CB_TRY(palloc(p, &d_cps, ncomp + 1)); CB_TRY(palloc(p, &d_cpts, cpts.size())); CB_TRY(palloc(p, &d_ccs, ncomp + 1));
-  CB_TRY(palloc(p, &d_ccons, nc)); CB_TRY(palloc(p, &d_loff, ncomp)); CB_TRY(palloc(p, &p->d_pt_comp, npts));
-  for (int k = 0; k < 2; ++k) { CB_TRY(palloc(p, &p->d_c_rs[k], nc)); CB_TRY(palloc(p, &p->d_c_dirw[k], 3 * (size_t)nc)); }
-  CB_TRY(palloc(p, &p->d_compL, (size_t)ltot));
-#define CB_UP(dst, vec) CB_CUDA(cudaMemcpyAsync(dst, (vec).data(), sizeof((vec)[0]) * (vec).size(), cudaMemcpyHostToDevice, st))
-  CB_UP(d_nu, cnu); CB_UP(d_g, cg); CB_UP(d_l, cl); CB_UP(d_coef, ccoef); CB_UP(d_cps, cps); CB_UP(d_cpts, cpts);
-  CB_UP(d_ccs, ccs); CB_UP(d_ccons, ccons); CB_UP(d_loff, loff); CB_UP(p->d_pt_comp, pt_comp);
-#undef CB_UP
-  CB_CUDA(cudaMemcpyAsync(d_dist, distances, sizeof(double) * nc, cudaMemcpyHostToDevice, st));
-  CB_CUDA(cudaMemcpyAsync(d_w, weights, sizeof(double) * nc, cudaMemcpyHostToDevice, st));
-  p->n_cblk = cdiv(nc, cb::CC_THREADS);
-  // the cost / step partial-sum arrays grow by the constraint blocks / components
-  const int NACC = (p->P == 6) ? 28 : 55;
-  CB_TRY(palloc(p, &p->d_camcost, (size_t)p->n_cams + p->n_cblk));
-  CB_TRY(palloc(p, &p->d_partial, (size_t)std::max(p->n_chunks, 1) * NACC + p->n_cblk));
-  CB_TRY(palloc(p, &p->d_bpart, 3 * ((size_t)p->pt_grid + ncomp)));
-  // captured launches hold the old buffer addresses
-  destroy_graph(p->trial_graph);
-  destroy_graph(p->loop_graph);
-  CB_CUDA(cudaStreamSynchronize(st));
-  p->ct.n_c = nc; p->ct.n_comp = ncomp; p->ct.n_dim_max = ndmax;
-  p->ct.c_nu = d_nu; p->ct.c_gidx = d_g; p->ct.c_lidx = d_l; p->ct.c_coef = d_coef; p->ct.c_dist = d_dist; p->ct.c_w = d_w;
-  p->ct.comp_pt_start = d_cps; p->ct.comp_pts = d_cpts; p->ct.comp_c_start = d_ccs; p->ct.comp_cons = d_ccons;
-  p->ct.comp_L_off = d_loff; p->ct.pt_comp = p->d_pt_comp;
-  p->n_c = nc; p->n_comp = ncomp; p->n_dim_max = ndmax;
-  const int esm = std::min(ndmax, cb::CC_SMEM_DIM);
-  p->comp_build_smem = sizeof(double) * ((size_t)ndmax * (1 + p->P) + (size_t)esm * esm) + 4 * ((size_t)(p->n_cams + 31) / 32 + 4);
-  p->comp_back_smem = sizeof(double) * ((size_t)p->nP + ndmax);
-  if (p->P == 6)
-    CB_CUDA(cudaFuncSetAttribute(cb::comp_build_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_build_smem));
-  else
-    CB_CUDA(cudaFuncSetAttribute(cb::comp_build_kernel<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_build_smem));
-  CB_CUDA(cudaFuncSetAttribute(cb::comp_backsub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_back_smem));
-  // merging the components' tile masks only adds incidences, so problems on the dense product stay on it unchanged
-  if (p->schur_sparse) CB_TRY(rebuild_schur_items(p, st));
-  p->h_ga.assign(groups_a, groups_a + 4 * (size_t)nc); p->h_gb.assign(groups_b, groups_b + 4 * (size_t)nc);
-  p->h_cdist.assign(distances, distances + nc); p->h_cw.assign(weights, weights + nc);
-  return CB_OK;
-}
-
-int64_t cb_ba_problem_n_constraints(const CbBaProblem* p) { return p ? p->n_c : -1; }
-
 // Constraint rows at x: r (n_c, == the tail of joint_residuals) and dir (n_c x 3) = w * unit(mean(P[ga]) - mean(P[gb]));
 // the Jacobian entry of member point q of group a (b) is +(-) dir / 4, summed over repeats (reprojection.py:207-226).
 int cb_ba_constraint_rows(CbBaProblem* p, const double* x, double* r_out, double* dir_out, void* stream) {
@@ -2676,12 +2639,14 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
     }
     CB_LAUNCH(cb::gather_obs_kernel, cdiv(nsel, 256), 256, 0, st, d_sel, nsel, p->d_obs_cam, p->d_obs_pt,
               reinterpret_cast<const double2*>(p->d_obs_xy), c_cam, c_pt, reinterpret_cast<double2*>(c_xy));
-    CbBaProblemDesc d2;
+    CbBaProblemDesc d2 = {};
     d2.n_cams = nc; d2.n_pts = p->n_pts; d2.n_obs = nsel;
     d2.cam_flags = p->h_cam_flags.data(); d2.cam_const = p->h_cam_const.data();
     d2.obs_cam = c_cam; d2.obs_pt = c_pt; d2.obs_xy = c_xy; d2.obs_on_device = 1;
     d2.obs_cam_bits = 32;
     d2.cam_order = p->h_perm.data();  // the filtered problem keeps this problem's camera order
+    d2.n_constraints = p->n_c;
+    d2.groups_a = p->h_ga.data(); d2.groups_b = p->h_gb.data(); d2.distances = p->h_cdist.data(); d2.weights = p->h_cw.data();
     CbBaProblem* q = new CbBaProblem();
     q->allocs.push_back(c_cam); q->allocs.push_back(c_pt); q->allocs.push_back(c_xy);  // owned by the new problem
     rc = problem_create_impl(&d2, p->device, st, q);
@@ -2690,17 +2655,8 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
       cb_ba_problem_destroy(q);
       g_last_error = keep;
     } else {
-      if (p->n_c)
-        rc = cb_ba_problem_set_constraints(q, p->n_c, p->h_ga.data(), p->h_gb.data(), p->h_cdist.data(), p->h_cw.data(),
-                                           stream);
-      if (rc != CB_OK) {
-        std::string keep = g_last_error;
-        cb_ba_problem_destroy(q);
-        g_last_error = keep;
-      } else {
-        q->order_auto = p->order_auto;
-        *out = q;
-      }
+      q->order_auto = p->order_auto;
+      *out = q;
     }
   }
   if (n_kept) *n_kept = nsel;

@@ -161,31 +161,26 @@ class BAProblem:
         order = None if cam_order is None else np.ascontiguousarray(cam_order, dtype=np.int32)
         if order is not None and order.shape != (self.n_cams,):
             raise ValueError(f"cam_order must have shape ({self.n_cams},)")
-        desc = L.ProblemDesc(
-            self.n_cams, self.n_pts, n_obs, _ptr(self.cam_flags), _ptr(self.cam_const), ptrs[0], ptrs[1], ptrs[2],
-            1 if on_dev else 0, cam_bits, _ptr(order) if order is not None else None,
-        )  # fmt: skip
-        h = C.c_void_p()
-        L.check(lib.cb_ba_problem_create(C.byref(desc), self.device, C.c_void_p(stream), C.byref(h)), "problem_create")
-        self._h = h
-        self.cam_stride = int(lib.cb_ba_cam_stride(h))
         self.n_constraints = 0
+        cons_ptrs = (None,) * 4
         if constraints is not None and constraints[0] is not None and len(constraints[0]) > 0:
             ga = np.ascontiguousarray(constraints[0], dtype=np.int32).reshape(-1, 4)
             gb = np.ascontiguousarray(constraints[1], dtype=np.int32).reshape(-1, 4)
             dist = np.ascontiguousarray(constraints[2], dtype=np.float64)
             w = np.ascontiguousarray(constraints[3], dtype=np.float64)
             if not (len(ga) == len(gb) == len(dist) == len(w)):
-                self.close()
                 raise ValueError("constraint arrays must have the same length")
-            try:
-                L.check(lib.cb_ba_problem_set_constraints(h, len(ga), _ptr(ga), _ptr(gb), _ptr(dist), _ptr(w),
-                                                          C.c_void_p(stream)), "set_constraints")  # fmt: skip
-            except Exception:
-                self.close()
-                raise
             self.n_constraints = len(ga)
             self.constraints = (ga, gb, dist, w)
+            cons_ptrs = tuple(_ptr(a) for a in self.constraints)
+        desc = L.ProblemDesc(
+            self.n_cams, self.n_pts, n_obs, _ptr(self.cam_flags), _ptr(self.cam_const), ptrs[0], ptrs[1], ptrs[2],
+            1 if on_dev else 0, cam_bits, _ptr(order) if order is not None else None, self.n_constraints, *cons_ptrs,
+        )  # fmt: skip
+        h = C.c_void_p()
+        L.check(lib.cb_ba_problem_create(C.byref(desc), self.device, C.c_void_p(stream), C.byref(h)), "problem_create")
+        self._h = h
+        self.cam_stride = int(lib.cb_ba_cam_stride(h))
 
     # -- lifetime -----------------------------------------------------------------------------
     def close(self) -> None:

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define CB_BA_ABI_VERSION 2
+#define CB_BA_ABI_VERSION 3
 
 /* cam_flags bits (CameraBlock.free_intrinsics / .fisheye, bundle_parameterization.py:36-51) */
 #define CB_CAM_FREE_INTRINSICS 1
@@ -81,6 +81,17 @@ typedef struct {
    * so that whole 96-column tile pairs of the Schur product are empty); no input or output of the ABI is reordered.
    * Every rank of a sharded solve MUST pass the same order (caliscope_b200.distributed does). */
   const int32_t* cam_order;
+  /* Rigid-distance constraint rows (reprojection.py:112-117 and :207-226): groups_a / groups_b are n_constraints x 4
+   * world-point row indices, distances and weights n_constraints doubles -- the arrays
+   * CaptureVolume._build_constraint_arrays produces (capture_volume.py:446-516) with
+   * weights = (pixel_sigma / f_median) / sigma (:377-381).  Host pointers, copied; ignored when n_constraints == 0.
+   * Under observation sharding every point a row touches must belong to the same rank (shard by connected component
+   * of the constraint graph). */
+  int64_t n_constraints;
+  const int32_t* groups_a;
+  const int32_t* groups_b;
+  const double* distances;
+  const double* weights;
 } CbBaProblemDesc;
 
 /*
@@ -149,7 +160,7 @@ const char* cb_ba_error_string(int code);
 const char* cb_ba_last_error(void);
 void cb_ba_default_options(CbBaOptions* opt);
 
-/* Upload + index build (sort by camera / by point, chunk and pair tables). */
+/* Upload + index build (sort by camera / by point, chunk and pair tables, constraint components). */
 int cb_ba_problem_create(const CbBaProblemDesc* desc, int device, void* stream, CbBaProblem** out);
 int cb_ba_problem_destroy(CbBaProblem* p);
 int64_t cb_ba_problem_n_params(const CbBaProblem* p);
@@ -163,17 +174,9 @@ int64_t cb_ba_problem_n_params(const CbBaProblem* p);
  * -1 for an unknown key. */
 double cb_ba_problem_stat(const CbBaProblem* p, int what);
 
-/* Rigid-distance constraint rows (reprojection.py:112-117 and :207-226): groups_a / groups_b are n_c x 4 world-point
- * row indices, distances and weights n_c doubles -- the arrays CaptureVolume._build_constraint_arrays produces
- * (capture_volume.py:446-516) with weights = (pixel_sigma / f_median) / sigma (:377-381).  Host pointers, copied.
- * Call at most once, after cb_ba_problem_create.  Under observation sharding every point a row touches must belong
- * to the same rank (shard by connected component of the constraint graph). */
-int cb_ba_problem_set_constraints(CbBaProblem* p, int64_t n_c, const int32_t* groups_a, const int32_t* groups_b,
-                                  const double* distances, const double* weights, void* stream);
-int64_t cb_ba_problem_n_constraints(const CbBaProblem* p);
-
-/* Constraint rows at x: r_out (n_c) == the tail of joint_residuals; dir_out (n_c x 3, nullable) = weight * unit vector
- * between the two endpoint means: the Jacobian entry of a group-a (group-b) member is +(-) dir / 4, repeats summed. */
+/* Constraint rows at x, n_c = CbBaProblemDesc.n_constraints: r_out (n_c) == the tail of joint_residuals; dir_out (n_c x 3,
+ * nullable) = weight * unit vector between the two endpoint means: the Jacobian entry of a group-a (group-b) member is
+ * +(-) dir / 4, repeats summed. */
 int cb_ba_constraint_rows(CbBaProblem* p, const double* x, double* r_out, double* dir_out, void* stream);
 
 /* Replaces least_squares(joint_residuals, x0, jac=joint_jacobian, method="trf", ...)

@@ -193,7 +193,7 @@ def test_constrained_camera_relabelling_permutes_every_output():
 
 
 def test_device_cull_of_a_constrained_problem(monkeypatch):
-    """cb_ba_cull builds the filtered problem and sets the constraints on it again; its reduced system (row lists in use)
+    """cb_ba_cull builds the filtered problem with this problem's constraints; its reduced system (row lists in use)
     must match the oracle on the filtered rig."""
     from caliscope_b200 import filtering
 

@@ -136,7 +136,7 @@ def test_shared_library_exports_every_declared_symbol():
     lib = _lib.load()
     for name in declared:
         assert hasattr(lib, name), name
-    assert lib.cb_ba_abi_version() == 2
+    assert lib.cb_ba_abi_version() == 3
     opt = _lib.Options()
     lib.cb_ba_default_options(ctypes.byref(opt))
     assert opt.ftol == 1e-8 and opt.xtol == 1e-8 and opt.gtol == 1e-8 and opt.use_bounds == 1
