@@ -1474,7 +1474,7 @@ double cb_ba_problem_stat(const CbBaProblem* p, int what) {
 }
 
 // Schur work items.  Dense visibility: off-diagonal tiles and pairs of diagonal tiles, each split over k so that the
-// grid is one CTA per SM with equal DMMA work (a diagonal pair costs 45/36 of a full tile per chunk).  Sparse
+// grid is one CTA per SM with equal DMMA work (a diagonal pair issues 84/72 of a full tile's MMAs per chunk).  Sparse
 // visibility (fewer than 70 % of the (point, tile pair) incidences exist): every tile pair gets the compacted list of
 // the k rows of the points BOTH its column tiles see, and CTAs are dealt in proportion to list length.
 static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
@@ -1483,8 +1483,12 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
   int nt = 0;
   for (int I = 0; I < nb; ++I)
     for (int J = I; J < nb; ++J) tof[(size_t)I * nb + J] = nt++;
-  const double w_pair = 1.55;  // measured cost of a diagonal-pair CTA per k chunk relative to an off-diagonal one
-  const double w_single = 0.75;
+  // measured cost of a diagonal-pair (single diagonal) CTA per k chunk relative to an off-diagonal one
+  // (profiles/microbench/syrk_feed.cu, H100 SXM at a 400 W power limit).  w_single also weighs the diagonal tiles in the choice between
+  // dense tiles and row lists below (listed < 0.7 * dense), so it moves that threshold: schur_sparse (stat key 0) can
+  // differ from earlier builds on rigs near it.
+  const double w_pair = 1.31;
+  const double w_single = 1.04;
 
   // per-pair row lists, if sparse: offset of each tile pair's list in d_klist (-1: no common point) and its point count
   std::vector<long long> pair_koff, pair_cnt;
@@ -1590,11 +1594,11 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
   }
   double W = 0.0;
   for (auto& g : groups) W += g.w * g.chunks;
-  // flops the product issues per launch: an off-diagonal tile is 96 x 96 outputs per k row, a diagonal tile its 10
-  // upper-triangular 24 x 24 blocks
+  // flops the product issues per launch: an off-diagonal tile is 96 x 96 outputs per k row, a diagonal tile its 42
+  // 16 x 8 blocks on or above the diagonal
   p->schur_flop_issued = 0.0;
   for (auto& g : groups) {
-    const double cols2 = g.kind == 0 ? 96.0 * 96.0 : (g.J >= 0 ? 2.0 : 1.0) * 10.0 * 24.0 * 24.0;
+    const double cols2 = g.kind == 0 ? 96.0 * 96.0 : (g.J >= 0 ? 2.0 : 1.0) * 42.0 * 16.0 * 8.0;
     p->schur_flop_issued += 2.0 * cols2 * (double)g.chunks * cb::SY_KC;
   }
   std::vector<cb::SyItem> items;

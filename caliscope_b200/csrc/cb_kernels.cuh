@@ -389,19 +389,89 @@ struct SyItem {
                // seen by cameras of BOTH column tiles; padded with the index of an all-zero row); -1: all rows
 };
 
-// Diagonal blocks (24 x 24, not a multiple of 16 rows) stay on m8n8k4.
-// Fragment ownership (PTX m8n8k4.f64): A[row = lane>>2][k = lane&3], B[k = lane&3][col = lane>>2],
-// C[row = lane>>2][col = 2*(lane&3) + {0,1}];  A[i][k] = Zt[k][I*96 + i], B[k][j] = Zt[k][J*96 + j].
-//
-// kind 0: 8 consumer warps as 2 (row groups of 48) x 4 (column groups of 24): 3 x 3 m16n8k16 tiles per warp
-//         (A[i][k] sits in shared memory at As[k*SY_LDS + i], B[k][j] likewise).
-// kind 1: only the 10 upper-triangular 24x24 blocks of each diagonal tile are formed; the 20 blocks of the
-//         pair are dealt 3/3/3/3/2/2/2/2 to warps 0..7 so every SM sub-partition (warps w and w+4) carries 5.
-__constant__ signed char SY_DIAG_BLOCKS[8][3][3] = {
-    // {tile select, block row, block col}; select -1 = no block
-    {{0, 0, 0}, {0, 0, 1}, {0, 0, 2}}, {{0, 0, 3}, {0, 1, 3}, {0, 2, 3}}, {{0, 1, 1}, {0, 1, 2}, {0, 2, 2}},
-    {{0, 3, 3}, {1, 3, 3}, {1, 2, 2}}, {{1, 0, 0}, {1, 0, 1}, {-1, 0, 0}}, {{1, 0, 2}, {1, 0, 3}, {-1, 0, 0}},
-    {{1, 1, 1}, {1, 1, 2}, {-1, 0, 0}}, {{1, 1, 3}, {1, 2, 3}, {-1, 0, 0}}};
+// Both kinds issue m16n8k16 (A[i][k] = Zt[k][I*96 + i] sits in shared memory at As[k*SY_LDS + i], B[k][j] likewise).
+// kind 0: 8 consumer warps as 2 (row groups of 48) x 4 (column groups of 24): 3 x 3 m16n8k16 tiles per warp.
+// kind 1: a diagonal tile is formed at 16x8 granularity, only the 42 of its 72 (16-row, 8-column) blocks that hold an
+//         element on or above the diagonal (block (rb, cb) with cb >= 2 rb).  A warp takes one or two runs of
+//         consecutive blocks along a block row, so it loads the A fragment of at most two block rows per k step.
+//         Pair: warps 0-3 form tile I, 4-7 tile I2, 11/11/10/10 blocks each (an SM sub-partition, warps w and w+4,
+//         carries 20-22 against 18 for an off-diagonal tile).  Single tile: the 42 blocks over all 8 warps, at most 6.
+struct SyDiagRuns {
+  signed char sel, rA, cA, nA, rB, cB, nB;  // tile (0: I, 1: I2), then runs {block row, first block column, length}
+};
+constexpr int SY_DIAG_MAX = 11;  // blocks of the longest warp share
+__constant__ SyDiagRuns SY_DIAG_RUNS[2][8] = {
+    {{0, 0, 0, 11, 0, 0, 0}, {0, 0, 11, 1, 1, 2, 10}, {0, 2, 4, 8, 5, 10, 2}, {0, 3, 6, 6, 4, 8, 4},
+     {1, 0, 0, 11, 0, 0, 0}, {1, 0, 11, 1, 1, 2, 10}, {1, 2, 4, 8, 5, 10, 2}, {1, 3, 6, 6, 4, 8, 4}},
+    {{0, 0, 0, 6, 0, 0, 0}, {0, 0, 6, 5, 0, 0, 0}, {0, 0, 11, 1, 1, 2, 4}, {0, 1, 6, 6, 0, 0, 0},
+     {0, 2, 4, 5, 0, 0, 0}, {0, 2, 9, 3, 5, 10, 2}, {0, 3, 6, 6, 0, 0, 0}, {0, 4, 8, 4, 0, 0, 0}}};
+
+// The MMAs of one pipeline stage (SY_KC k rows) for one consumer warp.  Split out of schur_syrk_kernel so that
+// profiles/microbench/syrk_feed.cu times exactly this math with and without the loads.
+// Off-diagonal tile: warp (wr, wc) of 2 x 4 forms rows wr*48 .. +47, columns wc*24 .. +23.
+__device__ __forceinline__ void syrk_offdiag_stage(double (&acc)[3][3][4], const double* __restrict__ As_stage,
+                                                   const double* __restrict__ Bs_stage, int wr, int wc, int fr, int fk) {
+  const double* As = As_stage + fk * SY_LDS + wr * 48 + fr;
+  const double* Bs = Bs_stage + fk * SY_LDS + wc * 24 + fr;
+#pragma unroll
+  for (int ks = 0; ks < SY_KC / 16; ++ks) {
+    double a[3][8], b[3][4];
+#pragma unroll
+    for (int u = 0; u < 3; ++u)
+#pragma unroll
+      for (int i = 0; i < 8; ++i) a[u][i] = As[(ks * 16 + 4 * (i >> 1)) * SY_LDS + u * 16 + 8 * (i & 1)];
+#pragma unroll
+    for (int v = 0; v < 3; ++v)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) b[v][j] = Bs[(ks * 16 + 4 * j) * SY_LDS + v * 8];
+#pragma unroll
+    for (int u = 0; u < 3; ++u)
+#pragma unroll
+      for (int v = 0; v < 3; ++v) dmma16816(acc[u][v], a[u], b[v]);
+  }
+}
+
+// Diagonal tile: the warp's runs of 16x8 blocks (SY_DIAG_RUNS) of the tile at T_stage.  Run A is blocks 0 .. nA-1, run B
+// nA .. nA+nB-1, each with its block row's A fragment.  The B fragments are loaded a batch of blocks at a time and the
+// MMAs follow the whole batch, so the loads of a batch overlap (a branch between each load and its MMA serialises them on
+// shared-memory latency).  Blocks of a batch outside the run are neither loaded nor multiplied; every condition is
+// warp-uniform.
+__device__ __forceinline__ void syrk_diag_stage(double (&acc)[SY_DIAG_MAX][4], const double* __restrict__ T_stage,
+                                                const SyDiagRuns& run, int fr, int fk) {
+  const int rA = run.rA, cA = run.cA, nA = run.nA, rB = run.rB, cB = run.cB, nB = run.nB;
+  const double* T = T_stage + fk * SY_LDS + fr;
+#pragma unroll
+  for (int ks = 0; ks < SY_KC / 16; ++ks) {
+    const double* Tk = T + ks * 16 * SY_LDS;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int lo = h ? nA : 0, hi = h ? nA + nB : nA, rb = h ? rB : rA, c0 = h ? cB - nA : cA;
+      if (lo >= hi) continue;
+      double a[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) a[i] = Tk[4 * (i >> 1) * SY_LDS + rb * 16 + 8 * (i & 1)];
+      constexpr int BATCH = 4;
+#pragma unroll
+      for (int j0 = 0; j0 < SY_DIAG_MAX; j0 += BATCH) {
+        if (j0 + BATCH <= lo || j0 >= hi) continue;
+        double b[BATCH][4];
+#pragma unroll
+        for (int jj = 0; jj < BATCH; ++jj) {
+          const int j = j0 + jj;
+          if (j < SY_DIAG_MAX && j >= lo && j < hi) {
+#pragma unroll
+            for (int q = 0; q < 4; ++q) b[jj][q] = Tk[4 * q * SY_LDS + (c0 + j) * 8];
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < BATCH; ++jj) {
+          const int j = j0 + jj;
+          if (j < SY_DIAG_MAX && j >= lo && j < hi) dmma16816(acc[j], a, b[jj]);
+        }
+      }
+    }
+  }
+}
 
 __global__ void __launch_bounds__(SY_THREADS, 1)
 schur_syrk_kernel(const LmState* __restrict__ st, const double* __restrict__ Zt, size_t LD,
@@ -464,24 +534,7 @@ schur_syrk_kernel(const LmState* __restrict__ st, const double* __restrict__ Zt,
     for (int it = 0; it < n_it; ++it) {
       const int stage = it % SY_STAGES;
       mbar_wait(&sm.full[stage], (uint32_t)((it / SY_STAGES) & 1));
-      const double* As = sm.A[stage] + fk * SY_LDS + wr * 48 + fr;
-      const double* Bs = sm.B[stage] + fk * SY_LDS + wc * 24 + fr;
-#pragma unroll
-      for (int ks = 0; ks < SY_KC / 16; ++ks) {
-        double a[3][8], b[3][4];
-#pragma unroll
-        for (int u = 0; u < 3; ++u)
-#pragma unroll
-          for (int i = 0; i < 8; ++i) a[u][i] = As[(ks * 16 + 4 * (i >> 1)) * SY_LDS + u * 16 + 8 * (i & 1)];
-#pragma unroll
-        for (int v = 0; v < 3; ++v)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) b[v][j] = Bs[(ks * 16 + 4 * j) * SY_LDS + v * 8];
-#pragma unroll
-        for (int u = 0; u < 3; ++u)
-#pragma unroll
-          for (int v = 0; v < 3; ++v) dmma16816(acc[u][v], a[u], b[v]);
-      }
+      syrk_offdiag_stage(acc, sm.A[stage], sm.B[stage], wr, wc, fr, fk);
       __syncwarp();
       if (lane == 0) mbar_arrive(&sm.empty[stage]);
     }
@@ -498,46 +551,19 @@ schur_syrk_kernel(const LmState* __restrict__ st, const double* __restrict__ Zt,
     return;
   }
 
-  // ---------------- diagonal pair ----------------
-  int bsel[3], brow[3], bcol[3];
-  const int wmap = wid;
+  // ---------------- diagonal pair (or single diagonal tile) ----------------
+  const SyDiagRuns run = SY_DIAG_RUNS[two ? 0 : 1][wid];
+  const int rA = run.rA, cA = run.cA, nA = run.nA, rB = run.rB, cB = run.cB, nB = run.nB;
+  double acc[SY_DIAG_MAX][4];
 #pragma unroll
-  for (int b = 0; b < 3; ++b) {
-    bsel[b] = SY_DIAG_BLOCKS[wmap][b][0];
-    brow[b] = SY_DIAG_BLOCKS[wmap][b][1];
-    bcol[b] = SY_DIAG_BLOCKS[wmap][b][2];
-    if (bsel[b] == 1 && !two) bsel[b] = -1;
-  }
-  double acc[3][3][3][2];
-#pragma unroll
-  for (int b = 0; b < 3; ++b)
-#pragma unroll
-    for (int u = 0; u < 3; ++u)
-#pragma unroll
-      for (int v = 0; v < 3; ++v) acc[b][u][v][0] = acc[b][u][v][1] = 0.0;
+  for (int j = 0; j < SY_DIAG_MAX; ++j) acc[j][0] = acc[j][1] = acc[j][2] = acc[j][3] = 0.0;
   double tacc = 0.0;
   const int trow = tid % SY_TILE, tsel = tid / SY_TILE;  // threads 0..191: one row of Z t each
   const bool tact = tid < 2 * SY_TILE && (tsel == 0 || two);
   for (int it = 0; it < n_it; ++it) {
     const int stage = it % SY_STAGES;
     mbar_wait(&sm.full[stage], (uint32_t)((it / SY_STAGES) & 1));
-#pragma unroll
-    for (int ks = 0; ks < SY_KC / 4; ++ks) {
-#pragma unroll
-      for (int b = 0; b < 3; ++b) {
-        if (bsel[b] < 0) continue;  // warp-uniform
-        const double* T = (bsel[b] == 0 ? sm.A[stage] : sm.B[stage]) + (ks * 4 + fk) * SY_LDS + fr;
-        double a[3], bb[3];
-#pragma unroll
-        for (int u = 0; u < 3; ++u) a[u] = T[brow[b] * 24 + u * 8];
-#pragma unroll
-        for (int v = 0; v < 3; ++v) bb[v] = T[bcol[b] * 24 + v * 8];
-#pragma unroll
-        for (int u = 0; u < 3; ++u)
-#pragma unroll
-          for (int v = 0; v < 3; ++v) dmma884(acc[b][u][v][0], acc[b][u][v][1], a[u], bb[v]);
-      }
-    }
+    syrk_diag_stage(acc, run.sel == 0 ? sm.A[stage] : sm.B[stage], run, fr, fk);
     if (tact) {
       const double* Ad = (tsel == 0 ? sm.A[stage] : sm.B[stage]);
 #pragma unroll 8
@@ -546,24 +572,23 @@ schur_syrk_kernel(const LmState* __restrict__ st, const double* __restrict__ Zt,
     __syncwarp();
     if (lane == 0) mbar_arrive(&sm.empty[stage]);
   }
+  double* out = part + (size_t)(run.sel == 0 ? item.slotA : item.slotB) * (SY_TILE * SY_TILE);
 #pragma unroll
-  for (int b = 0; b < 3; ++b) {
-    if (bsel[b] < 0) continue;
-    double* out = part + (size_t)(bsel[b] == 0 ? item.slotA : item.slotB) * (SY_TILE * SY_TILE);
+  for (int j = 0; j < SY_DIAG_MAX; ++j) {
+    if (j >= nA + nB) break;
+    const int rb = j < nA ? rA : rB, cb = j < nA ? cA + j : cB + (j - nA);
 #pragma unroll
-    for (int u = 0; u < 3; ++u)
-#pragma unroll
-      for (int v = 0; v < 3; ++v) {
-        const int r = brow[b] * 24 + u * 8 + fr, cc = bcol[b] * 24 + v * 8 + 2 * fk;
-        *reinterpret_cast<double2*>(out + r * SY_TILE + cc) = make_double2(acc[b][u][v][0], acc[b][u][v][1]);
-      }
+    for (int h = 0; h < 2; ++h) {
+      const int r = rb * 16 + 8 * h + fr, cc = cb * 8 + 2 * fk;
+      *reinterpret_cast<double2*>(out + r * SY_TILE + cc) = make_double2(acc[j][2 * h], acc[j][2 * h + 1]);
+    }
   }
   if (tact) tpart[(size_t)(tsel == 0 ? item.slotA : item.slotB) * SY_TILE + trow] = tacc;
 }
 
 // red = [ S (nP*nP) | b (nP) | gc (nP) | diagU (nP) | cost | gpmax slots ... ]   (local partials)
 // one output element of S = U - Z Z^T, b = g_c - Z t (+ g_c, diag U, cost) from the split-K partial tiles;
-// diagonal tiles hold only their upper-triangular 24x24 blocks
+// diagonal tiles hold only the 16x8 blocks that reach the diagonal or above it, which cover every element li <= lj
 template <int P>
 __device__ __forceinline__ void finalize_elem(size_t idx, int nP, int n_blk, const int* __restrict__ tile_of,
                                               const int* __restrict__ tile_slot_start,
@@ -577,7 +602,7 @@ __device__ __forceinline__ void finalize_elem(size_t idx, int nP, int n_blk, con
     const int i = (int)(idx / nP), j = (int)(idx % nP);
     int I = i / SY_TILE, J = j / SY_TILE, li = i % SY_TILE, lj = j % SY_TILE;
     if (I > J) { int t = I; I = J; J = t; t = li; li = lj; lj = t; }
-    if (I == J && li / 24 > lj / 24) { int t = li; li = lj; lj = t; }
+    if (I == J && li > lj) { int t = li; li = lj; lj = t; }
     const int tile = tile_of[I * n_blk + J];
     double s = 0.0;
     const int q1 = tile_slot_start[tile + 1];
