@@ -182,27 +182,8 @@ cov_point_kernel(const int* __restrict__ pt_start, const int* __restrict__ pm_ca
       if (pb < pa) continue;  // X_dc = X_cd^T: each unordered pair once
       const int ca = pm_cam[pa], cb = pm_cam[pb];
       if ((pa > s && pm_cam[pa - 1] == ca) || (pb > s && pm_cam[pb - 1] == cb)) continue;  // repeated rows of one camera
-      double zb[3][P];
-#pragma unroll
-      for (int b = 0; b < 3; ++b)
-#pragma unroll
-        for (int q = 0; q < P; ++q) zb[b][q] = zrow[(size_t)b * LD + (size_t)cb * P + q];
-      double x[3][3] = {{0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}};
-#pragma unroll
-      for (int p = 0; p < P; ++p) {
-        const double* srow = Sig + (size_t)(ca * P + p) * nP + (size_t)cb * P;
-        double y0 = 0.0, y1 = 0.0, y2 = 0.0;
-#pragma unroll
-        for (int q = 0; q < P; ++q) {
-          const double sv = srow[q];
-          y0 = fma(sv, zb[0][q], y0); y1 = fma(sv, zb[1][q], y1); y2 = fma(sv, zb[2][q], y2);
-        }
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-          const double za = zrow[(size_t)a * LD + (size_t)ca * P + p];
-          x[a][0] = fma(za, y0, x[a][0]); x[a][1] = fma(za, y1, x[a][1]); x[a][2] = fma(za, y2, x[a][2]);
-        }
-      }
+      double x[3][3];
+      cov_pair_gather<P>(zrow + (size_t)ca * P, zrow + (size_t)cb * P, LD, Sig, nP, ca, cb, x);
       const bool same = pa == pb;
 #pragma unroll
       for (int a = 0; a < 3; ++a)

@@ -21,6 +21,7 @@ constexpr int CT_SX = 31;    // fx / fx0
 constexpr int CT_SY = 32;    // fy / fx0
 constexpr int CT_FYR = 33;   // fy0 / fx0
 constexpr int CT_FLAGS = 34; // flags as double
+constexpr int CT_FX0 = 35;   // fx0
 constexpr int CT_SIZE = 36;
 // stride of a camera-table entry in SHARED memory when lanes of a warp read DIFFERENT cameras (point-major kernels): an odd
 // number of doubles, so that the same field of 16 consecutive cameras falls into 16 different 8-byte banks (stride 36 puts
@@ -243,6 +244,40 @@ __device__ __forceinline__ void obs_res_jx(const double* __restrict__ cam, doubl
   for (int k = 0; k < 3; ++k) {
     JX[k] = t0 * R[k] + t1 * R[3 + k] + t2 * R[6 + k];
     JX[3 + k] = t3 * R[k] + t4 * R[3 + k] + t5 * R[6 + k];
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// One camera pair of a point covariance gather: x = Z_a Sig_ab Z_b^T for the 3 x P blocks Z_a, Z_b (row stride ld) and
+// the P x P block (ca, cb) of Sig (row stride nP).  cov_point_kernel (Z = the point's Zt rows) and tri_cov_kernel
+// (Z = the per-camera blocks J_X^T J_c of a triangulated point) both sum these over the unordered camera pairs.
+// ---------------------------------------------------------------------------------------------
+template <int P>
+__device__ __forceinline__ void cov_pair_gather(const double* __restrict__ za, const double* __restrict__ zb, size_t ld,
+                                                const double* __restrict__ Sig, int nP, int ca, int cb, double x[3][3]) {
+  double zr[3][P];
+#pragma unroll
+  for (int b = 0; b < 3; ++b)
+#pragma unroll
+    for (int q = 0; q < P; ++q) zr[b][q] = zb[(size_t)b * ld + q];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) x[a][b] = 0.0;
+#pragma unroll
+  for (int p = 0; p < P; ++p) {
+    const double* srow = Sig + (size_t)(ca * P + p) * nP + (size_t)cb * P;
+    double y0 = 0.0, y1 = 0.0, y2 = 0.0;
+#pragma unroll
+    for (int q = 0; q < P; ++q) {
+      const double sv = srow[q];
+      y0 = fma(sv, zr[0][q], y0); y1 = fma(sv, zr[1][q], y1); y2 = fma(sv, zr[2][q], y2);
+    }
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      const double v = za[(size_t)a * ld + p];
+      x[a][0] = fma(v, y0, x[a][0]); x[a][1] = fma(v, y1, x[a][1]); x[a][2] = fma(v, y2, x[a][2]);
+    }
   }
 }
 

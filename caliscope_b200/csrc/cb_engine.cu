@@ -2799,38 +2799,33 @@ namespace {
 
 int group_by_key(const long long* d_key, int n, cudaStream_t st, ScopedFree& sf, int** d_rows, int** d_start, int* n_groups);
 
-// shared body of cb_triangulate_dlt / cb_undistort_triangulate: `undist` non-null = obs_xy are raw pixels,
-// undistorted on the device (normalised output) before the DLT, never leaving HBM in between.
-int triangulate_impl(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int64_t n_obs,
-                     const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
-                     int32_t max_groups, int32_t* n_groups_out, double* xyz_out, int32_t* count_out,
-                     int32_t* rep_row_out, uint64_t* camset_sig_out, CbTriStats* stats, int device, void* stream) {
-  if (n_cams <= 0 || !proj || n_obs < 0 || n_obs > 0x7fffffffLL || !n_groups_out || max_groups < 0 ||
-      (n_obs > 0 && (!obs_cam || !obs_key || !obs_xy)) ||
-      (max_groups > 0 && (!xyz_out || !count_out || !rep_row_out || !camset_sig_out))) {
-    g_last_error = "cb_triangulate_dlt: bad argument";
-    return CB_E_INVALID;
-  }
-  CB_TRY(select_device(device));
-  *n_groups_out = 0;
-  if (stats) std::memset(stats, 0, sizeof(*stats));
-  if (n_obs == 0) return CB_OK;
-  const long long launches0 = g_launches.load();
-  cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
-  const int n = (int)n_obs;
-  const int TB = 256, G = cdiv(n, TB);
-  cudaEvent_t ev[4];
-  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); } } evg{ev};
-  CB_CUDA(cudaEventRecord(ev[0], st));
+// device-side result of the grouping and the DLT (buffers owned by the caller's ScopedFree)
+struct TriDlt {
+  const int* cam = nullptr;  // obs_cam on the device
+  int* rows = nullptr;       // caller rows sorted by key (stable)
+  int* start = nullptr;      // group boundaries, n_groups + 1
+  int n_groups = 0;
+  int lanes = 8;             // lanes per group of the DLT kernel (8, or 32 when groups average > 96 rows)
+  double* xyz = nullptr;
+  int* count = nullptr;
+  int* rep = nullptr;
+  unsigned long long* sig = nullptr;
+};
 
+// upload + validation + (undistortion) + grouping + DLT, the stages every triangulation call shares.  Records ev[1] after
+// the grouping and ev[2] / ev[3] around the DLT kernel.  `undist` non-null = obs_xy are raw pixels, undistorted on the
+// device (normalised output) before the DLT, never leaving HBM in between.
+int tri_dlt_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int n,
+                  const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
+                  int32_t max_groups, int32_t* n_groups_out, const char* who, cudaEvent_t* ev, ScopedFree& sf,
+                  cudaStream_t st, TriDlt* out) {
+  const int TB = 256, G = cdiv(n, TB);
   const int* d_cam = nullptr;
   const long long* d_key = nullptr;
   const double* d_xy = nullptr;
   CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
   CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
-  CB_TRY(validate_rows(d_cam, d_key, n, n_cams, st, "cb_triangulate_dlt"));
+  CB_TRY(validate_rows(d_cam, d_key, n, n_cams, st, who));
   if (undist) {
     cb::UndistCam* d_tab = nullptr;
     CB_TRY(dalloc(&d_tab, (size_t)n_cams));
@@ -2863,7 +2858,7 @@ int triangulate_impl(int32_t n_cams, const std::vector<cb::UndistCam>* undist, c
   CB_CUDA(cudaEventRecord(ev[1], st));
   *n_groups_out = n_groups;
   if (n_groups > max_groups) {
-    g_last_error = "cb_triangulate_dlt: " + std::to_string(n_groups) + " groups but room for " + std::to_string(max_groups);
+    g_last_error = std::string(who) + ": " + std::to_string(n_groups) + " groups but room for " + std::to_string(max_groups);
     return CB_E_INVALID;
   }
   // (3) DLT per group
@@ -2889,10 +2884,48 @@ int triangulate_impl(int32_t n_cams, const std::vector<cb::UndistCam>* undist, c
               d_proj, n_cams, in_smem, d_start, v_out, d_cam, d_xy, n_groups, d_xyz, d_count, d_rep, d_sig);
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[3], st));
-  CB_CUDA(cudaMemcpyAsync(xyz_out, d_xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(count_out, d_count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rep_row_out, d_rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(camset_sig_out, d_sig, sizeof(unsigned long long) * 2 * (size_t)n_groups,
+  out->cam = d_cam;
+  out->rows = v_out;
+  out->start = d_start;
+  out->n_groups = n_groups;
+  out->lanes = lanes;
+  out->xyz = d_xyz;
+  out->count = d_count;
+  out->rep = d_rep;
+  out->sig = d_sig;
+  return CB_OK;
+}
+
+// shared body of cb_triangulate_dlt / cb_undistort_triangulate
+int triangulate_impl(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int64_t n_obs,
+                     const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
+                     int32_t max_groups, int32_t* n_groups_out, double* xyz_out, int32_t* count_out,
+                     int32_t* rep_row_out, uint64_t* camset_sig_out, CbTriStats* stats, int device, void* stream) {
+  if (n_cams <= 0 || !proj || n_obs < 0 || n_obs > 0x7fffffffLL || !n_groups_out || max_groups < 0 ||
+      (n_obs > 0 && (!obs_cam || !obs_key || !obs_xy)) ||
+      (max_groups > 0 && (!xyz_out || !count_out || !rep_row_out || !camset_sig_out))) {
+    g_last_error = "cb_triangulate_dlt: bad argument";
+    return CB_E_INVALID;
+  }
+  CB_TRY(select_device(device));
+  *n_groups_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf;
+  cudaEvent_t ev[4];
+  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
+  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  TriDlt t;
+  CB_TRY(tri_dlt_stage(n_cams, undist, proj, (int)n_obs, obs_cam, obs_key, obs_xy, obs_on_device, max_groups,
+                       n_groups_out, "cb_triangulate_dlt", ev, sf, st, &t));
+  const int n_groups = t.n_groups;
+  CB_CUDA(cudaMemcpyAsync(xyz_out, t.xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, t.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, t.rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(camset_sig_out, t.sig, sizeof(unsigned long long) * 2 * (size_t)n_groups,
                           cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   if (stats) {
@@ -2930,6 +2963,183 @@ int cb_undistort_triangulate(int32_t n_cams, const int32_t* cam_fisheye, const d
   CB_TRY(build_undist_table(n_cams, cam_fisheye, cam_k, cam_dist, tab));
   return triangulate_impl(n_cams, &tab, proj, n_obs, obs_cam, obs_key, obs_px, obs_on_device, max_groups, n_groups_out,
                           xyz_out, count_out, rep_row_out, camset_sig_out, stats, device, stream);
+}
+
+int cb_triangulate_refine(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                          const double* cam_cov, int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key,
+                          const double* obs_px, int obs_on_device, double pixel_sigma, int32_t max_iter, double xtol,
+                          int32_t max_groups, int32_t* n_groups_out, double* xyz_out, double* cov_out,
+                          double* rmse_px_out, int32_t* count_out, int32_t* rep_row_out, int32_t* status_out,
+                          CbTriRefineStats* stats, int device, void* stream) {
+  if (n_cams <= 0 || !cam_flags || !cam_const || !cam_x || n_obs < 0 || n_obs > 0x7fffffffLL || !n_groups_out ||
+      max_groups < 0 || (n_obs > 0 && (!obs_cam || !obs_key || !obs_px)) ||
+      (max_groups > 0 && (!xyz_out || !rmse_px_out || !count_out || !rep_row_out || !status_out)) ||
+      !(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma)) || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol))) {
+    g_last_error = "cb_triangulate_refine: bad argument";
+    return CB_E_INVALID;
+  }
+  // camera models in the BA parameter layout (x: [r t] or [r t s k1 k2] per camera) -> the DLT start's normalised
+  // projection matrices [R|t] and undistortion tables; intrinsics as cam_prep_one forms them
+  std::vector<int> xoff(n_cams + 1, 0);
+  bool any_free = false;
+  for (int c = 0; c < n_cams; ++c) {
+    if (cam_flags[c] < 0 || cam_flags[c] > 3) {
+      g_last_error = "cb_triangulate_refine: camera flags must be a combination of bits 0 and 1";
+      return CB_E_INVALID;
+    }
+    any_free = any_free || (cam_flags[c] & 1);
+    xoff[c + 1] = xoff[c] + ((cam_flags[c] & 1) ? 9 : 6);
+  }
+  const int ncp = xoff[n_cams];
+  std::vector<double> proj(12 * (size_t)n_cams);
+  std::vector<cb::UndistCam> tab(n_cams);
+  for (int c = 0; c < n_cams; ++c) {
+    const double* q = cam_x + xoff[c];
+    const double* k = cam_const + 9 * (size_t)c;
+    const bool free_i = cam_flags[c] & 1;
+    const double th = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+    double R[9];
+    if (th < 1e-12) {
+      const double r[9] = {1, -q[2], q[1], q[2], 1, -q[0], -q[1], q[0], 1};
+      std::memcpy(R, r, sizeof(R));
+    } else {
+      const double kx = q[0] / th, ky = q[1] / th, kz = q[2] / th, s = std::sin(th), co = std::cos(th), c1 = 1.0 - co;
+      const double r[9] = {co + c1 * kx * kx,      c1 * kx * ky - s * kz, c1 * kx * kz + s * ky,
+                           c1 * ky * kx + s * kz, co + c1 * ky * ky,      c1 * ky * kz - s * kx,
+                           c1 * kz * kx - s * ky, c1 * kz * ky + s * kx, co + c1 * kz * kz};
+      std::memcpy(R, r, sizeof(R));
+    }
+    for (int i = 0; i < 3; ++i) {
+      for (int j = 0; j < 3; ++j) proj[12 * (size_t)c + 4 * i + j] = R[3 * i + j];
+      proj[12 * (size_t)c + 4 * i + 3] = q[3 + i];
+    }
+    const double sc = free_i ? q[6] : 1.0, k1 = free_i ? q[7] : k[4], k2 = free_i ? q[8] : k[5];
+    cb::UndistCam& u = tab[c];
+    std::memset(&u, 0, sizeof(u));
+    u.fx = sc * k[0]; u.fy = sc * k[1]; u.cx = k[2]; u.cy = k[3]; u.skew = 0.0;
+    u.fisheye = (cam_flags[c] & 2) ? 1 : 0;
+    u.d[0] = k1; u.d[1] = k2; u.d[2] = k[6]; u.d[3] = k[7];
+    if (!u.fisheye) u.d[4] = k[8];
+    if (!(k[0] != 0.0) || !(u.fx != 0.0) || !(u.fy != 0.0)) {
+      g_last_error = "cb_triangulate_refine: zero focal length in the camera table";
+      return CB_E_INVALID;
+    }
+  }
+  CB_TRY(select_device(device));
+  *n_groups_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf;
+  const int n = (int)n_obs;
+  cudaEvent_t ev[8];
+  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
+  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 8; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  // fp64 pixels on the device: the refinement reads them at full precision; the DLT start rounds them to float32 as
+  // cb_undistort_triangulate does
+  const int* d_cam = nullptr;
+  const long long* d_key = nullptr;
+  const double* d_px = nullptr;
+  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
+  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
+  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
+  TriDlt t;
+  CB_TRY(tri_dlt_stage(n_cams, &tab, proj.data(), n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups, n_groups_out,
+                       "cb_triangulate_refine", ev, sf, st, &t));
+  const int n_groups = t.n_groups;
+
+  // camera table from the BA layout (cam_prep_kernel, P = 9 when any camera has free intrinsics)
+  const int P = any_free ? 9 : 6;
+  int *d_flags = nullptr, *d_xoff = nullptr;
+  double *d_const = nullptr, *d_x = nullptr, *d_xc = nullptr, *d_camtab = nullptr;
+  CB_TRY(dalloc(&d_flags, (size_t)n_cams)); sf.dev.push_back(d_flags);
+  CB_TRY(dalloc(&d_xoff, (size_t)n_cams)); sf.dev.push_back(d_xoff);
+  CB_TRY(dalloc(&d_const, 9 * (size_t)n_cams)); sf.dev.push_back(d_const);
+  CB_TRY(dalloc(&d_x, (size_t)ncp)); sf.dev.push_back(d_x);
+  CB_TRY(dalloc(&d_xc, (size_t)P * n_cams)); sf.dev.push_back(d_xc);
+  CB_TRY(dalloc(&d_camtab, (size_t)cb::CT_SIZE * n_cams)); sf.dev.push_back(d_camtab);
+  CB_CUDA(cudaMemcpyAsync(d_flags, cam_flags, sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(d_xoff, xoff.data(), sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(d_const, cam_const, sizeof(double) * 9 * n_cams, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(d_x, cam_x, sizeof(double) * ncp, cudaMemcpyHostToDevice, st));
+  CB_LAUNCH(cb::unpack_x_kernel, cdiv((long long)n_cams * P, 256), 256, 0, st, d_x, d_xoff, d_flags, d_const, n_cams, P,
+            0, ncp, d_xc, nullptr);
+  CB_LAUNCH(cb::cam_prep_kernel, cdiv(n_cams, 64), 64, 0, st, d_xc, d_flags, d_const, n_cams, P, d_camtab);
+
+  double *d_out_xyz = nullptr, *d_rmse = nullptr;
+  int* d_status = nullptr;
+  CB_TRY(dalloc(&d_out_xyz, 3 * (size_t)n_groups)); sf.dev.push_back(d_out_xyz);
+  CB_TRY(dalloc(&d_rmse, (size_t)n_groups)); sf.dev.push_back(d_rmse);
+  CB_TRY(dalloc(&d_status, (size_t)n_groups)); sf.dev.push_back(d_status);
+  const size_t cam_bytes = sizeof(double) * cb::CT_SMEM * (size_t)n_cams;  // odd stride, see tri_stage_camtab
+  const int cam_in_smem = cam_bytes <= 40 * 1024 ? 1 : 0;
+  const size_t smem = cam_in_smem ? cam_bytes : 0;
+  const int lanes = t.lanes;
+  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
+  CB_CUDA(cudaEventRecord(ev[4], st));
+  if (lanes == 32)
+    CB_LAUNCH(cb::tri_refine_kernel<32>, blocks, cb::TRI_THREADS, smem, st, d_camtab, n_cams, cam_in_smem, t.start,
+              t.rows, t.cam, d_px, n_groups, t.xyz, max_iter, xtol, d_out_xyz, d_rmse, d_status);
+  else
+    CB_LAUNCH(cb::tri_refine_kernel<8>, blocks, cb::TRI_THREADS, smem, st, d_camtab, n_cams, cam_in_smem, t.start,
+              t.rows, t.cam, d_px, n_groups, t.xyz, max_iter, xtol, d_out_xyz, d_rmse, d_status);
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaEventRecord(ev[5], st));
+
+  double* d_cov = nullptr;
+  if (cov_out) {
+    // camera covariance from x's layout to a uniform stride P (fixed / absent slots 0), uploaded once
+    double* d_sig = nullptr;
+    double* d_B = nullptr;
+    int* d_first = nullptr;
+    if (cam_cov) {
+      const size_t nP = (size_t)n_cams * P;
+      std::vector<double> sig(nP * nP, 0.0);
+      for (int c = 0; c < n_cams; ++c)
+        for (int p = 0; p < xoff[c + 1] - xoff[c]; ++p)
+          for (int d = 0; d < n_cams; ++d)
+            for (int q = 0; q < xoff[d + 1] - xoff[d]; ++q)
+              sig[((size_t)c * P + p) * nP + (size_t)d * P + q] = cam_cov[(size_t)(xoff[c] + p) * ncp + xoff[d] + q];
+      CB_TRY(dalloc(&d_sig, nP * nP)); sf.dev.push_back(d_sig);
+      CB_CUDA(cudaMemcpyAsync(d_sig, sig.data(), sizeof(double) * nP * nP, cudaMemcpyHostToDevice, st));
+      CB_TRY(dalloc(&d_B, 3 * (size_t)P * n)); sf.dev.push_back(d_B);
+      CB_TRY(dalloc(&d_first, (size_t)n)); sf.dev.push_back(d_first);
+      CB_CUDA(cudaStreamSynchronize(st));  // `sig` is a stack-lifetime upload
+    }
+    CB_TRY(dalloc(&d_cov, 9 * (size_t)n_groups)); sf.dev.push_back(d_cov);
+    const double s2 = pixel_sigma * pixel_sigma;
+    CB_CUDA(cudaEventRecord(ev[6], st));
+#define CB_TRI_COV(PP, LL)                                                                                           \
+  CB_LAUNCH((cb::tri_cov_kernel<PP, LL>), blocks, cb::TRI_THREADS, smem, st, d_camtab, n_cams, cam_in_smem, t.start, \
+            t.rows, t.cam, d_px, n_groups, d_out_xyz, d_status, d_sig, s2, d_B, d_first, d_cov)
+    if (P == 9 && lanes == 32) CB_TRI_COV(9, 32);
+    else if (P == 9) CB_TRI_COV(9, 8);
+    else if (lanes == 32) CB_TRI_COV(6, 32);
+    else CB_TRI_COV(6, 8);
+#undef CB_TRI_COV
+    CB_CUDA(cudaGetLastError());
+    CB_CUDA(cudaEventRecord(ev[7], st));
+  }
+  CB_CUDA(cudaMemcpyAsync(xyz_out, d_out_xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, t.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, t.rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  if (cov_out)
+    CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (stats) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
+    cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->dlt_ms = ms;
+    cudaEventElapsedTime(&ms, ev[4], ev[5]); stats->refine_ms = ms;
+    if (cov_out) { cudaEventElapsedTime(&ms, ev[6], ev[7]); stats->cov_ms = ms; }
+    cudaEventElapsedTime(&ms, ev[0], cov_out ? ev[7] : ev[5]); stats->total_ms = ms;
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
 }
 
 }  // extern "C"

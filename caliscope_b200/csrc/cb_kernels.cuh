@@ -148,7 +148,7 @@ __device__ __forceinline__ void cam_prep_one(const double* __restrict__ q, const
   o[CT_SY] = fy / k[0];
   o[CT_FYR] = k[1] / k[0];
   o[CT_FLAGS] = (double)flags;
-  o[35] = k[0];
+  o[CT_FX0] = k[0];
 }
 
 __global__ void cam_prep_kernel(const double* __restrict__ xc, const int* __restrict__ cam_flags,

@@ -280,4 +280,301 @@ tri_dlt_kernel(const double* __restrict__ proj, int n_cams, int proj_in_smem, co
   xyz[3 * g + 2] = w[2] / w[3];
 }
 
+// ---- refinement to the reprojection optimum and point covariance (cb_triangulate_refine, DESIGN.md section 4.7) -------
+// Group status codes, first match wins.
+enum { TRI_OK = 0, TRI_FEW_ROWS = 1, TRI_NOT_PD = 2, TRI_MAX_ITER = 3, TRI_BEHIND = 4 };
+constexpr double TRI_LAMBDA0 = 1e-3;  // initial Levenberg-Marquardt damping
+constexpr double TRI_PD_RTOL = 1e-12;
+
+// Cholesky factor (packed 00 10 20 11 21 22) of a symmetric 3x3 h (packed 00 01 02 11 12 22).  Returns false when a pivot
+// is at or below rtol times the largest diagonal entry of h (or is not a number): the depth of a point seen along
+// near-parallel rays is such a direction, although no single coordinate axis need be.
+__device__ __forceinline__ bool chol3(const double* h, double rtol, double* L) {
+  const double thr = rtol * fmax(h[0], fmax(h[3], h[5]));
+  const double p0 = h[0];
+  L[0] = sqrt(p0);
+  L[1] = h[1] / L[0];
+  L[2] = h[2] / L[0];
+  const double p1 = h[3] - L[1] * L[1];
+  L[3] = sqrt(p1);
+  L[4] = (h[4] - L[2] * L[1]) / L[3];
+  const double p2 = h[5] - L[2] * L[2] - L[4] * L[4];
+  L[5] = sqrt(p2);
+  return p0 > thr && p1 > thr && p2 > thr;
+}
+
+// (L L^T) d = -g
+__device__ __forceinline__ void chol3_solve_neg(const double* L, const double* g, double* d) {
+  const double y0 = -g[0] / L[0];
+  const double y1 = (-g[1] - L[1] * y0) / L[3];
+  const double y2 = (-g[2] - L[2] * y0 - L[4] * y1) / L[5];
+  d[2] = y2 / L[5];
+  d[1] = (y1 - L[4] * d[2]) / L[3];
+  d[0] = (y0 - L[1] * d[1] - L[2] * d[2]) / L[0];
+}
+
+// camera-table staging shared by the two kernels below: an odd stride in shared memory (CT_SMEM, lanes of a warp read
+// different cameras), the global table as it is otherwise
+__device__ __forceinline__ const double* tri_stage_camtab(const double* __restrict__ camtab, int n_cams, int in_smem,
+                                                          double* s_cam, int& stride) {
+  if (in_smem) {
+    for (int i = threadIdx.x; i < n_cams * CT_SIZE; i += blockDim.x) s_cam[(i / CT_SIZE) * CT_SMEM + i % CT_SIZE] = camtab[i];
+    __syncthreads();
+    stride = CT_SMEM;
+    return s_cam;
+  }
+  stride = CT_SIZE;
+  return camtab;
+}
+
+// Cost (squared pixels), J^T J and J^T r (pixels) of one group's rows at X, summed over the LANES lanes of the group: an
+// xor butterfly leaves the identical sums on every lane.  Lanes with `on` false contribute zero but still shuffle.
+template <int LANES>
+__device__ __forceinline__ void tri_normal_eq(const double* cams, int stride, const int* __restrict__ rows,
+                                              const int* __restrict__ obs_cam, const double* __restrict__ obs_px, int b,
+                                              int e, int lane, bool on, const double* X, double acc[10]) {
+#pragma unroll
+  for (int k = 0; k < 10; ++k) acc[k] = 0.0;
+  if (on)
+    for (int i = b + lane; i < e; i += LANES) {
+      const int r = rows[i];
+      const double* cam = cams + (size_t)stride * obs_cam[r];
+      const double2 px = reinterpret_cast<const double2*>(obs_px)[r];
+      double f[2], J[6];
+      obs_res_jx(cam, X[0], X[1], X[2], px.x, px.y, 0, 1.0, f, J);
+      const double fx0 = cam[CT_FX0];
+      const double r0 = f[0] * fx0, r1 = f[1] * fx0;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) J[k] *= fx0;
+      acc[0] = fma(J[0], J[0], fma(J[3], J[3], acc[0]));
+      acc[1] = fma(J[0], J[1], fma(J[3], J[4], acc[1]));
+      acc[2] = fma(J[0], J[2], fma(J[3], J[5], acc[2]));
+      acc[3] = fma(J[1], J[1], fma(J[4], J[4], acc[3]));
+      acc[4] = fma(J[1], J[2], fma(J[4], J[5], acc[4]));
+      acc[5] = fma(J[2], J[2], fma(J[5], J[5], acc[5]));
+      acc[6] = fma(J[0], r0, fma(J[3], r1, acc[6]));
+      acc[7] = fma(J[1], r0, fma(J[4], r1, acc[7]));
+      acc[8] = fma(J[2], r0, fma(J[5], r1, acc[8]));
+      acc[9] = fma(r0, r0, fma(r1, r1, acc[9]));
+    }
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1)
+#pragma unroll
+    for (int k = 0; k < 10; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], s);
+}
+
+// Per group, Levenberg-Marquardt on the pixel reprojection cost from the DLT point xyz0 (oracle/triangulation_refine.py
+// refine_points states the same rule):  solve (H + lam diag H) d = -g;  accept when the cost drops (lam /= 10), else
+// lam *= 10;  stop when |d| <= xtol (|X| + xtol) or after max_iter steps.  Every lane of a group holds the same reduced
+// sums, so every lane solves the same 3x3 system and takes the same decision; the loop runs until no group of the warp
+// is active, because the shuffles need the whole warp.  Writes xyz (the DLT point when H is not positive definite),
+// the pixel RMSE and the status code.
+template <int LANES>
+__global__ void __launch_bounds__(TRI_THREADS)
+tri_refine_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
+                  const int* __restrict__ rows, const int* __restrict__ obs_cam, const double* __restrict__ obs_px,
+                  int n_groups, const double* __restrict__ xyz0, int max_iter, double xtol, double* __restrict__ xyz,
+                  double* __restrict__ rmse, int* __restrict__ status) {
+  extern __shared__ double s_cam[];
+  int stride;
+  const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
+  const int lane = threadIdx.x & (LANES - 1);
+  const long long g = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LANES;
+  const bool live = g < n_groups;
+  const int b = live ? start[g] : 0, e = live ? start[g + 1] : 0, n = e - b;
+  double X[3] = {0.0, 0.0, 0.0};
+  if (live)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) X[k] = xyz0[3 * g + k];
+  int st = n < 2 ? TRI_FEW_ROWS : TRI_OK;
+  double acc[10], L[6];
+  tri_normal_eq<LANES>(cams, stride, rows, obs_cam, obs_px, b, e, lane, live && st == TRI_OK, X, acc);
+  const double cost0 = acc[9];
+  if (st == TRI_OK && !chol3(acc, TRI_PD_RTOL, L)) st = TRI_NOT_PD;
+  bool active = live && st == TRI_OK;
+  double lam = TRI_LAMBDA0;
+  int it = 0;
+  while (__any_sync(0xffffffffu, active)) {
+    if (active && it == max_iter) {
+      st = TRI_MAX_ITER;
+      active = false;
+    }
+    double d[3] = {0.0, 0.0, 0.0}, Xt[3];
+    if (active) {
+      double A[6] = {acc[0] * (1.0 + lam), acc[1], acc[2], acc[3] * (1.0 + lam), acc[4], acc[5] * (1.0 + lam)};
+      chol3(A, 0.0, L);
+      chol3_solve_neg(L, acc + 6, d);
+    }
+#pragma unroll
+    for (int k = 0; k < 3; ++k) Xt[k] = X[k] + d[k];
+    double tr[10];
+    tri_normal_eq<LANES>(cams, stride, rows, obs_cam, obs_px, b, e, lane, active, Xt, tr);
+    if (active) {
+      ++it;
+      const double dn = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+      const double xn = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
+      if (tr[9] < acc[9]) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) X[k] = Xt[k];
+#pragma unroll
+        for (int k = 0; k < 10; ++k) acc[k] = tr[k];
+        lam *= 0.1;
+      } else {
+        lam *= 10.0;
+      }
+      if (dn <= xtol * (xn + xtol)) active = false;
+    }
+  }
+  if ((st == TRI_OK || st == TRI_MAX_ITER) && !chol3(acc, TRI_PD_RTOL, L)) st = TRI_NOT_PD;
+  // behind a camera at the solution
+  int behind = 0;
+  if (live && st == TRI_OK)
+    for (int i = b + lane; i < e; i += LANES) {
+      const double* cam = cams + (size_t)stride * obs_cam[rows[i]];
+      const double z = fma(cam[CT_R + 6], X[0], fma(cam[CT_R + 7], X[1], fma(cam[CT_R + 8], X[2], cam[CT_T + 2])));
+      behind |= !(z > 0.0);
+    }
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1) behind |= __shfl_xor_sync(0xffffffffu, behind, s);
+  if (!live || lane != 0) return;
+  if (st == TRI_OK && behind) st = TRI_BEHIND;
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  const bool at_start = st == TRI_FEW_ROWS || st == TRI_NOT_PD;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) xyz[3 * g + k] = at_start ? xyz0[3 * g + k] : X[k];
+  rmse[g] = st == TRI_FEW_ROWS ? nan : sqrt((at_start ? cost0 : acc[9]) / n);
+  status[g] = st;
+}
+
+// Per group at the refined point X (status 0, 3 or 4; NaN otherwise), the first-order covariance
+//   Sigma_X = s2 H^-1 + H^-1 M H^-1,   M = sum_{c,d} B_c Sigma_cd B_d^T,   B_c = sum over the rows of camera c of J_X^T J_c
+// (pixels).  Sig (n_cams*P square, uniform stride P, nullptr: no camera term) is read from L2.  The lanes of a group write
+// each camera's B_c once (at the position of its first row in the group, scratch `Bs` / `first`), then gather the
+// unordered camera pairs with cov_pair_gather, the gather of cov_point_kernel.
+template <int P, int LANES>
+__global__ void __launch_bounds__(TRI_THREADS)
+tri_cov_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
+               const int* __restrict__ rows, const int* __restrict__ obs_cam, const double* __restrict__ obs_px,
+               int n_groups, const double* __restrict__ xyz, const int* __restrict__ status,
+               const double* __restrict__ Sig, double s2, double* __restrict__ Bs, int* __restrict__ first,
+               double* __restrict__ cov) {
+  extern __shared__ double s_cam[];
+  int stride;
+  const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
+  const int lane = threadIdx.x & (LANES - 1);
+  const long long g = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LANES;
+  const bool live = g < n_groups;
+  const int st = live ? status[g] : TRI_FEW_ROWS;
+  const bool on = st == TRI_OK || st == TRI_MAX_ITER || st == TRI_BEHIND;
+  const int b = on ? start[g] : 0, e = on ? start[g + 1] : 0, k = e - b;
+  const int nP = n_cams * P;
+  double X[3] = {0.0, 0.0, 0.0};
+  if (on)
+#pragma unroll
+    for (int q = 0; q < 3; ++q) X[q] = xyz[3 * g + q];
+  double h[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int i = b + lane; i < e; i += LANES) {
+    const int c = obs_cam[rows[i]];
+    bool is_first = true;
+    if (Sig)
+      for (int j = b; j < i && is_first; ++j) is_first = obs_cam[rows[j]] != c;
+    double Bc[3][P];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int q = 0; q < P; ++q) Bc[a][q] = 0.0;
+    // row i, then (first row of its camera only) the later rows of the same camera
+    for (int j = i; j < e; ++j) {
+      const int r = rows[j];
+      if (j > i && (!Sig || !is_first)) break;
+      if (obs_cam[r] != c) continue;
+      const double* cam = cams + (size_t)stride * c;
+      const double2 px = reinterpret_cast<const double2*>(obs_px)[r];
+      double f[2], J[6], Jc[2 * P];
+      obs_jac<P>(cam, X[0], X[1], X[2], px.x, px.y, 0, 1.0, f, J, Jc);
+      const double fx0 = cam[CT_FX0];
+#pragma unroll
+      for (int q = 0; q < 6; ++q) J[q] *= fx0;
+      if (j == i) {
+        h[0] = fma(J[0], J[0], fma(J[3], J[3], h[0]));
+        h[1] = fma(J[0], J[1], fma(J[3], J[4], h[1]));
+        h[2] = fma(J[0], J[2], fma(J[3], J[5], h[2]));
+        h[3] = fma(J[1], J[1], fma(J[4], J[4], h[3]));
+        h[4] = fma(J[1], J[2], fma(J[4], J[5], h[4]));
+        h[5] = fma(J[2], J[2], fma(J[5], J[5], h[5]));
+      }
+      if (Sig && is_first)
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+#pragma unroll
+          for (int q = 0; q < P; ++q) Bc[a][q] = fma(J[a], Jc[q] * fx0, fma(J[3 + a], Jc[P + q] * fx0, Bc[a][q]));
+    }
+    if (Sig) {
+      first[i] = is_first ? 1 : 0;
+      if (is_first)
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+#pragma unroll
+          for (int q = 0; q < P; ++q) Bs[(size_t)i * 3 * P + a * P + q] = Bc[a][q];
+    }
+  }
+  double m[3][3] = {{0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}, {0.0, 0.0, 0.0}};
+  if (Sig) {
+    __syncwarp();
+    for (int idx = lane; idx < k * k; idx += LANES) {
+      const int pa = b + idx / k, pb = b + idx % k;
+      if (pb < pa || !first[pa] || !first[pb]) continue;
+      double x[3][3];
+      cov_pair_gather<P>(Bs + (size_t)pa * 3 * P, Bs + (size_t)pb * 3 * P, P, Sig, nP, obs_cam[rows[pa]],
+                         obs_cam[rows[pb]], x);
+      const bool same = pa == pb;
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int c = 0; c < 3; ++c) m[a][c] += same ? x[a][c] : x[a][c] + x[c][a];
+    }
+  }
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1) {
+#pragma unroll
+    for (int q = 0; q < 6; ++q) h[q] += __shfl_xor_sync(0xffffffffu, h[q], s);
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) m[a][c] += __shfl_xor_sync(0xffffffffu, m[a][c], s);
+  }
+  if (!live || lane != 0) return;
+  double* out = cov + 9 * (size_t)g;
+  if (!on) {
+    for (int q = 0; q < 9; ++q) out[q] = __longlong_as_double(0x7ff8000000000000LL);
+    return;
+  }
+  // H^-1 = L^-T L^-1
+  double L[6];
+  chol3(h, 0.0, L);
+  const double i0 = 1.0 / L[0], i3 = 1.0 / L[3], i5 = 1.0 / L[5];
+  const double li[3][3] = {{i0, 0.0, 0.0},
+                           {-L[1] * i0 * i3, i3, 0.0},
+                           {(L[1] * L[4] * i3 - L[2]) * i0 * i5, -L[4] * i3 * i5, i5}};
+  double Hi[3][3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) Hi[a][c] = li[0][a] * li[0][c] + li[1][a] * li[1][c] + li[2][a] * li[2][c];
+  double t[3][3];  // M H^-1
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) t[a][c] = m[a][0] * Hi[0][c] + m[a][1] * Hi[1][c] + m[a][2] * Hi[2][c];
+  double o[3][3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[a][c] = s2 * Hi[a][c] + Hi[a][0] * t[0][c] + Hi[a][1] * t[1][c] + Hi[a][2] * t[2][c];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) out[3 * a + c] = 0.5 * (o[a][c] + o[c][a]);
+}
+
 }  // namespace cb

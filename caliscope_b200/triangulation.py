@@ -245,6 +245,111 @@ def triangulate(self, camera_array, static_object_ids: frozenset = frozenset()):
     return WorldPoints(pd.concat(parts, ignore_index=True))
 
 
+@dataclass
+class RefinedPoints:
+    """``triangulate_refined``: per group in ascending key order.  status: 0 ok, 1 fewer than 2 rows, 2 not positive
+    definite (xyz is the DLT point, cov NaN), 3 iteration limit, 4 behind a camera."""
+
+    xyz: np.ndarray  # (G, 3)
+    cov: np.ndarray  # (G, 3, 3)
+    rmse_px: np.ndarray  # (G,)
+    count: np.ndarray  # (G,) int32
+    rep_row: np.ndarray  # (G,) int32
+    status: np.ndarray  # (G,) int32
+
+
+@dataclass
+class RefineStats:
+    group_ms: float = 0.0
+    dlt_ms: float = 0.0
+    refine_ms: float = 0.0
+    cov_ms: float = 0.0
+    total_ms: float = 0.0
+    kernel_launches: int = 0
+    n_groups: int = 0
+
+
+def _check_device_tri_obs(obs_cam, obs_key, obs_px, device: int) -> int:
+    """Device-resident observations, read in place (no conversion): CUDA tensors on ``device``, contiguous; obs_cam
+    int32 (n,), obs_key int64 (n,), obs_px float64 (n, 2).  Returns n."""
+    dtypes = {"obs_cam": "torch.int32", "obs_key": "torch.int64", "obs_px": "torch.float64"}
+    arrays = {"obs_cam": obs_cam, "obs_key": obs_key, "obs_px": obs_px}
+    for name, a in arrays.items():
+        dev = getattr(a, "device", None)
+        if getattr(dev, "type", None) != "cuda" or dev.index != device:
+            raise ValueError(f"{name} must be a CUDA tensor on cuda:{device}, got device {dev}")
+        if str(getattr(a, "dtype", None)) != dtypes[name]:
+            raise ValueError(f"{name} must have dtype {dtypes[name]}, got {getattr(a, 'dtype', None)}")
+        if not a.is_contiguous():
+            raise ValueError(f"{name} must be contiguous")
+    n = int(obs_cam.shape[0])
+    if tuple(obs_cam.shape) != (n,) or tuple(obs_key.shape) != (n,):
+        raise ValueError(f"obs_cam and obs_key must be 1-D of the same length, got {tuple(obs_cam.shape)}, "
+                         f"{tuple(obs_key.shape)}")  # fmt: skip
+    if tuple(obs_px.shape) != (n, 2):
+        raise ValueError(f"obs_px must have shape ({n}, 2), got {tuple(obs_px.shape)}")
+    return n
+
+
+def triangulate_refined(cam_flags, cam_const, cam_x, obs_cam, obs_key, obs_px, *, pixel_sigma: float = 1.0,
+                        camera_cov=None, max_iter: int = 20, xtol: float = 1e-12, device: int = 0, stream: int = 0,
+                        stats: RefineStats | None = None) -> RefinedPoints:
+    """Maximum-likelihood triangulation with calibrated cameras and a covariance per point (``cb_triangulate_refine``,
+    DESIGN.md section 4.7).
+
+    The cameras are ``BAProblem.cam_flags``, ``BAProblem.cam_const`` and ``x[:n_camera_params]`` of a solution;
+    ``camera_cov`` is ``Covariance.cameras`` at that solution (None: pixel noise only).  Observations with equal
+    ``obs_key`` are one point; ``obs_px`` are raw pixels.  They may be host arrays or CUDA tensors on ``device``
+    (obs_cam int32, obs_key int64, obs_px float64 (n, 2)), read in place.  Each point starts at the DLT point and is
+    refined to the least-squares reprojection optimum; ``cov = pixel_sigma^2 H^-1 + H^-1 G camera_cov G^T H^-1``.  This
+    assumes the observations are independent of those the calibration used (for a point that was itself in the
+    bundle adjustment, use ``Covariance.points``), and the camera term is relative to ``camera_cov``'s gauge."""
+    lib = L.load()
+    flags = np.ascontiguousarray(cam_flags, dtype=np.int32).ravel()
+    nc = len(flags)
+    const = np.ascontiguousarray(cam_const, dtype=np.float64).reshape(nc, 9)
+    ncp = int(np.where(flags & L.CB_CAM_FREE_INTRINSICS, 9, 6).sum())
+    cx = np.ascontiguousarray(cam_x, dtype=np.float64).ravel()
+    if len(cx) < ncp:
+        raise ValueError(f"cam_x must hold the {ncp} camera parameters, got {len(cx)}")
+    cx = np.ascontiguousarray(cx[:ncp])
+    ccov = None
+    if camera_cov is not None:
+        ccov = np.ascontiguousarray(camera_cov, dtype=np.float64)
+        if ccov.shape != (ncp, ncp):
+            raise ValueError(f"camera_cov must be ({ncp}, {ncp}), got {ccov.shape}")
+    on_dev = hasattr(obs_px, "data_ptr")
+    if on_dev:
+        n = _check_device_tri_obs(obs_cam, obs_key, obs_px, device)
+        cam_p, key_p, px_p = (C.c_void_p(t.data_ptr()) for t in (obs_cam, obs_key, obs_px))
+    else:
+        cam = np.ascontiguousarray(obs_cam, dtype=np.int32)
+        key = np.ascontiguousarray(obs_key, dtype=np.int64)
+        px = np.ascontiguousarray(obs_px, dtype=np.float64).reshape(-1, 2)
+        n = len(cam)
+        if len(key) != n or len(px) != n:
+            raise ValueError("obs_cam, obs_key and obs_px must have one row per observation")
+        cam_p, key_p, px_p = _ptr(cam), _ptr(key), _ptr(px)
+    m = max(n, 1)
+    xyz, cov, rmse = np.empty((m, 3)), np.empty((m, 3, 3)), np.empty(m)
+    count, rep, status = np.empty(m, np.int32), np.empty(m, np.int32), np.empty(m, np.int32)
+    ng = C.c_int32(0)
+    st = L.TriRefineStats()
+    L.check(
+        lib.cb_triangulate_refine(nc, _ptr(flags), _ptr(const), _ptr(cx), None if ccov is None else _ptr(ccov), n, cam_p,
+                                  key_p, px_p, 1 if on_dev else 0, float(pixel_sigma), int(max_iter), float(xtol), n,
+                                  C.byref(ng), _ptr(xyz), _ptr(cov), _ptr(rmse), _ptr(count), _ptr(rep), _ptr(status),
+                                  C.byref(st), int(device), C.c_void_p(stream)),
+        "triangulate_refine",
+    )  # fmt: skip
+    g = ng.value
+    if stats is not None:
+        stats.group_ms, stats.dlt_ms, stats.refine_ms, stats.cov_ms = st.group_ms, st.dlt_ms, st.refine_ms, st.cov_ms
+        stats.total_ms, stats.kernel_launches, stats.n_groups = st.total_ms, st.kernel_launches, g
+    return RefinedPoints(xyz=xyz[:g], cov=cov[:g], rmse_px=rmse[:g], count=count[:g], rep_row=rep[:g],
+                         status=status[:g])  # fmt: skip
+
+
 def undistort_points(points, cam_rows, matrices, distortions, fisheye, *, output: str = "normalized", device: int = 0,
                      stream: int = 0) -> np.ndarray:
     """``CameraData.undistort_points`` for many cameras at once.

@@ -297,6 +297,40 @@ int cb_undistort_triangulate(int32_t n_cams, const int32_t* cam_fisheye, const d
                              double* xyz_out, int32_t* count_out, int32_t* rep_row_out, uint64_t* camset_sig_out,
                              CbTriStats* stats, int device, void* stream);
 
+typedef struct CbTriRefineStats {
+  double group_ms;   /* upload + undistortion + radix sort + group boundaries */
+  double dlt_ms;     /* the DLT start */
+  double refine_ms;  /* the Levenberg-Marquardt kernel */
+  double cov_ms;     /* the covariance kernel (0 without cov_out) */
+  double total_ms;
+  int32_t kernel_launches;
+  int32_t pad_;
+} CbTriRefineStats;
+
+/* Triangulation with calibrated cameras to the reprojection optimum, with a first-order covariance per point
+ * (DESIGN.md section 4.7).  Groups as cb_triangulate_dlt (equal obs_key, ascending key order).  The cameras are given in
+ * the bundle-adjustment layout: cam_flags / cam_const as CbBaProblemDesc, cam_x = the camera section of x
+ * (n_camera_params = sum of 6 or 9 per camera).  obs_px are raw pixels (float64, read at full precision).
+ * Per group with >= 2 rows: the DLT point of cb_undistort_triangulate (projection matrices and lens tables derived from
+ * cam_x) starts a Levenberg-Marquardt minimisation of sum_i |pi(X; c_i) - u_i|^2 in pixels (lambda0 = 1e-3, accept on a
+ * lower cost with lambda / 10, else lambda * 10; stop when |dX| <= xtol (|X| + xtol) or after max_iter steps).
+ *   cov = pixel_sigma^2 H^-1 + H^-1 G cam_cov G^T H^-1,  H = sum J_X^T J_X,  G = sum J_X^T J_c  (pixels; J_X, J_c the
+ *   derivatives of the projection by the point and the camera parameters).  cam_cov (nullable: the first term alone) is
+ *   the n_camera_params^2 camera covariance in x's camera layout (BAProblem.covariance's cameras).  It assumes the
+ *   triangulated observations are independent of those the calibration used, and is relative to cam_cov's gauge.
+ * Outputs (host, room for max_groups): xyz[g][3], cov[g][9] (nullable: no covariance stage), rmse_px[g] (reprojection
+ * RMSE over the group's rows), count[g], rep_row[g] (as cb_triangulate_dlt) and status[g], first match wins:
+ *   1 fewer than 2 rows (xyz, cov, rmse NaN);  2 H not positive definite at the start or at the solution (a Cholesky
+ *   pivot <= 1e-12 times H's largest diagonal entry: parallel rays, or every row from one camera; xyz = the DLT point,
+ *   rmse there, cov NaN);  3 max_iter reached;  4 behind a camera at the solution (some row with Xc.z <= 0);  0 none.
+ * No atomics: repeated calls return bit-identical outputs. */
+int cb_triangulate_refine(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                          const double* cam_cov, int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key,
+                          const double* obs_px, int obs_on_device, double pixel_sigma, int32_t max_iter, double xtol,
+                          int32_t max_groups, int32_t* n_groups_out, double* xyz_out, double* cov_out,
+                          double* rmse_px_out, int32_t* count_out, int32_t* rep_row_out, int32_t* status_out,
+                          CbTriRefineStats* stats, int device, void* stream);
+
 /* Optional NCCL transport owned by the engine (no host callback per all-reduce).  NCCL is resolved at run time from
  * the libnccl the process already has loaded (PyTorch's).  Rank 0 calls cb_nccl_unique_id and distributes the 128
  * bytes (e.g. torch.distributed.broadcast); every rank then calls cb_nccl_comm_create (collective). */
