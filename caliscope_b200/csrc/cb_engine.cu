@@ -1847,7 +1847,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
     p->pt_grid = std::max(1, std::min(cdiv(std::max(p->n_pts, 1), per_block), 2 * p->num_sms));
     const size_t tab_bytes = sizeof(double) * cb::CT_SMEM * (size_t)p->n_cams;
     p->cam_in_smem = tab_bytes <= 64 * 1024 ? 1 : 0;
-    p->pt_smem = p->cam_in_smem ? tab_bytes : 0;
+    p->pt_smem = p->cam_in_smem ? tab_bytes : 0;  // + the Zt staging, once build_indices has counted repeated rows
     p->bs_smem = sizeof(double) * (((size_t)p->nP + 3) & ~(size_t)3) + (p->cam_in_smem ? tab_bytes : 0);
   }
 
@@ -1910,6 +1910,11 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   p->h_cam_const.assign(d->cam_const, d->cam_const + 9 * (size_t)p->n_cams);
   lap("alloc + staged upload");
   CB_TRY(build_indices(p, d_cam, d_pt, d_xy, d->cam_order, st, xy_up.started ? &xy_up : nullptr));
+  // the point pass's Zt staging per point group (cfg4: 18.9 KB of table + 44.8 KB, 2 CTAs per SM); the run-summed
+  // variants store their pieces directly and get none, which leaves their register spills the L1 they had
+  if (!p->n_dups)
+    p->pt_smem += p->P == 6 ? (p->pt_lanes == 8 ? cb::pt_stage_bytes<6, 8>() : cb::pt_stage_bytes<6, 32>())
+                            : (p->pt_lanes == 8 ? cb::pt_stage_bytes<9, 8>() : cb::pt_stage_bytes<9, 32>());
   // camera tables by internal slot
   {
     std::vector<int> xoff(p->n_cams);
@@ -1996,6 +2001,14 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
       cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
       cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
       cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a);  \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
+      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
       cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);     \
       cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);    \
       cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);    \

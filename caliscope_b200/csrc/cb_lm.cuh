@@ -6,7 +6,7 @@
 //
 //   pt_pass_kernel        per point: recompute r, Jp, Jc of its observations from (pixel, camera table, point),
 //                         V = sum Jp^T Jp, g = sum Jp^T r, Marquardt scale, 3x3 damped Cholesky, t = L^-1 g and
-//                         Z = (Jc^T Jp) L^-T streamed straight into the k-major Schur factor   [reprojection.py:171-205]
+//                         Z = (Jc^T Jp) L^-T into the k-major Schur factor, as whole 64-byte granules   [reprojection.py:171-205]
 //   schur_syrk_kernel     Z Z^T (+ Z t), split-K                                               (cb_kernels.cuh)
 //   schur_finalize(_peer) S = U - Z Z^T, b = g_c - Z t (+ the all-reduce over NVLink peers)
 //   reduced_prep_kernel   damping, gradient norm, gtol / max_nfev tests, block-Jacobi inverses
@@ -71,6 +71,19 @@ __device__ __forceinline__ void pt_factor_rows(const double* JX, const double* L
   }
 }
 
+// Zt staging of one point group (dynamic shared memory after the camera table): the Z pieces of one round of LANES rows
+// (lane l's in slot l + 1; slot 0 keeps the last piece of the previous round), their cameras, and the 64-byte granules
+// the round writes as (granule << 12 | slot of the previous piece << 6 | owning slot).  A P-double piece touches at most
+// two granules of a row.
+template <int P, int LANES>
+struct PtStage {
+  double z[LANES + 1][3][P];
+  int cam[LANES + 1];
+  int list[2 * LANES];
+};
+template <int P, int LANES>
+constexpr size_t pt_stage_bytes() { return sizeof(PtStage<P, LANES>) * PT_WARPS * (32 / LANES); }
+
 template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false>
 __global__ void __launch_bounds__(PT_WARPS * 32, 2)
 pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start, const int* __restrict__ pm_cam,
@@ -101,6 +114,8 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
   constexpr int GPW = 32 / LANES;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int gl = lane % LANES, grp = lane / LANES;
+  constexpr unsigned LMASK = LANES == 32 ? 0xffffffffu : (1u << LANES) - 1u;
+  const unsigned gmask = LMASK << (grp * LANES);
   double gm = 0.0;
   for (int j0 = (blockIdx.x * PT_WARPS + wid) * GPW; j0 < n_pts; j0 += gridDim.x * PT_WARPS * GPW) {
     const int j = j0 + grp;
@@ -121,11 +136,13 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
     // 16 warps per SM, long_scoreboard 60 % of the stalls in the first version)
     int cam_n = 0;
     double2 xy_n = make_double2(0.0, 0.0);
+    bool unsorted = false;  // the point's rows are not in camera-slot order (the engine reordered the cameras)
     if (s + gl < e) { cam_n = pm_cam[s + gl]; xy_n = pm_xy[s + gl]; }
     for (int pos = s + gl; pos < e; pos += LANES) {
       const int cam = cam_n;
       const double2 xy = xy_n;
       if (pos + LANES < e) { cam_n = pm_cam[pos + LANES]; xy_n = pm_xy[pos + LANES]; }
+      if (!DUPS && pos + 1 < e && pm_cam[pos + 1] < cam) unsorted = true;
       double f[2], JX[6];
       obs_res_jx(cam_entry(cam), X0, X1, X2, xy.x, xy.y, loss, fscale, f, JX);
       v[0] += JX[0] * JX[0] + JX[3] * JX[3]; v[1] += JX[0] * JX[1] + JX[3] * JX[4]; v[2] += JX[0] * JX[2] + JX[3] * JX[5];
@@ -134,6 +151,8 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
     }
 #pragma unroll
     for (int k = 0; k < 9; ++k) v[k] = group_sum<LANES>(v[k]);
+    bool pieces_only = false;
+    if constexpr (!DUPS) pieces_only = ((__ballot_sync(0xffffffffu, unsorted) >> (grp * LANES)) & LMASK) != 0;
     double D[3] = {1.0, 1.0, 1.0};
     if (valid) {
       const double* d = Dp2 + (size_t)j * 3;
@@ -178,28 +197,15 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
         gm = fmax(gm, fmax(fabs(v[6]), fmax(fabs(v[7]), fabs(v[8]))));
       }
     }
-    // ---- phase 2: Z = (Jc^T Jp) Linv^T per (camera, point) pair, rows 3j..3j+2 of the k-major factor
-    if (s + gl < e) { cam_n = pm_cam[s + gl]; xy_n = pm_xy[s + gl]; }
-    for (int pos = s + gl; pos < e; pos += LANES) {
-      int cam;
-      double f[2], JX[6], Jc[2 * P];
-      double z[3][P];
-      if constexpr (!DUPS) {
-        cam = cam_n;
-        const double2 xy = xy_n;
-        if (pos + LANES < e) { cam_n = pm_cam[pos + LANES]; xy_n = pm_xy[pos + LANES]; }
-        obs_jac<P>(cam_entry(cam), X0, X1, X2, xy.x, xy.y, loss, fscale, f, JX, Jc);
-        double q00, q01, q02, q10, q11, q12;
-        pt_factor_rows<COV>(JX, Li, q00, q01, q02, q10, q11, q12);
-#pragma unroll
-        for (int p = 0; p < P; ++p) {
-          z[0][p] = fma(Jc[p], q00, Jc[P + p] * q10);
-          z[1][p] = fma(Jc[p], q01, Jc[P + p] * q11);
-          z[2][p] = fma(Jc[p], q02, Jc[P + p] * q12);
-        }
-      } else {
-        cam = pm_cam[pos];
+    // ---- phase 2: Z = (Jc^T Jp) Linv^T per (camera, point) pair, rows 3j..3j+2 of the k-major factor.
+    if constexpr (DUPS) {
+      // Run-summed pieces (rigs with few cameras whose points repeat rows) are stored as they are: staging does not pay
+      // on those shapes (cfg2, cfg3; DESIGN §7), and this loop is the one the kernel had before staging.
+      for (int pos = s + gl; pos < e; pos += LANES) {
+        const int cam = pm_cam[pos];
         if (pos > s && pm_cam[pos - 1] == cam) continue;  // not the first row of its (point, camera) run
+        double f[2], JX[6], Jc[2 * P];
+        double z[3][P];
 #pragma unroll
         for (int a = 0; a < 3; ++a)
 #pragma unroll
@@ -218,22 +224,116 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
           }
           ++r;
         } while (r < e && pm_cam[r] == cam);
-      }
-      (void)f;
-      double* z0 = Zt + (3 * (size_t)j) * LD + (size_t)cam * P;
-      if constexpr (P == 6) {
+        (void)f;
+        double* z0 = Zt + (3 * (size_t)j) * LD + (size_t)cam * P;
+        if constexpr (P == 6) {
 #pragma unroll
-        for (int a = 0; a < 3; ++a) {
-          double2* dst = reinterpret_cast<double2*>(z0 + a * LD);  // cam*48 B and LD*8 B are 16-byte multiples
-          dst[0] = make_double2(z[a][0], z[a][1]);
-          dst[1] = make_double2(z[a][2], z[a][3]);
-          dst[2] = make_double2(z[a][4], z[a][5]);
+          for (int a = 0; a < 3; ++a) {
+            double2* dst = reinterpret_cast<double2*>(z0 + a * LD);  // cam*48 B and LD*8 B are 16-byte multiples
+            dst[0] = make_double2(z[a][0], z[a][1]);
+            dst[1] = make_double2(z[a][2], z[a][3]);
+            dst[2] = make_double2(z[a][4], z[a][5]);
+          }
+        } else {
+#pragma unroll
+          for (int a = 0; a < 3; ++a)
+#pragma unroll
+            for (int p = 0; p < P; ++p) z0[a * LD + p] = z[a][p];
         }
-      } else {
+      }
+    } else {
+      // Written as whole 64-byte granules, four lanes per granule, from pieces staged in shared memory: stored piece by
+      // piece, most granules of a row reach L2 as partial pieces in many requests, and the store stream ran at a third
+      // of the rate of whole granules (profiles/microbench/zt_store.cu, DESIGN §7).  Each round of LANES rows writes the
+      // granules its pieces touch, zeros included where a granule covers a camera the point does not see (a structural
+      // zero), except a last granule the next camera's piece shares: the next round writes that one, reading this
+      // round's last piece from slot 0.
+      PtStage<P, LANES>& sg =
+          reinterpret_cast<PtStage<P, LANES>*>(pt_sm + (CAMSM ? (size_t)n_cams * CT_SMEM : 0))[wid * GPW + grp];
+      if (gl == 0) sg.cam[0] = -1;
+      if (s + gl < e) { cam_n = pm_cam[s + gl]; xy_n = pm_xy[s + gl]; }
+      for (int base = s; base < e; base += LANES) {
+        const int pos = base + gl;
+        int cam = -1, next = -1;
+        bool has = false;
+        double* zs = &sg.z[gl + 1][0][0];  // this lane's piece
+        if (pos < e) {
+          double f[2], JX[6], Jc[2 * P];
+          cam = cam_n;
+          const double2 xy = xy_n;
+          if (pos + LANES < e) { cam_n = pm_cam[pos + LANES]; xy_n = pm_xy[pos + LANES]; }
+          obs_jac<P>(cam_entry(cam), X0, X1, X2, xy.x, xy.y, loss, fscale, f, JX, Jc);
+          (void)f;
+          double q00, q01, q02, q10, q11, q12;
+          pt_factor_rows<COV>(JX, Li, q00, q01, q02, q10, q11, q12);
 #pragma unroll
-        for (int a = 0; a < 3; ++a)
+          for (int p = 0; p < P; ++p) {
+            zs[p] = fma(Jc[p], q00, Jc[P + p] * q10);
+            zs[P + p] = fma(Jc[p], q01, Jc[P + p] * q11);
+            zs[2 * P + p] = fma(Jc[p], q02, Jc[P + p] * q12);
+          }
+          has = true;
+        }
+        // camera of row pos + 1: the next lane's, or for the last lane the one lane 0 has just prefetched
+        const int nx = __shfl_sync(gmask, gl == 0 ? cam_n : cam, (gl + 1) % LANES, LANES);
+        if (pos + 1 < e) next = nx;
+        if (pieces_only) {  // the granule ownership below needs rows in slot order: store each piece as it is
+          if (has) {
+            double* z0 = Zt + (3 * (size_t)j) * LD + (size_t)cam * P;
 #pragma unroll
-          for (int p = 0; p < P; ++p) z0[a * LD + p] = z[a][p];
+            for (int a = 0; a < 3; ++a)
+#pragma unroll
+              for (int p = 0; p < P; p += (P == 6 ? 2 : 1)) {
+                if constexpr (P == 6)  // cam*48 B and LD*8 B are 16-byte multiples
+                  *reinterpret_cast<double2*>(z0 + a * LD + p) = make_double2(zs[a * P + p], zs[a * P + p + 1]);
+                else z0[a * LD + p] = zs[a * P + p];
+              }
+          }
+          continue;
+        }
+        // lanes with a piece, in camera order; the previous camera the point sees is the piece of the next lower such
+        // lane, or of slot 0 for the lowest
+        const unsigned bal = (__ballot_sync(gmask, has) >> (grp * LANES)) & LMASK;
+        const unsigned below = bal & ((1u << gl) - 1u);
+        const int prev = below ? 32 - __clz(below) : 0;  // slot of the previous piece
+        int g0 = 0, ng = 0;
+        if (has) {
+          sg.cam[gl + 1] = cam;
+          g0 = (cam * P) >> 3;
+          const int g1 = (cam * P + P - 1) >> 3;
+          ng = g1 - g0 + 1;
+          if (next == cam + 1 && ((cam + 1) * P) >> 3 == g1) --ng;  // shared with the next piece: written with it
+        }
+        int off = ng;  // inclusive scan of the granule counts over the group
+#pragma unroll
+        for (int o = 1; o < LANES; o <<= 1) {
+          const int t = __shfl_up_sync(gmask, off, o, LANES);
+          if (gl >= o) off += t;
+        }
+        const int total = __shfl_sync(gmask, off, LANES - 1, LANES);
+        for (int q = 0; q < ng; ++q) sg.list[off - ng + q] = ((g0 + q) << 12) | (prev << 6) | (gl + 1);
+        __syncwarp(gmask);
+        double* zrow = Zt + (3 * (size_t)j) * LD;
+        for (int it = gl; it < total * 12; it += LANES) {  // (granule, row, 16-byte quarter)
+          const int ent = sg.list[it / 12], a = (it >> 2) % 3, col0 = 8 * (ent >> 12) + 2 * (it & 3);
+          const int sl = ent & 63, ps = (ent >> 6) & 63;
+          const int oc = sg.cam[sl] * P, pc = sg.cam[ps] * P;
+          double v[2];
+#pragma unroll
+          for (int u = 0; u < 2; ++u) {
+            const int col = col0 + u;
+            if (col >= oc) v[u] = col < oc + P ? sg.z[sl][a][col - oc] : 0.0;
+            else v[u] = pc == oc - P ? sg.z[ps][a][col - pc] : 0.0;
+          }
+          *reinterpret_cast<double2*>(zrow + a * LD + col0) = make_double2(v[0], v[1]);  // LD*8 B is a multiple of 64
+        }
+        __syncwarp(gmask);
+        if (bal) {  // the round's last piece becomes slot 0 of the next
+          const int last = 32 - __clz(bal);
+          for (int i = gl; i < 3 * P; i += LANES) sg.z[0][i / P][i % P] = sg.z[last][i / P][i % P];
+          if (gl == 0) sg.cam[0] = sg.cam[last];
+        }
+        __syncwarp(gmask);
       }
     }
   }
