@@ -1,5 +1,6 @@
 // Device-side helpers for the caliscope_b200 bundle-adjustment engine (sm_90a).
 #pragma once
+#include <cuda.h>  // CUtensorMap (type only: the encoder is reached through cudaGetDriverEntryPoint)
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -84,6 +85,15 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src_gmem, u
                    smem_u32(dst_smem)),
                "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
+}
+// global -> shared 2-D tensor copy of one box of `map` at element coordinates (c0 innermost, c1), completion signalled
+// on `bar` with the whole box's bytes (out-of-bounds elements arrive as zeros); dst 128-byte aligned (SASS: UTMALDG)
+__device__ __forceinline__ void tma_load_2d(void* dst_smem, const CUtensorMap* map, int c0, int c1, unsigned long long* bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(
+          smem_u32(dst_smem)),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar))
+      : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------

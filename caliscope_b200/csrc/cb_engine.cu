@@ -471,6 +471,7 @@ struct CbBaProblem {
   int *d_tile_of = nullptr, *d_tile_slot_start = nullptr, *d_tile_slots = nullptr;
   cb::SyItem* d_items = nullptr;
   int n_items = 0, n_slots = 0;
+  CUtensorMap zt_map{};  // d_Zt for the product's dense-path feed (Zt is allocated once and never moves)
   unsigned char* d_active = nullptr;
   double *d_lo = nullptr, *d_hi = nullptr;
   // work buffers (index [2]: current / trial point, selected on the device by LmState::cur)
@@ -874,8 +875,9 @@ int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const 
               p->ct, p->d_pt_start, p->d_pm_cam, p->d_V6, p->d_gp, p->d_Dp2, p->d_gpt, p->c_crs(), p->c_cdirw(), p->n_cams,
               p->d_compL, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax);
   if (ev) CB_CUDA(cudaEventRecord(ev[2], st));
-  CB_LAUNCH(cb::schur_syrk_kernel, p->n_items, cb::SY_THREADS, sizeof(cb::SyrkSmem), st, (const cb::LmState*)p->d_state,
-            p->d_Zt, (size_t)p->LD, p->d_tvec, p->d_items, (const int*)p->d_klist, p->d_part, p->d_tpart);
+  CB_LAUNCH(cb::schur_syrk_kernel, p->n_items, cb::SY_THREADS, sizeof(cb::SyrkSmem), st, p->zt_map,
+            (const cb::LmState*)p->d_state, p->d_Zt, (size_t)p->LD, p->d_tvec, p->d_items, (const int*)p->d_klist,
+            p->d_part, p->d_tpart);
   if (ev) CB_CUDA(cudaEventRecord(ev[3], st));
   const size_t nfin = (size_t)p->nP * p->nP + p->nP + 1;
   // gradient inf-norm over points: one slot per rank so a SUM all-reduce carries the max
@@ -1484,11 +1486,12 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
   for (int I = 0; I < nb; ++I)
     for (int J = I; J < nb; ++J) tof[(size_t)I * nb + J] = nt++;
   // measured cost of a diagonal-pair (single diagonal) CTA per k chunk relative to an off-diagonal one
-  // (profiles/microbench/syrk_feed.cu, H100 SXM at a 400 W power limit).  w_single also weighs the diagonal tiles in the choice between
-  // dense tiles and row lists below (listed < 0.7 * dense), so it moves that threshold: schur_sparse (stat key 0) can
-  // differ from earlier builds on rigs near it.
-  const double w_pair = 1.31;
-  const double w_single = 1.04;
+  // (profiles/microbench/syrk_feed.cu).  Dense tiles, fed by tensor boxes: H100 SXM at a 700 W power limit.  Row lists,
+  // fed row by row: H100 SXM at a 400 W power limit; w_list_single also weighs the diagonal tiles in the choice between
+  // dense tiles and row lists below (listed < 0.7 * dense), so it moves that threshold.
+  const double w_pair = 2.07;
+  const double w_single = 1.46;
+  const double w_list_single = 1.04;
 
   // per-pair row lists, if sparse: offset of each tile pair's list in d_klist (-1: no common point) and its point count
   std::vector<long long> pair_koff, pair_cnt;
@@ -1516,7 +1519,7 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
     double listed = 0.0, dense = 0.0;
     for (int I = 0; I < nb; ++I)
       for (int J = I; J < nb; ++J) {
-        const double w = (I == J) ? w_single : 1.0;
+        const double w = (I == J) ? w_list_single : 1.0;
         listed += w * (double)cnt[tof[(size_t)I * nb + J]];
         dense += w * (double)p->n_pts;
       }
@@ -1588,7 +1591,7 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
         if (pair_cnt[(size_t)t] == 0) continue;
         const int koff = (int)pair_koff[(size_t)t];
         const int chunks = (int)cdiv(3 * pair_cnt[(size_t)t], (long long)cb::SY_KC);
-        if (I == J) groups.push_back({1, I, -1, w_single, chunks, koff});
+        if (I == J) groups.push_back({1, I, -1, w_list_single, chunks, koff});
         else groups.push_back({0, I, J, 1.0, chunks, koff});
       }
   }
@@ -1963,6 +1966,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   // + one chunk of rows that stay zero for good: the padding target of the compacted k-lists
   CB_TRY(palloc(p, &p->d_tvec, (size_t)p->K_pad + cb::SY_KC));
   CB_TRY(palloc(p, &p->d_Zt, ((size_t)p->K_pad + cb::SY_KC) * p->LD));
+  CB_CUDA(cb::make_zt_tensor_map(&p->zt_map, p->d_Zt, (size_t)p->LD, (size_t)p->K_pad + cb::SY_KC));
   CB_TRY(palloc(p, &p->d_part, (size_t)p->n_slots * cb::SY_TILE * cb::SY_TILE));
   CB_TRY(palloc(p, &p->d_tpart, (size_t)p->n_slots * cb::SY_TILE));
   CB_TRY(palloc(p, &p->d_red, p->red_len()));

@@ -346,11 +346,13 @@ __device__ __forceinline__ void chol3_inv(const double* V6, const double* D2, do
 
 // ---------------------------------------------------------------------------------------------
 // Schur product  part[split][tile] = A_I^T A_J  over a slab of k rows (k = 3*point + axis), where
-// Zt is k-major: Zt[k][col], col = camera*P + p.  Tiles are staged through shared memory with
-// 1-D bulk async copies (TMA engine, mbarrier completion), SY_STAGES deep; each thread owns a
-// 6x6 register tile.  Diagonal tiles also accumulate Z t (the reduced right-hand side).
+// Zt is k-major: Zt[k][col], col = camera*P + p.  Tiles are staged through shared memory by the
+// TMA engine (2-D tensor boxes over consecutive rows, 1-D row copies for row lists; mbarrier
+// completion), SY_STAGES deep.  Diagonal tiles also accumulate Z t (the reduced right-hand side).
 // ---------------------------------------------------------------------------------------------
 constexpr int SY_LDS = SY_TILE + 4;  // padded smem row stride (doubles): conflict-free DMMA fragment loads
+// every stage starts 128-byte aligned, as a tensor copy's destination must
+static_assert(SY_KC * SY_LDS * sizeof(double) % 128 == 0, "Schur stage size");
 
 struct SyrkSmem {
   double A[SY_STAGES][SY_KC * SY_LDS];
@@ -473,10 +475,14 @@ __device__ __forceinline__ void syrk_diag_stage(double (&acc)[SY_DIAG_MAX][4], c
   }
 }
 
+// zt_map: Zt as a 2-D tensor (LD columns x rows), box SY_LDS columns x SY_KC rows (make_zt_tensor_map).  A box lands on a
+// stage exactly in its padded layout; its SY_LDS - SY_TILE extra columns are the next tile's (or, past the last tile,
+// zeros) and are never read.
 __global__ void __launch_bounds__(SY_THREADS, 1)
-schur_syrk_kernel(const LmState* __restrict__ st, const double* __restrict__ Zt, size_t LD,
-                  const double* __restrict__ tvec, const SyItem* __restrict__ items, const int* __restrict__ klist,
-                  double* __restrict__ part, double* __restrict__ tpart) {
+schur_syrk_kernel(const __grid_constant__ CUtensorMap zt_map, const LmState* __restrict__ st,
+                  const double* __restrict__ Zt, size_t LD, const double* __restrict__ tvec,
+                  const SyItem* __restrict__ items, const int* __restrict__ klist, double* __restrict__ part,
+                  double* __restrict__ tpart) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   SyrkSmem& sm = *reinterpret_cast<SyrkSmem*>(smem_raw);
   if (st->done) return;
@@ -496,22 +502,34 @@ schur_syrk_kernel(const LmState* __restrict__ st, const double* __restrict__ Zt,
   __syncthreads();
 
   const uint32_t row_bytes = SY_TILE * 8;
-  const uint32_t stage_bytes = SY_KC * row_bytes * (two ? 2u : 1u);
+  const bool listed = item.koff >= 0;
+  // a tensor box fills the padding columns too, and they count towards the transaction
+  const uint32_t stage_bytes = SY_KC * (listed ? row_bytes : SY_LDS * 8u) * (two ? 2u : 1u);
   const int n_it = item.c1 - item.c0;
 
   if (wid == SY_CONSUMER_WARPS) {
-    // ---- producer warp: runs ahead, one k row per lane per tile, stage recycled on `empty` ----
+    // ---- producer warp: runs ahead, stage recycled on `empty` ----
     for (int it = 0; it < n_it; ++it) {
-      const int stage = it % SY_STAGES, round = it / SY_STAGES;
+      const int stage = it % SY_STAGES, round = it / SY_STAGES, chunk = item.c0 + it;
       if (round > 0) mbar_wait(&sm.empty[stage], (uint32_t)((round - 1) & 1));
       // row of this lane: straight through k, or through the item's compacted list (rows of points that both
       // column tiles see; everything else would multiply structural zeros)
-      const size_t k = item.koff >= 0 ? (size_t)klist[(size_t)item.koff + (size_t)(item.c0 + it) * SY_KC + lane]
-                                      : (size_t)(item.c0 + it) * SY_KC + lane;
+      const size_t k = listed ? (size_t)klist[(size_t)item.koff + (size_t)chunk * SY_KC + lane]
+                              : (size_t)chunk * SY_KC + lane;
       // t rides along as a plain shared-memory store: ordered before lane 0's arrive (release) by the warp barrier,
       // visible to the consumers after their acquire on `full`
       if (diag) sm.t[stage][lane] = tvec[k];
       __syncwarp();
+      if (!listed) {
+        // consecutive rows: one tensor box per tile
+        if (lane == 0) {
+          mbar_expect_tx(&sm.full[stage], stage_bytes);
+          tma_load_2d(sm.A[stage], &zt_map, item.I * SY_TILE, chunk * SY_KC, &sm.full[stage]);
+          if (two) tma_load_2d(sm.B[stage], &zt_map, item.J * SY_TILE, chunk * SY_KC, &sm.full[stage]);
+        }
+        continue;
+      }
+      // listed rows: one row copy per lane per tile
       if (lane == 0) mbar_expect_tx(&sm.full[stage], stage_bytes);
       __syncwarp();
       bulk_g2s(&sm.A[stage][lane * SY_LDS], Zt + k * LD + (size_t)item.I * SY_TILE, row_bytes, &sm.full[stage]);
@@ -584,6 +602,26 @@ schur_syrk_kernel(const LmState* __restrict__ st, const double* __restrict__ Zt,
     }
   }
   if (tact) tpart[(size_t)(tsel == 0 ? item.slotA : item.slotB) * SY_TILE + trow] = tacc;
+}
+
+// schur_syrk_kernel's tensor map of Zt (rows x ld doubles, ld a multiple of SY_TILE).  The encoder is a driver entry
+// point, reached through the runtime so that nothing links against the driver library.
+inline cudaError_t make_zt_tensor_map(CUtensorMap* map, const double* Zt, size_t ld, size_t rows) {
+  using Encode = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                              const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                              CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  void* fn = nullptr;
+  cudaDriverEntryPointQueryResult q = cudaDriverEntryPointSymbolNotFound;
+  const cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q);
+  if (e != cudaSuccess) return e;
+  if (q != cudaDriverEntryPointSuccess || !fn) return cudaErrorSymbolNotFound;
+  // row stride ld * 8 bytes and box row SY_LDS * 8 = 800 bytes: both multiples of 16; box edges <= 256 elements
+  const cuuint64_t dim[2] = {ld, rows}, stride[1] = {ld * sizeof(double)};
+  const cuuint32_t box[2] = {SY_LDS, SY_KC}, estride[2] = {1, 1};
+  const CUresult r = ((Encode)fn)(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT64, 2, const_cast<double*>(Zt), dim, stride, box,
+                                  estride, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? cudaSuccess : cudaErrorInvalidValue;
 }
 
 // red = [ S (nP*nP) | b (nP) | gc (nP) | diagU (nP) | cost | gpmax slots ... ]   (local partials)

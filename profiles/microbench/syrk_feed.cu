@@ -9,7 +9,11 @@
 //   (e) the engine's schur_syrk_kernel (cb_kernels.cuh) per item kind, which gives the split weights of
 //       build_schur_items, and on the cfg4 schedule built with them;
 //   (d) the engine's per-stage math (diagonal tiles on m16n8k16) in the modes of (a)-(c) at that schedule: the same
-//       stop test on the kernel as it is now.
+//       stop test on the kernel as it is now.  The feed alone (loads only) in four variants: (i) one 768-byte row copy
+//       per lane per tile, (ii) one 2-D tensor box per tile per stage (what the engine's dense path does), (iii) the row
+//       copies of (i) in lock-step chunk order (CTA s of a group of n takes chunks s, s + n, ...: every group sweeps k at
+//       the same pace, so a row's readers meet in L2), and (ii) in that order.  Last, the MMAs alone on a schedule
+//       weighted by MMA-only costs: the product's MMA bound.
 // Prints us per launch, GB/s of global -> shared feed and TFLOP/s of issued MMA work.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o syrk_feed syrk_feed.cu && ./syrk_feed
 #include <algorithm>
@@ -163,9 +167,13 @@ __global__ void __launch_bounds__(THREADS, 1) old_feed(const double* __restrict_
 // cb::syrk_offdiag_stage / cb::syrk_diag_stage, diagonal tiles on m16n8k16) with the same three modes as (a)-(c):
 // MODE 0: loads + MMA, 1: loads only, 2: MMA only.  Z t and the output stores are left out (one store per thread).
 // ---------------------------------------------------------------------------------------------
-template <int MODE>
-__global__ void __launch_bounds__(cb::SY_THREADS, 1) engine_feed(const double* __restrict__ Zt,
+// BOX: the producer loads a stage with one 2-D tensor box per tile (as the engine's dense path does) instead of one
+// 768-byte row copy per lane per tile.  CTA b walks chunks c0, c0 + cstep[b], ... below c1.
+template <int MODE, bool BOX = false>
+__global__ void __launch_bounds__(cb::SY_THREADS, 1) engine_feed(const __grid_constant__ CUtensorMap zt_map,
+                                                                const double* __restrict__ Zt,
                                                                 const cb::SyItem* __restrict__ items,
+                                                                const int* __restrict__ cstep,
                                                                 double* __restrict__ out) {
   extern __shared__ __align__(128) unsigned char raw[];
   cb::SyrkSmem& sm = *reinterpret_cast<cb::SyrkSmem*>(raw);
@@ -177,18 +185,26 @@ __global__ void __launch_bounds__(cb::SY_THREADS, 1) engine_feed(const double* _
     mbar_fence_init();
   }
   __syncthreads();
-  const int n_it = item.c1 - item.c0;
+  const int step = cstep[blockIdx.x], n_it = (item.c1 - item.c0 + step - 1) / step;
   const uint32_t row_bytes = TILE * 8;
   if (wid == cb::SY_CONSUMER_WARPS) {
     if constexpr (MODE != 2) {
       for (int it = 0; it < n_it; ++it) {
-        const int stage = it % cb::SY_STAGES, round = it / cb::SY_STAGES;
+        const int stage = it % cb::SY_STAGES, round = it / cb::SY_STAGES, chunk = item.c0 + it * step;
         if (round > 0) mbar_wait(&sm.empty[stage], (uint32_t)((round - 1) & 1));
-        const size_t k = (size_t)(item.c0 + it) * cb::SY_KC + lane;
-        if (lane == 0) mbar_expect_tx(&sm.full[stage], cb::SY_KC * row_bytes * (two ? 2u : 1u));
-        __syncwarp();
-        bulk_g2s(&sm.A[stage][lane * LDS], Zt + k * LD + (size_t)item.I * TILE, row_bytes, &sm.full[stage]);
-        if (two) bulk_g2s(&sm.B[stage][lane * LDS], Zt + k * LD + (size_t)item.J * TILE, row_bytes, &sm.full[stage]);
+        if constexpr (BOX) {
+          if (lane == 0) {
+            mbar_expect_tx(&sm.full[stage], cb::SY_KC * LDS * 8 * (two ? 2u : 1u));
+            cb::tma_load_2d(sm.A[stage], &zt_map, item.I * TILE, chunk * cb::SY_KC, &sm.full[stage]);
+            if (two) cb::tma_load_2d(sm.B[stage], &zt_map, item.J * TILE, chunk * cb::SY_KC, &sm.full[stage]);
+          }
+        } else {
+          const size_t k = (size_t)chunk * cb::SY_KC + lane;
+          if (lane == 0) mbar_expect_tx(&sm.full[stage], cb::SY_KC * row_bytes * (two ? 2u : 1u));
+          __syncwarp();
+          bulk_g2s(&sm.A[stage][lane * LDS], Zt + k * LD + (size_t)item.I * TILE, row_bytes, &sm.full[stage]);
+          if (two) bulk_g2s(&sm.B[stage][lane * LDS], Zt + k * LD + (size_t)item.J * TILE, row_bytes, &sm.full[stage]);
+        }
       }
     }
     return;
@@ -329,8 +345,9 @@ int main() {
     cudaFree(d_items);
   }
   {
-    // (e) the engine's schur_syrk_kernel (diagonal tiles on m16n8k16): cost per k chunk of each item kind, one CTA per
-    // SM, which sets build_schur_items' split weights; then the cfg4 schedule built with those weights
+    // (e) the engine's schur_syrk_kernel (diagonal tiles on m16n8k16, dense items fed by tensor boxes): cost per k chunk
+    // of each item kind, one CTA per SM, which sets build_schur_items' split weights; then the cfg4 schedule built with
+    // those weights
     cb::LmState h_st{};
     cb::LmState* d_st;
     cudaMalloc(&d_st, sizeof(cb::LmState));
@@ -338,6 +355,11 @@ int main() {
     double *part, *tpart;
     cudaMalloc(&part, (size_t)2 * sms * TILE * TILE * sizeof(double));
     cudaMalloc(&tpart, (size_t)2 * sms * TILE * sizeof(double));
+    CUtensorMap zmap;
+    if (cb::make_zt_tensor_map(&zmap, Zt, LD, (size_t)K_pad + KC_OLD) != cudaSuccess) {
+      printf("tensor map encoding failed\n");
+      return 1;
+    }
     const int smem = sizeof(cb::SyrkSmem);
     cudaFuncSetAttribute(cb::schur_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cb::SyItem* d_it;
@@ -345,7 +367,7 @@ int main() {
     auto run = [&](const std::vector<cb::SyItem>& v) {
       cudaMemcpy(d_it, v.data(), v.size() * sizeof(cb::SyItem), cudaMemcpyHostToDevice);
       return time_ms([&] {
-        cb::schur_syrk_kernel<<<(int)v.size(), cb::SY_THREADS, smem>>>(d_st, Zt, LD, Zt, d_it, nullptr, part, tpart);
+        cb::schur_syrk_kernel<<<(int)v.size(), cb::SY_THREADS, smem>>>(zmap, d_st, Zt, LD, Zt, d_it, nullptr, part, tpart);
       }, reps);
     };
     auto mk = [&](int kind, int I, int J, int c0, int c1, int s) { return cb::SyItem{kind, I, J, c0, c1, s, s + sms, -1}; };
@@ -363,37 +385,77 @@ int main() {
     report("(e) engine kernel, single-diagonal CTAs only", t_single, 1.0 * ch * KC_OLD * TILE * 8 * sms, fl_off * 42 / 72);
     printf("engine kernel: diagonal pair / off-diagonal = %.3f, single diagonal / off-diagonal = %.3f\n", t_pair / t_off,
            t_single / t_off);
-    const std::vector<Item> sched = old_items(sms, K_pad / KC_OLD, t_pair / t_off);
-    std::vector<cb::SyItem> v;
+    // cfg4 schedule at pair weight w: contiguous k slabs per CTA, or lock-step (CTA s of a group of n takes chunks s,
+    // s + n, s + 2n, ...: every group sweeps k at the same pace, so a row's readers meet in L2)
     double bytes = 0.0, flop = 0.0;
-    for (size_t i = 0; i < sched.size(); ++i) {
-      const Item& x = sched[i];
-      v.push_back(mk(x.kind, x.I, x.J, x.c0, x.c1, (int)i));
-      bytes += 2.0 * (x.c1 - x.c0) * KC_OLD * TILE * 8;
-      flop += 2.0 * (x.kind == 0 ? 96.0 * 96.0 : 84.0 * 16 * 8) * (x.c1 - x.c0) * KC_OLD;
-    }
+    std::vector<int> steps;  // cstep of engine_feed, per CTA, for the schedule sched() built last
+    auto sched = [&](double w, bool lockstep) {
+      const std::vector<Item> g = old_items(sms, K_pad / KC_OLD, w);
+      std::vector<cb::SyItem> v;
+      steps.clear();
+      bytes = flop = 0.0;
+      for (size_t i = 0; i < g.size();) {
+        size_t e = i;
+        while (e < g.size() && g[e].kind == g[i].kind && g[e].I == g[i].I && g[e].J == g[i].J) ++e;
+        const int n = (int)(e - i);
+        for (size_t q = i; q < e; ++q) {
+          const Item& x = g[q];
+          v.push_back(lockstep ? mk(x.kind, x.I, x.J, (int)(q - i), K_pad / KC_OLD, (int)q)
+                               : mk(x.kind, x.I, x.J, x.c0, x.c1, (int)q));
+          steps.push_back(lockstep ? n : 1);
+          bytes += 2.0 * (x.c1 - x.c0) * KC_OLD * TILE * 8;
+          flop += 2.0 * (x.kind == 0 ? 96.0 * 96.0 : 84.0 * 16 * 8) * (x.c1 - x.c0) * KC_OLD;
+        }
+        i = e;
+      }
+      return v;
+    };
+    report("(e) engine kernel, cfg4 schedule at w_pair 1.31", run(sched(1.31, false)), bytes, flop);
+    const std::vector<cb::SyItem> vl = sched(t_pair / t_off, true);
+    const std::vector<int> steps_l = steps;
+    const std::vector<cb::SyItem> v = sched(t_pair / t_off, false);
     report("(e) engine kernel, cfg4 schedule at the measured weight", run(v), bytes, flop);
-    // (d) the stop test of (a)-(c) repeated on the engine's math at that schedule
+    // (d) the stop test of (a)-(c) repeated on the engine's math at that schedule, and the feed alone (loads only):
+    //   (i) row copies, (ii) one tensor box per tile per stage, (iii) row copies in lock-step order, and boxes in lock-step
     cudaFuncSetAttribute(engine_feed<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(engine_feed<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     cudaFuncSetAttribute(engine_feed<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    auto run_mode = [&](int mode, const std::vector<cb::SyItem>& items) {
+    cudaFuncSetAttribute(engine_feed<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(engine_feed<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    int* d_step;
+    cudaMalloc(&d_step, 2 * sms * sizeof(int));
+    auto run_mode = [&](int mode, const std::vector<cb::SyItem>& items, const std::vector<int>* st = nullptr) {
+      const std::vector<int> ones(items.size(), 1);
       cudaMemcpy(d_it, items.data(), items.size() * sizeof(cb::SyItem), cudaMemcpyHostToDevice);
+      cudaMemcpy(d_step, (st ? *st : ones).data(), items.size() * sizeof(int), cudaMemcpyHostToDevice);
       const int g = (int)items.size();
       return time_ms([&] {
-        if (mode == 0) engine_feed<0><<<g, cb::SY_THREADS, smem>>>(Zt, d_it, out);
-        else if (mode == 1) engine_feed<1><<<g, cb::SY_THREADS, smem>>>(Zt, d_it, out);
-        else engine_feed<2><<<g, cb::SY_THREADS, smem>>>(Zt, d_it, out);
+        if (mode == 0) engine_feed<0><<<g, cb::SY_THREADS, smem>>>(zmap, Zt, d_it, d_step, out);
+        else if (mode == 1) engine_feed<1><<<g, cb::SY_THREADS, smem>>>(zmap, Zt, d_it, d_step, out);
+        else if (mode == 2) engine_feed<2><<<g, cb::SY_THREADS, smem>>>(zmap, Zt, d_it, d_step, out);
+        else if (mode == 3) engine_feed<0, true><<<g, cb::SY_THREADS, smem>>>(zmap, Zt, d_it, d_step, out);
+        else engine_feed<1, true><<<g, cb::SY_THREADS, smem>>>(zmap, Zt, d_it, d_step, out);
       }, reps);
     };
-    report("(d) engine math, cfg4 schedule, loads + MMA", run_mode(0, v), bytes, flop);
-    report("(d) engine math, cfg4 schedule, loads only", run_mode(1, v), bytes, 0.0);
+    report("(d) engine math, cfg4 schedule, loads + MMA (row copies)", run_mode(0, v), bytes, flop);
+    report("(d) engine math, cfg4 schedule, loads + MMA (boxes)", run_mode(3, v), bytes, flop);
+    report("(d) engine math, lock-step schedule, loads + MMA (row copies)", run_mode(0, vl, &steps_l), bytes, flop);
+    report("(d) engine math, lock-step schedule, loads + MMA (boxes)", run_mode(3, vl, &steps_l), bytes, flop);
+    report("(d)(i) loads only, row copies", run_mode(1, v), bytes, 0.0);
+    report("(d)(ii) loads only, tensor boxes", run_mode(4, v), bytes, 0.0);
+    report("(d)(iii) loads only, row copies, lock-step", run_mode(1, vl, &steps_l), bytes, 0.0);
+    report("(d)(ii+iii) loads only, tensor boxes, lock-step", run_mode(4, vl, &steps_l), bytes, 0.0);
     report("(d) engine math, cfg4 schedule, MMA only", run_mode(2, v), 0.0, flop);
     const float m_off = run_mode(2, off), m_pair = run_mode(2, pair), m_single = run_mode(2, single);
     report("(d) engine math, off-diagonal CTAs only, MMA only", m_off, 0.0, fl_off);
     report("(d) engine math, diagonal-pair CTAs only, MMA only", m_pair, 0.0, fl_off * 84 / 72);
     report("(d) engine math, single-diagonal CTAs only, MMA only", m_single, 0.0, fl_off * 42 / 72);
-    cudaFree(d_it); cudaFree(part); cudaFree(tpart); cudaFree(d_st);
+    printf("engine math, MMA only: diagonal pair / off-diagonal = %.3f, single diagonal / off-diagonal = %.3f\n",
+           m_pair / m_off, m_single / m_off);
+    // the MMA bound of the product: MMA only on a schedule weighted by MMA-only costs
+    const std::vector<cb::SyItem> vm = sched(m_pair / m_off, false);
+    report("(d) engine math, schedule at the MMA-only weight, MMA only", run_mode(2, vm), 0.0, flop);
+    cudaFree(d_step); cudaFree(d_it); cudaFree(part); cudaFree(tpart); cudaFree(d_st);
   }
   cudaFree(Zt);
   cudaFree(out);
