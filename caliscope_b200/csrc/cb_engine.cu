@@ -2818,24 +2818,25 @@ int group_by_key(const long long* d_key, int n, cudaStream_t st, ScopedFree& sf,
 
 // device-side result of the grouping and the DLT (buffers owned by the caller's ScopedFree)
 struct TriDlt {
-  const int* cam = nullptr;  // obs_cam on the device
-  int* rows = nullptr;       // caller rows sorted by key (stable)
-  int* start = nullptr;      // group boundaries, n_groups + 1
+  const int* cam = nullptr;   // obs_cam on the device
+  const double* xy = nullptr; // the DLT's coordinates on the device (undistorted and float32-rounded with `undist`)
+  double* proj = nullptr;     // [n_cams][3][4] projection matrices on the device
+  int* rows = nullptr;        // caller rows sorted by key (stable)
+  int* start = nullptr;       // group boundaries, n_groups + 1
   int n_groups = 0;
-  int lanes = 8;             // lanes per group of the DLT kernel (8, or 32 when groups average > 96 rows)
+  int lanes = 8;              // lanes per group of the DLT kernel (8, or 32 when groups average > 96 rows)
   double* xyz = nullptr;
   int* count = nullptr;
   int* rep = nullptr;
   unsigned long long* sig = nullptr;
 };
 
-// upload + validation + (undistortion) + grouping + DLT, the stages every triangulation call shares.  Records ev[1] after
-// the grouping and ev[2] / ev[3] around the DLT kernel.  `undist` non-null = obs_xy are raw pixels, undistorted on the
-// device (normalised output) before the DLT, never leaving HBM in between.
-int tri_dlt_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int n,
-                  const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
-                  int32_t max_groups, int32_t* n_groups_out, const char* who, cudaEvent_t* ev, ScopedFree& sf,
-                  cudaStream_t st, TriDlt* out) {
+// upload + validation + (undistortion) + grouping, the stages every triangulation call shares.  Records ev[1] after the
+// grouping.  `undist` non-null = obs_xy are raw pixels, undistorted on the device (normalised output), never leaving HBM.
+int tri_group_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int n,
+                    const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
+                    int32_t max_groups, int32_t* n_groups_out, const char* who, cudaEvent_t* ev, ScopedFree& sf,
+                    cudaStream_t st, TriDlt* out) {
   const int TB = 256, G = cdiv(n, TB);
   const int* d_cam = nullptr;
   const long long* d_key = nullptr;
@@ -2878,7 +2879,25 @@ int tri_dlt_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, cons
     g_last_error = std::string(who) + ": " + std::to_string(n_groups) + " groups but room for " + std::to_string(max_groups);
     return CB_E_INVALID;
   }
-  // (3) DLT per group
+  out->cam = d_cam;
+  out->xy = d_xy;
+  out->proj = d_proj;
+  out->rows = v_out;
+  out->start = d_start;
+  out->n_groups = n_groups;
+  // 8 lanes per group: the serial 4x4 eigen-solve of one lane per group, not the gather, bounds the DLT kernel, so
+  // more groups per warp wins until groups get very long
+  out->lanes = (n / std::max(n_groups, 1) > 96) ? 32 : 8;
+  return CB_OK;
+}
+
+// the DLT of every group of `t`, ev[2] / ev[3] around the kernel
+int tri_dlt_launch(int32_t n_cams, cudaEvent_t* ev, ScopedFree& sf, cudaStream_t st, TriDlt* t) {
+  const int n_groups = t->n_groups, lanes = t->lanes;
+  const int* d_cam = t->cam;
+  const double* d_xy = t->xy;
+  const double* d_proj = t->proj;
+  const int *d_start = t->start, *v_out = t->rows;
   double* d_xyz = nullptr;
   int *d_count = nullptr, *d_rep = nullptr;
   unsigned long long* d_sig = nullptr;
@@ -2888,9 +2907,6 @@ int tri_dlt_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, cons
   CB_TRY(dalloc(&d_sig, 2 * (size_t)n_groups)); sf.dev.push_back(d_sig);
   const size_t proj_bytes = sizeof(double) * 13 * (size_t)n_cams;  // padded stride, see tri_dlt_kernel
   const int in_smem = proj_bytes <= 40 * 1024 ? 1 : 0;
-  // 8 lanes per group: the serial 4x4 eigen-solve of one lane per group, not the gather, bounds this kernel, so
-  // more groups per warp wins until groups get very long
-  const int lanes = (n / std::max(n_groups, 1) > 96) ? 32 : 8;
   const long long threads = (long long)n_groups * lanes;
   CB_CUDA(cudaEventRecord(ev[2], st));
   if (lanes == 32)
@@ -2901,15 +2917,178 @@ int tri_dlt_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, cons
               d_proj, n_cams, in_smem, d_start, v_out, d_cam, d_xy, n_groups, d_xyz, d_count, d_rep, d_sig);
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[3], st));
-  out->cam = d_cam;
-  out->rows = v_out;
-  out->start = d_start;
-  out->n_groups = n_groups;
-  out->lanes = lanes;
-  out->xyz = d_xyz;
-  out->count = d_count;
-  out->rep = d_rep;
-  out->sig = d_sig;
+  t->xyz = d_xyz;
+  t->count = d_count;
+  t->rep = d_rep;
+  t->sig = d_sig;
+  return CB_OK;
+}
+
+int tri_dlt_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int n,
+                  const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
+                  int32_t max_groups, int32_t* n_groups_out, const char* who, cudaEvent_t* ev, ScopedFree& sf,
+                  cudaStream_t st, TriDlt* out) {
+  CB_TRY(tri_group_stage(n_cams, undist, proj, n, obs_cam, obs_key, obs_xy, obs_on_device, max_groups, n_groups_out, who,
+                         ev, sf, st, out));
+  return tri_dlt_launch(n_cams, ev, sf, st, out);
+}
+
+// Cameras of the calibrated triangulation calls, given in the bundle-adjustment layout (x: [r t] or [r t s k1 k2] per
+// camera).  tri_cams_prepare validates them on the host and derives the DLT start's normalised projection matrices [R|t]
+// and undistortion tables (intrinsics as cam_prep_one forms them); tri_cams_upload builds the device camera table with
+// cam_prep_kernel (P = 9 when any camera has free intrinsics).
+struct TriCams {
+  std::vector<int> xoff;  // offset of each camera in cam_x, n_cams + 1
+  int ncp = 0;
+  int P = 6;
+  std::vector<double> proj;
+  std::vector<cb::UndistCam> tab;
+  double* camtab = nullptr;  // [n_cams][CT_SIZE] on the device, after tri_cams_upload
+};
+
+int tri_cams_prepare(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                     const char* who, TriCams* out) {
+  std::vector<int>& xoff = out->xoff;
+  xoff.assign(n_cams + 1, 0);
+  bool any_free = false;
+  for (int c = 0; c < n_cams; ++c) {
+    if (cam_flags[c] < 0 || cam_flags[c] > 3) {
+      g_last_error = std::string(who) + ": camera flags must be a combination of bits 0 and 1";
+      return CB_E_INVALID;
+    }
+    any_free = any_free || (cam_flags[c] & 1);
+    xoff[c + 1] = xoff[c] + ((cam_flags[c] & 1) ? 9 : 6);
+  }
+  out->ncp = xoff[n_cams];
+  out->P = any_free ? 9 : 6;
+  std::vector<double>& proj = out->proj;
+  std::vector<cb::UndistCam>& tab = out->tab;
+  proj.assign(12 * (size_t)n_cams, 0.0);
+  tab.assign(n_cams, cb::UndistCam{});
+  for (int c = 0; c < n_cams; ++c) {
+    const double* q = cam_x + xoff[c];
+    const double* k = cam_const + 9 * (size_t)c;
+    const bool free_i = cam_flags[c] & 1;
+    const double th = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
+    double R[9];
+    if (th < 1e-12) {
+      const double r[9] = {1, -q[2], q[1], q[2], 1, -q[0], -q[1], q[0], 1};
+      std::memcpy(R, r, sizeof(R));
+    } else {
+      const double kx = q[0] / th, ky = q[1] / th, kz = q[2] / th, s = std::sin(th), co = std::cos(th), c1 = 1.0 - co;
+      const double r[9] = {co + c1 * kx * kx,      c1 * kx * ky - s * kz, c1 * kx * kz + s * ky,
+                           c1 * ky * kx + s * kz, co + c1 * ky * ky,      c1 * ky * kz - s * kx,
+                           c1 * kz * kx - s * ky, c1 * kz * ky + s * kx, co + c1 * kz * kz};
+      std::memcpy(R, r, sizeof(R));
+    }
+    for (int i = 0; i < 3; ++i) {
+      for (int j = 0; j < 3; ++j) proj[12 * (size_t)c + 4 * i + j] = R[3 * i + j];
+      proj[12 * (size_t)c + 4 * i + 3] = q[3 + i];
+    }
+    const double sc = free_i ? q[6] : 1.0, k1 = free_i ? q[7] : k[4], k2 = free_i ? q[8] : k[5];
+    cb::UndistCam& u = tab[c];
+    std::memset(&u, 0, sizeof(u));
+    u.fx = sc * k[0]; u.fy = sc * k[1]; u.cx = k[2]; u.cy = k[3]; u.skew = 0.0;
+    u.fisheye = (cam_flags[c] & 2) ? 1 : 0;
+    u.d[0] = k1; u.d[1] = k2; u.d[2] = k[6]; u.d[3] = k[7];
+    if (!u.fisheye) u.d[4] = k[8];
+    if (!(k[0] != 0.0) || !(u.fx != 0.0) || !(u.fy != 0.0)) {
+      g_last_error = std::string(who) + ": zero focal length in the camera table";
+      return CB_E_INVALID;
+    }
+  }
+  return CB_OK;
+}
+
+int tri_cams_upload(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                    TriCams* c, ScopedFree& sf, cudaStream_t st) {
+  const int P = c->P, ncp = c->ncp;
+  int *d_flags = nullptr, *d_xoff = nullptr;
+  double *d_const = nullptr, *d_x = nullptr, *d_xc = nullptr, *d_camtab = nullptr;
+  CB_TRY(dalloc(&d_flags, (size_t)n_cams)); sf.dev.push_back(d_flags);
+  CB_TRY(dalloc(&d_xoff, (size_t)n_cams)); sf.dev.push_back(d_xoff);
+  CB_TRY(dalloc(&d_const, 9 * (size_t)n_cams)); sf.dev.push_back(d_const);
+  CB_TRY(dalloc(&d_x, (size_t)ncp)); sf.dev.push_back(d_x);
+  CB_TRY(dalloc(&d_xc, (size_t)P * n_cams)); sf.dev.push_back(d_xc);
+  CB_TRY(dalloc(&d_camtab, (size_t)cb::CT_SIZE * n_cams)); sf.dev.push_back(d_camtab);
+  CB_CUDA(cudaMemcpyAsync(d_flags, cam_flags, sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(d_xoff, c->xoff.data(), sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(d_const, cam_const, sizeof(double) * 9 * n_cams, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaMemcpyAsync(d_x, cam_x, sizeof(double) * ncp, cudaMemcpyHostToDevice, st));
+  CB_LAUNCH(cb::unpack_x_kernel, cdiv((long long)n_cams * P, 256), 256, 0, st, d_x, d_xoff, d_flags, d_const, n_cams, P,
+            0, ncp, d_xc, nullptr);
+  CB_LAUNCH(cb::cam_prep_kernel, cdiv(n_cams, 64), 64, 0, st, d_xc, d_flags, d_const, n_cams, P, d_camtab);
+  c->camtab = d_camtab;
+  return CB_OK;
+}
+
+// the camera table of tri_refine_kernel / tri_cov_kernel / tri_consensus_kernel goes to shared memory (odd stride, see
+// tri_stage_camtab) when it takes at most 40 KB
+size_t tri_camtab_smem(int32_t n_cams) {
+  const size_t cam_bytes = sizeof(double) * cb::CT_SMEM * (size_t)n_cams;
+  return cam_bytes <= 40 * 1024 ? cam_bytes : 0;
+}
+
+// tri_refine_kernel over the row list (start, rows) from xyz0
+int tri_refine_launch(int32_t n_cams, const TriCams& c, int lanes, const int* start, const int* rows, const int* cam,
+                      const double* px, int n_groups, const double* xyz0, int32_t max_iter, double xtol, double* xyz,
+                      double* rmse, int* status, cudaStream_t st) {
+  const size_t smem = tri_camtab_smem(n_cams);
+  const int cam_in_smem = smem ? 1 : 0;
+  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
+  if (lanes == 32)
+    CB_LAUNCH(cb::tri_refine_kernel<32>, blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem, start, rows,
+              cam, px, n_groups, xyz0, max_iter, xtol, xyz, rmse, status);
+  else
+    CB_LAUNCH(cb::tri_refine_kernel<8>, blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem, start, rows,
+              cam, px, n_groups, xyz0, max_iter, xtol, xyz, rmse, status);
+  CB_CUDA(cudaGetLastError());
+  return CB_OK;
+}
+
+// tri_cov_kernel over the row list (start, rows; n rows at most), recorded between ev_a and ev_b.  The camera covariance
+// (nullable) goes from x's layout to a uniform stride P (fixed / absent slots 0) and is uploaded once.
+int tri_cov_launch(int32_t n_cams, const TriCams& c, const double* cam_cov, double pixel_sigma, int lanes,
+                   const int* start, const int* rows, const int* cam, const double* px, int n, int n_groups,
+                   const double* xyz, const int* status, cudaEvent_t ev_a, cudaEvent_t ev_b, ScopedFree& sf,
+                   cudaStream_t st, double** d_cov_out) {
+  const int P = c.P, ncp = c.ncp;
+  const std::vector<int>& xoff = c.xoff;
+  double* d_sig = nullptr;
+  double* d_B = nullptr;
+  int* d_first = nullptr;
+  if (cam_cov) {
+    const size_t nP = (size_t)n_cams * P;
+    std::vector<double> sig(nP * nP, 0.0);
+    for (int a = 0; a < n_cams; ++a)
+      for (int p = 0; p < xoff[a + 1] - xoff[a]; ++p)
+        for (int d = 0; d < n_cams; ++d)
+          for (int q = 0; q < xoff[d + 1] - xoff[d]; ++q)
+            sig[((size_t)a * P + p) * nP + (size_t)d * P + q] = cam_cov[(size_t)(xoff[a] + p) * ncp + xoff[d] + q];
+    CB_TRY(dalloc(&d_sig, nP * nP)); sf.dev.push_back(d_sig);
+    CB_CUDA(cudaMemcpyAsync(d_sig, sig.data(), sizeof(double) * nP * nP, cudaMemcpyHostToDevice, st));
+    CB_TRY(dalloc(&d_B, 3 * (size_t)P * n)); sf.dev.push_back(d_B);
+    CB_TRY(dalloc(&d_first, (size_t)n)); sf.dev.push_back(d_first);
+    CB_CUDA(cudaStreamSynchronize(st));  // `sig` is a stack-lifetime upload
+  }
+  double* d_cov = nullptr;
+  CB_TRY(dalloc(&d_cov, 9 * (size_t)n_groups)); sf.dev.push_back(d_cov);
+  const double s2 = pixel_sigma * pixel_sigma;
+  const size_t smem = tri_camtab_smem(n_cams);
+  const int cam_in_smem = smem ? 1 : 0;
+  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
+  CB_CUDA(cudaEventRecord(ev_a, st));
+#define CB_TRI_COV(PP, LL)                                                                                             \
+  CB_LAUNCH((cb::tri_cov_kernel<PP, LL>), blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem, start, rows, \
+            cam, px, n_groups, xyz, status, d_sig, s2, d_B, d_first, d_cov)
+  if (P == 9 && lanes == 32) CB_TRI_COV(9, 32);
+  else if (P == 9) CB_TRI_COV(9, 8);
+  else if (lanes == 32) CB_TRI_COV(6, 32);
+  else CB_TRI_COV(6, 8);
+#undef CB_TRI_COV
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaEventRecord(ev_b, st));
+  *d_cov_out = d_cov;
   return CB_OK;
 }
 
@@ -2995,53 +3174,8 @@ int cb_triangulate_refine(int32_t n_cams, const int32_t* cam_flags, const double
     g_last_error = "cb_triangulate_refine: bad argument";
     return CB_E_INVALID;
   }
-  // camera models in the BA parameter layout (x: [r t] or [r t s k1 k2] per camera) -> the DLT start's normalised
-  // projection matrices [R|t] and undistortion tables; intrinsics as cam_prep_one forms them
-  std::vector<int> xoff(n_cams + 1, 0);
-  bool any_free = false;
-  for (int c = 0; c < n_cams; ++c) {
-    if (cam_flags[c] < 0 || cam_flags[c] > 3) {
-      g_last_error = "cb_triangulate_refine: camera flags must be a combination of bits 0 and 1";
-      return CB_E_INVALID;
-    }
-    any_free = any_free || (cam_flags[c] & 1);
-    xoff[c + 1] = xoff[c] + ((cam_flags[c] & 1) ? 9 : 6);
-  }
-  const int ncp = xoff[n_cams];
-  std::vector<double> proj(12 * (size_t)n_cams);
-  std::vector<cb::UndistCam> tab(n_cams);
-  for (int c = 0; c < n_cams; ++c) {
-    const double* q = cam_x + xoff[c];
-    const double* k = cam_const + 9 * (size_t)c;
-    const bool free_i = cam_flags[c] & 1;
-    const double th = std::sqrt(q[0] * q[0] + q[1] * q[1] + q[2] * q[2]);
-    double R[9];
-    if (th < 1e-12) {
-      const double r[9] = {1, -q[2], q[1], q[2], 1, -q[0], -q[1], q[0], 1};
-      std::memcpy(R, r, sizeof(R));
-    } else {
-      const double kx = q[0] / th, ky = q[1] / th, kz = q[2] / th, s = std::sin(th), co = std::cos(th), c1 = 1.0 - co;
-      const double r[9] = {co + c1 * kx * kx,      c1 * kx * ky - s * kz, c1 * kx * kz + s * ky,
-                           c1 * ky * kx + s * kz, co + c1 * ky * ky,      c1 * ky * kz - s * kx,
-                           c1 * kz * kx - s * ky, c1 * kz * ky + s * kx, co + c1 * kz * kz};
-      std::memcpy(R, r, sizeof(R));
-    }
-    for (int i = 0; i < 3; ++i) {
-      for (int j = 0; j < 3; ++j) proj[12 * (size_t)c + 4 * i + j] = R[3 * i + j];
-      proj[12 * (size_t)c + 4 * i + 3] = q[3 + i];
-    }
-    const double sc = free_i ? q[6] : 1.0, k1 = free_i ? q[7] : k[4], k2 = free_i ? q[8] : k[5];
-    cb::UndistCam& u = tab[c];
-    std::memset(&u, 0, sizeof(u));
-    u.fx = sc * k[0]; u.fy = sc * k[1]; u.cx = k[2]; u.cy = k[3]; u.skew = 0.0;
-    u.fisheye = (cam_flags[c] & 2) ? 1 : 0;
-    u.d[0] = k1; u.d[1] = k2; u.d[2] = k[6]; u.d[3] = k[7];
-    if (!u.fisheye) u.d[4] = k[8];
-    if (!(k[0] != 0.0) || !(u.fx != 0.0) || !(u.fy != 0.0)) {
-      g_last_error = "cb_triangulate_refine: zero focal length in the camera table";
-      return CB_E_INVALID;
-    }
-  }
+  TriCams cams;
+  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, "cb_triangulate_refine", &cams));
   CB_TRY(select_device(device));
   *n_groups_out = 0;
   if (stats) std::memset(stats, 0, sizeof(*stats));
@@ -3063,82 +3197,25 @@ int cb_triangulate_refine(int32_t n_cams, const int32_t* cam_flags, const double
   CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
   CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
   TriDlt t;
-  CB_TRY(tri_dlt_stage(n_cams, &tab, proj.data(), n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups, n_groups_out,
-                       "cb_triangulate_refine", ev, sf, st, &t));
+  CB_TRY(tri_dlt_stage(n_cams, &cams.tab, cams.proj.data(), n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups,
+                       n_groups_out, "cb_triangulate_refine", ev, sf, st, &t));
   const int n_groups = t.n_groups;
-
-  // camera table from the BA layout (cam_prep_kernel, P = 9 when any camera has free intrinsics)
-  const int P = any_free ? 9 : 6;
-  int *d_flags = nullptr, *d_xoff = nullptr;
-  double *d_const = nullptr, *d_x = nullptr, *d_xc = nullptr, *d_camtab = nullptr;
-  CB_TRY(dalloc(&d_flags, (size_t)n_cams)); sf.dev.push_back(d_flags);
-  CB_TRY(dalloc(&d_xoff, (size_t)n_cams)); sf.dev.push_back(d_xoff);
-  CB_TRY(dalloc(&d_const, 9 * (size_t)n_cams)); sf.dev.push_back(d_const);
-  CB_TRY(dalloc(&d_x, (size_t)ncp)); sf.dev.push_back(d_x);
-  CB_TRY(dalloc(&d_xc, (size_t)P * n_cams)); sf.dev.push_back(d_xc);
-  CB_TRY(dalloc(&d_camtab, (size_t)cb::CT_SIZE * n_cams)); sf.dev.push_back(d_camtab);
-  CB_CUDA(cudaMemcpyAsync(d_flags, cam_flags, sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
-  CB_CUDA(cudaMemcpyAsync(d_xoff, xoff.data(), sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
-  CB_CUDA(cudaMemcpyAsync(d_const, cam_const, sizeof(double) * 9 * n_cams, cudaMemcpyHostToDevice, st));
-  CB_CUDA(cudaMemcpyAsync(d_x, cam_x, sizeof(double) * ncp, cudaMemcpyHostToDevice, st));
-  CB_LAUNCH(cb::unpack_x_kernel, cdiv((long long)n_cams * P, 256), 256, 0, st, d_x, d_xoff, d_flags, d_const, n_cams, P,
-            0, ncp, d_xc, nullptr);
-  CB_LAUNCH(cb::cam_prep_kernel, cdiv(n_cams, 64), 64, 0, st, d_xc, d_flags, d_const, n_cams, P, d_camtab);
+  CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
 
   double *d_out_xyz = nullptr, *d_rmse = nullptr;
   int* d_status = nullptr;
   CB_TRY(dalloc(&d_out_xyz, 3 * (size_t)n_groups)); sf.dev.push_back(d_out_xyz);
   CB_TRY(dalloc(&d_rmse, (size_t)n_groups)); sf.dev.push_back(d_rmse);
   CB_TRY(dalloc(&d_status, (size_t)n_groups)); sf.dev.push_back(d_status);
-  const size_t cam_bytes = sizeof(double) * cb::CT_SMEM * (size_t)n_cams;  // odd stride, see tri_stage_camtab
-  const int cam_in_smem = cam_bytes <= 40 * 1024 ? 1 : 0;
-  const size_t smem = cam_in_smem ? cam_bytes : 0;
-  const int lanes = t.lanes;
-  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
   CB_CUDA(cudaEventRecord(ev[4], st));
-  if (lanes == 32)
-    CB_LAUNCH(cb::tri_refine_kernel<32>, blocks, cb::TRI_THREADS, smem, st, d_camtab, n_cams, cam_in_smem, t.start,
-              t.rows, t.cam, d_px, n_groups, t.xyz, max_iter, xtol, d_out_xyz, d_rmse, d_status);
-  else
-    CB_LAUNCH(cb::tri_refine_kernel<8>, blocks, cb::TRI_THREADS, smem, st, d_camtab, n_cams, cam_in_smem, t.start,
-              t.rows, t.cam, d_px, n_groups, t.xyz, max_iter, xtol, d_out_xyz, d_rmse, d_status);
-  CB_CUDA(cudaGetLastError());
+  CB_TRY(tri_refine_launch(n_cams, cams, t.lanes, t.start, t.rows, t.cam, d_px, n_groups, t.xyz, max_iter, xtol, d_out_xyz,
+                           d_rmse, d_status, st));
   CB_CUDA(cudaEventRecord(ev[5], st));
 
   double* d_cov = nullptr;
-  if (cov_out) {
-    // camera covariance from x's layout to a uniform stride P (fixed / absent slots 0), uploaded once
-    double* d_sig = nullptr;
-    double* d_B = nullptr;
-    int* d_first = nullptr;
-    if (cam_cov) {
-      const size_t nP = (size_t)n_cams * P;
-      std::vector<double> sig(nP * nP, 0.0);
-      for (int c = 0; c < n_cams; ++c)
-        for (int p = 0; p < xoff[c + 1] - xoff[c]; ++p)
-          for (int d = 0; d < n_cams; ++d)
-            for (int q = 0; q < xoff[d + 1] - xoff[d]; ++q)
-              sig[((size_t)c * P + p) * nP + (size_t)d * P + q] = cam_cov[(size_t)(xoff[c] + p) * ncp + xoff[d] + q];
-      CB_TRY(dalloc(&d_sig, nP * nP)); sf.dev.push_back(d_sig);
-      CB_CUDA(cudaMemcpyAsync(d_sig, sig.data(), sizeof(double) * nP * nP, cudaMemcpyHostToDevice, st));
-      CB_TRY(dalloc(&d_B, 3 * (size_t)P * n)); sf.dev.push_back(d_B);
-      CB_TRY(dalloc(&d_first, (size_t)n)); sf.dev.push_back(d_first);
-      CB_CUDA(cudaStreamSynchronize(st));  // `sig` is a stack-lifetime upload
-    }
-    CB_TRY(dalloc(&d_cov, 9 * (size_t)n_groups)); sf.dev.push_back(d_cov);
-    const double s2 = pixel_sigma * pixel_sigma;
-    CB_CUDA(cudaEventRecord(ev[6], st));
-#define CB_TRI_COV(PP, LL)                                                                                           \
-  CB_LAUNCH((cb::tri_cov_kernel<PP, LL>), blocks, cb::TRI_THREADS, smem, st, d_camtab, n_cams, cam_in_smem, t.start, \
-            t.rows, t.cam, d_px, n_groups, d_out_xyz, d_status, d_sig, s2, d_B, d_first, d_cov)
-    if (P == 9 && lanes == 32) CB_TRI_COV(9, 32);
-    else if (P == 9) CB_TRI_COV(9, 8);
-    else if (lanes == 32) CB_TRI_COV(6, 32);
-    else CB_TRI_COV(6, 8);
-#undef CB_TRI_COV
-    CB_CUDA(cudaGetLastError());
-    CB_CUDA(cudaEventRecord(ev[7], st));
-  }
+  if (cov_out)
+    CB_TRY(tri_cov_launch(n_cams, cams, cam_cov, pixel_sigma, t.lanes, t.start, t.rows, t.cam, d_px, n, n_groups,
+                          d_out_xyz, d_status, ev[6], ev[7], sf, st, &d_cov));
   CB_CUDA(cudaMemcpyAsync(xyz_out, d_out_xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(count_out, t.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
@@ -3151,6 +3228,141 @@ int cb_triangulate_refine(int32_t n_cams, const int32_t* cam_flags, const double
     float ms = 0.f;
     cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
     cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->dlt_ms = ms;
+    cudaEventElapsedTime(&ms, ev[4], ev[5]); stats->refine_ms = ms;
+    if (cov_out) { cudaEventElapsedTime(&ms, ev[6], ev[7]); stats->cov_ms = ms; }
+    cudaEventElapsedTime(&ms, ev[0], cov_out ? ev[7] : ev[5]); stats->total_ms = ms;
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
+}
+
+int cb_triangulate_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                          const double* cam_cov, int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key,
+                          const double* obs_px, int obs_on_device, double threshold_px, int32_t min_inliers,
+                          int32_t max_pairs, double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups,
+                          int32_t* n_groups_out, double* xyz_out, double* cov_out, double* rmse_px_out,
+                          int32_t* count_out, int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out,
+                          uint8_t* inlier_out, CbTriRobustStats* stats, int device, void* stream) {
+  if (n_cams <= 0 || !cam_flags || !cam_const || !cam_x || n_obs < 0 || n_obs > 0x7fffffffLL || !n_groups_out ||
+      max_groups < 0 || (n_obs > 0 && (!obs_cam || !obs_key || !obs_px || !inlier_out)) ||
+      (max_groups > 0 && (!xyz_out || !rmse_px_out || !count_out || !n_inliers_out || !rep_row_out || !status_out)) ||
+      !(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma)) || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol)) ||
+      !(threshold_px > 0.0 && std::isfinite(threshold_px)) || min_inliers < 2 || max_pairs < 1) {
+    g_last_error = "cb_triangulate_robust: bad argument";
+    return CB_E_INVALID;
+  }
+  TriCams cams;
+  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, "cb_triangulate_robust", &cams));
+  CB_TRY(select_device(device));
+  *n_groups_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf;
+  const int n = (int)n_obs;
+  cudaEvent_t ev[8];
+  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
+  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 8; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  const int* d_cam = nullptr;
+  const long long* d_key = nullptr;
+  const double* d_px = nullptr;
+  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
+  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
+  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
+  // grouping and undistortion only: a DLT over the whole group would be contaminated by the outliers
+  TriDlt t;
+  CB_TRY(tri_group_stage(n_cams, &cams.tab, cams.proj.data(), n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups,
+                         n_groups_out, "cb_triangulate_robust", ev, sf, st, &t));
+  const int n_groups = t.n_groups;
+  CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
+
+  // (1) consensus: hypothesis, count, rep_row, n_inliers (+ a zero past the end for the scan), status 0 / 1 / 5, flags
+  double* d_hyp = nullptr;
+  int *d_count = nullptr, *d_rep = nullptr, *d_nin = nullptr, *d_cstatus = nullptr;
+  unsigned char *d_flag = nullptr, *d_inl = nullptr;
+  CB_TRY(dalloc(&d_hyp, 3 * (size_t)n_groups)); sf.dev.push_back(d_hyp);
+  CB_TRY(dalloc(&d_count, (size_t)n_groups)); sf.dev.push_back(d_count);
+  CB_TRY(dalloc(&d_rep, (size_t)n_groups)); sf.dev.push_back(d_rep);
+  CB_TRY(dalloc(&d_nin, (size_t)n_groups + 1)); sf.dev.push_back(d_nin);
+  CB_TRY(dalloc(&d_cstatus, (size_t)n_groups)); sf.dev.push_back(d_cstatus);
+  CB_TRY(dalloc(&d_flag, (size_t)n)); sf.dev.push_back(d_flag);
+  CB_TRY(dalloc(&d_inl, (size_t)n)); sf.dev.push_back(d_inl);
+  // (2) compaction: the consensus rows of every group, in key-sorted order, and their group starts
+  int *d_rows_c = nullptr, *d_start_c = nullptr, *d_nsel = nullptr;
+  CB_TRY(dalloc(&d_rows_c, (size_t)n)); sf.dev.push_back(d_rows_c);
+  CB_TRY(dalloc(&d_start_c, (size_t)n_groups + 1)); sf.dev.push_back(d_start_c);
+  CB_TRY(dalloc(&d_nsel, 1)); sf.dev.push_back(d_nsel);
+  size_t tb_sel = 0, tb_scan = 0;
+  CB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb_sel, t.rows, d_flag, d_rows_c, d_nsel, n, st));
+  CB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb_scan, d_nin, d_start_c, n_groups + 1, st));
+  void* d_tmp = nullptr;
+  const size_t tb = std::max<size_t>(std::max(tb_sel, tb_scan), 16);
+  CB_TRY(cached_malloc(&d_tmp, tb));
+  sf.dev.push_back(d_tmp);
+
+  // camera table and projection table each in shared memory when it takes at most 40 KB
+  const size_t cam_smem = tri_camtab_smem(n_cams);
+  const size_t proj_bytes = sizeof(double) * 13 * (size_t)n_cams;  // padded stride, see tri_dlt_kernel
+  const size_t proj_smem = proj_bytes <= 40 * 1024 ? proj_bytes : 0;
+  const size_t smem = cam_smem + proj_smem;
+  if (smem > 48 * 1024) {
+    CB_CUDA(cudaFuncSetAttribute(cb::tri_consensus_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CB_CUDA(cudaFuncSetAttribute(cb::tri_consensus_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  const int lanes = t.lanes;
+  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
+  CB_CUDA(cudaMemsetAsync(d_nin + n_groups, 0, sizeof(int), st));
+  CB_CUDA(cudaEventRecord(ev[2], st));
+#define CB_TRI_CONSENSUS(LL)                                                                                           \
+  CB_LAUNCH(cb::tri_consensus_kernel<LL>, blocks, cb::TRI_THREADS, smem, st, cams.camtab, cam_smem ? 1 : 0, t.proj,     \
+            proj_smem ? 1 : 0, n_cams, t.start, t.rows, t.cam, t.xy, d_px, n_groups, threshold_px, min_inliers,         \
+            max_pairs, d_hyp, d_count, d_rep, d_nin, d_cstatus, d_flag, d_inl)
+  if (lanes == 32) CB_TRI_CONSENSUS(32);
+  else CB_TRI_CONSENSUS(8);
+#undef CB_TRI_CONSENSUS
+  CB_CUDA(cudaGetLastError());
+  size_t tb_run = tb;
+  CB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb_run, t.rows, d_flag, d_rows_c, d_nsel, n, st));
+  tb_run = tb;
+  CB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tb_run, d_nin, d_start_c, n_groups + 1, st));
+  g_launches.fetch_add(4);
+  CB_CUDA(cudaEventRecord(ev[3], st));
+
+  // (3) refinement and covariance on the consensus rows, from the selected hypotheses; a status-5 group has no rows
+  // there, so the refinement reports 1 for it and the covariance is NaN
+  double *d_out_xyz = nullptr, *d_rmse = nullptr;
+  int* d_status = nullptr;
+  CB_TRY(dalloc(&d_out_xyz, 3 * (size_t)n_groups)); sf.dev.push_back(d_out_xyz);
+  CB_TRY(dalloc(&d_rmse, (size_t)n_groups)); sf.dev.push_back(d_rmse);
+  CB_TRY(dalloc(&d_status, (size_t)n_groups)); sf.dev.push_back(d_status);
+  CB_CUDA(cudaEventRecord(ev[4], st));
+  CB_TRY(tri_refine_launch(n_cams, cams, lanes, d_start_c, d_rows_c, t.cam, d_px, n_groups, d_hyp, max_iter, xtol,
+                           d_out_xyz, d_rmse, d_status, st));
+  CB_CUDA(cudaEventRecord(ev[5], st));
+  double* d_cov = nullptr;
+  if (cov_out)
+    CB_TRY(tri_cov_launch(n_cams, cams, cam_cov, pixel_sigma, lanes, d_start_c, d_rows_c, t.cam, d_px, n, n_groups,
+                          d_out_xyz, d_status, ev[6], ev[7], sf, st, &d_cov));
+  std::vector<int> cstatus(n_groups);
+  CB_CUDA(cudaMemcpyAsync(xyz_out, d_out_xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, d_count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(n_inliers_out, d_nin, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, d_rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(cstatus.data(), d_cstatus, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(inlier_out, d_inl, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (cov_out)
+    CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  for (int g = 0; g < n_groups; ++g)
+    if (cstatus[g] == cb::TRI_NO_CONSENSUS) status_out[g] = cb::TRI_NO_CONSENSUS;
+  if (stats) {
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
+    cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->consensus_ms = ms;
     cudaEventElapsedTime(&ms, ev[4], ev[5]); stats->refine_ms = ms;
     if (cov_out) { cudaEventElapsedTime(&ms, ev[6], ev[7]); stats->cov_ms = ms; }
     cudaEventElapsedTime(&ms, ev[0], cov_out ? ev[7] : ev[5]); stats->total_ms = ms;

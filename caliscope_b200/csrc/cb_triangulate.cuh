@@ -282,7 +282,7 @@ tri_dlt_kernel(const double* __restrict__ proj, int n_cams, int proj_in_smem, co
 
 // ---- refinement to the reprojection optimum and point covariance (cb_triangulate_refine, DESIGN.md section 4.7) -------
 // Group status codes, first match wins.
-enum { TRI_OK = 0, TRI_FEW_ROWS = 1, TRI_NOT_PD = 2, TRI_MAX_ITER = 3, TRI_BEHIND = 4 };
+enum { TRI_OK = 0, TRI_FEW_ROWS = 1, TRI_NOT_PD = 2, TRI_MAX_ITER = 3, TRI_BEHIND = 4, TRI_NO_CONSENSUS = 5 };
 constexpr double TRI_LAMBDA0 = 1e-3;  // initial Levenberg-Marquardt damping
 constexpr double TRI_PD_RTOL = 1e-12;
 
@@ -575,6 +575,178 @@ tri_cov_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, c
   for (int a = 0; a < 3; ++a)
 #pragma unroll
     for (int c = 0; c < 3; ++c) out[3 * a + c] = 0.5 * (o[a][c] + o[c][a]);
+}
+
+// ---- consensus over view pairs (cb_triangulate_robust, DESIGN.md section 4.8) ------------------------------------------
+// Positions (i, j), i < j, of the m-th candidate pair of a group of k rows with T = k (k - 1) / 2 pairs: lexicographic rank
+// m when T <= max_pairs, else floor(m T / max_pairs), computed exactly as m q + floor(m rem / max_pairs) with
+// T = q max_pairs + rem (m rem < max_pairs^2 < 2^62).  rank(i, j) = i k - i (i + 1) / 2 + (j - i - 1).
+__device__ __forceinline__ long long tri_pair_base(long long i, long long k) { return i * k - i * (i + 1) / 2; }
+
+__device__ __forceinline__ void tri_candidate_pair(long long m, long long T, int max_pairs, int k, int& i, int& j) {
+  long long r = m;
+  if (T > max_pairs) r = m * (T / max_pairs) + (m * (T % max_pairs)) / max_pairs;
+  const double kk = 2.0 * k - 1.0;
+  long long a = (long long)(0.5 * (kk - sqrt(kk * kk - 8.0 * (double)r)));  // largest a with base(a) <= r, up to rounding
+  a = max(0LL, min(a, (long long)k - 2));
+  while (a > 0 && tri_pair_base(a, k) > r) --a;
+  while (a < k - 2 && tri_pair_base(a + 1, k) <= r) ++a;
+  i = (int)a;
+  j = (int)(r - tri_pair_base(a, k) + a + 1);
+}
+
+// squared pixel error of one row at X and whether the row is in front of its camera
+__device__ __forceinline__ double tri_row_err2(const double* cam, const double* X, double2 px, bool& front) {
+  ProjOut o;
+  project_obs<false>(cam, (((int)cam[CT_FLAGS]) & 2) != 0, X[0], X[1], X[2], o);
+  front = o.Xc[2] > 0.0;
+  const double du = o.u - px.x, dv = o.v - px.y;
+  return du * du + dv * dv;
+}
+
+// One group per LANES lanes (the lane choice of tri_dlt_kernel).  The lanes stride over the group's candidate pairs; each
+// builds its pair's DLT point (tri_dlt_kernel's normal matrix on the undistorted float32-rounded coordinates `obs_xy`,
+// then sym4_min_eigvec) and scores it by MSAC over all k rows, sum min(e_r^2, tau^2) in raw pixels (a row behind its camera
+// or with a non-finite error costs tau^2).  A pair of rows from one camera, a non-finite point or one not in front of both
+// of the pair's cameras is no hypothesis.  An xor butterfly over (score, candidate index) picks the lowest score, the
+// lowest rank on a tie (rank grows with the index); the winner's point reaches the group's lanes by shuffle.  Each lane
+// then classifies its rows (in front and e_r^2 <= tau^2) into `pos_flag` (key-sorted position) and `inlier` (caller row);
+// both are cleared when the group has no hypothesis or fewer than min_inliers consensus rows (status 5).  Writes count,
+// rep_row, n_inliers, status (0, 1 or 5) and xyz0 = the selected hypothesis (NaN for status 1 and 5).
+// `camtab` and `proj` are staged in shared memory independently (camera table first) when their flags say so.
+template <int LANES>
+__global__ void __launch_bounds__(TRI_THREADS)
+tri_consensus_kernel(const double* __restrict__ camtab, int cam_in_smem, const double* __restrict__ proj, int proj_in_smem,
+                     int n_cams, const int* __restrict__ start, const int* __restrict__ rows,
+                     const int* __restrict__ obs_cam, const double* __restrict__ obs_xy, const double* __restrict__ obs_px,
+                     int n_groups, double tau, int min_inliers, int max_pairs, double* __restrict__ xyz0,
+                     int* __restrict__ count, int* __restrict__ rep_row, int* __restrict__ n_inliers,
+                     int* __restrict__ status, unsigned char* __restrict__ pos_flag, unsigned char* __restrict__ inlier) {
+  extern __shared__ double s_cam[];
+  int stride;
+  const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
+  constexpr int PSTRIDE_SM = 13;  // odd stride, see tri_dlt_kernel
+  double* s_proj = s_cam + (cam_in_smem ? (size_t)CT_SMEM * n_cams : 0);
+  if (proj_in_smem) {
+    for (int i = threadIdx.x; i < n_cams * 12; i += blockDim.x) s_proj[(i / 12) * PSTRIDE_SM + i % 12] = proj[i];
+    __syncthreads();
+  }
+  const double* Pt = proj_in_smem ? s_proj : proj;
+  const int pstride = proj_in_smem ? PSTRIDE_SM : 12;
+  const int lane = threadIdx.x & (LANES - 1);
+  const long long g = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LANES;
+  const bool live = g < n_groups;
+  const int b = live ? start[g] : 0, e = live ? start[g + 1] : 0, k = e - b;
+  const double tau2 = tau * tau;
+  const double inf = __longlong_as_double(0x7ff0000000000000LL);
+  const long long T = (long long)k * (k - 1) / 2;
+  const long long nh = T < max_pairs ? T : (long long)max_pairs;
+  double best = inf, X[3] = {0.0, 0.0, 0.0};
+  long long best_m = 0x7fffffffffffffffLL;
+  for (long long m = lane; m < nh; m += LANES) {
+    int i, j;
+    tri_candidate_pair(m, T, max_pairs, k, i, j);
+    const int ri = rows[b + i], rj = rows[b + j];
+    const int ci = obs_cam[ri], cj = obs_cam[rj];
+    if (ci == cj) continue;
+    double mm[10];
+#pragma unroll
+    for (int t = 0; t < 10; ++t) mm[t] = 0.0;
+#pragma unroll
+    for (int s = 0; s < 2; ++s) {
+      const int r = s ? rj : ri;
+      const double2 xy = reinterpret_cast<const double2*>(obs_xy)[r];
+      const double* Pc = Pt + (size_t)pstride * (size_t)(s ? cj : ci);
+      double a[4], bb[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const double p2 = Pc[8 + q];
+        a[q] = xy.x * p2 - Pc[q];
+        bb[q] = xy.y * p2 - Pc[4 + q];
+      }
+      int t = 0;
+#pragma unroll
+      for (int p = 0; p < 4; ++p)
+#pragma unroll
+        for (int q = p; q < 4; ++q) {
+          mm[t] = fma(a[p], a[q], fma(bb[p], bb[q], mm[t]));
+          ++t;
+        }
+    }
+    double A[4][4], w[4];
+    int t = 0;
+#pragma unroll
+    for (int p = 0; p < 4; ++p)
+#pragma unroll
+      for (int q = p; q < 4; ++q) {
+        A[p][q] = mm[t];
+        A[q][p] = mm[t];
+        ++t;
+      }
+    sym4_min_eigvec(A, w);
+    const double h[3] = {w[0] / w[3], w[1] / w[3], w[2] / w[3]};
+    if (!isfinite(h[0]) || !isfinite(h[1]) || !isfinite(h[2])) continue;
+    const double* Ci = cams + (size_t)stride * ci;
+    const double* Cj = cams + (size_t)stride * cj;
+    const double zi = fma(Ci[CT_R + 6], h[0], fma(Ci[CT_R + 7], h[1], fma(Ci[CT_R + 8], h[2], Ci[CT_T + 2])));
+    const double zj = fma(Cj[CT_R + 6], h[0], fma(Cj[CT_R + 7], h[1], fma(Cj[CT_R + 8], h[2], Cj[CT_T + 2])));
+    if (!(zi > 0.0) || !(zj > 0.0)) continue;
+    double score = 0.0;
+    for (int p = b; p < e; ++p) {
+      const int r = rows[p];
+      bool front;
+      const double e2 = tri_row_err2(cams + (size_t)stride * obs_cam[r], h, reinterpret_cast<const double2*>(obs_px)[r], front);
+      score += (front && e2 <= tau2) ? e2 : tau2;
+    }
+    if (score < best) {  // candidates of a lane come in increasing rank: the first of equal scores stays
+      best = score;
+      best_m = m;
+#pragma unroll
+      for (int q = 0; q < 3; ++q) X[q] = h[q];
+    }
+  }
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1) {
+    const double ob = __shfl_xor_sync(0xffffffffu, best, s);
+    const long long om = __shfl_xor_sync(0xffffffffu, best_m, s);
+    if (ob < best || (ob == best && om < best_m)) {
+      best = ob;
+      best_m = om;
+    }
+  }
+  const bool found = best < inf;
+  const int owner = found ? (int)(best_m % LANES) : 0;
+#pragma unroll
+  for (int q = 0; q < 3; ++q) X[q] = __shfl_sync(0xffffffffu, X[q], owner, LANES);
+  int nin = 0;
+  for (int i = b + lane; i < e; i += LANES) {
+    const int r = rows[i];
+    bool in = false;
+    if (found) {
+      bool front;
+      const double e2 = tri_row_err2(cams + (size_t)stride * obs_cam[r], X, reinterpret_cast<const double2*>(obs_px)[r], front);
+      in = front && e2 <= tau2;
+    }
+    pos_flag[i] = in ? 1 : 0;
+    inlier[r] = in ? 1 : 0;
+    nin += in ? 1 : 0;
+  }
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1) nin += __shfl_xor_sync(0xffffffffu, nin, s);
+  const bool ok = found && nin >= min_inliers;
+  if (!ok && nin > 0)
+    for (int i = b + lane; i < e; i += LANES) {
+      pos_flag[i] = 0;
+      inlier[rows[i]] = 0;
+    }
+  if (!live || lane != 0) return;
+  const double nan = __longlong_as_double(0x7ff8000000000000LL);
+  count[g] = k;
+  rep_row[g] = rows[b];
+  n_inliers[g] = ok ? nin : 0;
+  status[g] = k < 2 ? TRI_FEW_ROWS : ok ? TRI_OK : TRI_NO_CONSENSUS;
+#pragma unroll
+  for (int q = 0; q < 3; ++q) xyz0[3 * g + q] = ok ? X[q] : nan;
 }
 
 }  // namespace cb

@@ -291,20 +291,10 @@ def _check_device_tri_obs(obs_cam, obs_key, obs_px, device: int) -> int:
     return n
 
 
-def triangulate_refined(cam_flags, cam_const, cam_x, obs_cam, obs_key, obs_px, *, pixel_sigma: float = 1.0,
-                        camera_cov=None, max_iter: int = 20, xtol: float = 1e-12, device: int = 0, stream: int = 0,
-                        stats: RefineStats | None = None) -> RefinedPoints:
-    """Maximum-likelihood triangulation with calibrated cameras and a covariance per point (``cb_triangulate_refine``,
-    DESIGN.md section 4.7).
-
-    The cameras are ``BAProblem.cam_flags``, ``BAProblem.cam_const`` and ``x[:n_camera_params]`` of a solution;
-    ``camera_cov`` is ``Covariance.cameras`` at that solution (None: pixel noise only).  Observations with equal
-    ``obs_key`` are one point; ``obs_px`` are raw pixels.  They may be host arrays or CUDA tensors on ``device``
-    (obs_cam int32, obs_key int64, obs_px float64 (n, 2)), read in place.  Each point starts at the DLT point and is
-    refined to the least-squares reprojection optimum; ``cov = pixel_sigma^2 H^-1 + H^-1 G camera_cov G^T H^-1``.  This
-    assumes the observations are independent of those the calibration used (for a point that was itself in the
-    bundle adjustment, use ``Covariance.points``), and the camera term is relative to ``camera_cov``'s gauge."""
-    lib = L.load()
+def _calibrated_inputs(cam_flags, cam_const, cam_x, camera_cov, obs_cam, obs_key, obs_px, device: int):
+    """Cameras in the BA layout and observations (host arrays or CUDA tensors read in place) of the calibrated
+    triangulation calls as the C ABI takes them: (n_cams, flags, const, cam_x, camera_cov or None, n, on_device,
+    observation pointers, host arrays the pointers refer to)."""
     flags = np.ascontiguousarray(cam_flags, dtype=np.int32).ravel()
     nc = len(flags)
     const = np.ascontiguousarray(cam_const, dtype=np.float64).reshape(nc, 9)
@@ -330,6 +320,26 @@ def triangulate_refined(cam_flags, cam_const, cam_x, obs_cam, obs_key, obs_px, *
         if len(key) != n or len(px) != n:
             raise ValueError("obs_cam, obs_key and obs_px must have one row per observation")
         cam_p, key_p, px_p = _ptr(cam), _ptr(key), _ptr(px)
+        return nc, flags, const, cx, ccov, n, False, (cam_p, key_p, px_p), (cam, key, px)
+    return nc, flags, const, cx, ccov, n, True, (cam_p, key_p, px_p), ()
+
+
+def triangulate_refined(cam_flags, cam_const, cam_x, obs_cam, obs_key, obs_px, *, pixel_sigma: float = 1.0,
+                        camera_cov=None, max_iter: int = 20, xtol: float = 1e-12, device: int = 0, stream: int = 0,
+                        stats: RefineStats | None = None) -> RefinedPoints:
+    """Maximum-likelihood triangulation with calibrated cameras and a covariance per point (``cb_triangulate_refine``,
+    DESIGN.md section 4.7).
+
+    The cameras are ``BAProblem.cam_flags``, ``BAProblem.cam_const`` and ``x[:n_camera_params]`` of a solution;
+    ``camera_cov`` is ``Covariance.cameras`` at that solution (None: pixel noise only).  Observations with equal
+    ``obs_key`` are one point; ``obs_px`` are raw pixels.  They may be host arrays or CUDA tensors on ``device``
+    (obs_cam int32, obs_key int64, obs_px float64 (n, 2)), read in place.  Each point starts at the DLT point and is
+    refined to the least-squares reprojection optimum; ``cov = pixel_sigma^2 H^-1 + H^-1 G camera_cov G^T H^-1``.  This
+    assumes the observations are independent of those the calibration used (for a point that was itself in the
+    bundle adjustment, use ``Covariance.points``), and the camera term is relative to ``camera_cov``'s gauge."""
+    lib = L.load()
+    nc, flags, const, cx, ccov, n, on_dev, (cam_p, key_p, px_p), _keep = _calibrated_inputs(
+        cam_flags, cam_const, cam_x, camera_cov, obs_cam, obs_key, obs_px, device)
     m = max(n, 1)
     xyz, cov, rmse = np.empty((m, 3)), np.empty((m, 3, 3)), np.empty(m)
     count, rep, status = np.empty(m, np.int32), np.empty(m, np.int32), np.empty(m, np.int32)
@@ -348,6 +358,71 @@ def triangulate_refined(cam_flags, cam_const, cam_x, obs_cam, obs_key, obs_px, *
         stats.total_ms, stats.kernel_launches, stats.n_groups = st.total_ms, st.kernel_launches, g
     return RefinedPoints(xyz=xyz[:g], cov=cov[:g], rmse_px=rmse[:g], count=count[:g], rep_row=rep[:g],
                          status=status[:g])  # fmt: skip
+
+
+@dataclass
+class RobustPoints(RefinedPoints):
+    """``triangulate_robust``: the ``RefinedPoints`` fields over each group's consensus rows (``count`` is still every
+    row of the group), plus n_inliers per group and the caller-order inlier mask.  status 5: no consensus (xyz, cov and
+    rmse NaN, n_inliers 0)."""
+
+    n_inliers: np.ndarray = None  # (G,) int32
+    inlier: np.ndarray = None  # (n_obs,) bool, caller order
+
+
+@dataclass
+class RobustStats:
+    group_ms: float = 0.0
+    consensus_ms: float = 0.0
+    refine_ms: float = 0.0
+    cov_ms: float = 0.0
+    total_ms: float = 0.0
+    kernel_launches: int = 0
+    n_groups: int = 0
+
+
+def triangulate_robust(cam_flags, cam_const, cam_x, obs_cam, obs_key, obs_px, *, threshold_px: float,
+                       min_inliers: int = 2, max_pairs: int = 64, pixel_sigma: float = 1.0, camera_cov=None,
+                       max_iter: int = 20, xtol: float = 1e-12, device: int = 0, stream: int = 0,
+                       stats: RobustStats | None = None) -> RobustPoints:
+    """``triangulate_refined`` on each point's agreeing views (``cb_triangulate_robust``, DESIGN.md section 4.8).
+
+    Inputs as ``triangulate_refined``.  Inside each group the DLT points of up to ``max_pairs`` view pairs (every pair,
+    or an evenly spaced deterministic subset of the lexicographically ranked pairs) are scored by MSAC over all rows of
+    the group, sum min(e^2, threshold_px^2) in raw pixels; the lowest score wins (the lowest rank on a tie).  The rows
+    within ``threshold_px`` of the winner, in front of their camera, are the consensus set; the point is refined on them
+    alone from the winner and gets its covariance from them.  Fewer than ``min_inliers`` consensus rows, or no valid
+    pair (every row from one camera, for example), gives status 5.  There is one consensus round (rows are not
+    re-classified at the refined point), and in a two-view group an error along the epipolar line cannot be seen."""
+    if not (np.isfinite(threshold_px) and threshold_px > 0):
+        raise ValueError(f"threshold_px must be finite and > 0, got {threshold_px}")
+    if int(min_inliers) < 2:
+        raise ValueError(f"min_inliers must be >= 2, got {min_inliers}")
+    if int(max_pairs) < 1:
+        raise ValueError(f"max_pairs must be >= 1, got {max_pairs}")
+    lib = L.load()
+    nc, flags, const, cx, ccov, n, on_dev, (cam_p, key_p, px_p), _keep = _calibrated_inputs(
+        cam_flags, cam_const, cam_x, camera_cov, obs_cam, obs_key, obs_px, device)
+    m = max(n, 1)
+    xyz, cov, rmse = np.empty((m, 3)), np.empty((m, 3, 3)), np.empty(m)
+    count, nin, rep, status = (np.empty(m, np.int32) for _ in range(4))
+    inlier = np.zeros(m, np.uint8)
+    ng = C.c_int32(0)
+    st = L.TriRobustStats()
+    L.check(
+        lib.cb_triangulate_robust(nc, _ptr(flags), _ptr(const), _ptr(cx), None if ccov is None else _ptr(ccov), n, cam_p,
+                                  key_p, px_p, 1 if on_dev else 0, float(threshold_px), int(min_inliers), int(max_pairs),
+                                  float(pixel_sigma), int(max_iter), float(xtol), n, C.byref(ng), _ptr(xyz), _ptr(cov),
+                                  _ptr(rmse), _ptr(count), _ptr(nin), _ptr(rep), _ptr(status), _ptr(inlier), C.byref(st),
+                                  int(device), C.c_void_p(stream)),
+        "triangulate_robust",
+    )  # fmt: skip
+    g = ng.value
+    if stats is not None:
+        stats.group_ms, stats.consensus_ms, stats.refine_ms = st.group_ms, st.consensus_ms, st.refine_ms
+        stats.cov_ms, stats.total_ms, stats.kernel_launches, stats.n_groups = st.cov_ms, st.total_ms, st.kernel_launches, g
+    return RobustPoints(xyz=xyz[:g], cov=cov[:g], rmse_px=rmse[:g], count=count[:g], rep_row=rep[:g], status=status[:g],
+                        n_inliers=nin[:g], inlier=inlier[:n].astype(bool))  # fmt: skip
 
 
 def undistort_points(points, cam_rows, matrices, distortions, fisheye, *, output: str = "normalized", device: int = 0,

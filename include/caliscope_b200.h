@@ -331,6 +331,45 @@ int cb_triangulate_refine(int32_t n_cams, const int32_t* cam_flags, const double
                           double* rmse_px_out, int32_t* count_out, int32_t* rep_row_out, int32_t* status_out,
                           CbTriRefineStats* stats, int device, void* stream);
 
+typedef struct CbTriRobustStats {
+  double group_ms;      /* upload + undistortion + radix sort + group boundaries */
+  double consensus_ms;  /* the consensus kernel and the compaction of the consensus rows */
+  double refine_ms;     /* the Levenberg-Marquardt kernel on the consensus rows */
+  double cov_ms;        /* the covariance kernel (0 without cov_out) */
+  double total_ms;
+  int32_t kernel_launches;
+  int32_t pad_;
+} CbTriRobustStats;
+
+/* cb_triangulate_refine on each group's consensus rows, chosen by view-pair consensus (DESIGN.md section 4.8).  Inputs
+ * as cb_triangulate_refine, plus threshold_px tau (finite, > 0), min_inliers (>= 2) and max_pairs (>= 1).  Inside a
+ * group of k rows (key-sorted, caller order within a key, positions 0..k-1):
+ *   candidate pairs: the pairs i < j ranked lexicographically, rank(i,j) = i k - i (i + 1) / 2 + (j - i - 1),
+ *     T = k (k - 1) / 2; every rank when T <= max_pairs, else the ranks floor(m T / max_pairs), m = 0..max_pairs-1 (exact
+ *     64-bit integers; no random sampling).
+ *   hypothesis of a pair: none when both rows come from one camera; else the DLT point of the two rows (the normal
+ *     matrix of cb_undistort_triangulate on float32-rounded undistorted coordinates, smallest eigenvector,
+ *     de-homogenised); none when it is not finite or has Xc.z <= 0 in either of the pair's cameras.
+ *   score (MSAC): sum over all k rows of min(e_r^2, tau^2), e_r = |pi(X; c_r) - u_r| in raw pixels with the engine's
+ *     projection; a row with Xc.z <= 0 or a non-finite e_r adds tau^2.  The lowest score wins, the lowest rank on a tie.
+ *   consensus set: the rows with Xc.z > 0 and e_r <= tau at the winner.
+ * The refinement and covariance of cb_triangulate_refine then run on the consensus rows alone, started from the winning
+ * hypothesis; rmse_px is over the consensus rows.  There is one consensus round: rows are not re-classified at the
+ * refined point.  In a two-view group an error along the epipolar line cannot be seen.
+ * Outputs (host, room for max_groups): xyz, cov (nullable), rmse_px, count (all rows of the group), n_inliers, rep_row
+ * and status per group; inlier[n_obs] (1 = the caller row is in its group's consensus set).  status, first match wins:
+ *   1 fewer than 2 rows;  5 no consensus: no valid hypothesis, or fewer than min_inliers consensus rows (xyz, cov, rmse
+ *   NaN, n_inliers 0, no row inlier; a group whose rows all come from one camera is 5);  2, 3, 4 as cb_triangulate_refine
+ *   (for 2, xyz = the hypothesis);  0 none.
+ * No atomics: repeated calls return bit-identical outputs. */
+int cb_triangulate_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                          const double* cam_cov, int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key,
+                          const double* obs_px, int obs_on_device, double threshold_px, int32_t min_inliers,
+                          int32_t max_pairs, double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups,
+                          int32_t* n_groups_out, double* xyz_out, double* cov_out, double* rmse_px_out,
+                          int32_t* count_out, int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out,
+                          uint8_t* inlier_out, CbTriRobustStats* stats, int device, void* stream);
+
 /* Optional NCCL transport owned by the engine (no host callback per all-reduce).  NCCL is resolved at run time from
  * the libnccl the process already has loaded (PyTorch's).  Rank 0 calls cb_nccl_unique_id and distributes the 128
  * bytes (e.g. torch.distributed.broadcast); every rank then calls cb_nccl_comm_create (collective). */
