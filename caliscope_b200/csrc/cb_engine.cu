@@ -257,11 +257,76 @@ void cached_free_host(void* p) {
   g_cache.live_host.erase(it);
 }
 
+template <typename T>
+int dalloc(T** p, size_t n) {
+  return cached_malloc((void**)p, std::max<size_t>(n, 1) * sizeof(T));
+}
+
+// The workspace of one call: device and pinned blocks from the cache, held until the scope ends.  It is bound to the
+// stream the call queues its work on, and waits for that stream before any block goes back to the cache: a return
+// partway through, after kernels or copies were queued, must not hand a block they still use to another thread.  An
+// unbound workspace (XyUpload::pinned) belongs to an owner that waits for its copies itself.
 struct ScopedFree {
-  std::vector<void*> dev, host;
+  ScopedFree() = default;
+  explicit ScopedFree(cudaStream_t s) : st(s), bound(true) {}
+  ScopedFree(const ScopedFree&) = delete;
+  ScopedFree& operator=(const ScopedFree&) = delete;
   ~ScopedFree() {
+    if (bound) cudaStreamSynchronize(st);  // its error, if any, is left to the caller's own checks: g_last_error stays
     for (void* q : dev) cached_free(q);
     for (void* q : host) cached_free_host(q);
+  }
+  template <typename T>
+  int alloc(T** p, size_t n) {
+    CB_TRY(dalloc(p, n));
+    dev.push_back((void*)*p);
+    return CB_OK;
+  }
+  template <typename T>
+  int alloc_pinned(T** p, size_t n) {
+    CB_TRY(cached_malloc_host((void**)p, std::max<size_t>(n, 1) * sizeof(T)));
+    host.push_back((void*)*p);
+    return CB_OK;
+  }
+
+ private:
+  std::vector<void*> dev, host;
+  cudaStream_t st = nullptr;
+  bool bound = false;
+};
+
+// Runs the cub device algorithm `algo` on one argument list: queries its temporary storage, takes it (16 B at least)
+// from the workspace `sf` and makes the call.
+#define CB_CUB(sf, algo, ...)                                    \
+  do {                                                           \
+    size_t _tb = 0;                                              \
+    CB_CUDA(algo(nullptr, _tb, __VA_ARGS__));                    \
+    unsigned char* _tmp = nullptr;                               \
+    CB_TRY((sf).alloc(&_tmp, std::max<size_t>(_tb, 16)));        \
+    CB_CUDA(algo(_tmp, _tb, __VA_ARGS__));                       \
+  } while (0)
+
+// The timing events of one call's stages, destroyed on every path
+template <int N>
+struct StageEvents {
+  cudaEvent_t e[N] = {};
+  StageEvents() = default;
+  StageEvents(const StageEvents&) = delete;
+  StageEvents& operator=(const StageEvents&) = delete;
+  ~StageEvents() {
+    for (cudaEvent_t x : e)
+      if (x) cudaEventDestroy(x);
+  }
+  int create() {
+    for (cudaEvent_t& x : e) CB_CUDA(cudaEventCreate(&x));
+    return CB_OK;
+  }
+  cudaEvent_t operator[](int i) const { return e[i]; }
+  // milliseconds from event a to event b
+  float ms(int a, int b) const {
+    float v = 0.f;
+    cudaEventElapsedTime(&v, e[a], e[b]);
+    return v;
   }
 };
 
@@ -339,13 +404,11 @@ class WorkerPool {
 // buffer, well below PCIe speed, so the caller's arrays (NumPy, pageable) are copied by pool threads into a pinned block in
 // chunks; the calling thread queues each chunk's DMA in order as soon as it is staged (one thread talks to the driver)
 // and copies chunks itself while it would otherwise wait.  Returns once the source has been read completely (the caller
-// may free it); the pinned block must stay alive until `st` has drained (sf.host frees it at scope exit of the caller,
-// which synchronises first).
+// may free it); the pinned block must stay alive until `st` has drained (the caller's workspace `sf` holds it).
 int staged_h2d(void* d_dst, const void* h_src, size_t bytes, cudaStream_t st, ScopedFree& sf, int n_threads = 6) {
   if (bytes == 0) return CB_OK;
-  void* pin = nullptr;
-  CB_TRY(cached_malloc_host(&pin, bytes));
-  sf.host.push_back(pin);
+  char* pin = nullptr;
+  CB_TRY(sf.alloc_pinned(&pin, bytes));
   // Two granularities.  Host threads copy 512 KB units (enough units to keep 6-8 threads busy on a 4 MB array); the DMA is
   // queued in 4 MB blocks: every cudaMemcpyAsync has a fixed copy-engine cost on top of its bytes, so small blocks
   // throttle the engine and large ones expose the staging.
@@ -418,11 +481,6 @@ int select_device(int device) {
   if (device < 0 || device >= ndev) { g_last_error = "device index out of range"; return CB_E_INVALID; }
   CB_CUDA(cudaSetDevice(device));
   return CB_OK;
-}
-
-template <typename T>
-int dalloc(T** p, size_t n) {
-  return cached_malloc((void**)p, std::max<size_t>(n, 1) * sizeof(T));
 }
 
 }  // namespace
@@ -599,8 +657,8 @@ int choose_camera_order(CbBaProblem* p, const int* cam_order, cudaStream_t st) {
       p->order_auto = true;
       const int stride = std::max(1, p->n_pts / 8192), ns = cdiv(p->n_pts, stride);
       unsigned int* d_W;
-      CB_TRY(dalloc(&d_W, (size_t)nc * nc));
-      ScopedFree sf; sf.dev.push_back(d_W);
+      ScopedFree sf(st);
+      CB_TRY(sf.alloc(&d_W, (size_t)nc * nc));
       CB_CUDA(cudaMemsetAsync(d_W, 0, sizeof(unsigned int) * nc * nc, st));
       CB_LAUNCH(cb::covis_kernel, cdiv((long long)ns * 32, 256), 256, 0, st, p->d_pt_start, p->d_pm_cam, p->n_pts, stride, nc, d_W);
       std::vector<unsigned int> W((size_t)nc * nc);
@@ -685,31 +743,25 @@ int build_indices(CbBaProblem* p, const int* d_obs_cam, const int* d_obs_pt, con
                   const int* cam_order, cudaStream_t st, XyUpload* xy_upload) {
   const int n = p->n_obs;
   const int TB = 256, G = cdiv(std::max(n, 1), TB);
-  ScopedFree sf;
+  ScopedFree sf(st);
   int* d_bad;
-  CB_TRY(dalloc(&d_bad, 2)); sf.dev.push_back(d_bad);
+  CB_TRY(sf.alloc(&d_bad, 2));
   CB_CUDA(cudaMemsetAsync(d_bad, 0, 2 * sizeof(int), st));
   CB_LAUNCH(cb::validate_kernel, G, TB, 0, st, d_obs_cam, d_obs_pt, n, p->n_cams, p->n_pts, d_bad);
 
   unsigned long long *k_in, *k_out;
   int *v_in, *v_out, *pm_pt, *pm_cam, *cm_cam;
-  CB_TRY(dalloc(&k_in, n)); sf.dev.push_back(k_in);
-  CB_TRY(dalloc(&k_out, n)); sf.dev.push_back(k_out);
-  CB_TRY(dalloc(&v_in, n)); sf.dev.push_back(v_in);
-  CB_TRY(dalloc(&v_out, n)); sf.dev.push_back(v_out);
-  CB_TRY(dalloc(&cm_cam, n)); sf.dev.push_back(cm_cam);
+  CB_TRY(sf.alloc(&k_in, n));
+  CB_TRY(sf.alloc(&k_out, n));
+  CB_TRY(sf.alloc(&v_in, n));
+  CB_TRY(sf.alloc(&v_out, n));
+  CB_TRY(sf.alloc(&cm_cam, n));
   pm_pt = p->d_pm_pt; pm_cam = p->d_pm_cam;
-
-  // temp storage for cub
-  size_t tb = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tb, k_in, k_out, v_in, v_out, n, 0, 64, st);
-  void* d_tmp;
-  CB_TRY(cached_malloc(&d_tmp, std::max<size_t>(tb, 16))); sf.dev.push_back(d_tmp);
 
   // (1) point-major order: key = pt * n_cams + cam, stable -> ties keep caller order
   CB_LAUNCH(cb::make_keys_kernel, G, TB, 0, st, d_obs_pt, d_obs_cam, (long long)p->n_cams, n, k_in, v_in);
   const int kb = bits_for((unsigned long long)p->n_pts * (unsigned long long)p->n_cams);
-  CB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, k_in, k_out, v_in, p->d_pm_orig, n, 0, kb, st));
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, k_in, k_out, v_in, p->d_pm_orig, n, 0, kb, st);
   g_launches.fetch_add(4);
   CB_LAUNCH(cb::split_keys_kernel, G, TB, 0, st, k_out, (long long)p->n_cams, n, pm_pt, pm_cam);
   CB_LAUNCH(cb::lower_bound_kernel, cdiv(p->n_pts + 1, TB), TB, 0, st, pm_pt, n, p->n_pts, p->d_pt_start);
@@ -719,7 +771,7 @@ int build_indices(CbBaProblem* p, const int* d_obs_cam, const int* d_obs_pt, con
   if (!p->order_identity) CB_LAUNCH(cb::remap_kernel, G, TB, 0, st, pm_cam, (const int*)p->d_cam_slot, n);
   // (2) camera-major order: key = cam * n_pts + pt over the point-major positions (stable)
   CB_LAUNCH(cb::make_keys_kernel, G, TB, 0, st, pm_cam, pm_pt, (long long)p->n_pts, n, k_in, v_in);
-  CB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, k_in, k_out, v_in, v_out, n, 0, kb, st));
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, k_in, k_out, v_in, v_out, n, 0, kb, st);
   g_launches.fetch_add(4);
   CB_LAUNCH(cb::split_keys_kernel, G, TB, 0, st, k_out, (long long)p->n_pts, n, cm_cam, v_in);
   CB_LAUNCH(cb::lower_bound_kernel, cdiv(p->n_cams + 1, TB), TB, 0, st, cm_cam, n, p->n_cams, p->d_cam_start);
@@ -1500,16 +1552,15 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
   if (const char* ev = std::getenv("CB_SY_SPARSE")) want_sparse = std::atoi(ev);
   if (nb >= 2 && nb <= 64 && p->n_pts > 0 && want_sparse != 0) {
     unsigned long long* d_mask;
-    CB_TRY(dalloc(&d_mask, (size_t)p->n_pts));
-    ScopedFree sf; sf.dev.push_back(d_mask);
+    ScopedFree sf(st);
+    CB_TRY(sf.alloc(&d_mask, (size_t)p->n_pts));
     CB_LAUNCH(cb::pt_tile_mask_kernel, cdiv(p->n_pts, 256), 256, 0, st, p->d_pt_start, p->d_pm_cam, p->n_pts, p->P, d_mask);
     if (p->n_comp)  // comp_build_kernel fills a component point's Zt rows in every column its component's cameras reach
       CB_LAUNCH(cb::comp_tile_mask_kernel, cdiv(p->n_comp, 256), 256, 0, st, p->ct.comp_pt_start, p->ct.comp_pts, p->n_comp,
                 d_mask);
     // incidence counts per tile pair (dense rigs stop here: no mask download, no host pass over the points)
     unsigned long long* d_cnt;
-    CB_TRY(dalloc(&d_cnt, (size_t)nt));
-    sf.dev.push_back(d_cnt);
+    CB_TRY(sf.alloc(&d_cnt, (size_t)nt));
     CB_CUDA(cudaMemsetAsync(d_cnt, 0, sizeof(unsigned long long) * nt, st));
     CB_LAUNCH(cb::tile_pair_count_kernel, cdiv(p->n_pts, 256), 256, sizeof(unsigned) * nt, st, d_mask, p->n_pts, nb, d_cnt);
     std::vector<unsigned long long> cnt_u((size_t)nt);
@@ -1543,27 +1594,20 @@ static int build_schur_items(CbBaProblem* p, cudaStream_t st) {
       int *d_ninc = nullptr, *d_incoff = nullptr;
       unsigned long long *d_keys = nullptr, *d_keys_s = nullptr;
       long long *d_pair_start = nullptr, *d_koff = nullptr;
-      CB_TRY(dalloc(&d_ninc, (size_t)p->n_pts + 1)); sf.dev.push_back(d_ninc);
-      CB_TRY(dalloc(&d_incoff, (size_t)p->n_pts + 1)); sf.dev.push_back(d_incoff);
-      CB_TRY(dalloc(&d_keys, (size_t)n_inc)); sf.dev.push_back(d_keys);
-      CB_TRY(dalloc(&d_keys_s, (size_t)n_inc)); sf.dev.push_back(d_keys_s);
-      CB_TRY(dalloc(&d_pair_start, (size_t)nt + 1)); sf.dev.push_back(d_pair_start);
-      CB_TRY(dalloc(&d_koff, (size_t)nt)); sf.dev.push_back(d_koff);
+      CB_TRY(sf.alloc(&d_ninc, (size_t)p->n_pts + 1));
+      CB_TRY(sf.alloc(&d_incoff, (size_t)p->n_pts + 1));
+      CB_TRY(sf.alloc(&d_keys, (size_t)n_inc));
+      CB_TRY(sf.alloc(&d_keys_s, (size_t)n_inc));
+      CB_TRY(sf.alloc(&d_pair_start, (size_t)nt + 1));
+      CB_TRY(sf.alloc(&d_koff, (size_t)nt));
       CB_TRY(palloc(p, &p->d_klist, (size_t)klen));
       CB_CUDA(cudaMemsetAsync(d_ninc + p->n_pts, 0, sizeof(int), st));
       CB_LAUNCH(cb::inc_count_kernel, cdiv(p->n_pts, 256), 256, 0, st, (const unsigned long long*)d_mask, p->n_pts, d_ninc);
-      size_t tb_a = 0, tb_b = 0;
       const int key_bits = bits_for((unsigned long long)nt * (unsigned long long)p->n_pts);
-      cub::DeviceScan::ExclusiveSum(nullptr, tb_a, d_ninc, d_incoff, p->n_pts + 1, st);
-      cub::DeviceRadixSort::SortKeys(nullptr, tb_b, d_keys, d_keys_s, (int)n_inc, 0, key_bits, st);
-      void* d_tmp = nullptr;
-      size_t tbm = std::max(tb_a, tb_b);
-      CB_TRY(cached_malloc(&d_tmp, std::max<size_t>(tbm, 16))); sf.dev.push_back(d_tmp);
-      CB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tbm, d_ninc, d_incoff, p->n_pts + 1, st));
+      CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_ninc, d_incoff, p->n_pts + 1, st);
       CB_LAUNCH(cb::inc_emit_kernel, cdiv(p->n_pts, 256), 256, 0, st, (const unsigned long long*)d_mask, (const int*)d_incoff,
                 p->n_pts, nb, d_keys);
-      tbm = std::max(tb_a, tb_b);
-      CB_CUDA(cub::DeviceRadixSort::SortKeys(d_tmp, tbm, d_keys, d_keys_s, (int)n_inc, 0, key_bits, st));
+      CB_CUB(sf, cub::DeviceRadixSort::SortKeys, d_keys, d_keys_s, (int)n_inc, 0, key_bits, st);
       g_launches.fetch_add(5);
       CB_CUDA(cudaMemcpyAsync(d_pair_start, pair_start.data(), sizeof(long long) * pair_start.size(), cudaMemcpyHostToDevice, st));
       CB_CUDA(cudaMemcpyAsync(d_koff, koff_h.data(), sizeof(long long) * koff_h.size(), cudaMemcpyHostToDevice, st));
@@ -1870,7 +1914,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   const double* d_xy = d->obs_xy;
   int *t_cam = nullptr, *t_pt = nullptr;
   double* t_xy = nullptr;
-  ScopedFree stage;  // pinned staging blocks: released when this function returns (it synchronises before)
+  ScopedFree stage(st);  // staging blocks of the observation upload
   XyUpload xy_up;    // declared after `stage`: its destructor joins the staging thread before the pinned blocks go
   if (!d->obs_on_device) {
     CB_TRY(dalloc(&t_cam, n)); CB_TRY(dalloc(&t_pt, n)); CB_TRY(dalloc(&t_xy, 2 * (size_t)n));
@@ -1893,8 +1937,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
     }
     if (d->obs_cam_bits == 16) {
       short* t16 = nullptr;
-      CB_TRY(dalloc(&t16, n));
-      stage.dev.push_back(t16);
+      CB_TRY(stage.alloc(&t16, n));
       CB_TRY(staged_h2d(t16, d->obs_cam, sizeof(short) * (size_t)n, st, stage));
       CB_LAUNCH(cb::widen_i16_kernel, cdiv(n, 256), 256, 0, st, (const short*)t16, n, t_cam);
     } else {
@@ -2128,9 +2171,10 @@ int cb_ba_jacobian_blocks(CbBaProblem* p, const double* x, double* Jc, double* J
   cudaStream_t st = (cudaStream_t)stream;
   const int n = p->n_obs;
   CB_TRY(upload_x(p, x, st));
+  ScopedFree sf(st);
   double *dJc, *dJp;
-  CB_TRY(dalloc(&dJc, 18 * (size_t)std::max(n, 1)));
-  CB_TRY(dalloc(&dJp, 6 * (size_t)std::max(n, 1)));
+  CB_TRY(sf.alloc(&dJc, 18 * (size_t)std::max(n, 1)));
+  CB_TRY(sf.alloc(&dJp, 6 * (size_t)std::max(n, 1)));
   if (p->P == 6) {
     CB_TRY(run_cam_prep<6>(p, p->d_xc[0], p->d_camtab[0], st));
     if (n) CB_LAUNCH((cb::jac_blocks_kernel<6>), cdiv(n, 128), 128, 0, st, p->d_obs_cam, (const int*)p->d_cam_slot, p->d_obs_pt,
@@ -2140,11 +2184,9 @@ int cb_ba_jacobian_blocks(CbBaProblem* p, const double* x, double* Jc, double* J
     if (n) CB_LAUNCH((cb::jac_blocks_kernel<9>), cdiv(n, 128), 128, 0, st, p->d_obs_cam, (const int*)p->d_cam_slot, p->d_obs_pt,
                      reinterpret_cast<const double2*>(p->d_obs_xy), n, (const double*)p->d_camtab[0], (const double*)p->d_xp4[0], dJc, dJp);
   }
-  cudaError_t e1 = cudaMemcpyAsync(Jc, dJc, sizeof(double) * 18 * (size_t)n, cudaMemcpyDeviceToHost, st);
-  cudaError_t e2 = cudaMemcpyAsync(Jp, dJp, sizeof(double) * 6 * (size_t)n, cudaMemcpyDeviceToHost, st);
-  cudaError_t e3 = cudaStreamSynchronize(st);
-  cached_free(dJc); cached_free(dJp);
-  CB_CUDA(e1); CB_CUDA(e2); CB_CUDA(e3);
+  CB_CUDA(cudaMemcpyAsync(Jc, dJc, sizeof(double) * 18 * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(Jp, dJp, sizeof(double) * 6 * (size_t)n, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
   return CB_OK;
 }
 
@@ -2465,37 +2507,32 @@ int cb_debug_fp64_peak(int device, double* dmma_tflops, double* dfma_tflops) {
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
   const int warps = 8, threads = warps * 32, iters = 20000;
   double* out = nullptr;
-  CB_TRY(dalloc(&out, (size_t)sms * threads));
-  ScopedFree sf; sf.dev.push_back(out);
-  cudaEvent_t e0, e1;
-  CB_CUDA(cudaEventCreate(&e0)); CB_CUDA(cudaEventCreate(&e1));
-  float ms = 0.f;
+  ScopedFree sf((cudaStream_t)0);  // the kernels below run on the legacy default stream
+  CB_TRY(sf.alloc(&out, (size_t)sms * threads));
+  StageEvents<2> ev;
+  CB_TRY(ev.create());
   double best_mma = 0.0, best_fma = 0.0;
   for (int rep = 0; rep < 3; ++rep) {
     fp64_dmma_peak_kernel<16><<<sms, threads>>>(out, rep == 0 ? 200 : iters, 1.0000001, 1e-9);
     if (rep == 0) { cudaDeviceSynchronize(); continue; }
-    cudaEventRecord(e0);
+    cudaEventRecord(ev[0]);
     fp64_dmma_peak_kernel<16><<<sms, threads>>>(out, iters, 1.0000001, 1e-9);
-    cudaEventRecord(e1);
-    cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-    best_mma = std::max(best_mma, 2.0 * 256 * 16 * iters * (double)warps * sms / ms * 1e-9);
+    cudaEventRecord(ev[1]);
+    cudaEventSynchronize(ev[1]);
+    best_mma = std::max(best_mma, 2.0 * 256 * 16 * iters * (double)warps * sms / ev.ms(0, 1) * 1e-9);
     // the m16n8k16 shape the off-diagonal Schur tiles issue
     if (rep == 1) fp64_dmma16816_peak_kernel<8><<<sms, threads>>>(out, 200, 1.0000001, 1e-9);
-    cudaEventRecord(e0);
+    cudaEventRecord(ev[0]);
     fp64_dmma16816_peak_kernel<8><<<sms, threads>>>(out, iters / 4, 1.0000001, 1e-9);
-    cudaEventRecord(e1);
-    cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-    best_mma = std::max(best_mma, 2.0 * 2048 * 8 * (iters / 4) * (double)warps * sms / ms * 1e-9);
-    cudaEventRecord(e0);
+    cudaEventRecord(ev[1]);
+    cudaEventSynchronize(ev[1]);
+    best_mma = std::max(best_mma, 2.0 * 2048 * 8 * (iters / 4) * (double)warps * sms / ev.ms(0, 1) * 1e-9);
+    cudaEventRecord(ev[0]);
     fp64_dfma_peak_kernel<16><<<sms, threads>>>(out, iters, 1.0000001, 1e-9);
-    cudaEventRecord(e1);
-    cudaEventSynchronize(e1);
-    cudaEventElapsedTime(&ms, e0, e1);
-    best_fma = std::max(best_fma, 2.0 * 16 * iters * (double)threads * sms / ms * 1e-9);
+    cudaEventRecord(ev[1]);
+    cudaEventSynchronize(ev[1]);
+    best_fma = std::max(best_fma, 2.0 * 16 * iters * (double)threads * sms / ev.ms(0, 1) * 1e-9);
   }
-  cudaEventDestroy(e0); cudaEventDestroy(e1);
   CB_CUDA(cudaGetLastError());
   *dmma_tflops = best_mma;
   *dfma_tflops = best_fma;
@@ -2510,23 +2547,22 @@ int cb_ba_error_order_stats(CbBaProblem* p, const double* x, double q_percent, d
   cudaStream_t st = (cudaStream_t)stream;
   const int n = p->n_obs;
   CB_TRY(p->P == 6 ? (eval_mode<6, 4>(p, x, st)) : (eval_mode<9, 4>(p, x, st)));
+  ScopedFree sf(st);
   double *d_lo, *d_hi;
   long long* d_cnt;
-  CB_TRY(dalloc(&d_lo, p->n_cams)); CB_TRY(dalloc(&d_hi, p->n_cams)); CB_TRY(dalloc(&d_cnt, p->n_cams));
+  CB_TRY(sf.alloc(&d_lo, p->n_cams)); CB_TRY(sf.alloc(&d_hi, p->n_cams)); CB_TRY(sf.alloc(&d_cnt, p->n_cams));
   CB_LAUNCH(cb::order_stats_kernel, p->n_cams, 256, 0, st, p->d_out2, p->d_cam_start, q_percent / 100.0, d_lo, d_hi,
             d_cnt);
   if (err && n) {
     CB_LAUNCH(cb::cm_to_orig_kernel, cdiv(n, 256), 256, 0, st, p->d_out2, p->d_cm_orig, n, p->d_out2 + n);
-    cudaMemcpyAsync(err, p->d_out2 + n, sizeof(double) * n, cudaMemcpyDeviceToHost, st);
+    CB_CUDA(cudaMemcpyAsync(err, p->d_out2 + n, sizeof(double) * n, cudaMemcpyDeviceToHost, st));
   }
   std::vector<long long> hc(p->n_cams);
   std::vector<double> hlo(p->n_cams), hhi(p->n_cams);
-  cudaMemcpyAsync(hlo.data(), d_lo, sizeof(double) * p->n_cams, cudaMemcpyDeviceToHost, st);
-  cudaMemcpyAsync(hhi.data(), d_hi, sizeof(double) * p->n_cams, cudaMemcpyDeviceToHost, st);
-  cudaMemcpyAsync(hc.data(), d_cnt, sizeof(long long) * p->n_cams, cudaMemcpyDeviceToHost, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  cached_free(d_lo); cached_free(d_hi); cached_free(d_cnt);
-  CB_CUDA(e);
+  CB_CUDA(cudaMemcpyAsync(hlo.data(), d_lo, sizeof(double) * p->n_cams, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(hhi.data(), d_hi, sizeof(double) * p->n_cams, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(hc.data(), d_cnt, sizeof(long long) * p->n_cams, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
   for (int i = 0; i < p->n_cams; ++i) {  // internal slot -> caller's camera index
     const int c = p->h_perm[i];
     count[c] = hc[i]; lo[c] = hlo[i]; hi[c] = hhi[i];
@@ -2542,15 +2578,14 @@ int cb_ba_constraint_rows(CbBaProblem* p, const double* x, double* r_out, double
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
   CB_TRY(upload_x(p, x, st));
+  ScopedFree sf(st);
   double *d_r, *d_rs, *d_dir;
-  CB_TRY(dalloc(&d_r, p->n_c)); CB_TRY(dalloc(&d_rs, p->n_c)); CB_TRY(dalloc(&d_dir, 3 * (size_t)p->n_c));
+  CB_TRY(sf.alloc(&d_r, p->n_c)); CB_TRY(sf.alloc(&d_rs, p->n_c)); CB_TRY(sf.alloc(&d_dir, 3 * (size_t)p->n_c));
   CB_LAUNCH((cb::constraint_eval_kernel<false>), p->n_cblk, cb::CC_THREADS, 0, st, (const cb::LmState*)nullptr, 0, p->ct,
             p->c_xp(), 0, 1.0, (cb::Ptr2{{d_rs, d_rs}}), (cb::Ptr2{{d_dir, d_dir}}), d_r, (double*)nullptr);
-  cudaMemcpyAsync(r_out, d_r, sizeof(double) * p->n_c, cudaMemcpyDeviceToHost, st);
-  if (dir_out) cudaMemcpyAsync(dir_out, d_dir, sizeof(double) * 3 * (size_t)p->n_c, cudaMemcpyDeviceToHost, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  cached_free(d_r); cached_free(d_rs); cached_free(d_dir);
-  CB_CUDA(e);
+  CB_CUDA(cudaMemcpyAsync(r_out, d_r, sizeof(double) * p->n_c, cudaMemcpyDeviceToHost, st));
+  if (dir_out) CB_CUDA(cudaMemcpyAsync(dir_out, d_dir, sizeof(double) * 3 * (size_t)p->n_c, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
   return CB_OK;
 }
 
@@ -2561,17 +2596,16 @@ int cb_ba_rmse_px(CbBaProblem* p, const double* x, double* overall, double* per_
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
   CB_TRY(p->P == 6 ? (eval_mode<6, 4>(p, x, st)) : (eval_mode<9, 4>(p, x, st)));
+  ScopedFree sf(st);
   double* d_ss;
-  CB_TRY(dalloc(&d_ss, p->n_cams));
+  CB_TRY(sf.alloc(&d_ss, p->n_cams));
   CB_LAUNCH(cb::cam_err_stats_kernel, p->n_cams, 256, 0, st, p->d_out2, p->d_cam_start, (const double*)nullptr,
             (long long*)nullptr, d_ss);
   std::vector<double> ss(p->n_cams);
   std::vector<int> cs(p->n_cams + 1);
-  cudaMemcpyAsync(ss.data(), d_ss, sizeof(double) * p->n_cams, cudaMemcpyDeviceToHost, st);
-  cudaMemcpyAsync(cs.data(), p->d_cam_start, sizeof(int) * (p->n_cams + 1), cudaMemcpyDeviceToHost, st);
-  cudaError_t e = cudaStreamSynchronize(st);
-  cached_free(d_ss);
-  CB_CUDA(e);
+  CB_CUDA(cudaMemcpyAsync(ss.data(), d_ss, sizeof(double) * p->n_cams, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(cs.data(), p->d_cam_start, sizeof(int) * (p->n_cams + 1), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
   double tot = 0.0;
   for (int c = 0; c < p->n_cams; ++c) {
     tot += ss[c];
@@ -2598,14 +2632,14 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
   long long* d_kept;
   unsigned char* d_flag;
   int *d_iota, *d_sel, *d_nsel;
-  ScopedFree sf;  // every early return below releases the temporaries
-  CB_TRY(dalloc(&d_thr, nc)); sf.dev.push_back(d_thr);
-  CB_TRY(dalloc(&d_ss, nc)); sf.dev.push_back(d_ss);
-  CB_TRY(dalloc(&d_kept, nc)); sf.dev.push_back(d_kept);
-  CB_TRY(dalloc(&d_flag, n)); sf.dev.push_back(d_flag);
-  CB_TRY(dalloc(&d_iota, n)); sf.dev.push_back(d_iota);
-  CB_TRY(dalloc(&d_sel, n)); sf.dev.push_back(d_sel);
-  CB_TRY(dalloc(&d_nsel, 1)); sf.dev.push_back(d_nsel);
+  ScopedFree sf(st);
+  CB_TRY(sf.alloc(&d_thr, nc));
+  CB_TRY(sf.alloc(&d_ss, nc));
+  CB_TRY(sf.alloc(&d_kept, nc));
+  CB_TRY(sf.alloc(&d_flag, n));
+  CB_TRY(sf.alloc(&d_iota, n));
+  CB_TRY(sf.alloc(&d_sel, n));
+  CB_TRY(sf.alloc(&d_nsel, 1));
   std::vector<double> thr(nc);
   for (int i = 0; i < nc; ++i) thr[i] = thresholds[p->h_perm[i]];  // by internal camera slot
   std::vector<long long> kept(nc);
@@ -2636,12 +2670,7 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
   CB_LAUNCH(cb::keep_flag_kernel, cdiv(n, 256), 256, 0, st, p->d_out2, p->d_cm_orig, p->d_cam_start, nc,
             (const double*)d_thr, n, d_flag);
   CB_LAUNCH(cb::iota_kernel, cdiv(n, 256), 256, 0, st, d_iota, n);
-  size_t tb = 0;
-  cub::DeviceSelect::Flagged(nullptr, tb, d_iota, d_flag, d_sel, d_nsel, n, st);
-  void* d_tmp;
-  CB_TRY(cached_malloc(&d_tmp, std::max<size_t>(tb, 16)));
-  sf.dev.push_back(d_tmp);
-  CB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb, d_iota, d_flag, d_sel, d_nsel, n, st));
+  CB_CUB(sf, cub::DeviceSelect::Flagged, d_iota, d_flag, d_sel, d_nsel, n, st);
   g_launches.fetch_add(2);
   int nsel = 0;
   CB_CUDA(cudaMemcpyAsync(&nsel, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -2712,16 +2741,14 @@ template <typename T>
 int to_device(const T* src, size_t n, int on_device, const T** out, ScopedFree& sf, cudaStream_t st) {
   if (on_device) { *out = src; return CB_OK; }
   T* d = nullptr;
-  CB_TRY(dalloc(&d, n));
-  sf.dev.push_back(d);
+  CB_TRY(sf.alloc(&d, n));
   if (sizeof(T) * n >= ((size_t)2 << 20)) {  // large arrays: pool threads stage, the DMA is queued block by block
     CB_TRY(staged_h2d(d, src, sizeof(T) * n, st, sf, 8));
     *out = d;
     return CB_OK;
   }
   T* h = nullptr;
-  CB_TRY(cached_malloc_host((void**)&h, sizeof(T) * std::max<size_t>(n, 1)));
-  sf.host.push_back(h);
+  CB_TRY(sf.alloc_pinned(&h, n));
   stream_copy(h, src, sizeof(T) * n);  // non-temporal: the DMA reads it next (see stream_copy)
   CB_CUDA(cudaMemcpyAsync(d, h, sizeof(T) * n, cudaMemcpyHostToDevice, st));
   *out = d;
@@ -2731,11 +2758,9 @@ int to_device(const T* src, size_t n, int on_device, const T** out, ScopedFree& 
 // host doubles -> device floats, converted while staging into the pinned bounce buffer
 int to_device_f32(const double* src, size_t n, const float** out, ScopedFree& sf, cudaStream_t st) {
   float* d = nullptr;
-  CB_TRY(dalloc(&d, n));
-  sf.dev.push_back(d);
+  CB_TRY(sf.alloc(&d, n));
   float* h = nullptr;
-  CB_TRY(cached_malloc_host((void**)&h, sizeof(float) * std::max<size_t>(n, 1)));
-  sf.host.push_back(h);
+  CB_TRY(sf.alloc_pinned(&h, n));
   const size_t chunk = (size_t)1 << 20;  // elements
   for (size_t off = 0; off < n; off += chunk) {
     const size_t m = std::min(chunk, n - off);
@@ -2746,19 +2771,28 @@ int to_device_f32(const double* src, size_t n, const float** out, ScopedFree& sf
   return CB_OK;
 }
 
-int validate_rows(const int* d_cam, const long long* d_key, long long n, int n_cams, cudaStream_t st, const char* who) {
+int validate_rows(const int* d_cam, const long long* d_key, long long n, int n_cams, const char* who, ScopedFree& sf,
+                  cudaStream_t st) {
   int* d_bad = nullptr;
-  CB_TRY(dalloc(&d_bad, 1));
+  CB_TRY(sf.alloc(&d_bad, 1));
   CB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
   CB_LAUNCH(cb::tri_validate_kernel, cdiv(n, 256), 256, 0, st, d_cam, d_key, n, n_cams, d_bad);
   int bad = 0;
   CB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
-  cached_free(d_bad);
   if (bad) {
     g_last_error = std::string(who) + ": camera index out of range or negative group key in " + std::to_string(bad) + " rows";
     return CB_E_INVALID;
   }
+  return CB_OK;
+}
+
+// the undistortion table on the device (`tab` must outlive the queued copy: the call's workspace waits for it)
+int upload_undist_table(const std::vector<cb::UndistCam>& tab, ScopedFree& sf, cudaStream_t st, const cb::UndistCam** out) {
+  cb::UndistCam* d_tab = nullptr;
+  CB_TRY(sf.alloc(&d_tab, tab.size()));
+  CB_CUDA(cudaMemcpyAsync(d_tab, tab.data(), sizeof(cb::UndistCam) * tab.size(), cudaMemcpyHostToDevice, st));
+  *out = d_tab;
   return CB_OK;
 }
 
@@ -2777,13 +2811,11 @@ int cb_undistort_points(int32_t n_cams, const int32_t* cam_fisheye, const double
   CB_TRY(select_device(device));
   if (n == 0) return CB_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
   std::vector<cb::UndistCam> tab;
   CB_TRY(build_undist_table(n_cams, cam_fisheye, cam_k, cam_dist, tab));
-  cb::UndistCam* d_tab = nullptr;
-  CB_TRY(dalloc(&d_tab, (size_t)n_cams));
-  sf.dev.push_back(d_tab);
-  CB_CUDA(cudaMemcpyAsync(d_tab, tab.data(), sizeof(cb::UndistCam) * n_cams, cudaMemcpyHostToDevice, st));
+  ScopedFree sf(st);
+  const cb::UndistCam* d_tab = nullptr;
+  CB_TRY(upload_undist_table(tab, sf, st, &d_tab));
   const int* d_cam = nullptr;
   const double* d_in = nullptr;
   if (obs_cam) CB_TRY(to_device(obs_cam, (size_t)n, on_device, &d_cam, sf, st));
@@ -2791,22 +2823,17 @@ int cb_undistort_points(int32_t n_cams, const int32_t* cam_fisheye, const double
   double* d_out = xy_out;
   double* h_out = nullptr;
   if (!on_device) {
-    CB_TRY(dalloc(&d_out, 2 * (size_t)n));
-    sf.dev.push_back(d_out);
-    CB_TRY(cached_malloc_host((void**)&h_out, sizeof(double) * 2 * (size_t)n));
-    sf.host.push_back(h_out);
+    CB_TRY(sf.alloc(&d_out, 2 * (size_t)n));
+    CB_TRY(sf.alloc_pinned(&h_out, 2 * (size_t)n));
   }
-  if (d_cam) CB_TRY(validate_rows(d_cam, nullptr, n, n_cams, st, "cb_undistort_points"));
+  if (d_cam) CB_TRY(validate_rows(d_cam, nullptr, n, n_cams, "cb_undistort_points", sf, st));
   CB_LAUNCH(cb::undistort_kernel<double>, cdiv(n, 256), 256, 0, st, d_tab, d_cam, d_in, d_out, (long long)n,
             to_pixels ? 1 : 0);
   CB_CUDA(cudaGetLastError());
-  if (!on_device) {
+  if (!on_device)
     CB_CUDA(cudaMemcpyAsync(h_out, d_out, sizeof(double) * 2 * (size_t)n, cudaMemcpyDeviceToHost, st));
-    CB_CUDA(cudaStreamSynchronize(st));
-    std::memcpy(xy_out, h_out, sizeof(double) * 2 * (size_t)n);
-  } else {
-    CB_CUDA(cudaStreamSynchronize(st));  // the camera table is a stack-lifetime upload
-  }
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (!on_device) std::memcpy(xy_out, h_out, sizeof(double) * 2 * (size_t)n);
   return CB_OK;
 }
 
@@ -2814,44 +2841,67 @@ int cb_undistort_points(int32_t n_cams, const int32_t* cam_fisheye, const double
 
 namespace {
 
-int group_by_key(const long long* d_key, int n, cudaStream_t st, ScopedFree& sf, int** d_rows, int** d_start, int* n_groups);
+// stable sort of the rows by key, group boundaries: d_rows (n), d_start (n_groups + 1)
+int group_by_key(const long long* d_key, int n, cudaStream_t st, ScopedFree& sf, int** d_rows, int** d_start, int* n_groups) {
+  const int TB = 256, G = cdiv(n, TB);
+  unsigned long long* k_out = nullptr;
+  int *v_in = nullptr, *v_out = nullptr, *d_head = nullptr, *d_gid = nullptr, *dstart = nullptr;
+  CB_TRY(sf.alloc(&k_out, (size_t)n));
+  CB_TRY(sf.alloc(&v_in, (size_t)n));
+  CB_TRY(sf.alloc(&v_out, (size_t)n));
+  CB_TRY(sf.alloc(&d_head, (size_t)n));
+  CB_TRY(sf.alloc(&d_gid, (size_t)n));
+  CB_TRY(sf.alloc(&dstart, (size_t)n + 1));
+  CB_LAUNCH(cb::tri_iota_kernel, G, TB, 0, st, v_in, (long long)n);
+  // radix passes only over the key's significant bits (a packed (sync, object, keypoint) key of a 50k-point rig has 16)
+  unsigned long long* d_max = nullptr;
+  CB_TRY(sf.alloc(&d_max, 1));
+  CB_CUB(sf, cub::DeviceReduce::Max, (const unsigned long long*)d_key, d_max, n, st);
+  unsigned long long h_max = 0;
+  CB_CUDA(cudaMemcpyAsync(&h_max, d_max, sizeof(h_max), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  const int key_bits = std::min(63, bits_for(h_max));
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, (const unsigned long long*)d_key, k_out, v_in, v_out, n, 0, key_bits, st);
+  g_launches.fetch_add(2 + 2 * ((key_bits + 7) / 8));
+  CB_LAUNCH(cb::tri_heads_kernel, G, TB, 0, st, k_out, (long long)n, d_head);
+  CB_CUB(sf, cub::DeviceScan::InclusiveSum, d_head, d_gid, n, st);
+  g_launches.fetch_add(2);
+  CB_LAUNCH(cb::tri_starts_kernel, G, TB, 0, st, d_head, d_gid, (long long)n, dstart);
+  CB_CUDA(cudaMemcpyAsync(n_groups, d_gid + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  *d_rows = v_out;
+  *d_start = dstart;
+  return CB_OK;
+}
 
-// device-side result of the grouping and the DLT (buffers owned by the caller's ScopedFree)
-struct TriDlt {
+// the rows of an array-level call on the device, grouped by key (buffers held by the call's workspace)
+struct ObsGroups {
   const int* cam = nullptr;   // obs_cam on the device
-  const double* xy = nullptr; // the DLT's coordinates on the device (undistorted and float32-rounded with `undist`)
-  double* proj = nullptr;     // [n_cams][3][4] projection matrices on the device
+  const double* xy = nullptr; // the coordinates on the device (undistorted to the normalised plane with `undist`)
   int* rows = nullptr;        // caller rows sorted by key (stable)
   int* start = nullptr;       // group boundaries, n_groups + 1
   int n_groups = 0;
-  int lanes = 8;              // lanes per group of the DLT kernel (8, or 32 when groups average > 96 rows)
-  double* xyz = nullptr;
-  int* count = nullptr;
-  int* rep = nullptr;
-  unsigned long long* sig = nullptr;
 };
 
-// upload + validation + (undistortion) + grouping, the stages every triangulation call shares.  Records ev[1] after the
-// grouping.  `undist` non-null = obs_xy are raw pixels, undistorted on the device (normalised output), never leaving HBM.
-int tri_group_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int n,
-                    const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
-                    int32_t max_groups, int32_t* n_groups_out, const char* who, cudaEvent_t* ev, ScopedFree& sf,
-                    cudaStream_t st, TriDlt* out) {
+// Upload + validation + (undistortion) + grouping, the observation stage of every call that groups rows by key.  Records
+// `ev` after the grouping, reports the group count and refuses more than max_groups groups.  `undist` non-null = obs_xy
+// are raw pixels, undistorted on the device to the normalised plane, never leaving HBM.
+int obs_group_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, int n, const int32_t* obs_cam,
+                    const int64_t* obs_key, const double* obs_xy, int obs_on_device, int32_t max_groups,
+                    int32_t* n_groups_out, const char* who, cudaEvent_t ev, ScopedFree& sf, cudaStream_t st,
+                    ObsGroups* out) {
   const int TB = 256, G = cdiv(n, TB);
   const int* d_cam = nullptr;
   const long long* d_key = nullptr;
   const double* d_xy = nullptr;
   CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
   CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
-  CB_TRY(validate_rows(d_cam, d_key, n, n_cams, st, who));
+  CB_TRY(validate_rows(d_cam, d_key, n, n_cams, who, sf, st));
   if (undist) {
-    cb::UndistCam* d_tab = nullptr;
-    CB_TRY(dalloc(&d_tab, (size_t)n_cams));
-    sf.dev.push_back(d_tab);
-    CB_CUDA(cudaMemcpyAsync(d_tab, undist->data(), sizeof(cb::UndistCam) * n_cams, cudaMemcpyHostToDevice, st));
+    const cb::UndistCam* d_tab = nullptr;
+    CB_TRY(upload_undist_table(*undist, sf, st, &d_tab));
     double* d_und = nullptr;
-    CB_TRY(dalloc(&d_und, 2 * (size_t)n));
-    sf.dev.push_back(d_und);
+    CB_TRY(sf.alloc(&d_und, 2 * (size_t)n));
     if (obs_on_device) {
       CB_LAUNCH(cb::undistort_kernel<double>, G, TB, 0, st, d_tab, d_cam, obs_xy, d_und, (long long)n, 0);
     } else {
@@ -2865,15 +2915,11 @@ int tri_group_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, co
   } else {
     CB_TRY(to_device(obs_xy, 2 * (size_t)n, obs_on_device, &d_xy, sf, st));
   }
-  double* d_proj = nullptr;
-  CB_TRY(dalloc(&d_proj, 12 * (size_t)n_cams));
-  sf.dev.push_back(d_proj);
-  CB_CUDA(cudaMemcpyAsync(d_proj, proj, sizeof(double) * 12 * (size_t)n_cams, cudaMemcpyHostToDevice, st));
 
   // (1) stable radix sort of (key, row) -> rows of one group adjacent, in caller order inside the group; (2) boundaries
   int *v_out = nullptr, *d_start = nullptr, n_groups = 0;
   CB_TRY(group_by_key(d_key, n, st, sf, &v_out, &d_start, &n_groups));
-  CB_CUDA(cudaEventRecord(ev[1], st));
+  CB_CUDA(cudaEventRecord(ev, st));
   *n_groups_out = n_groups;
   if (n_groups > max_groups) {
     g_last_error = std::string(who) + ": " + std::to_string(n_groups) + " groups but room for " + std::to_string(max_groups);
@@ -2881,56 +2927,45 @@ int tri_group_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, co
   }
   out->cam = d_cam;
   out->xy = d_xy;
-  out->proj = d_proj;
   out->rows = v_out;
   out->start = d_start;
   out->n_groups = n_groups;
-  // 8 lanes per group: the serial 4x4 eigen-solve of one lane per group, not the gather, bounds the DLT kernel, so
-  // more groups per warp wins until groups get very long
-  out->lanes = (n / std::max(n_groups, 1) > 96) ? 32 : 8;
   return CB_OK;
 }
 
-// the DLT of every group of `t`, ev[2] / ev[3] around the kernel
-int tri_dlt_launch(int32_t n_cams, cudaEvent_t* ev, ScopedFree& sf, cudaStream_t st, TriDlt* t) {
-  const int n_groups = t->n_groups, lanes = t->lanes;
-  const int* d_cam = t->cam;
-  const double* d_xy = t->xy;
-  const double* d_proj = t->proj;
-  const int *d_start = t->start, *v_out = t->rows;
-  double* d_xyz = nullptr;
-  int *d_count = nullptr, *d_rep = nullptr;
-  unsigned long long* d_sig = nullptr;
-  CB_TRY(dalloc(&d_xyz, 3 * (size_t)n_groups)); sf.dev.push_back(d_xyz);
-  CB_TRY(dalloc(&d_count, (size_t)n_groups)); sf.dev.push_back(d_count);
-  CB_TRY(dalloc(&d_rep, (size_t)n_groups)); sf.dev.push_back(d_rep);
-  CB_TRY(dalloc(&d_sig, 2 * (size_t)n_groups)); sf.dev.push_back(d_sig);
+// Lanes per group of the triangulation kernels.  8: the serial 4x4 eigen-solve of one lane per group, not the gather,
+// bounds the DLT kernel, so more groups per warp wins until groups get very long (more than 96 rows on average).
+int tri_lanes(int n, int n_groups) { return (n / std::max(n_groups, 1) > 96) ? 32 : 8; }
+
+// the DLT of every group (buffers held by the call's workspace)
+struct TriDlt {
+  double* xyz = nullptr;
+  int* count = nullptr;
+  int* rep = nullptr;
+  unsigned long long* sig = nullptr;
+};
+
+// the DLT of every group of `g` with the [n_cams][3][4] projection matrices d_proj, ev_a / ev_b around the kernel
+int tri_dlt_launch(int32_t n_cams, const double* d_proj, const ObsGroups& g, int lanes, cudaEvent_t ev_a,
+                   cudaEvent_t ev_b, ScopedFree& sf, cudaStream_t st, TriDlt* t) {
+  const int n_groups = g.n_groups;
+  CB_TRY(sf.alloc(&t->xyz, 3 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&t->count, (size_t)n_groups));
+  CB_TRY(sf.alloc(&t->rep, (size_t)n_groups));
+  CB_TRY(sf.alloc(&t->sig, 2 * (size_t)n_groups));
   const size_t proj_bytes = sizeof(double) * 13 * (size_t)n_cams;  // padded stride, see tri_dlt_kernel
   const int in_smem = proj_bytes <= 40 * 1024 ? 1 : 0;
   const long long threads = (long long)n_groups * lanes;
-  CB_CUDA(cudaEventRecord(ev[2], st));
+  CB_CUDA(cudaEventRecord(ev_a, st));
   if (lanes == 32)
     CB_LAUNCH(cb::tri_dlt_kernel<32>, cdiv(threads, cb::TRI_THREADS), cb::TRI_THREADS, in_smem ? proj_bytes : 0, st,
-              d_proj, n_cams, in_smem, d_start, v_out, d_cam, d_xy, n_groups, d_xyz, d_count, d_rep, d_sig);
+              d_proj, n_cams, in_smem, g.start, g.rows, g.cam, g.xy, n_groups, t->xyz, t->count, t->rep, t->sig);
   else
     CB_LAUNCH(cb::tri_dlt_kernel<8>, cdiv(threads, cb::TRI_THREADS), cb::TRI_THREADS, in_smem ? proj_bytes : 0, st,
-              d_proj, n_cams, in_smem, d_start, v_out, d_cam, d_xy, n_groups, d_xyz, d_count, d_rep, d_sig);
+              d_proj, n_cams, in_smem, g.start, g.rows, g.cam, g.xy, n_groups, t->xyz, t->count, t->rep, t->sig);
   CB_CUDA(cudaGetLastError());
-  CB_CUDA(cudaEventRecord(ev[3], st));
-  t->xyz = d_xyz;
-  t->count = d_count;
-  t->rep = d_rep;
-  t->sig = d_sig;
+  CB_CUDA(cudaEventRecord(ev_b, st));
   return CB_OK;
-}
-
-int tri_dlt_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, const double* proj, int n,
-                  const int32_t* obs_cam, const int64_t* obs_key, const double* obs_xy, int obs_on_device,
-                  int32_t max_groups, int32_t* n_groups_out, const char* who, cudaEvent_t* ev, ScopedFree& sf,
-                  cudaStream_t st, TriDlt* out) {
-  CB_TRY(tri_group_stage(n_cams, undist, proj, n, obs_cam, obs_key, obs_xy, obs_on_device, max_groups, n_groups_out, who,
-                         ev, sf, st, out));
-  return tri_dlt_launch(n_cams, ev, sf, st, out);
 }
 
 // Cameras of the calibrated triangulation calls, given in the bundle-adjustment layout (x: [r t] or [r t s k1 k2] per
@@ -3005,12 +3040,12 @@ int tri_cams_upload(int32_t n_cams, const int32_t* cam_flags, const double* cam_
   const int P = c->P, ncp = c->ncp;
   int *d_flags = nullptr, *d_xoff = nullptr;
   double *d_const = nullptr, *d_x = nullptr, *d_xc = nullptr, *d_camtab = nullptr;
-  CB_TRY(dalloc(&d_flags, (size_t)n_cams)); sf.dev.push_back(d_flags);
-  CB_TRY(dalloc(&d_xoff, (size_t)n_cams)); sf.dev.push_back(d_xoff);
-  CB_TRY(dalloc(&d_const, 9 * (size_t)n_cams)); sf.dev.push_back(d_const);
-  CB_TRY(dalloc(&d_x, (size_t)ncp)); sf.dev.push_back(d_x);
-  CB_TRY(dalloc(&d_xc, (size_t)P * n_cams)); sf.dev.push_back(d_xc);
-  CB_TRY(dalloc(&d_camtab, (size_t)cb::CT_SIZE * n_cams)); sf.dev.push_back(d_camtab);
+  CB_TRY(sf.alloc(&d_flags, (size_t)n_cams));
+  CB_TRY(sf.alloc(&d_xoff, (size_t)n_cams));
+  CB_TRY(sf.alloc(&d_const, 9 * (size_t)n_cams));
+  CB_TRY(sf.alloc(&d_x, (size_t)ncp));
+  CB_TRY(sf.alloc(&d_xc, (size_t)P * n_cams));
+  CB_TRY(sf.alloc(&d_camtab, (size_t)cb::CT_SIZE * n_cams));
   CB_CUDA(cudaMemcpyAsync(d_flags, cam_flags, sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaMemcpyAsync(d_xoff, c->xoff.data(), sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaMemcpyAsync(d_const, cam_const, sizeof(double) * 9 * n_cams, cudaMemcpyHostToDevice, st));
@@ -3027,6 +3062,68 @@ int tri_cams_upload(int32_t n_cams, const int32_t* cam_flags, const double* cam_
 size_t tri_camtab_smem(int32_t n_cams) {
   const size_t cam_bytes = sizeof(double) * cb::CT_SMEM * (size_t)n_cams;
   return cam_bytes <= 40 * 1024 ? cam_bytes : 0;
+}
+
+// robust triangulation's consensus rule (cb_triangulate_robust) and its outputs beyond the refinement's
+struct TriConsensusArgs {
+  double threshold_px;
+  int32_t min_inliers, max_pairs;
+  int32_t* n_inliers_out;
+  uint8_t* inlier_out;
+};
+
+// the consensus of every group of `g` and the compaction of its rows (buffers held by the call's workspace)
+struct TriConsensus {
+  double* hyp = nullptr;         // the selected hypothesis of every group
+  int *count = nullptr, *rep = nullptr, *nin = nullptr, *status = nullptr;
+  unsigned char* inl = nullptr;  // caller-order inlier mask
+  int *rows = nullptr, *start = nullptr;  // the consensus rows of every group, in key-sorted order, and their group starts
+};
+
+// tri_consensus_kernel over the groups of `g`, then the compaction of the consensus rows; ev_a / ev_b around both
+int tri_consensus_launch(int32_t n_cams, const TriCams& cams, const double* d_proj, const ObsGroups& g, int lanes, int n,
+                         const double* px, const TriConsensusArgs& a, cudaEvent_t ev_a, cudaEvent_t ev_b, ScopedFree& sf,
+                         cudaStream_t st, TriConsensus* c) {
+  const int n_groups = g.n_groups;
+  // hypothesis, count, rep_row, n_inliers (+ a zero past the end for the scan), status 0 / 1 / 5, flags
+  unsigned char* d_flag = nullptr;
+  int* d_nsel = nullptr;
+  CB_TRY(sf.alloc(&c->hyp, 3 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&c->count, (size_t)n_groups));
+  CB_TRY(sf.alloc(&c->rep, (size_t)n_groups));
+  CB_TRY(sf.alloc(&c->nin, (size_t)n_groups + 1));
+  CB_TRY(sf.alloc(&c->status, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_flag, (size_t)n));
+  CB_TRY(sf.alloc(&c->inl, (size_t)n));
+  CB_TRY(sf.alloc(&c->rows, (size_t)n));
+  CB_TRY(sf.alloc(&c->start, (size_t)n_groups + 1));
+  CB_TRY(sf.alloc(&d_nsel, 1));
+
+  // camera table and projection table each in shared memory when it takes at most 40 KB
+  const size_t cam_smem = tri_camtab_smem(n_cams);
+  const size_t proj_bytes = sizeof(double) * 13 * (size_t)n_cams;  // padded stride, see tri_dlt_kernel
+  const size_t proj_smem = proj_bytes <= 40 * 1024 ? proj_bytes : 0;
+  const size_t smem = cam_smem + proj_smem;
+  if (smem > 48 * 1024) {
+    CB_CUDA(cudaFuncSetAttribute(cb::tri_consensus_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CB_CUDA(cudaFuncSetAttribute(cb::tri_consensus_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
+  CB_CUDA(cudaMemsetAsync(c->nin + n_groups, 0, sizeof(int), st));
+  CB_CUDA(cudaEventRecord(ev_a, st));
+#define CB_TRI_CONSENSUS(LL)                                                                                           \
+  CB_LAUNCH(cb::tri_consensus_kernel<LL>, blocks, cb::TRI_THREADS, smem, st, cams.camtab, cam_smem ? 1 : 0, d_proj,     \
+            proj_smem ? 1 : 0, n_cams, g.start, g.rows, g.cam, g.xy, px, n_groups, a.threshold_px, a.min_inliers,       \
+            a.max_pairs, c->hyp, c->count, c->rep, c->nin, c->status, d_flag, c->inl)
+  if (lanes == 32) CB_TRI_CONSENSUS(32);
+  else CB_TRI_CONSENSUS(8);
+#undef CB_TRI_CONSENSUS
+  CB_CUDA(cudaGetLastError());
+  CB_CUB(sf, cub::DeviceSelect::Flagged, g.rows, d_flag, c->rows, d_nsel, n, st);
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, c->nin, c->start, n_groups + 1, st);
+  g_launches.fetch_add(4);
+  CB_CUDA(cudaEventRecord(ev_b, st));
+  return CB_OK;
 }
 
 // tri_refine_kernel over the row list (start, rows) from xyz0
@@ -3065,14 +3162,14 @@ int tri_cov_launch(int32_t n_cams, const TriCams& c, const double* cam_cov, doub
         for (int d = 0; d < n_cams; ++d)
           for (int q = 0; q < xoff[d + 1] - xoff[d]; ++q)
             sig[((size_t)a * P + p) * nP + (size_t)d * P + q] = cam_cov[(size_t)(xoff[a] + p) * ncp + xoff[d] + q];
-    CB_TRY(dalloc(&d_sig, nP * nP)); sf.dev.push_back(d_sig);
+    CB_TRY(sf.alloc(&d_sig, nP * nP));
     CB_CUDA(cudaMemcpyAsync(d_sig, sig.data(), sizeof(double) * nP * nP, cudaMemcpyHostToDevice, st));
-    CB_TRY(dalloc(&d_B, 3 * (size_t)P * n)); sf.dev.push_back(d_B);
-    CB_TRY(dalloc(&d_first, (size_t)n)); sf.dev.push_back(d_first);
+    CB_TRY(sf.alloc(&d_B, 3 * (size_t)P * n));
+    CB_TRY(sf.alloc(&d_first, (size_t)n));
     CB_CUDA(cudaStreamSynchronize(st));  // `sig` is a stack-lifetime upload
   }
   double* d_cov = nullptr;
-  CB_TRY(dalloc(&d_cov, 9 * (size_t)n_groups)); sf.dev.push_back(d_cov);
+  CB_TRY(sf.alloc(&d_cov, 9 * (size_t)n_groups));
   const double s2 = pixel_sigma * pixel_sigma;
   const size_t smem = tri_camtab_smem(n_cams);
   const int cam_in_smem = smem ? 1 : 0;
@@ -3108,16 +3205,20 @@ int triangulate_impl(int32_t n_cams, const std::vector<cb::UndistCam>* undist, c
   if (stats) std::memset(stats, 0, sizeof(*stats));
   if (n_obs == 0) return CB_OK;
   const long long launches0 = g_launches.load();
+  const int n = (int)n_obs;
   cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
-  cudaEvent_t ev[4];
-  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  ScopedFree sf(st);
+  StageEvents<4> ev;
+  CB_TRY(ev.create());
   CB_CUDA(cudaEventRecord(ev[0], st));
+  const double* d_proj = nullptr;
+  CB_TRY(to_device(proj, 12 * (size_t)n_cams, 0, &d_proj, sf, st));
+  ObsGroups g;
+  CB_TRY(obs_group_stage(n_cams, undist, n, obs_cam, obs_key, obs_xy, obs_on_device, max_groups, n_groups_out,
+                         "cb_triangulate_dlt", ev[1], sf, st, &g));
   TriDlt t;
-  CB_TRY(tri_dlt_stage(n_cams, undist, proj, (int)n_obs, obs_cam, obs_key, obs_xy, obs_on_device, max_groups,
-                       n_groups_out, "cb_triangulate_dlt", ev, sf, st, &t));
-  const int n_groups = t.n_groups;
+  CB_TRY(tri_dlt_launch(n_cams, d_proj, g, tri_lanes(n, g.n_groups), ev[2], ev[3], sf, st, &t));
+  const int n_groups = g.n_groups;
   CB_CUDA(cudaMemcpyAsync(xyz_out, t.xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(count_out, t.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(rep_row_out, t.rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
@@ -3125,10 +3226,107 @@ int triangulate_impl(int32_t n_cams, const std::vector<cb::UndistCam>* undist, c
                           cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   if (stats) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
-    cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->dlt_ms = ms;
-    cudaEventElapsedTime(&ms, ev[0], ev[3]); stats->total_ms = ms;
+    stats->group_ms = ev.ms(0, 1);
+    stats->dlt_ms = ev.ms(2, 3);
+    stats->total_ms = ev.ms(0, 3);
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
+}
+
+static_assert(sizeof(CbTriRefineStats) == sizeof(CbTriRobustStats) &&
+                  offsetof(CbTriRefineStats, dlt_ms) == offsetof(CbTriRobustStats, consensus_ms) &&
+                  offsetof(CbTriRefineStats, kernel_launches) == offsetof(CbTriRobustStats, kernel_launches),
+              "the calibrated triangulation calls fill one stats layout");
+
+// Shared body of cb_triangulate_refine / cb_triangulate_robust after their argument checks: upload, undistortion and
+// grouping, the start of every group, the refinement and the covariance.  The start is the DLT of all rows of a group,
+// or with `robust` the hypothesis of the view-pair consensus, and then only the consensus rows go on: a DLT over the
+// whole group would be contaminated by the outliers.  The start's time goes to the stats' second field (dlt_ms /
+// consensus_ms).
+int tri_calibrated(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                   const double* cam_cov, int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key,
+                   const double* obs_px, int obs_on_device, const TriConsensusArgs* robust, double pixel_sigma,
+                   int32_t max_iter, double xtol, int32_t max_groups, int32_t* n_groups_out, double* xyz_out,
+                   double* cov_out, double* rmse_px_out, int32_t* count_out, int32_t* rep_row_out, int32_t* status_out,
+                   CbTriRefineStats* stats, const char* who, int device, void* stream) {
+  TriCams cams;
+  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, who, &cams));
+  CB_TRY(select_device(device));
+  *n_groups_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf(st);
+  const int n = (int)n_obs;
+  StageEvents<8> ev;
+  CB_TRY(ev.create());
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  // fp64 pixels on the device: the refinement reads them at full precision
+  const int* d_cam = nullptr;
+  const long long* d_key = nullptr;
+  const double *d_px = nullptr, *d_proj = nullptr;
+  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
+  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
+  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
+  CB_TRY(to_device(cams.proj.data(), cams.proj.size(), 0, &d_proj, sf, st));
+  ObsGroups g;
+  CB_TRY(obs_group_stage(n_cams, &cams.tab, n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups, n_groups_out, who,
+                         ev[1], sf, st, &g));
+  const int n_groups = g.n_groups, lanes = tri_lanes(n, n_groups);
+  const double* xyz0 = nullptr;
+  const int *count = nullptr, *rep = nullptr, *start = g.start, *rows = g.rows;
+  TriConsensus cs;
+  if (robust) {
+    CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
+    CB_TRY(tri_consensus_launch(n_cams, cams, d_proj, g, lanes, n, d_px, *robust, ev[2], ev[3], sf, st, &cs));
+    xyz0 = cs.hyp; count = cs.count; rep = cs.rep; start = cs.start; rows = cs.rows;
+  } else {
+    TriDlt t;
+    CB_TRY(tri_dlt_launch(n_cams, d_proj, g, lanes, ev[2], ev[3], sf, st, &t));
+    CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
+    xyz0 = t.xyz; count = t.count; rep = t.rep;
+  }
+
+  // refinement and covariance from the starts; a status-5 group of the consensus has no rows, so the refinement reports
+  // 1 for it and the covariance is NaN
+  double *d_out_xyz = nullptr, *d_rmse = nullptr;
+  int* d_status = nullptr;
+  CB_TRY(sf.alloc(&d_out_xyz, 3 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_rmse, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_status, (size_t)n_groups));
+  CB_CUDA(cudaEventRecord(ev[4], st));
+  CB_TRY(tri_refine_launch(n_cams, cams, lanes, start, rows, g.cam, d_px, n_groups, xyz0, max_iter, xtol, d_out_xyz,
+                           d_rmse, d_status, st));
+  CB_CUDA(cudaEventRecord(ev[5], st));
+  double* d_cov = nullptr;
+  if (cov_out)
+    CB_TRY(tri_cov_launch(n_cams, cams, cam_cov, pixel_sigma, lanes, start, rows, g.cam, d_px, n, n_groups, d_out_xyz,
+                          d_status, ev[6], ev[7], sf, st, &d_cov));
+  CB_CUDA(cudaMemcpyAsync(xyz_out, d_out_xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  if (cov_out)
+    CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  std::vector<int> cstatus;
+  if (robust) {
+    cstatus.resize(n_groups);
+    CB_CUDA(cudaMemcpyAsync(robust->n_inliers_out, cs.nin, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(cstatus.data(), cs.status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(robust->inlier_out, cs.inl, (size_t)n, cudaMemcpyDeviceToHost, st));
+  }
+  CB_CUDA(cudaStreamSynchronize(st));
+  for (int i = 0; i < (int)cstatus.size(); ++i)
+    if (cstatus[i] == cb::TRI_NO_CONSENSUS) status_out[i] = cb::TRI_NO_CONSENSUS;
+  if (stats) {
+    stats->group_ms = ev.ms(0, 1);
+    stats->dlt_ms = ev.ms(2, 3);
+    stats->refine_ms = ev.ms(4, 5);
+    if (cov_out) stats->cov_ms = ev.ms(6, 7);
+    stats->total_ms = ev.ms(0, cov_out ? 7 : 5);
     stats->kernel_launches = (int)(g_launches.load() - launches0);
   }
   return CB_OK;
@@ -3174,66 +3372,9 @@ int cb_triangulate_refine(int32_t n_cams, const int32_t* cam_flags, const double
     g_last_error = "cb_triangulate_refine: bad argument";
     return CB_E_INVALID;
   }
-  TriCams cams;
-  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, "cb_triangulate_refine", &cams));
-  CB_TRY(select_device(device));
-  *n_groups_out = 0;
-  if (stats) std::memset(stats, 0, sizeof(*stats));
-  if (n_obs == 0) return CB_OK;
-  const long long launches0 = g_launches.load();
-  cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
-  const int n = (int)n_obs;
-  cudaEvent_t ev[8];
-  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 8; ++i) cudaEventDestroy(e[i]); } } evg{ev};
-  CB_CUDA(cudaEventRecord(ev[0], st));
-  // fp64 pixels on the device: the refinement reads them at full precision; the DLT start rounds them to float32 as
-  // cb_undistort_triangulate does
-  const int* d_cam = nullptr;
-  const long long* d_key = nullptr;
-  const double* d_px = nullptr;
-  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
-  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
-  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
-  TriDlt t;
-  CB_TRY(tri_dlt_stage(n_cams, &cams.tab, cams.proj.data(), n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups,
-                       n_groups_out, "cb_triangulate_refine", ev, sf, st, &t));
-  const int n_groups = t.n_groups;
-  CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
-
-  double *d_out_xyz = nullptr, *d_rmse = nullptr;
-  int* d_status = nullptr;
-  CB_TRY(dalloc(&d_out_xyz, 3 * (size_t)n_groups)); sf.dev.push_back(d_out_xyz);
-  CB_TRY(dalloc(&d_rmse, (size_t)n_groups)); sf.dev.push_back(d_rmse);
-  CB_TRY(dalloc(&d_status, (size_t)n_groups)); sf.dev.push_back(d_status);
-  CB_CUDA(cudaEventRecord(ev[4], st));
-  CB_TRY(tri_refine_launch(n_cams, cams, t.lanes, t.start, t.rows, t.cam, d_px, n_groups, t.xyz, max_iter, xtol, d_out_xyz,
-                           d_rmse, d_status, st));
-  CB_CUDA(cudaEventRecord(ev[5], st));
-
-  double* d_cov = nullptr;
-  if (cov_out)
-    CB_TRY(tri_cov_launch(n_cams, cams, cam_cov, pixel_sigma, t.lanes, t.start, t.rows, t.cam, d_px, n, n_groups,
-                          d_out_xyz, d_status, ev[6], ev[7], sf, st, &d_cov));
-  CB_CUDA(cudaMemcpyAsync(xyz_out, d_out_xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(count_out, t.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rep_row_out, t.rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  if (cov_out)
-    CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaStreamSynchronize(st));
-  if (stats) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
-    cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->dlt_ms = ms;
-    cudaEventElapsedTime(&ms, ev[4], ev[5]); stats->refine_ms = ms;
-    if (cov_out) { cudaEventElapsedTime(&ms, ev[6], ev[7]); stats->cov_ms = ms; }
-    cudaEventElapsedTime(&ms, ev[0], cov_out ? ev[7] : ev[5]); stats->total_ms = ms;
-    stats->kernel_launches = (int)(g_launches.load() - launches0);
-  }
-  return CB_OK;
+  return tri_calibrated(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_obs, obs_cam, obs_key, obs_px, obs_on_device,
+                        nullptr, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, xyz_out, cov_out, rmse_px_out,
+                        count_out, rep_row_out, status_out, stats, "cb_triangulate_refine", device, stream);
 }
 
 int cb_triangulate_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
@@ -3251,197 +3392,16 @@ int cb_triangulate_robust(int32_t n_cams, const int32_t* cam_flags, const double
     g_last_error = "cb_triangulate_robust: bad argument";
     return CB_E_INVALID;
   }
-  TriCams cams;
-  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, "cb_triangulate_robust", &cams));
-  CB_TRY(select_device(device));
-  *n_groups_out = 0;
-  if (stats) std::memset(stats, 0, sizeof(*stats));
-  if (n_obs == 0) return CB_OK;
-  const long long launches0 = g_launches.load();
-  cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
-  const int n = (int)n_obs;
-  cudaEvent_t ev[8];
-  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 8; ++i) cudaEventDestroy(e[i]); } } evg{ev};
-  CB_CUDA(cudaEventRecord(ev[0], st));
-  const int* d_cam = nullptr;
-  const long long* d_key = nullptr;
-  const double* d_px = nullptr;
-  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
-  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
-  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
-  // grouping and undistortion only: a DLT over the whole group would be contaminated by the outliers
-  TriDlt t;
-  CB_TRY(tri_group_stage(n_cams, &cams.tab, cams.proj.data(), n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups,
-                         n_groups_out, "cb_triangulate_robust", ev, sf, st, &t));
-  const int n_groups = t.n_groups;
-  CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
-
-  // (1) consensus: hypothesis, count, rep_row, n_inliers (+ a zero past the end for the scan), status 0 / 1 / 5, flags
-  double* d_hyp = nullptr;
-  int *d_count = nullptr, *d_rep = nullptr, *d_nin = nullptr, *d_cstatus = nullptr;
-  unsigned char *d_flag = nullptr, *d_inl = nullptr;
-  CB_TRY(dalloc(&d_hyp, 3 * (size_t)n_groups)); sf.dev.push_back(d_hyp);
-  CB_TRY(dalloc(&d_count, (size_t)n_groups)); sf.dev.push_back(d_count);
-  CB_TRY(dalloc(&d_rep, (size_t)n_groups)); sf.dev.push_back(d_rep);
-  CB_TRY(dalloc(&d_nin, (size_t)n_groups + 1)); sf.dev.push_back(d_nin);
-  CB_TRY(dalloc(&d_cstatus, (size_t)n_groups)); sf.dev.push_back(d_cstatus);
-  CB_TRY(dalloc(&d_flag, (size_t)n)); sf.dev.push_back(d_flag);
-  CB_TRY(dalloc(&d_inl, (size_t)n)); sf.dev.push_back(d_inl);
-  // (2) compaction: the consensus rows of every group, in key-sorted order, and their group starts
-  int *d_rows_c = nullptr, *d_start_c = nullptr, *d_nsel = nullptr;
-  CB_TRY(dalloc(&d_rows_c, (size_t)n)); sf.dev.push_back(d_rows_c);
-  CB_TRY(dalloc(&d_start_c, (size_t)n_groups + 1)); sf.dev.push_back(d_start_c);
-  CB_TRY(dalloc(&d_nsel, 1)); sf.dev.push_back(d_nsel);
-  size_t tb_sel = 0, tb_scan = 0;
-  CB_CUDA(cub::DeviceSelect::Flagged(nullptr, tb_sel, t.rows, d_flag, d_rows_c, d_nsel, n, st));
-  CB_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb_scan, d_nin, d_start_c, n_groups + 1, st));
-  void* d_tmp = nullptr;
-  const size_t tb = std::max<size_t>(std::max(tb_sel, tb_scan), 16);
-  CB_TRY(cached_malloc(&d_tmp, tb));
-  sf.dev.push_back(d_tmp);
-
-  // camera table and projection table each in shared memory when it takes at most 40 KB
-  const size_t cam_smem = tri_camtab_smem(n_cams);
-  const size_t proj_bytes = sizeof(double) * 13 * (size_t)n_cams;  // padded stride, see tri_dlt_kernel
-  const size_t proj_smem = proj_bytes <= 40 * 1024 ? proj_bytes : 0;
-  const size_t smem = cam_smem + proj_smem;
-  if (smem > 48 * 1024) {
-    CB_CUDA(cudaFuncSetAttribute(cb::tri_consensus_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    CB_CUDA(cudaFuncSetAttribute(cb::tri_consensus_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  }
-  const int lanes = t.lanes;
-  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
-  CB_CUDA(cudaMemsetAsync(d_nin + n_groups, 0, sizeof(int), st));
-  CB_CUDA(cudaEventRecord(ev[2], st));
-#define CB_TRI_CONSENSUS(LL)                                                                                           \
-  CB_LAUNCH(cb::tri_consensus_kernel<LL>, blocks, cb::TRI_THREADS, smem, st, cams.camtab, cam_smem ? 1 : 0, t.proj,     \
-            proj_smem ? 1 : 0, n_cams, t.start, t.rows, t.cam, t.xy, d_px, n_groups, threshold_px, min_inliers,         \
-            max_pairs, d_hyp, d_count, d_rep, d_nin, d_cstatus, d_flag, d_inl)
-  if (lanes == 32) CB_TRI_CONSENSUS(32);
-  else CB_TRI_CONSENSUS(8);
-#undef CB_TRI_CONSENSUS
-  CB_CUDA(cudaGetLastError());
-  size_t tb_run = tb;
-  CB_CUDA(cub::DeviceSelect::Flagged(d_tmp, tb_run, t.rows, d_flag, d_rows_c, d_nsel, n, st));
-  tb_run = tb;
-  CB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tb_run, d_nin, d_start_c, n_groups + 1, st));
-  g_launches.fetch_add(4);
-  CB_CUDA(cudaEventRecord(ev[3], st));
-
-  // (3) refinement and covariance on the consensus rows, from the selected hypotheses; a status-5 group has no rows
-  // there, so the refinement reports 1 for it and the covariance is NaN
-  double *d_out_xyz = nullptr, *d_rmse = nullptr;
-  int* d_status = nullptr;
-  CB_TRY(dalloc(&d_out_xyz, 3 * (size_t)n_groups)); sf.dev.push_back(d_out_xyz);
-  CB_TRY(dalloc(&d_rmse, (size_t)n_groups)); sf.dev.push_back(d_rmse);
-  CB_TRY(dalloc(&d_status, (size_t)n_groups)); sf.dev.push_back(d_status);
-  CB_CUDA(cudaEventRecord(ev[4], st));
-  CB_TRY(tri_refine_launch(n_cams, cams, lanes, d_start_c, d_rows_c, t.cam, d_px, n_groups, d_hyp, max_iter, xtol,
-                           d_out_xyz, d_rmse, d_status, st));
-  CB_CUDA(cudaEventRecord(ev[5], st));
-  double* d_cov = nullptr;
-  if (cov_out)
-    CB_TRY(tri_cov_launch(n_cams, cams, cam_cov, pixel_sigma, lanes, d_start_c, d_rows_c, t.cam, d_px, n, n_groups,
-                          d_out_xyz, d_status, ev[6], ev[7], sf, st, &d_cov));
-  std::vector<int> cstatus(n_groups);
-  CB_CUDA(cudaMemcpyAsync(xyz_out, d_out_xyz, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(count_out, d_count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(n_inliers_out, d_nin, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rep_row_out, d_rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(cstatus.data(), d_cstatus, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(inlier_out, d_inl, (size_t)n, cudaMemcpyDeviceToHost, st));
-  if (cov_out)
-    CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaStreamSynchronize(st));
-  for (int g = 0; g < n_groups; ++g)
-    if (cstatus[g] == cb::TRI_NO_CONSENSUS) status_out[g] = cb::TRI_NO_CONSENSUS;
-  if (stats) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
-    cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->consensus_ms = ms;
-    cudaEventElapsedTime(&ms, ev[4], ev[5]); stats->refine_ms = ms;
-    if (cov_out) { cudaEventElapsedTime(&ms, ev[6], ev[7]); stats->cov_ms = ms; }
-    cudaEventElapsedTime(&ms, ev[0], cov_out ? ev[7] : ev[5]); stats->total_ms = ms;
-    stats->kernel_launches = (int)(g_launches.load() - launches0);
-  }
-  return CB_OK;
+  const TriConsensusArgs robust = {threshold_px, min_inliers, max_pairs, n_inliers_out, inlier_out};
+  return tri_calibrated(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_obs, obs_cam, obs_key, obs_px, obs_on_device,
+                        &robust, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, xyz_out, cov_out, rmse_px_out,
+                        count_out, rep_row_out, status_out, reinterpret_cast<CbTriRefineStats*>(stats),
+                        "cb_triangulate_robust", device, stream);
 }
-
-}  // extern "C"
 
 // ------------------------------------------------------------------------------------------
 // extrinsic bootstrap: batched planar PnP and stereo RMSE (SURVEY.md §8(f) rank 1)
 // ------------------------------------------------------------------------------------------
-namespace {
-
-// stable sort of the rows by key, group boundaries: d_rows (n), d_start (n_groups + 1)
-int group_by_key(const long long* d_key, int n, cudaStream_t st, ScopedFree& sf, int** d_rows, int** d_start, int* n_groups) {
-  const int TB = 256, G = cdiv(n, TB);
-  unsigned long long* k_out = nullptr;
-  int *v_in = nullptr, *v_out = nullptr, *d_head = nullptr, *d_gid = nullptr, *dstart = nullptr;
-  CB_TRY(dalloc(&k_out, (size_t)n)); sf.dev.push_back(k_out);
-  CB_TRY(dalloc(&v_in, (size_t)n)); sf.dev.push_back(v_in);
-  CB_TRY(dalloc(&v_out, (size_t)n)); sf.dev.push_back(v_out);
-  CB_TRY(dalloc(&d_head, (size_t)n)); sf.dev.push_back(d_head);
-  CB_TRY(dalloc(&d_gid, (size_t)n)); sf.dev.push_back(d_gid);
-  CB_TRY(dalloc(&dstart, (size_t)n + 1)); sf.dev.push_back(dstart);
-  size_t tb_sort = 0, tb_scan = 0, tb_red = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tb_sort, (const unsigned long long*)d_key, k_out, v_in, v_out, n, 0, 64, st);
-  cub::DeviceScan::InclusiveSum(nullptr, tb_scan, d_head, d_gid, n, st);
-  cub::DeviceReduce::Max(nullptr, tb_red, (const unsigned long long*)d_key, (unsigned long long*)nullptr, n, st);
-  void* d_tmp = nullptr;
-  size_t tb = std::max(std::max(tb_sort, tb_scan), tb_red);
-  CB_TRY(cached_malloc(&d_tmp, std::max<size_t>(tb, 16)));
-  sf.dev.push_back(d_tmp);
-  CB_LAUNCH(cb::tri_iota_kernel, G, TB, 0, st, v_in, (long long)n);
-  // radix passes only over the key's significant bits (a packed (sync, object, keypoint) key of a 50k-point rig has 16)
-  unsigned long long* d_max = nullptr;
-  CB_TRY(dalloc(&d_max, 1)); sf.dev.push_back(d_max);
-  size_t tb_max = tb;
-  CB_CUDA(cub::DeviceReduce::Max(d_tmp, tb_max, (const unsigned long long*)d_key, d_max, n, st));
-  unsigned long long h_max = 0;
-  CB_CUDA(cudaMemcpyAsync(&h_max, d_max, sizeof(h_max), cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaStreamSynchronize(st));
-  const int key_bits = std::min(63, bits_for(h_max));
-  CB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, (const unsigned long long*)d_key, k_out, v_in, v_out, n, 0, key_bits, st));
-  g_launches.fetch_add(2 + 2 * ((key_bits + 7) / 8));
-  CB_LAUNCH(cb::tri_heads_kernel, G, TB, 0, st, k_out, (long long)n, d_head);
-  CB_CUDA(cub::DeviceScan::InclusiveSum(d_tmp, tb, d_head, d_gid, n, st));
-  g_launches.fetch_add(2);
-  CB_LAUNCH(cb::tri_starts_kernel, G, TB, 0, st, d_head, d_gid, (long long)n, dstart);
-  CB_CUDA(cudaMemcpyAsync(n_groups, d_gid + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaStreamSynchronize(st));
-  *d_rows = v_out;
-  *d_start = dstart;
-  return CB_OK;
-}
-
-// pixels (host, double) -> device, undistorted to the normalised plane with the reference's float32 rounding
-int upload_undistorted(int32_t n_cams, const int32_t* cam_fisheye, const double* cam_k, const double* cam_dist, int n,
-                       const int* d_cam, const double* obs_px, ScopedFree& sf, cudaStream_t st, double** d_norm) {
-  std::vector<cb::UndistCam> tab;
-  CB_TRY(build_undist_table(n_cams, cam_fisheye, cam_k, cam_dist, tab));
-  cb::UndistCam* d_tab = nullptr;
-  CB_TRY(dalloc(&d_tab, (size_t)n_cams));
-  sf.dev.push_back(d_tab);
-  CB_CUDA(cudaMemcpy(d_tab, tab.data(), sizeof(cb::UndistCam) * n_cams, cudaMemcpyHostToDevice));
-  double* d_und = nullptr;
-  CB_TRY(dalloc(&d_und, 2 * (size_t)n));
-  sf.dev.push_back(d_und);
-  const float* d_px = nullptr;
-  CB_TRY(to_device_f32(obs_px, 2 * (size_t)n, &d_px, sf, st));
-  CB_LAUNCH(cb::undistort_kernel<float>, cdiv(n, 256), 256, 0, st, d_tab, d_cam, d_px, d_und, (long long)n, 0);
-  *d_norm = d_und;
-  return CB_OK;
-}
-
-}  // namespace
-
-extern "C" {
 
 int cb_pnp_ippe(int32_t n_cams, const int32_t* cam_fisheye, const double* cam_k, const double* cam_dist, int64_t n_obs,
                 const int32_t* obs_cam, const int64_t* obs_key, const double* obs_px, const double* obs_obj,
@@ -3458,42 +3418,32 @@ int cb_pnp_ippe(int32_t n_cams, const int32_t* cam_fisheye, const double* cam_k,
   *n_groups_out = 0;
   if (stats) std::memset(stats, 0, sizeof(*stats));
   if (n_obs == 0) return CB_OK;
+  std::vector<cb::UndistCam> tab;
+  CB_TRY(build_undist_table(n_cams, cam_fisheye, cam_k, cam_dist, tab));
   const long long launches0 = g_launches.load();
   cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
+  ScopedFree sf(st);
   const int n = (int)n_obs;
-  cudaEvent_t ev[4];
-  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  StageEvents<4> ev;
+  CB_TRY(ev.create());
   CB_CUDA(cudaEventRecord(ev[0], st));
-  const int* d_cam = nullptr;
-  const long long* d_key = nullptr;
   const double* d_obj = nullptr;
-  CB_TRY(to_device(obs_cam, (size_t)n, 0, &d_cam, sf, st));
-  CB_TRY(to_device((const long long*)obs_key, (size_t)n, 0, &d_key, sf, st));
   CB_TRY(to_device(obs_obj, 3 * (size_t)n, 0, &d_obj, sf, st));
-  CB_TRY(validate_rows(d_cam, d_key, n, n_cams, st, "cb_pnp_ippe"));
-  double* d_norm = nullptr;
-  CB_TRY(upload_undistorted(n_cams, cam_fisheye, cam_k, cam_dist, n, d_cam, obs_px, sf, st, &d_norm));
-  int *d_rows = nullptr, *d_start = nullptr, n_groups = 0;
-  CB_TRY(group_by_key(d_key, n, st, sf, &d_rows, &d_start, &n_groups));
-  CB_CUDA(cudaEventRecord(ev[1], st));
-  *n_groups_out = n_groups;
-  if (n_groups > max_groups) {
-    g_last_error = "cb_pnp_ippe: " + std::to_string(n_groups) + " groups but room for " + std::to_string(max_groups);
-    return CB_E_INVALID;
-  }
+  ObsGroups g;
+  CB_TRY(obs_group_stage(n_cams, &tab, n, obs_cam, obs_key, obs_px, 0, max_groups, n_groups_out, "cb_pnp_ippe", ev[1], sf,
+                         st, &g));
+  const int n_groups = g.n_groups;
   double *d_R, *d_t, *d_rmse;
   int *d_status, *d_count, *d_rep;
-  CB_TRY(dalloc(&d_R, 9 * (size_t)n_groups)); sf.dev.push_back(d_R);
-  CB_TRY(dalloc(&d_t, 3 * (size_t)n_groups)); sf.dev.push_back(d_t);
-  CB_TRY(dalloc(&d_rmse, (size_t)n_groups)); sf.dev.push_back(d_rmse);
-  CB_TRY(dalloc(&d_status, (size_t)n_groups)); sf.dev.push_back(d_status);
-  CB_TRY(dalloc(&d_count, (size_t)n_groups)); sf.dev.push_back(d_count);
-  CB_TRY(dalloc(&d_rep, (size_t)n_groups)); sf.dev.push_back(d_rep);
+  CB_TRY(sf.alloc(&d_R, 9 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_t, 3 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_rmse, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_status, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_count, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_rep, (size_t)n_groups));
   CB_CUDA(cudaEventRecord(ev[2], st));
-  CB_LAUNCH(cb::pnp_ippe_kernel, cdiv((long long)n_groups * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, d_start, d_rows, d_obj,
-            (const double*)d_norm, n_groups, (int)min_points, d_R, d_t, d_rmse, d_status, d_count, d_rep);
+  CB_LAUNCH(cb::pnp_ippe_kernel, cdiv((long long)n_groups * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, g.start, g.rows, d_obj,
+            g.xy, n_groups, (int)min_points, d_R, d_t, d_rmse, d_status, d_count, d_rep);
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[3], st));
   CB_CUDA(cudaMemcpyAsync(R_out, d_R, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
@@ -3504,10 +3454,9 @@ int cb_pnp_ippe(int32_t n_cams, const int32_t* cam_fisheye, const double* cam_k,
   CB_CUDA(cudaMemcpyAsync(rep_row_out, d_rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   if (stats) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
-    cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->dlt_ms = ms;
-    cudaEventElapsedTime(&ms, ev[0], ev[3]); stats->total_ms = ms;
+    stats->group_ms = ev.ms(0, 1);
+    stats->dlt_ms = ev.ms(2, 3);
+    stats->total_ms = ev.ms(0, 3);
     stats->kernel_launches = (int)(g_launches.load() - launches0);
   }
   return CB_OK;
@@ -3530,7 +3479,6 @@ int cb_stereo_rmse(int32_t n_cams, const int32_t* cam_fisheye, const double* cam
   if (n_pairs == 0 || n_obs == 0) return CB_OK;
   const long long launches0 = g_launches.load();
   cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
   const int n = (int)n_obs;
   std::vector<int> pair_of((size_t)n_cams * n_cams, -1);
   for (int p = 0; p < n_pairs; ++p) {
@@ -3541,35 +3489,28 @@ int cb_stereo_rmse(int32_t n_cams, const int32_t* cam_fisheye, const double* cam
     }
     pair_of[(size_t)a * n_cams + b] = p;
   }
-  cudaEvent_t ev[4];
-  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  std::vector<cb::UndistCam> tab;
+  CB_TRY(build_undist_table(n_cams, cam_fisheye, cam_k, cam_dist, tab));
+  ScopedFree sf(st);
+  StageEvents<4> ev;
+  CB_TRY(ev.create());
   CB_CUDA(cudaEventRecord(ev[0], st));
-  const int* d_cam = nullptr;
-  const long long* d_key = nullptr;
   const int* d_pair_of = nullptr;
   const double* d_Rt = nullptr;
-  CB_TRY(to_device(obs_cam, (size_t)n, 0, &d_cam, sf, st));
-  CB_TRY(to_device((const long long*)obs_key, (size_t)n, 0, &d_key, sf, st));
   CB_TRY(to_device(pair_of.data(), pair_of.size(), 0, &d_pair_of, sf, st));
   CB_TRY(to_device(pair_Rt, 12 * (size_t)n_pairs, 0, &d_Rt, sf, st));
-  CB_TRY(validate_rows(d_cam, d_key, n, n_cams, st, "cb_stereo_rmse"));
-  double* d_norm = nullptr;
-  CB_TRY(upload_undistorted(n_cams, cam_fisheye, cam_k, cam_dist, n, d_cam, obs_px, sf, st, &d_norm));
-  int *d_rows = nullptr, *d_start = nullptr, n_groups = 0;
-  CB_TRY(group_by_key(d_key, n, st, sf, &d_rows, &d_start, &n_groups));
-  CB_CUDA(cudaEventRecord(ev[1], st));
+  ObsGroups g;
+  int32_t n_groups = 0;  // every group has room: the call's outputs are per camera pair
+  CB_TRY(obs_group_stage(n_cams, &tab, n, obs_cam, obs_key, obs_px, 0, INT32_MAX, &n_groups, "cb_stereo_rmse", ev[1], sf,
+                         st, &g));
+  const int* d_start = g.start;
   // slots per group, exclusive scan
   long long *d_nslots = nullptr, *d_slot_start = nullptr;
-  CB_TRY(dalloc(&d_nslots, (size_t)n_groups + 1)); sf.dev.push_back(d_nslots);
-  CB_TRY(dalloc(&d_slot_start, (size_t)n_groups + 1)); sf.dev.push_back(d_slot_start);
+  CB_TRY(sf.alloc(&d_nslots, (size_t)n_groups + 1));
+  CB_TRY(sf.alloc(&d_slot_start, (size_t)n_groups + 1));
   CB_CUDA(cudaMemsetAsync(d_nslots, 0, sizeof(long long) * ((size_t)n_groups + 1), st));
   CB_LAUNCH(cb::stereo_slots_kernel, cdiv(n_groups, 256), 256, 0, st, d_start, n_groups, d_nslots);
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, d_nslots, d_slot_start, n_groups + 1, st);
-  void* d_tmp = nullptr;
-  CB_TRY(cached_malloc(&d_tmp, std::max<size_t>(tb, 16))); sf.dev.push_back(d_tmp);
-  CB_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp, tb, d_nslots, d_slot_start, n_groups + 1, st));
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_nslots, d_slot_start, n_groups + 1, st);
   g_launches.fetch_add(2);
   long long total = 0;
   CB_CUDA(cudaMemcpyAsync(&total, d_slot_start + n_groups, sizeof(long long), cudaMemcpyDeviceToHost, st));
@@ -3579,51 +3520,41 @@ int cb_stereo_rmse(int32_t n_cams, const int32_t* cam_fisheye, const double* cam
   const int m = (int)total;
   int *d_k = nullptr, *d_ks = nullptr;
   double *d_v = nullptr, *d_vs = nullptr;
-  CB_TRY(dalloc(&d_k, (size_t)m)); sf.dev.push_back(d_k);
-  CB_TRY(dalloc(&d_ks, (size_t)m)); sf.dev.push_back(d_ks);
-  CB_TRY(dalloc(&d_v, (size_t)m)); sf.dev.push_back(d_v);
-  CB_TRY(dalloc(&d_vs, (size_t)m)); sf.dev.push_back(d_vs);
+  CB_TRY(sf.alloc(&d_k, (size_t)m));
+  CB_TRY(sf.alloc(&d_ks, (size_t)m));
+  CB_TRY(sf.alloc(&d_v, (size_t)m));
+  CB_TRY(sf.alloc(&d_vs, (size_t)m));
   CB_CUDA(cudaEventRecord(ev[2], st));
   const int lanes = (n / std::max(n_groups, 1) > 12) ? 32 : 8;
   if (lanes == 32)
-    CB_LAUNCH(cb::stereo_pairs_kernel<32>, cdiv((long long)n_groups * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, d_start, d_rows,
-              d_cam, (const double*)d_norm, n_groups, (const long long*)d_slot_start, (int)n_cams, d_pair_of, d_Rt, (int)n_pairs, d_k, d_v);
+    CB_LAUNCH(cb::stereo_pairs_kernel<32>, cdiv((long long)n_groups * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, d_start, g.rows,
+              g.cam, g.xy, n_groups, (const long long*)d_slot_start, (int)n_cams, d_pair_of, d_Rt, (int)n_pairs, d_k, d_v);
   else
-    CB_LAUNCH(cb::stereo_pairs_kernel<8>, cdiv((long long)n_groups * 8, cb::BS_THREADS), cb::BS_THREADS, 0, st, d_start, d_rows,
-              d_cam, (const double*)d_norm, n_groups, (const long long*)d_slot_start, (int)n_cams, d_pair_of, d_Rt, (int)n_pairs, d_k, d_v);
+    CB_LAUNCH(cb::stereo_pairs_kernel<8>, cdiv((long long)n_groups * 8, cb::BS_THREADS), cb::BS_THREADS, 0, st, d_start, g.rows,
+              g.cam, g.xy, n_groups, (const long long*)d_slot_start, (int)n_cams, d_pair_of, d_Rt, (int)n_pairs, d_k, d_v);
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[3], st));
   // stable sort by pair id, then one segmented sum per pair (fixed order => reproducible sums)
-  size_t tb2 = 0, tb3 = 0;
   const int kbits = bits_for((unsigned long long)n_pairs);
-  cub::DeviceRadixSort::SortPairs(nullptr, tb2, d_k, d_ks, d_v, d_vs, m, 0, kbits, st);
   int *d_uk = nullptr, *d_nruns = nullptr;
   double* d_sum = nullptr;
-  CB_TRY(dalloc(&d_uk, (size_t)n_pairs + 2)); sf.dev.push_back(d_uk);
-  CB_TRY(dalloc(&d_sum, (size_t)n_pairs + 2)); sf.dev.push_back(d_sum);
-  CB_TRY(dalloc(&d_nruns, 1)); sf.dev.push_back(d_nruns);
-  cub::DeviceReduce::ReduceByKey(nullptr, tb3, d_ks, d_uk, d_vs, d_sum, d_nruns, cub::Sum(), m, st);
-  void* d_tmp2 = nullptr;
-  CB_TRY(cached_malloc(&d_tmp2, std::max<size_t>(std::max(tb2, tb3), 16))); sf.dev.push_back(d_tmp2);
-  size_t tbs = std::max(tb2, tb3);
-  CB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp2, tbs, d_k, d_ks, d_v, d_vs, m, 0, kbits, st));
-  CB_CUDA(cub::DeviceReduce::ReduceByKey(d_tmp2, tbs, d_ks, d_uk, d_vs, d_sum, d_nruns, cub::Sum(), m, st));
+  CB_TRY(sf.alloc(&d_uk, (size_t)n_pairs + 2));
+  CB_TRY(sf.alloc(&d_sum, (size_t)n_pairs + 2));
+  CB_TRY(sf.alloc(&d_nruns, 1));
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, d_v, d_vs, m, 0, kbits, st);
+  CB_CUB(sf, cub::DeviceReduce::ReduceByKey, d_ks, d_uk, d_vs, d_sum, d_nruns, cub::Sum(), m, st);
   g_launches.fetch_add(6);
   // counts per pair: run lengths of the sorted keys (same run order as the segmented sums)
   int *d_uk2 = nullptr, *d_len = nullptr;
-  CB_TRY(dalloc(&d_uk2, (size_t)n_pairs + 2)); sf.dev.push_back(d_uk2);
-  CB_TRY(dalloc(&d_len, (size_t)n_pairs + 2)); sf.dev.push_back(d_len);
-  size_t tb4 = 0;
-  cub::DeviceRunLengthEncode::Encode(nullptr, tb4, d_ks, d_uk2, d_len, d_nruns, m, st);
-  void* d_tmp3 = nullptr;
-  CB_TRY(cached_malloc(&d_tmp3, std::max<size_t>(tb4, 16))); sf.dev.push_back(d_tmp3);
+  CB_TRY(sf.alloc(&d_uk2, (size_t)n_pairs + 2));
+  CB_TRY(sf.alloc(&d_len, (size_t)n_pairs + 2));
   std::vector<int> uk((size_t)n_pairs + 2), len((size_t)n_pairs + 2);
   std::vector<double> sums((size_t)n_pairs + 2);
   int nruns = 0;
   CB_CUDA(cudaMemcpyAsync(&nruns, d_nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(uk.data(), d_uk, sizeof(int) * ((size_t)n_pairs + 1), cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(sums.data(), d_sum, sizeof(double) * ((size_t)n_pairs + 1), cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cub::DeviceRunLengthEncode::Encode(d_tmp3, tb4, d_ks, d_uk2, d_len, d_nruns, m, st));
+  CB_CUB(sf, cub::DeviceRunLengthEncode::Encode, d_ks, d_uk2, d_len, d_nruns, m, st);
   g_launches.fetch_add(2);
   CB_CUDA(cudaMemcpyAsync(len.data(), d_len, sizeof(int) * ((size_t)n_pairs + 1), cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
@@ -3635,10 +3566,9 @@ int cb_stereo_rmse(int32_t n_cams, const int32_t* cam_fisheye, const double* cam
     if (cnt >= min_common) rmse_out[pid] = std::sqrt(sums[r] / (2.0 * (double)cnt));  // mean over the 2N stacked rows
   }
   if (stats) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
-    cudaEventElapsedTime(&ms, ev[2], ev[3]); stats->dlt_ms = ms;
-    cudaEventElapsedTime(&ms, ev[0], ev[3]); stats->total_ms = ms;
+    stats->group_ms = ev.ms(0, 1);
+    stats->dlt_ms = ev.ms(2, 3);
+    stats->total_ms = ev.ms(0, 3);
     stats->kernel_launches = (int)(g_launches.load() - launches0);
   }
   return CB_OK;
@@ -3684,10 +3614,9 @@ int cb_relative_pose_network(int32_t n_groups, int32_t n_frames, const int32_t* 
   CB_TRY(select_device(device));
   const long long launches0 = g_launches.load();
   cudaStream_t st = (cudaStream_t)stream;
-  ScopedFree sf;
-  cudaEvent_t ev[3];
-  for (auto& e : ev) CB_CUDA(cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 3; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  ScopedFree sf(st);
+  StageEvents<3> ev;
+  CB_TRY(ev.create());
   CB_CUDA(cudaEventRecord(ev[0], st));
   const long long* d_pair_off = nullptr;
   const int *d_fs = nullptr, *d_id = nullptr, *d_pos = nullptr;
@@ -3702,17 +3631,17 @@ int cb_relative_pose_network(int32_t n_groups, int32_t n_frames, const int32_t* 
   unsigned *d_key = nullptr, *d_idx = nullptr, *d_key_s = nullptr, *d_perm = nullptr;
   double *d_Rr = nullptr, *d_tr = nullptr, *d_q = nullptr, *d_tm = nullptr;
   unsigned char *d_valid = nullptr, *d_keep = nullptr;
-  CB_TRY(dalloc(&d_key, m)); sf.dev.push_back(d_key);
-  CB_TRY(dalloc(&d_idx, m)); sf.dev.push_back(d_idx);
-  CB_TRY(dalloc(&d_key_s, m)); sf.dev.push_back(d_key_s);
-  CB_TRY(dalloc(&d_perm, m)); sf.dev.push_back(d_perm);
-  CB_TRY(dalloc(&d_Rr, 9 * m)); sf.dev.push_back(d_Rr);
-  CB_TRY(dalloc(&d_tr, 3 * m)); sf.dev.push_back(d_tr);
-  CB_TRY(dalloc(&d_q, 4 * m)); sf.dev.push_back(d_q);
-  CB_TRY(dalloc(&d_tm, m)); sf.dev.push_back(d_tm);
-  if (rel_valid) { CB_TRY(dalloc(&d_valid, m)); sf.dev.push_back(d_valid); }
+  CB_TRY(sf.alloc(&d_key, m));
+  CB_TRY(sf.alloc(&d_idx, m));
+  CB_TRY(sf.alloc(&d_key_s, m));
+  CB_TRY(sf.alloc(&d_perm, m));
+  CB_TRY(sf.alloc(&d_Rr, 9 * m));
+  CB_TRY(sf.alloc(&d_tr, 3 * m));
+  CB_TRY(sf.alloc(&d_q, 4 * m));
+  CB_TRY(sf.alloc(&d_tm, m));
+  if (rel_valid) CB_TRY(sf.alloc(&d_valid, m));
   if (rel_keep) {
-    CB_TRY(dalloc(&d_keep, m)); sf.dev.push_back(d_keep);
+    CB_TRY(sf.alloc(&d_keep, m));
     CB_CUDA(cudaMemsetAsync(d_keep, 0, m, st));
   }
   CB_LAUNCH(cb::rel_pose_kernel, cdiv(M, 256), 256, 0, st, d_pair_off, d_fs, (int)n_frames, M, d_id, d_pos, d_R, d_t, span,
@@ -3722,18 +3651,11 @@ int cb_relative_pose_network(int32_t n_groups, int32_t n_frames, const int32_t* 
   const int max_runs = (int)std::min<long long>(M, (long long)span * (span - 1) / 2 + 1) + 1;
   unsigned* d_uk = nullptr;
   int *d_len = nullptr, *d_nruns = nullptr;
-  CB_TRY(dalloc(&d_uk, (size_t)max_runs)); sf.dev.push_back(d_uk);
-  CB_TRY(dalloc(&d_len, (size_t)max_runs)); sf.dev.push_back(d_len);
-  CB_TRY(dalloc(&d_nruns, 1)); sf.dev.push_back(d_nruns);
-  size_t tb1 = 0, tb2 = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, tb1, d_key, d_key_s, d_idx, d_perm, (int)M, 0, kbits, st);
-  cub::DeviceRunLengthEncode::Encode(nullptr, tb2, d_key_s, d_uk, d_len, d_nruns, (int)M, st);
-  void* d_tmp = nullptr;
-  size_t tb = std::max(tb1, tb2);
-  CB_TRY(cached_malloc(&d_tmp, std::max<size_t>(tb, 16))); sf.dev.push_back(d_tmp);
-  CB_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp, tb, d_key, d_key_s, d_idx, d_perm, (int)M, 0, kbits, st));
-  tb = std::max(tb1, tb2);
-  CB_CUDA(cub::DeviceRunLengthEncode::Encode(d_tmp, tb, d_key_s, d_uk, d_len, d_nruns, (int)M, st));
+  CB_TRY(sf.alloc(&d_uk, (size_t)max_runs));
+  CB_TRY(sf.alloc(&d_len, (size_t)max_runs));
+  CB_TRY(sf.alloc(&d_nruns, 1));
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_key, d_key_s, d_idx, d_perm, (int)M, 0, kbits, st);
+  CB_CUB(sf, cub::DeviceRunLengthEncode::Encode, d_key_s, d_uk, d_len, d_nruns, (int)M, st);
   g_launches.fetch_add(6);
   int nruns = 0;
   CB_CUDA(cudaMemcpyAsync(&nruns, d_nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -3764,36 +3686,32 @@ int cb_relative_pose_network(int32_t n_groups, int32_t n_frames, const int32_t* 
   double *d_Rs = nullptr, *d_ts = nullptr, *d_qs = nullptr, *d_tms = nullptr, *d_sorted = nullptr, *d_ang = nullptr;
   int* d_seg = nullptr;
   unsigned char* d_ok = nullptr;
-  CB_TRY(dalloc(&d_Rs, 9 * mv)); sf.dev.push_back(d_Rs);
-  CB_TRY(dalloc(&d_ts, 3 * mv)); sf.dev.push_back(d_ts);
-  CB_TRY(dalloc(&d_qs, 4 * mv)); sf.dev.push_back(d_qs);
-  CB_TRY(dalloc(&d_tms, mv)); sf.dev.push_back(d_tms);
-  CB_TRY(dalloc(&d_sorted, mv)); sf.dev.push_back(d_sorted);
-  CB_TRY(dalloc(&d_ang, mv)); sf.dev.push_back(d_ang);
-  CB_TRY(dalloc(&d_seg, mv)); sf.dev.push_back(d_seg);
-  CB_TRY(dalloc(&d_ok, mv)); sf.dev.push_back(d_ok);
+  CB_TRY(sf.alloc(&d_Rs, 9 * mv));
+  CB_TRY(sf.alloc(&d_ts, 3 * mv));
+  CB_TRY(sf.alloc(&d_qs, 4 * mv));
+  CB_TRY(sf.alloc(&d_tms, mv));
+  CB_TRY(sf.alloc(&d_sorted, mv));
+  CB_TRY(sf.alloc(&d_ang, mv));
+  CB_TRY(sf.alloc(&d_seg, mv));
+  CB_TRY(sf.alloc(&d_ok, mv));
   double *d_Rm = nullptr, *d_tmn = nullptr, *d_q13 = nullptr;
   long long* d_cnt = nullptr;
-  CB_TRY(dalloc(&d_Rm, 9 * (size_t)n_seg)); sf.dev.push_back(d_Rm);
-  CB_TRY(dalloc(&d_tmn, 3 * (size_t)n_seg)); sf.dev.push_back(d_tmn);
-  CB_TRY(dalloc(&d_q13, 4 * (size_t)n_seg)); sf.dev.push_back(d_q13);
-  CB_TRY(dalloc(&d_cnt, (size_t)n_seg)); sf.dev.push_back(d_cnt);
+  CB_TRY(sf.alloc(&d_Rm, 9 * (size_t)n_seg));
+  CB_TRY(sf.alloc(&d_tmn, 3 * (size_t)n_seg));
+  CB_TRY(sf.alloc(&d_q13, 4 * (size_t)n_seg));
+  CB_TRY(sf.alloc(&d_cnt, (size_t)n_seg));
   CB_LAUNCH(cb::rel_gather_kernel, cdiv(Mv, 256), 256, 0, st, (const unsigned*)d_perm, Mv, (const double*)d_Rr,
             (const double*)d_tr, (const double*)d_q, (const double*)d_tm, d_Rs, d_ts, d_qs, d_tms);
   CB_LAUNCH(cb::seg_fill_kernel, n_seg, 128, 0, st, d_off, n_seg, d_seg);
   CB_CUDA(cudaEventRecord(ev[1], st));
   // quartiles of |t| per pair
-  size_t tb3 = 0;
-  cub::DeviceSegmentedSort::SortKeys(nullptr, tb3, (const double*)d_tms, d_sorted, (int)Mv, n_seg, d_off, d_off + 1, st);
-  void* d_tmp2 = nullptr;
-  CB_TRY(cached_malloc(&d_tmp2, std::max<size_t>(tb3, 16))); sf.dev.push_back(d_tmp2);
-  CB_CUDA(cub::DeviceSegmentedSort::SortKeys(d_tmp2, tb3, (const double*)d_tms, d_sorted, (int)Mv, n_seg, d_off, d_off + 1, st));
+  CB_CUB(sf, cub::DeviceSegmentedSort::SortKeys, (const double*)d_tms, d_sorted, (int)Mv, n_seg, d_off, d_off + 1, st);
   CB_LAUNCH(cb::seg_quartile_kernel, cdiv(n_seg, 128), 128, 0, st, (const double*)d_sorted, d_off, n_seg, d_q13, d_q13 + n_seg);
   // mean rotation per pair, angle of every sample to it, quartiles of the angle
   CB_LAUNCH(cb::quat_average_kernel, n_seg, cb::REL_THREADS, 0, st, d_off, n_seg, (const double*)d_qs, (const double*)d_ts,
             (const double*)d_Rs, (const unsigned char*)nullptr, d_Rm, d_tmn, d_cnt);
   CB_LAUNCH(cb::rel_angle_kernel, cdiv(Mv, 256), 256, 0, st, (const double*)d_Rs, (const int*)d_seg, (const double*)d_Rm, Mv, d_ang);
-  CB_CUDA(cub::DeviceSegmentedSort::SortKeys(d_tmp2, tb3, (const double*)d_ang, d_sorted, (int)Mv, n_seg, d_off, d_off + 1, st));
+  CB_CUB(sf, cub::DeviceSegmentedSort::SortKeys, (const double*)d_ang, d_sorted, (int)Mv, n_seg, d_off, d_off + 1, st);
   CB_LAUNCH(cb::seg_quartile_kernel, cdiv(n_seg, 128), 128, 0, st, (const double*)d_sorted, d_off, n_seg, d_q13 + 2 * (size_t)n_seg,
             d_q13 + 3 * (size_t)n_seg);
   g_launches.fetch_add(4);
@@ -3823,10 +3741,9 @@ int cb_relative_pose_network(int32_t n_groups, int32_t n_frames, const int32_t* 
   }
   *n_pairs_out = np;
   if (stats) {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev[0], ev[1]); stats->group_ms = ms;
-    cudaEventElapsedTime(&ms, ev[1], ev[2]); stats->dlt_ms = ms;
-    cudaEventElapsedTime(&ms, ev[0], ev[2]); stats->total_ms = ms;
+    stats->group_ms = ev.ms(0, 1);
+    stats->dlt_ms = ev.ms(1, 2);
+    stats->total_ms = ev.ms(0, 2);
     stats->kernel_launches = (int)(g_launches.load() - launches0);
   }
   return CB_OK;
