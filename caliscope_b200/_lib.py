@@ -132,6 +132,18 @@ class TriRobustStats(C.Structure):
     ]
 
 
+class ResectStats(C.Structure):
+    _fields_ = [
+        ("group_ms", C.c_double),
+        ("consensus_ms", C.c_double),
+        ("refine_ms", C.c_double),
+        ("cov_ms", C.c_double),
+        ("total_ms", C.c_double),
+        ("kernel_launches", C.c_int32),
+        ("pad_", C.c_int32),
+    ]
+
+
 # every symbol include/caliscope_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 _D = C.POINTER(C.c_double)
@@ -194,6 +206,12 @@ SYMBOLS = {
         [C.c_int32, _P, _P, _P, _P, C.c_int64, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32, C.c_double,
          C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, _P, _P, _P, _P, _P,
          C.POINTER(TriRobustStats), C.c_int, _P],
+    ),
+    "cb_resect_robust": (
+        C.c_int,
+        [C.c_int32, _P, _P, _P, C.c_int32, _P, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32,
+         C.c_int32, C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, _P, _P, _P, _P, _P,
+         _P, C.POINTER(ResectStats), C.c_int, _P],
     ),
     "cb_peer_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, C.POINTER(_P), _P]),
     "cb_peer_connect": (C.c_int, [_P, _P]),

@@ -35,6 +35,7 @@
 #include "cb_kernels.cuh"
 #include "cb_constraints.cuh"
 #include "cb_triangulate.cuh"
+#include "cb_resect.cuh"
 #include "cb_bootstrap.cuh"
 #include "cb_peer.cuh"
 
@@ -3397,6 +3398,231 @@ int cb_triangulate_robust(int32_t n_cams, const int32_t* cam_flags, const double
                         &robust, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, xyz_out, cov_out, rmse_px_out,
                         count_out, rep_row_out, status_out, reinterpret_cast<CbTriRefineStats*>(stats),
                         "cb_triangulate_robust", device, stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// Shape of cb_resect_robust's consensus stage: the long shape (hypothesis table, (chunk, hypothesis) tiles) when groups
+// average more than RES_LONG_ROWS rows and the table fits in RES_TABLE_BYTES; else res_consensus_kernel with
+// tri_lanes' 8 or 32 lanes per group.  Lanes per group elsewhere: 32 for the long shape.
+constexpr int RES_LONG_ROWS = 512;
+constexpr size_t RES_TABLE_BYTES = (size_t)1 << 30;
+
+int resect_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x, int32_t n_pts,
+                const double* pts_xyz, const double* pts_cov, int64_t n_obs, const int32_t* obs_cam,
+                const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px, int obs_on_device, double tau,
+                int32_t min_inliers, int32_t max_samples, int32_t use_prior, double pixel_sigma, int32_t max_iter,
+                double xtol, int32_t max_groups, int32_t* n_groups_out, int32_t* cam_out, double* pose_out,
+                double* cov_out, double* rmse_px_out, int32_t* count_out, int32_t* n_inliers_out,
+                int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out, CbResectStats* stats, int device,
+                void* stream) {
+  const char* who = "cb_resect_robust";
+  TriCams cams;
+  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, who, &cams));
+  CB_TRY(select_device(device));
+  *n_groups_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf(st);
+  const int n = (int)n_obs;
+  StageEvents<8> ev;
+  CB_TRY(ev.create());
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  const int *d_cam = nullptr, *d_pt = nullptr;
+  const long long* d_key = nullptr;
+  const double *d_px = nullptr, *d_pts = nullptr, *d_pcov = nullptr;
+  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
+  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
+  CB_TRY(to_device(obs_pt, (size_t)n, obs_on_device, &d_pt, sf, st));
+  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
+  CB_TRY(to_device(pts_xyz, 3 * (size_t)n_pts, 0, &d_pts, sf, st));
+  if (pts_cov && cov_out) CB_TRY(to_device(pts_cov, 9 * (size_t)n_pts, 0, &d_pcov, sf, st));
+  {  // point indices in range (tri_validate_kernel's count with the point table as the "cameras")
+    int* d_bad = nullptr;
+    CB_TRY(sf.alloc(&d_bad, 1));
+    CB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+    CB_LAUNCH(cb::tri_validate_kernel, cdiv(n, 256), 256, 0, st, d_pt, nullptr, (long long)n, n_pts, d_bad);
+    int bad = 0;
+    CB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaStreamSynchronize(st));
+    if (bad) {
+      g_last_error = std::string(who) + ": point index out of range in " + std::to_string(bad) + " rows";
+      return CB_E_INVALID;
+    }
+  }
+  ObsGroups g;
+  CB_TRY(obs_group_stage(n_cams, &cams.tab, n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups, n_groups_out, who,
+                         ev[1], sf, st, &g));
+  CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
+  const int n_groups = g.n_groups;
+  const int S = 1 + cb::RES_SLOTS_PER_SAMPLE * max_samples;
+  const bool long_shape = n / std::max(n_groups, 1) > RES_LONG_ROWS &&
+                          (size_t)n_groups * S * cb::RES_HYP * sizeof(double) <= RES_TABLE_BYTES;
+  const int lanes = long_shape ? 32 : tri_lanes(n, n_groups);
+
+  // consensus: winner, cam, count, rep_row, n_inliers (+ a zero past the end for the scan), status 0 / 1 / 5 / 6, flags
+  double* d_hyp = nullptr;
+  int *d_gcam = nullptr, *d_count = nullptr, *d_rep = nullptr, *d_nin = nullptr, *d_cst = nullptr, *d_nsel = nullptr;
+  int *d_crows = nullptr, *d_cstart = nullptr;
+  unsigned char *d_flag = nullptr, *d_inl = nullptr;
+  CB_TRY(sf.alloc(&d_hyp, (size_t)cb::RES_HYP * n_groups));
+  CB_TRY(sf.alloc(&d_gcam, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_count, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_rep, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_nin, (size_t)n_groups + 1));
+  CB_TRY(sf.alloc(&d_cst, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_flag, (size_t)n));
+  CB_TRY(sf.alloc(&d_inl, (size_t)n));
+  CB_TRY(sf.alloc(&d_crows, (size_t)n));
+  CB_TRY(sf.alloc(&d_cstart, (size_t)n_groups + 1));
+  CB_TRY(sf.alloc(&d_nsel, 1));
+  CB_CUDA(cudaMemsetAsync(d_nin + n_groups, 0, sizeof(int), st));
+  CB_CUDA(cudaEventRecord(ev[2], st));
+  if (long_shape) {
+    double *d_tab = nullptr, *d_part = nullptr;
+    int *d_nchunk = nullptr, *d_choff = nullptr, *d_best = nullptr;
+    CB_TRY(sf.alloc(&d_tab, (size_t)n_groups * S * cb::RES_HYP));
+    CB_TRY(sf.alloc(&d_nchunk, (size_t)n_groups + 1));
+    CB_TRY(sf.alloc(&d_choff, (size_t)n_groups + 1));
+    CB_TRY(sf.alloc(&d_best, (size_t)n_groups));
+    const long long n_tasks = (long long)n_groups * (1 + max_samples);
+    CB_LAUNCH(cb::res_hyp_kernel, cdiv(n_tasks, 128), 128, 0, st, cams.camtab, g.start, g.rows, g.cam, d_pt, g.xy, d_pts,
+              n_groups, max_samples, use_prior, d_tab);
+    CB_LAUNCH(cb::res_chunks_kernel, cdiv(n_groups + 1, 256), 256, 0, st, g.start, n_groups, d_nchunk);
+    CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_nchunk, d_choff, n_groups + 1, st);
+    g_launches.fetch_add(2);
+    int n_chunks = 0;
+    CB_CUDA(cudaMemcpyAsync(&n_chunks, d_choff + n_groups, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaStreamSynchronize(st));
+    CB_TRY(sf.alloc(&d_part, (size_t)n_chunks * S));
+    CB_LAUNCH(cb::res_score_kernel, dim3(n_chunks, cdiv(S, cb::RES_SCORE_THREADS)), cb::RES_SCORE_THREADS, 0, st,
+              cams.camtab, g.start, d_choff, g.rows, g.cam, d_pt, d_px, d_pts, n_groups, S, d_tab, tau, d_part);
+    CB_LAUNCH(cb::res_select_kernel, n_groups, cb::RES_SCORE_THREADS, 0, st, d_choff, S, d_part, d_best);
+    CB_LAUNCH(cb::res_classify_kernel, cdiv((long long)n_groups * 32, cb::TRI_THREADS), cb::TRI_THREADS, 0, st,
+              cams.camtab, g.start, g.rows, g.cam, d_pt, d_px, d_pts, n_groups, S, d_tab, d_best, tau, min_inliers,
+              d_hyp, d_gcam, d_count, d_rep, d_nin, d_cst, d_flag, d_inl);
+  } else {
+#define CB_RES_CONSENSUS(LL)                                                                                           \
+  CB_LAUNCH(cb::res_consensus_kernel<LL>, cdiv((long long)n_groups * LL, cb::TRI_THREADS), cb::TRI_THREADS, 0, st,       \
+            cams.camtab, g.start, g.rows, g.cam, d_pt, g.xy, d_px, d_pts, n_groups, tau, min_inliers, max_samples,      \
+            use_prior, d_hyp, d_gcam, d_count, d_rep, d_nin, d_cst, d_flag, d_inl)
+    if (lanes == 32) CB_RES_CONSENSUS(32);
+    else CB_RES_CONSENSUS(8);
+#undef CB_RES_CONSENSUS
+  }
+  CB_CUDA(cudaGetLastError());
+  CB_CUB(sf, cub::DeviceSelect::Flagged, g.rows, d_flag, d_crows, d_nsel, n, st);
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_nin, d_cstart, n_groups + 1, st);
+  g_launches.fetch_add(4);
+  CB_CUDA(cudaEventRecord(ev[3], st));
+
+  // refinement on the consensus rows from the winners
+  double *d_pose = nullptr, *d_rmse = nullptr;
+  int* d_status = nullptr;
+  CB_TRY(sf.alloc(&d_pose, 6 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_rmse, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_status, (size_t)n_groups));
+  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
+  CB_CUDA(cudaEventRecord(ev[4], st));
+#define CB_RES_REFINE(LL)                                                                                              \
+  CB_LAUNCH(cb::res_refine_kernel<LL>, blocks, cb::TRI_THREADS, 0, st, cams.camtab, d_cstart, d_crows, d_pt, d_px,      \
+            d_pts, n_groups, d_gcam, d_cst, d_hyp, max_iter, xtol, d_pose, d_rmse, d_status)
+  if (lanes == 32) CB_RES_REFINE(32);
+  else CB_RES_REFINE(8);
+#undef CB_RES_REFINE
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaEventRecord(ev[5], st));
+
+  // covariance: with a point covariance, the consensus rows of each group sorted by point (stable) so that each point's
+  // rows are adjacent
+  double* d_cov = nullptr;
+  if (cov_out) {
+    CB_TRY(sf.alloc(&d_cov, 36 * (size_t)n_groups));
+    CB_CUDA(cudaEventRecord(ev[6], st));
+    const int* cov_rows = d_crows;
+    if (d_pcov) {
+      const int pt_bits = std::max(1, bits_for((unsigned long long)std::max(n_pts - 1, 0)));
+      const int key_bits = std::min(64, pt_bits + bits_for((unsigned long long)n_groups));
+      unsigned long long *d_k = nullptr, *d_ks = nullptr;
+      int* d_prow = nullptr;
+      CB_TRY(sf.alloc(&d_k, (size_t)n));
+      CB_TRY(sf.alloc(&d_ks, (size_t)n));
+      CB_TRY(sf.alloc(&d_prow, (size_t)n));
+      int n_cons = 0;
+      CB_CUDA(cudaMemcpyAsync(&n_cons, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CB_CUDA(cudaStreamSynchronize(st));
+      if (n_cons > 0) {
+#define CB_RES_KEY(LL)                                                                                                 \
+  CB_LAUNCH(cb::res_pt_key_kernel<LL>, blocks, cb::TRI_THREADS, 0, st, d_cstart, d_crows, d_pt, n_groups, pt_bits, d_k)
+        if (lanes == 32) CB_RES_KEY(32);
+        else CB_RES_KEY(8);
+#undef CB_RES_KEY
+        CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, d_crows, d_prow, n_cons, 0, key_bits, st);
+        g_launches.fetch_add(2 * ((key_bits + 7) / 8));
+      }
+      cov_rows = d_prow;
+    }
+#define CB_RES_COV(LL)                                                                                                 \
+  CB_LAUNCH(cb::res_cov_kernel<LL>, blocks, cb::TRI_THREADS, 0, st, cams.camtab, d_cstart, cov_rows, d_pt, d_px, d_pts,  \
+            d_pcov, n_groups, d_gcam, d_status, d_pose, pixel_sigma * pixel_sigma, d_cov)
+    if (lanes == 32) CB_RES_COV(32);
+    else CB_RES_COV(8);
+#undef CB_RES_COV
+    CB_CUDA(cudaGetLastError());
+    CB_CUDA(cudaEventRecord(ev[7], st));
+  }
+  CB_CUDA(cudaMemcpyAsync(cam_out, d_gcam, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(pose_out, d_pose, sizeof(double) * 6 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, d_count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(n_inliers_out, d_nin, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, d_rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(inlier_out, d_inl, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (cov_out) CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 36 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (stats) {
+    stats->group_ms = ev.ms(0, 1);
+    stats->consensus_ms = ev.ms(2, 3);
+    stats->refine_ms = ev.ms(4, 5);
+    if (cov_out) stats->cov_ms = ev.ms(6, 7);
+    stats->total_ms = ev.ms(0, cov_out ? 7 : 5);
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                     int32_t n_pts, const double* pts_xyz, const double* pts_cov, int64_t n_obs, const int32_t* obs_cam,
+                     const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px, int obs_on_device,
+                     double threshold_px, int32_t min_inliers, int32_t max_samples, int32_t use_prior,
+                     double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups, int32_t* n_groups_out,
+                     int32_t* cam_out, double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
+                     int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
+                     CbResectStats* stats, int device, void* stream) {
+  if (n_cams <= 0 || !cam_flags || !cam_const || !cam_x || n_pts < 0 || (n_pts > 0 && !pts_xyz) || n_obs < 0 ||
+      n_obs > 0x7fffffffLL || !n_groups_out || max_groups < 0 ||
+      (n_obs > 0 && (!obs_cam || !obs_key || !obs_pt || !obs_px || !inlier_out || n_pts == 0)) ||
+      (max_groups > 0 && (!cam_out || !pose_out || !rmse_px_out || !count_out || !n_inliers_out || !rep_row_out ||
+                          !status_out)) ||
+      !(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma)) || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol)) ||
+      !(threshold_px > 0.0 && std::isfinite(threshold_px)) || min_inliers < 4 || max_samples < 1 ||
+      max_samples > 4096) {
+    g_last_error = "cb_resect_robust: bad argument";
+    return CB_E_INVALID;
+  }
+  return resect_impl(n_cams, cam_flags, cam_const, cam_x, n_pts, pts_xyz, pts_cov, n_obs, obs_cam, obs_key, obs_pt,
+                     obs_px, obs_on_device, threshold_px, min_inliers, max_samples, use_prior ? 1 : 0, pixel_sigma,
+                     max_iter, xtol, max_groups, n_groups_out, cam_out, pose_out, cov_out, rmse_px_out, count_out,
+                     n_inliers_out, rep_row_out, status_out, inlier_out, stats, device, stream);
 }
 
 // ------------------------------------------------------------------------------------------

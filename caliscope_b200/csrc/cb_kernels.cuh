@@ -104,11 +104,8 @@ struct CPtr2 {
   const double* p[2];
 };
 
-// camera table entry: Rodrigues, SO(3) right Jacobian, intrinsics  [bundle_parameterization.py:166-186]
-__device__ __forceinline__ void cam_prep_one(const double* __restrict__ q, const double* __restrict__ k, int flags,
-                                             double* __restrict__ o) {
-  const bool free_i = (flags & 1) != 0;
-  const double r0 = q[0], r1 = q[1], r2 = q[2];
+// rotation half of a camera table entry: Rodrigues R(r) and the SO(3) right Jacobian (CT_R, CT_JR)
+__device__ __forceinline__ void cam_prep_rot(double r0, double r1, double r2, double* __restrict__ o) {
   const double th2 = r0 * r0 + r1 * r1 + r2 * r2, th = sqrt(th2);
   double R[9];
   double s = 0.0, co = 1.0;
@@ -137,6 +134,13 @@ __device__ __forceinline__ void cam_prep_one(const double* __restrict__ q, const
     o[CT_R + i] = R[i];
     o[CT_JR + i] = ((i % 4 == 0) ? 1.0 : 0.0) - B * Km[i] + C * K2[i];
   }
+}
+
+// camera table entry: Rodrigues, SO(3) right Jacobian, intrinsics  [bundle_parameterization.py:166-186]
+__device__ __forceinline__ void cam_prep_one(const double* __restrict__ q, const double* __restrict__ k, int flags,
+                                             double* __restrict__ o) {
+  const bool free_i = (flags & 1) != 0;
+  cam_prep_rot(q[0], q[1], q[2], o);
   o[CT_T + 0] = q[3]; o[CT_T + 1] = q[4]; o[CT_T + 2] = q[5];
   double sc = 1.0, k1 = k[4], k2 = k[5];
   if (free_i) { sc = q[6]; k1 = q[7]; k2 = q[8]; }

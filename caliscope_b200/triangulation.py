@@ -291,10 +291,11 @@ def _check_device_tri_obs(obs_cam, obs_key, obs_px, device: int) -> int:
     return n
 
 
-def _calibrated_inputs(cam_flags, cam_const, cam_x, camera_cov, obs_cam, obs_key, obs_px, device: int):
+def _calibrated_inputs(cam_flags, cam_const, cam_x, camera_cov, obs_cam, obs_key, obs_px, device: int, obs_pt=None):
     """Cameras in the BA layout and observations (host arrays or CUDA tensors read in place) of the calibrated
     triangulation calls as the C ABI takes them: (n_cams, flags, const, cam_x, camera_cov or None, n, on_device,
-    observation pointers, host arrays the pointers refer to)."""
+    observation pointers, host arrays the pointers refer to).  With ``obs_pt`` (the point of each row, int32; resection)
+    its pointer follows the other three."""
     flags = np.ascontiguousarray(cam_flags, dtype=np.int32).ravel()
     nc = len(flags)
     const = np.ascontiguousarray(cam_const, dtype=np.float64).reshape(nc, 9)
@@ -311,17 +312,30 @@ def _calibrated_inputs(cam_flags, cam_const, cam_x, camera_cov, obs_cam, obs_key
     on_dev = hasattr(obs_px, "data_ptr")
     if on_dev:
         n = _check_device_tri_obs(obs_cam, obs_key, obs_px, device)
-        cam_p, key_p, px_p = (C.c_void_p(t.data_ptr()) for t in (obs_cam, obs_key, obs_px))
-    else:
-        cam = np.ascontiguousarray(obs_cam, dtype=np.int32)
-        key = np.ascontiguousarray(obs_key, dtype=np.int64)
-        px = np.ascontiguousarray(obs_px, dtype=np.float64).reshape(-1, 2)
-        n = len(cam)
-        if len(key) != n or len(px) != n:
-            raise ValueError("obs_cam, obs_key and obs_px must have one row per observation")
-        cam_p, key_p, px_p = _ptr(cam), _ptr(key), _ptr(px)
-        return nc, flags, const, cx, ccov, n, False, (cam_p, key_p, px_p), (cam, key, px)
-    return nc, flags, const, cx, ccov, n, True, (cam_p, key_p, px_p), ()
+        ptrs = tuple(C.c_void_p(t.data_ptr()) for t in (obs_cam, obs_key, obs_px))
+        if obs_pt is not None:
+            dev = getattr(obs_pt, "device", None)
+            if getattr(dev, "type", None) != "cuda" or dev.index != device:
+                raise ValueError(f"obs_pt must be a CUDA tensor on cuda:{device}, got device {dev}")
+            if str(getattr(obs_pt, "dtype", None)) != "torch.int32" or not obs_pt.is_contiguous():
+                raise ValueError(f"obs_pt must be a contiguous torch.int32 tensor, got {getattr(obs_pt, 'dtype', None)}")
+            if tuple(obs_pt.shape) != (n,):
+                raise ValueError(f"obs_pt must have shape ({n},), got {tuple(obs_pt.shape)}")
+            ptrs += (C.c_void_p(obs_pt.data_ptr()),)
+        return nc, flags, const, cx, ccov, n, True, ptrs, ()
+    cam = np.ascontiguousarray(obs_cam, dtype=np.int32)
+    key = np.ascontiguousarray(obs_key, dtype=np.int64)
+    px = np.ascontiguousarray(obs_px, dtype=np.float64).reshape(-1, 2)
+    n = len(cam)
+    if len(key) != n or len(px) != n:
+        raise ValueError("obs_cam, obs_key and obs_px must have one row per observation")
+    keep = (cam, key, px)
+    if obs_pt is not None:
+        pt = np.ascontiguousarray(obs_pt, dtype=np.int32)
+        if pt.shape != (n,):
+            raise ValueError(f"obs_pt must have one entry per observation, got shape {pt.shape}")
+        keep += (pt,)
+    return nc, flags, const, cx, ccov, n, False, tuple(_ptr(a) for a in keep), keep
 
 
 def triangulate_refined(cam_flags, cam_const, cam_x, obs_cam, obs_key, obs_px, *, pixel_sigma: float = 1.0,

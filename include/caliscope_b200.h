@@ -370,6 +370,61 @@ int cb_triangulate_robust(int32_t n_cams, const int32_t* cam_flags, const double
                           int32_t* count_out, int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out,
                           uint8_t* inlier_out, CbTriRobustStats* stats, int device, void* stream);
 
+typedef struct CbResectStats {
+  double group_ms;      /* upload + undistortion + radix sort + group boundaries */
+  double consensus_ms;  /* hypotheses, MSAC scoring, selection and the compaction of the consensus rows */
+  double refine_ms;     /* the Levenberg-Marquardt kernel on the consensus rows */
+  double cov_ms;        /* the point sort and the covariance kernel (0 without cov_out) */
+  double total_ms;
+  int32_t kernel_launches;
+  int32_t pad_;
+} CbResectStats;
+
+/* Robust resection: the pose of a camera from 2-D detections of points whose 3-D positions are known (DESIGN.md
+ * section 4.9).  Cameras in the bundle-adjustment layout as cb_triangulate_refine; pts_xyz[n_pts][3] and pts_cov
+ * (nullable) [n_pts][3][3] are host arrays; obs_pt[n_obs] indexes them.  Observations (raw pixels) are host arrays or,
+ * with obs_on_device, device pointers (obs_cam, obs_key, obs_pt, obs_px).  A group is the rows of one obs_key: one pose
+ * of one camera (key = camera, or (camera, frame)), k rows key-sorted and in caller order within a key, positions 0..k-1.
+ *   1. rows from more than one camera: status 6.  2. k < 4: status 1.
+ *   3. a row whose point is not finite is unusable: it scores tau^2, is in no sample's solution set, never an inlier.
+ *   4. candidate samples, T = C(k, 3): every triple i < j < l in lexicographic order when T <= max_samples; else sample
+ *      m = 0..max_samples-1 draws positions splitmix64(m 2^32 + t) mod k, t = 0, 1, ... (exact unsigned 64-bit;
+ *      splitmix64(x) = the standard finaliser of x + 0x9e3779b97f4a7c15), keeps the first three distinct, sorted, and
+ *      gives up after 16 draws.  No random state.
+ *   5. hypotheses of a sample of three usable rows: the Lambda Twist P3P solutions (Persson & Nordberg, ECCV 2018; up
+ *      to 4, in the solver's order) on the bearings of the float32-rounded undistorted normalised coordinates; a
+ *      solution that is not finite or puts one of its three points at Xc.z <= 0 is none.  With use_prior the pose of
+ *      the group's camera in cam_x is one more hypothesis, ranked before every sample.
+ *   6. score (MSAC): sum over all k rows of min(e_r^2, tau^2), e_r = |pi(X_r; R, t, intrinsics) - u_r| in raw pixels with
+ *      the engine's projection and the hypothesis's R; a row with Xc.z <= 0, a non-finite e_r or an unusable point adds
+ *      tau^2.  The lowest score wins, ties to the lowest (prior, sample m, solution index).
+ *   7. consensus set: the usable rows with Xc.z > 0 and e_r^2 <= tau^2 at the winner.  No hypothesis, or fewer than
+ *      min_inliers such rows: status 5 (pose, cov, rmse NaN, n_inliers 0, no row inlier).
+ *   8. Levenberg-Marquardt over q = (r, t) on the consensus rows (intrinsics fixed), from the winner's R as a rotation
+ *      vector with theta in [0, pi] (cv2.Rodrigues): H = sum J^T J, g = sum J^T r (pixels, J = d pi / d q); solve
+ *      (H + lambda diag H) d = -g, lambda0 = 1e-3; accept when the cost drops (lambda / 10) else lambda * 10; q += d;
+ *      stop when |d| <= xtol (|q| + xtol) or after max_iter steps.
+ *   9. cov = pixel_sigma^2 H^-1 + H^-1 M H^-1, M = sum_p G_p Sigma_p G_p^T, G_p = sum over the consensus rows of point p
+ *      of J_q^T J_X (6 x 3, pixels), Sigma_p = pts_cov[p] (without pts_cov the first term alone; a NaN Sigma_p in the
+ *      consensus set makes cov NaN).  It assumes the points are independent of each other and of the group's own
+ *      observations and uses only each point's marginal: triangulate them without the resected camera's rows.
+ *  10. status, first match wins: 6;  1;  5;  2 H not positive definite at the start or at the solution (a Cholesky
+ *      pivot <= 1e-12 of the Jacobi-scaled D^-1/2 H D^-1/2; pose = the hypothesis, cov NaN);  3 max_iter reached;  4 a
+ *      consensus row has Xc.z <= 0 at q*;  0 none.
+ * Arguments: threshold_px tau finite > 0, min_inliers >= 4, 1 <= max_samples <= 4096, max_iter >= 1, finite
+ * pixel_sigma >= 0 and xtol >= 0; obs_pt in [0, n_pts).
+ * Outputs per group in ascending key order (host, room for max_groups): cam (the camera slot), pose[6] = (r, t) in x's
+ * camera layout, cov[36] (nullable), rmse_px over the consensus rows, count, n_inliers, rep_row, status; inlier[n_obs]
+ * (caller order).  No floating-point atomics: repeated calls return bit-identical outputs. */
+int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                     int32_t n_pts, const double* pts_xyz, const double* pts_cov, int64_t n_obs, const int32_t* obs_cam,
+                     const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px, int obs_on_device,
+                     double threshold_px, int32_t min_inliers, int32_t max_samples, int32_t use_prior,
+                     double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups, int32_t* n_groups_out,
+                     int32_t* cam_out, double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
+                     int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
+                     CbResectStats* stats, int device, void* stream);
+
 /* Optional NCCL transport owned by the engine (no host callback per all-reduce).  NCCL is resolved at run time from
  * the libnccl the process already has loaded (PyTorch's).  Rank 0 calls cb_nccl_unique_id and distributes the 128
  * bytes (e.g. torch.distributed.broadcast); every rank then calls cb_nccl_comm_create (collective). */
