@@ -337,4 +337,54 @@ __device__ __forceinline__ double obs_jac(const double* __restrict__ cam, double
   return cost;
 }
 
+// ---- the lanes of one group ----------------------------------------------------------------------------------------
+// A group owns LANES consecutive, aligned lanes of a warp, so xor offsets below LANES stay inside it.  The reductions
+// are xor butterflies over s = LANES/2 ... 1: every lane of the group ends with the identical result, summed in one
+// fixed order.  Every lane of the warp must take part, live group or not.
+
+// the group's sum of a scalar
+template <int LANES, typename T>
+[[nodiscard]] __device__ __forceinline__ T group_sum(T v) {
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1) v += __shfl_xor_sync(0xffffffffu, v, s);
+  return v;
+}
+
+// the group's sums of an array, in place
+template <int LANES, typename T, int N>
+__device__ __forceinline__ void group_sum(T (&v)[N]) {
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1)
+#pragma unroll
+    for (int k = 0; k < N; ++k) v[k] += __shfl_xor_sync(0xffffffffu, v[k], s);
+}
+
+template <int LANES>
+[[nodiscard]] __device__ __forceinline__ int group_or(int v) {
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1) v |= __shfl_xor_sync(0xffffffffu, v, s);
+  return v;
+}
+
+// the lowest score of the group, the lowest index on a tie, in place
+template <int LANES>
+__device__ __forceinline__ void group_argmin(double& score, long long& index) {
+#pragma unroll
+  for (int s = LANES / 2; s > 0; s >>= 1) {
+    const double os = __shfl_xor_sync(0xffffffffu, score, s);
+    const long long oi = __shfl_xor_sync(0xffffffffu, index, s);
+    if (os < score || (os == score && oi < index)) {
+      score = os;
+      index = oi;
+    }
+  }
+}
+
+// v from lane `owner` of the group to all its lanes
+template <int LANES, int N>
+__device__ __forceinline__ void group_bcast(double (&v)[N], int owner) {
+#pragma unroll
+  for (int q = 0; q < N; ++q) v[q] = __shfl_sync(0xffffffffu, v[q], owner, LANES);
+}
+
 }  // namespace cb

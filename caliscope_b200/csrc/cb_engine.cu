@@ -29,6 +29,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/caliscope_b200.h"
@@ -2938,6 +2939,14 @@ int obs_group_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, in
 // bounds the DLT kernel, so more groups per warp wins until groups get very long (more than 96 rows on average).
 int tri_lanes(int n, int n_groups) { return (n / std::max(n_groups, 1) > 96) ? 32 : 8; }
 
+// f(L) with L a std::integral_constant of the lanes per group (32, else 8), for launching the kernel instantiated
+// for them
+template <typename F>
+void with_lanes(int lanes, F&& f) {
+  if (lanes == 32) f(std::integral_constant<int, 32>{});
+  else f(std::integral_constant<int, 8>{});
+}
+
 // the DLT of every group (buffers held by the call's workspace)
 struct TriDlt {
   double* xyz = nullptr;
@@ -2958,12 +2967,10 @@ int tri_dlt_launch(int32_t n_cams, const double* d_proj, const ObsGroups& g, int
   const int in_smem = proj_bytes <= 40 * 1024 ? 1 : 0;
   const long long threads = (long long)n_groups * lanes;
   CB_CUDA(cudaEventRecord(ev_a, st));
-  if (lanes == 32)
-    CB_LAUNCH(cb::tri_dlt_kernel<32>, cdiv(threads, cb::TRI_THREADS), cb::TRI_THREADS, in_smem ? proj_bytes : 0, st,
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::tri_dlt_kernel<L.value>, cdiv(threads, cb::TRI_THREADS), cb::TRI_THREADS, in_smem ? proj_bytes : 0, st,
               d_proj, n_cams, in_smem, g.start, g.rows, g.cam, g.xy, n_groups, t->xyz, t->count, t->rep, t->sig);
-  else
-    CB_LAUNCH(cb::tri_dlt_kernel<8>, cdiv(threads, cb::TRI_THREADS), cb::TRI_THREADS, in_smem ? proj_bytes : 0, st,
-              d_proj, n_cams, in_smem, g.start, g.rows, g.cam, g.xy, n_groups, t->xyz, t->count, t->rep, t->sig);
+  });
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev_b, st));
   return CB_OK;
@@ -3073,32 +3080,50 @@ struct TriConsensusArgs {
   uint8_t* inlier_out;
 };
 
-// the consensus of every group of `g` and the compaction of its rows (buffers held by the call's workspace)
-struct TriConsensus {
-  double* hyp = nullptr;         // the selected hypothesis of every group
-  int *count = nullptr, *rep = nullptr, *nin = nullptr, *status = nullptr;
+// The outputs of a consensus stage (tri_consensus_kernel, the resection consensus kernels) and the compaction of its
+// rows, buffers held by the call's workspace
+struct Consensus {
+  double* hyp = nullptr;         // the selected hypothesis of every group, hyp_width doubles each
+  int* cam = nullptr;            // the camera of every group (resection only)
+  int *count = nullptr, *rep = nullptr, *status = nullptr;
+  int* nin = nullptr;            // consensus rows per group, and a zero past the end for the scan
+  unsigned char* flag = nullptr;  // consensus rows, key-sorted position
   unsigned char* inl = nullptr;  // caller-order inlier mask
   int *rows = nullptr, *start = nullptr;  // the consensus rows of every group, in key-sorted order, and their group starts
+  int* n_rows = nullptr;         // the number of consensus rows
 };
 
-// tri_consensus_kernel over the groups of `g`, then the compaction of the consensus rows; ev_a / ev_b around both
-int tri_consensus_launch(int32_t n_cams, const TriCams& cams, const double* d_proj, const ObsGroups& g, int lanes, int n,
-                         const double* px, const TriConsensusArgs& a, cudaEvent_t ev_a, cudaEvent_t ev_b, ScopedFree& sf,
-                         cudaStream_t st, TriConsensus* c) {
-  const int n_groups = g.n_groups;
-  // hypothesis, count, rep_row, n_inliers (+ a zero past the end for the scan), status 0 / 1 / 5, flags
-  unsigned char* d_flag = nullptr;
-  int* d_nsel = nullptr;
-  CB_TRY(sf.alloc(&c->hyp, 3 * (size_t)n_groups));
+// allocates the outputs of a consensus stage over n rows in n_groups groups (with_cam: and the camera of each group)
+int consensus_alloc(int n_groups, int n, int hyp_width, bool with_cam, ScopedFree& sf, cudaStream_t st, Consensus* c) {
+  CB_TRY(sf.alloc(&c->hyp, (size_t)hyp_width * n_groups));
+  if (with_cam) CB_TRY(sf.alloc(&c->cam, (size_t)n_groups));
   CB_TRY(sf.alloc(&c->count, (size_t)n_groups));
   CB_TRY(sf.alloc(&c->rep, (size_t)n_groups));
   CB_TRY(sf.alloc(&c->nin, (size_t)n_groups + 1));
   CB_TRY(sf.alloc(&c->status, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_flag, (size_t)n));
+  CB_TRY(sf.alloc(&c->flag, (size_t)n));
   CB_TRY(sf.alloc(&c->inl, (size_t)n));
   CB_TRY(sf.alloc(&c->rows, (size_t)n));
   CB_TRY(sf.alloc(&c->start, (size_t)n_groups + 1));
-  CB_TRY(sf.alloc(&d_nsel, 1));
+  CB_TRY(sf.alloc(&c->n_rows, 1));
+  CB_CUDA(cudaMemsetAsync(c->nin + n_groups, 0, sizeof(int), st));
+  return CB_OK;
+}
+
+// the flagged rows of the key-sorted `rows` into c->rows, and the start of each group's among them into c->start
+int consensus_compact(int* rows, int n, int n_groups, ScopedFree& sf, cudaStream_t st, Consensus* c) {
+  CB_CUB(sf, cub::DeviceSelect::Flagged, rows, c->flag, c->rows, c->n_rows, n, st);
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, c->nin, c->start, n_groups + 1, st);
+  g_launches.fetch_add(4);
+  return CB_OK;
+}
+
+// tri_consensus_kernel over the groups of `g`, then the compaction of the consensus rows; ev_a / ev_b around both
+int tri_consensus_launch(int32_t n_cams, const TriCams& cams, const double* d_proj, const ObsGroups& g, int lanes, int n,
+                         const double* px, const TriConsensusArgs& a, cudaEvent_t ev_a, cudaEvent_t ev_b, ScopedFree& sf,
+                         cudaStream_t st, Consensus* c) {
+  const int n_groups = g.n_groups;
+  CB_TRY(consensus_alloc(n_groups, n, 3, false, sf, st, c));
 
   // camera table and projection table each in shared memory when it takes at most 40 KB
   const size_t cam_smem = tri_camtab_smem(n_cams);
@@ -3110,19 +3135,14 @@ int tri_consensus_launch(int32_t n_cams, const TriCams& cams, const double* d_pr
     CB_CUDA(cudaFuncSetAttribute(cb::tri_consensus_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   }
   const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
-  CB_CUDA(cudaMemsetAsync(c->nin + n_groups, 0, sizeof(int), st));
   CB_CUDA(cudaEventRecord(ev_a, st));
-#define CB_TRI_CONSENSUS(LL)                                                                                           \
-  CB_LAUNCH(cb::tri_consensus_kernel<LL>, blocks, cb::TRI_THREADS, smem, st, cams.camtab, cam_smem ? 1 : 0, d_proj,     \
-            proj_smem ? 1 : 0, n_cams, g.start, g.rows, g.cam, g.xy, px, n_groups, a.threshold_px, a.min_inliers,       \
-            a.max_pairs, c->hyp, c->count, c->rep, c->nin, c->status, d_flag, c->inl)
-  if (lanes == 32) CB_TRI_CONSENSUS(32);
-  else CB_TRI_CONSENSUS(8);
-#undef CB_TRI_CONSENSUS
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::tri_consensus_kernel<L.value>, blocks, cb::TRI_THREADS, smem, st, cams.camtab, cam_smem ? 1 : 0,
+              d_proj, proj_smem ? 1 : 0, n_cams, g.start, g.rows, g.cam, g.xy, px, n_groups, a.threshold_px,
+              a.min_inliers, a.max_pairs, c->hyp, c->count, c->rep, c->nin, c->status, c->flag, c->inl);
+  });
   CB_CUDA(cudaGetLastError());
-  CB_CUB(sf, cub::DeviceSelect::Flagged, g.rows, d_flag, c->rows, d_nsel, n, st);
-  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, c->nin, c->start, n_groups + 1, st);
-  g_launches.fetch_add(4);
+  CB_TRY(consensus_compact(g.rows, n, n_groups, sf, st, c));
   CB_CUDA(cudaEventRecord(ev_b, st));
   return CB_OK;
 }
@@ -3134,12 +3154,10 @@ int tri_refine_launch(int32_t n_cams, const TriCams& c, int lanes, const int* st
   const size_t smem = tri_camtab_smem(n_cams);
   const int cam_in_smem = smem ? 1 : 0;
   const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
-  if (lanes == 32)
-    CB_LAUNCH(cb::tri_refine_kernel<32>, blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem, start, rows,
-              cam, px, n_groups, xyz0, max_iter, xtol, xyz, rmse, status);
-  else
-    CB_LAUNCH(cb::tri_refine_kernel<8>, blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem, start, rows,
-              cam, px, n_groups, xyz0, max_iter, xtol, xyz, rmse, status);
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::tri_refine_kernel<L.value>, blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem, start,
+              rows, cam, px, n_groups, xyz0, max_iter, xtol, xyz, rmse, status);
+  });
   CB_CUDA(cudaGetLastError());
   return CB_OK;
 }
@@ -3176,14 +3194,14 @@ int tri_cov_launch(int32_t n_cams, const TriCams& c, const double* cam_cov, doub
   const int cam_in_smem = smem ? 1 : 0;
   const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
   CB_CUDA(cudaEventRecord(ev_a, st));
-#define CB_TRI_COV(PP, LL)                                                                                             \
-  CB_LAUNCH((cb::tri_cov_kernel<PP, LL>), blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem, start, rows, \
-            cam, px, n_groups, xyz, status, d_sig, s2, d_B, d_first, d_cov)
-  if (P == 9 && lanes == 32) CB_TRI_COV(9, 32);
-  else if (P == 9) CB_TRI_COV(9, 8);
-  else if (lanes == 32) CB_TRI_COV(6, 32);
-  else CB_TRI_COV(6, 8);
-#undef CB_TRI_COV
+  with_lanes(lanes, [&](auto L) {
+    if (P == 9)
+      CB_LAUNCH((cb::tri_cov_kernel<9, L.value>), blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem,
+                start, rows, cam, px, n_groups, xyz, status, d_sig, s2, d_B, d_first, d_cov);
+    else
+      CB_LAUNCH((cb::tri_cov_kernel<6, L.value>), blocks, cb::TRI_THREADS, smem, st, c.camtab, n_cams, cam_in_smem,
+                start, rows, cam, px, n_groups, xyz, status, d_sig, s2, d_B, d_first, d_cov);
+  });
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev_b, st));
   *d_cov_out = d_cov;
@@ -3278,7 +3296,7 @@ int tri_calibrated(int32_t n_cams, const int32_t* cam_flags, const double* cam_c
   const int n_groups = g.n_groups, lanes = tri_lanes(n, n_groups);
   const double* xyz0 = nullptr;
   const int *count = nullptr, *rep = nullptr, *start = g.start, *rows = g.rows;
-  TriConsensus cs;
+  Consensus cs;
   if (robust) {
     CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
     CB_TRY(tri_consensus_launch(n_cams, cams, d_proj, g, lanes, n, d_px, *robust, ev[2], ev[3], sf, st, &cs));
@@ -3464,23 +3482,9 @@ int resect_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_cons
                           (size_t)n_groups * S * cb::RES_HYP * sizeof(double) <= RES_TABLE_BYTES;
   const int lanes = long_shape ? 32 : tri_lanes(n, n_groups);
 
-  // consensus: winner, cam, count, rep_row, n_inliers (+ a zero past the end for the scan), status 0 / 1 / 5 / 6, flags
-  double* d_hyp = nullptr;
-  int *d_gcam = nullptr, *d_count = nullptr, *d_rep = nullptr, *d_nin = nullptr, *d_cst = nullptr, *d_nsel = nullptr;
-  int *d_crows = nullptr, *d_cstart = nullptr;
-  unsigned char *d_flag = nullptr, *d_inl = nullptr;
-  CB_TRY(sf.alloc(&d_hyp, (size_t)cb::RES_HYP * n_groups));
-  CB_TRY(sf.alloc(&d_gcam, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_count, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_rep, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_nin, (size_t)n_groups + 1));
-  CB_TRY(sf.alloc(&d_cst, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_flag, (size_t)n));
-  CB_TRY(sf.alloc(&d_inl, (size_t)n));
-  CB_TRY(sf.alloc(&d_crows, (size_t)n));
-  CB_TRY(sf.alloc(&d_cstart, (size_t)n_groups + 1));
-  CB_TRY(sf.alloc(&d_nsel, 1));
-  CB_CUDA(cudaMemsetAsync(d_nin + n_groups, 0, sizeof(int), st));
+  // consensus: winner, cam, count, rep_row, n_inliers, status 0 / 1 / 5 / 6, flags
+  Consensus cs;
+  CB_TRY(consensus_alloc(n_groups, n, cb::RES_HYP, true, sf, st, &cs));
   CB_CUDA(cudaEventRecord(ev[2], st));
   if (long_shape) {
     double *d_tab = nullptr, *d_part = nullptr;
@@ -3504,20 +3508,17 @@ int resect_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_cons
     CB_LAUNCH(cb::res_select_kernel, n_groups, cb::RES_SCORE_THREADS, 0, st, d_choff, S, d_part, d_best);
     CB_LAUNCH(cb::res_classify_kernel, cdiv((long long)n_groups * 32, cb::TRI_THREADS), cb::TRI_THREADS, 0, st,
               cams.camtab, g.start, g.rows, g.cam, d_pt, d_px, d_pts, n_groups, S, d_tab, d_best, tau, min_inliers,
-              d_hyp, d_gcam, d_count, d_rep, d_nin, d_cst, d_flag, d_inl);
+              cs.hyp, cs.cam, cs.count, cs.rep, cs.nin, cs.status, cs.flag, cs.inl);
   } else {
-#define CB_RES_CONSENSUS(LL)                                                                                           \
-  CB_LAUNCH(cb::res_consensus_kernel<LL>, cdiv((long long)n_groups * LL, cb::TRI_THREADS), cb::TRI_THREADS, 0, st,       \
-            cams.camtab, g.start, g.rows, g.cam, d_pt, g.xy, d_px, d_pts, n_groups, tau, min_inliers, max_samples,      \
-            use_prior, d_hyp, d_gcam, d_count, d_rep, d_nin, d_cst, d_flag, d_inl)
-    if (lanes == 32) CB_RES_CONSENSUS(32);
-    else CB_RES_CONSENSUS(8);
-#undef CB_RES_CONSENSUS
+    with_lanes(lanes, [&](auto L) {
+      CB_LAUNCH(cb::res_consensus_kernel<L.value>, cdiv((long long)n_groups * L.value, cb::TRI_THREADS),
+                cb::TRI_THREADS, 0, st, cams.camtab, g.start, g.rows, g.cam, d_pt, g.xy, d_px, d_pts, n_groups, tau,
+                min_inliers, max_samples, use_prior, cs.hyp, cs.cam, cs.count, cs.rep, cs.nin, cs.status, cs.flag,
+                cs.inl);
+    });
   }
   CB_CUDA(cudaGetLastError());
-  CB_CUB(sf, cub::DeviceSelect::Flagged, g.rows, d_flag, d_crows, d_nsel, n, st);
-  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_nin, d_cstart, n_groups + 1, st);
-  g_launches.fetch_add(4);
+  CB_TRY(consensus_compact(g.rows, n, n_groups, sf, st, &cs));
   CB_CUDA(cudaEventRecord(ev[3], st));
 
   // refinement on the consensus rows from the winners
@@ -3528,12 +3529,10 @@ int resect_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_cons
   CB_TRY(sf.alloc(&d_status, (size_t)n_groups));
   const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
   CB_CUDA(cudaEventRecord(ev[4], st));
-#define CB_RES_REFINE(LL)                                                                                              \
-  CB_LAUNCH(cb::res_refine_kernel<LL>, blocks, cb::TRI_THREADS, 0, st, cams.camtab, d_cstart, d_crows, d_pt, d_px,      \
-            d_pts, n_groups, d_gcam, d_cst, d_hyp, max_iter, xtol, d_pose, d_rmse, d_status)
-  if (lanes == 32) CB_RES_REFINE(32);
-  else CB_RES_REFINE(8);
-#undef CB_RES_REFINE
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::res_refine_kernel<L.value>, blocks, cb::TRI_THREADS, 0, st, cams.camtab, cs.start, cs.rows, d_pt,
+              d_px, d_pts, n_groups, cs.cam, cs.status, cs.hyp, max_iter, xtol, d_pose, d_rmse, d_status);
+  });
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[5], st));
 
@@ -3543,7 +3542,7 @@ int resect_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_cons
   if (cov_out) {
     CB_TRY(sf.alloc(&d_cov, 36 * (size_t)n_groups));
     CB_CUDA(cudaEventRecord(ev[6], st));
-    const int* cov_rows = d_crows;
+    const int* cov_rows = cs.rows;
     if (d_pcov) {
       const int pt_bits = std::max(1, bits_for((unsigned long long)std::max(n_pts - 1, 0)));
       const int key_bits = std::min(64, pt_bits + bits_for((unsigned long long)n_groups));
@@ -3553,36 +3552,33 @@ int resect_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_cons
       CB_TRY(sf.alloc(&d_ks, (size_t)n));
       CB_TRY(sf.alloc(&d_prow, (size_t)n));
       int n_cons = 0;
-      CB_CUDA(cudaMemcpyAsync(&n_cons, d_nsel, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CB_CUDA(cudaMemcpyAsync(&n_cons, cs.n_rows, sizeof(int), cudaMemcpyDeviceToHost, st));
       CB_CUDA(cudaStreamSynchronize(st));
       if (n_cons > 0) {
-#define CB_RES_KEY(LL)                                                                                                 \
-  CB_LAUNCH(cb::res_pt_key_kernel<LL>, blocks, cb::TRI_THREADS, 0, st, d_cstart, d_crows, d_pt, n_groups, pt_bits, d_k)
-        if (lanes == 32) CB_RES_KEY(32);
-        else CB_RES_KEY(8);
-#undef CB_RES_KEY
-        CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, d_crows, d_prow, n_cons, 0, key_bits, st);
+        with_lanes(lanes, [&](auto L) {
+          CB_LAUNCH(cb::res_pt_key_kernel<L.value>, blocks, cb::TRI_THREADS, 0, st, cs.start, cs.rows, d_pt, n_groups,
+                    pt_bits, d_k);
+        });
+        CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, cs.rows, d_prow, n_cons, 0, key_bits, st);
         g_launches.fetch_add(2 * ((key_bits + 7) / 8));
       }
       cov_rows = d_prow;
     }
-#define CB_RES_COV(LL)                                                                                                 \
-  CB_LAUNCH(cb::res_cov_kernel<LL>, blocks, cb::TRI_THREADS, 0, st, cams.camtab, d_cstart, cov_rows, d_pt, d_px, d_pts,  \
-            d_pcov, n_groups, d_gcam, d_status, d_pose, pixel_sigma * pixel_sigma, d_cov)
-    if (lanes == 32) CB_RES_COV(32);
-    else CB_RES_COV(8);
-#undef CB_RES_COV
+    with_lanes(lanes, [&](auto L) {
+      CB_LAUNCH(cb::res_cov_kernel<L.value>, blocks, cb::TRI_THREADS, 0, st, cams.camtab, cs.start, cov_rows, d_pt,
+                d_px, d_pts, d_pcov, n_groups, cs.cam, d_status, d_pose, pixel_sigma * pixel_sigma, d_cov);
+    });
     CB_CUDA(cudaGetLastError());
     CB_CUDA(cudaEventRecord(ev[7], st));
   }
-  CB_CUDA(cudaMemcpyAsync(cam_out, d_gcam, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(cam_out, cs.cam, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(pose_out, d_pose, sizeof(double) * 6 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(count_out, d_count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(n_inliers_out, d_nin, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rep_row_out, d_rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, cs.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(n_inliers_out, cs.nin, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, cs.rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(inlier_out, d_inl, (size_t)n, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(inlier_out, cs.inl, (size_t)n, cudaMemcpyDeviceToHost, st));
   if (cov_out) CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 36 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   if (stats) {
@@ -3751,13 +3747,11 @@ int cb_stereo_rmse(int32_t n_cams, const int32_t* cam_fisheye, const double* cam
   CB_TRY(sf.alloc(&d_v, (size_t)m));
   CB_TRY(sf.alloc(&d_vs, (size_t)m));
   CB_CUDA(cudaEventRecord(ev[2], st));
-  const int lanes = (n / std::max(n_groups, 1) > 12) ? 32 : 8;
-  if (lanes == 32)
-    CB_LAUNCH(cb::stereo_pairs_kernel<32>, cdiv((long long)n_groups * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, d_start, g.rows,
-              g.cam, g.xy, n_groups, (const long long*)d_slot_start, (int)n_cams, d_pair_of, d_Rt, (int)n_pairs, d_k, d_v);
-  else
-    CB_LAUNCH(cb::stereo_pairs_kernel<8>, cdiv((long long)n_groups * 8, cb::BS_THREADS), cb::BS_THREADS, 0, st, d_start, g.rows,
-              g.cam, g.xy, n_groups, (const long long*)d_slot_start, (int)n_cams, d_pair_of, d_Rt, (int)n_pairs, d_k, d_v);
+  with_lanes((n / std::max(n_groups, 1) > 12) ? 32 : 8, [&](auto L) {
+    CB_LAUNCH(cb::stereo_pairs_kernel<L.value>, cdiv((long long)n_groups * L.value, cb::BS_THREADS), cb::BS_THREADS, 0,
+              st, d_start, g.rows, g.cam, g.xy, n_groups, (const long long*)d_slot_start, (int)n_cams, d_pair_of, d_Rt,
+              (int)n_pairs, d_k, d_v);
+  });
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[3], st));
   // stable sort by pair id, then one segmented sum per pair (fixed order => reproducible sums)

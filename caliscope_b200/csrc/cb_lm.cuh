@@ -33,14 +33,6 @@ struct LmLogRow {
   double nit, nfev, cost, cost_new, ratio, lam, step, gnorm, pcg;
 };
 
-// sum over the LANES lanes of a sub-warp group (groups are aligned, so xor offsets below LANES stay inside one)
-template <int LANES>
-__device__ __forceinline__ double group_sum(double v) {
-#pragma unroll
-  for (int o = LANES / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ---------------------------------------------------------------------------------------------
 // Point pass.  LANES lanes per point (32 / LANES points per warp), persistent grid-stride over points so the camera
 // table is staged into shared memory once per CTA.  DUPS: repeated (camera, point) rows exist (static objects seen

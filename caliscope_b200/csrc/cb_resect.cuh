@@ -326,7 +326,7 @@ __device__ __forceinline__ double res_score_rows(const double* cam, const double
     const double* X = pts + 3 * (size_t)obs_pt[r];
     bool front;
     const double e2 = res_row_err2(cam, R, t, X[0], X[1], X[2], reinterpret_cast<const double2*>(obs_px)[r], front);
-    score += (front && e2 <= tau2) ? e2 : tau2;
+    score += msac_term(front, e2, tau2);
   }
   return score;
 }
@@ -338,16 +338,13 @@ __device__ __forceinline__ int res_group_cam(const int* __restrict__ rows, const
   const int c0 = live && e > b ? obs_cam[rows[b]] : 0;
   int m = 0;
   for (int i = b + lane; i < e; i += LANES) m |= obs_cam[rows[i]] != c0;
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) m |= __shfl_xor_sync(0xffffffffu, m, s);
+  m = group_or<LANES>(m);
   multi = m != 0;
   return c0;
 }
 
-// Classification at the winner (R, t) (found: there is one) and the group's outputs: each lane flags its rows (usable,
-// in front, e_r^2 <= tau^2) into `pos_flag` (key-sorted position) and `inlier` (caller row); both are cleared when the
-// group has fewer than min_inliers consensus rows.  Lane 0 writes cam, count, rep_row, n_inliers, status (6, 1, 5 or 0)
-// and the winner (NaN without consensus).
+// consensus_classify at the winner (R, t) (found: there is one), then the group's outputs: lane 0 writes cam, count,
+// rep_row, n_inliers, status (6, 1, 5 or 0) and the winner (NaN without consensus).
 template <int LANES>
 __device__ __forceinline__ void res_classify(const double* cam, const double* R, const double* t, bool found, int st,
                                              int c0, const int* __restrict__ rows, const int* __restrict__ obs_pt,
@@ -357,28 +354,14 @@ __device__ __forceinline__ void res_classify(const double* cam, const double* R,
                                              int* __restrict__ rep_row, int* __restrict__ n_inliers,
                                              int* __restrict__ status, unsigned char* __restrict__ pos_flag,
                                              unsigned char* __restrict__ inlier) {
-  int nin = 0;
-  for (int i = b + lane; i < e; i += LANES) {
-    const int r = rows[i];
-    bool in = false;
-    if (found) {
-      const double* X = pts + 3 * (size_t)obs_pt[r];
-      bool front;
-      const double e2 = res_row_err2(cam, R, t, X[0], X[1], X[2], reinterpret_cast<const double2*>(obs_px)[r], front);
-      in = front && e2 <= tau2;
-    }
-    pos_flag[i] = in ? 1 : 0;
-    inlier[r] = in ? 1 : 0;
-    nin += in ? 1 : 0;
-  }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) nin += __shfl_xor_sync(0xffffffffu, nin, s);
-  const bool ok = found && nin >= min_inliers;
-  if (!ok && nin > 0)
-    for (int i = b + lane; i < e; i += LANES) {
-      pos_flag[i] = 0;
-      inlier[rows[i]] = 0;
-    }
+  int nin;
+  const bool ok = consensus_classify<LANES>(
+      found, rows, b, e, lane, tau2, min_inliers,
+      [&](int r, bool& front) {
+        const double* X = pts + 3 * (size_t)obs_pt[r];
+        return res_row_err2(cam, R, t, X[0], X[1], X[2], reinterpret_cast<const double2*>(obs_px)[r], front);
+      },
+      pos_flag, inlier, nin);
   if (!live || lane != 0) return;
   cam_out[g] = c0;
   count[g] = e - b;
@@ -400,7 +383,7 @@ __device__ __forceinline__ int res_pre_status(bool multi, int k) {
 // One group per LANES lanes.  Task 0 is the prior (the camera's pose in the table, when use_prior), task 1 + m sample m;
 // the lanes stride over the tasks, each scores its task's hypotheses over all k rows and keeps the lowest score (slots
 // increase along a lane's tasks, so the first of equal scores stays).  An xor butterfly over (score, slot) picks the
-// winner, which reaches the group's lanes by shuffle from the lane that owns its task; then res_classify.
+// winner (group_argmin), which reaches the group's lanes by shuffle from the lane that owns its task; then res_classify.
 template <int LANES>
 __global__ void __launch_bounds__(TRI_THREADS)
 res_consensus_kernel(const double* __restrict__ camtab, const int* __restrict__ start, const int* __restrict__ rows,
@@ -471,22 +454,12 @@ res_consensus_kernel(const double* __restrict__ camtab, const int* __restrict__ 
       }
     }
   }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) {
-    const double ob = __shfl_xor_sync(0xffffffffu, best, s);
-    const long long os = __shfl_xor_sync(0xffffffffu, best_s, s);
-    if (ob < best || (ob == best && os < best_s)) {
-      best = ob;
-      best_s = os;
-    }
-  }
+  group_argmin<LANES>(best, best_s);
   const bool found = best < inf;
   const long long task = found ? (best_s == 0 ? 0 : 1 + (best_s - 1) / RES_SLOTS_PER_SAMPLE) : 0;
   const int owner = (int)(task % LANES);
-#pragma unroll
-  for (int q = 0; q < 9; ++q) bR[q] = __shfl_sync(0xffffffffu, bR[q], owner, LANES);
-#pragma unroll
-  for (int q = 0; q < 3; ++q) bt[q] = __shfl_sync(0xffffffffu, bt[q], owner, LANES);
+  group_bcast<LANES>(bR, owner);
+  group_bcast<LANES>(bt, owner);
   res_classify<LANES>(cam, bR, bt, found, st, c0, rows, obs_pt, obs_px, pts, b, e, lane, live, g, tau2, min_inliers, hyp,
                       cam_out, count, rep_row, n_inliers, status, pos_flag, inlier);
 }
@@ -586,7 +559,7 @@ res_score_kernel(const double* __restrict__ camtab, const int* __restrict__ star
       bool front;
       const double* v = s_row + 5 * i;
       const double e2 = res_row_err2(cam, R, t, v[0], v[1], v[2], make_double2(v[3], v[4]), front);
-      score += (front && e2 <= tau2) ? e2 : tau2;
+      score += msac_term(front, e2, tau2);
     }
   }
   part[(size_t)chunk * S + s] = score;
@@ -721,7 +694,7 @@ template <int LANES>
 __device__ __forceinline__ void res_normal_eq(const double* cam, const double* q, const int* __restrict__ rows,
                                               const int* __restrict__ obs_pt, const double* __restrict__ obs_px,
                                               const double* __restrict__ pts, int b, int e, int lane, bool on,
-                                              double acc[28]) {
+                                              double (&acc)[28]) {
 #pragma unroll
   for (int k = 0; k < 28; ++k) acc[k] = 0.0;
   if (on) {
@@ -740,10 +713,7 @@ __device__ __forceinline__ void res_normal_eq(const double* cam, const double* q
       acc[27] = fma(rr[0], rr[0], fma(rr[1], rr[1], acc[27]));
     }
   }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1)
-#pragma unroll
-    for (int k = 0; k < 28; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], s);
+  group_sum<LANES>(acc);
 }
 
 // Cholesky factor L (row-major lower, 6x6) of packed symmetric h; returns whether every pivot exceeds `thr`
@@ -801,10 +771,8 @@ __device__ __forceinline__ void res_chol6_solve(const double L[6][6], double* v)
   }
 }
 
-// Per group with consensus (status 0 from the consensus stage), Levenberg-Marquardt over q = (r, t) on the consensus rows
-// (start, rows) from the winner hyp (R to a rotation vector by res_rot_log): solve (H + lam diag H) d = -g, accept when
-// the cost drops (lam /= 10) else lam *= 10, q += d; stop when |d| <= xtol (|q| + xtol) or after max_iter steps.  Every
-// lane of a group holds the same sums and takes the same decision.  Writes pose (the hypothesis for status 2, NaN
+// Per group with consensus (status 0 from the consensus stage), Levenberg-Marquardt (lm_iterate) over q = (r, t) on the
+// consensus rows (start, rows) from the winner hyp (R to a rotation vector by res_rot_log).  Writes pose (the hypothesis for status 2, NaN
 // without consensus), rmse over the consensus rows and status (the consensus stage's 1, 5, 6, else 2, 3, 4 or 0).
 template <int LANES>
 __global__ void __launch_bounds__(TRI_THREADS)
@@ -843,79 +811,55 @@ res_refine_kernel(const double* __restrict__ camtab, const int* __restrict__ sta
       for (int k = 0; k < 28; ++k) sa[k] = acc[k];
     cost = acc[27];
   }
-  __syncwarp();
   const double cost0 = cost;
-  bool active = on && st == TRI_OK;
-  double lam = TRI_LAMBDA0;
-  int it = 0;
-  while (__any_sync(0xffffffffu, active)) {
-    if (active && it == max_iter) {
-      st = TRI_MAX_ITER;
-      active = false;
-    }
-    double d[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0}, qt[6];
-    if (active) {
-      double A[21], L[6][6];
+  double tr[28];  // the sums at the trial pose
+  st = lm_iterate<6>(
+      q, on && st == TRI_OK, st, max_iter, xtol,
+      [&](double lam, bool on_, double* d) {
+        __syncwarp();  // lane 0's last write of sa is visible
+        if (!on_) return;
+        double A[21], L[6][6];
 #pragma unroll
-      for (int k = 0; k < 21; ++k) A[k] = sa[k];
+        for (int k = 0; k < 21; ++k) A[k] = sa[k];
 #pragma unroll
-      for (int k = 0; k < 6; ++k) {
-        A[res_ut(k, k)] = sa[res_ut(k, k)] * (1.0 + lam);
-        d[k] = -sa[21 + k];
-      }
-      res_chol6(A, 0.0, L);
-      res_chol6_solve(L, d);
-    }
-#pragma unroll
-    for (int k = 0; k < 6; ++k) qt[k] = q[k] + d[k];
-    double tr[28];
-    res_normal_eq<LANES>(ce, qt, rows, obs_pt, obs_px, pts, b, e, lane, active, tr);
-    __syncwarp();  // every lane has read sa
-    if (active) {
-      ++it;
-      double dn = 0.0, qn = 0.0;
-#pragma unroll
-      for (int k = 0; k < 6; ++k) {
-        dn += d[k] * d[k];
-        qn += q[k] * q[k];
-      }
-      dn = sqrt(dn);
-      qn = sqrt(qn);
-      if (tr[27] < cost) {
-#pragma unroll
-        for (int k = 0; k < 6; ++k) q[k] = qt[k];
+        for (int k = 0; k < 6; ++k) {
+          A[res_ut(k, k)] = sa[res_ut(k, k)] * (1.0 + lam);
+          d[k] = -sa[21 + k];
+        }
+        res_chol6(A, 0.0, L);
+        res_chol6_solve(L, d);
+      },
+      [&](const double* qt, bool on_) {
+        res_normal_eq<LANES>(ce, qt, rows, obs_pt, obs_px, pts, b, e, lane, on_, tr);
+        __syncwarp();  // every lane has read sa
+        return tr[27] < cost;
+      },
+      [&] {
         if (lane == 0)
 #pragma unroll
           for (int k = 0; k < 28; ++k) sa[k] = tr[k];
         cost = tr[27];
-        lam *= 0.1;
-      } else {
-        lam *= 10.0;
-      }
-      if (dn <= xtol * (qn + xtol)) active = false;
-    }
-    __syncwarp();
-  }
+      },
+      [](const double* v) {
+        double s2 = 0.0;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) s2 += v[k] * v[k];
+        return sqrt(s2);
+      });
+  __syncwarp();  // lane 0's last write of sa is visible
   if ((st == TRI_OK || st == TRI_MAX_ITER)) {
     double h[21];
 #pragma unroll
     for (int k = 0; k < 21; ++k) h[k] = sa[k];
     if (!res_pd6(h)) st = TRI_NOT_PD;
   }
-  int behind = 0;
-  if (live && st == TRI_OK) {
-    double E[CT_SIZE];
-    res_entry(ce, q, E);
-    for (int i = b + lane; i < e; i += LANES) {
-      const double* X = pts + 3 * (size_t)obs_pt[rows[i]];
-      const double z = fma(E[CT_R + 6], X[0], fma(E[CT_R + 7], X[1], fma(E[CT_R + 8], X[2], E[CT_T + 2])));
-      behind |= !(z > 0.0);
-    }
-  }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) behind |= __shfl_xor_sync(0xffffffffu, behind, s);
+  double E[CT_SIZE];
+  if (live && st == TRI_OK) res_entry(ce, q, E);
+  st = status_behind<LANES>(st, live, b, e, lane, [&](int i) {
+    const double* X = pts + 3 * (size_t)obs_pt[rows[i]];
+    return fma(E[CT_R + 6], X[0], fma(E[CT_R + 7], X[1], fma(E[CT_R + 8], X[2], E[CT_T + 2])));
+  });
   if (!live || lane != 0) return;
-  if (st == TRI_OK && behind) st = TRI_BEHIND;
   const double nan = res_nan();
   const bool at_start = st == TRI_NOT_PD;
 #pragma unroll

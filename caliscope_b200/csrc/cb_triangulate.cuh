@@ -192,6 +192,44 @@ __device__ __forceinline__ void sym4_min_eigvec(double a[4][4], double out[4]) {
   for (int k = 0; k < 4; ++k) out[k] = (m == 0) ? V[k][0] : (m == 1) ? V[k][1] : (m == 2) ? V[k][2] : V[k][3];
 }
 
+// Adds the two DLT rows of the undistorted point xy under the 3x4 projection Pc (row-major) to the packed normal matrix
+// m (00 01 02 03 11 12 13 22 23 33):  M += (x P2 - P0)(x P2 - P0)^T + (y P2 - P1)(y P2 - P1)^T.
+__device__ __forceinline__ void dlt_accumulate(const double* Pc, double2 xy, double m[10]) {
+  double a[4], bb[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const double p2 = Pc[8 + k];
+    a[k] = xy.x * p2 - Pc[k];
+    bb[k] = xy.y * p2 - Pc[4 + k];
+  }
+  int t = 0;
+#pragma unroll
+  for (int p = 0; p < 4; ++p)
+#pragma unroll
+    for (int q = p; q < 4; ++q) {
+      m[t] = fma(a[p], a[q], fma(bb[p], bb[q], m[t]));
+      ++t;
+    }
+}
+
+// The DLT point X (3) of packed normal matrix m: its smallest eigenvector, de-homogenised
+__device__ __forceinline__ void dlt_solve(const double m[10], double* X) {
+  double A[4][4];
+  int t = 0;
+#pragma unroll
+  for (int p = 0; p < 4; ++p)
+#pragma unroll
+    for (int q = p; q < 4; ++q) {
+      A[p][q] = m[t];
+      A[q][p] = m[t];
+      ++t;
+    }
+  double w[4];
+  sym4_min_eigvec(A, w);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) X[k] = w[k] / w[3];
+}
+
 constexpr int TRI_THREADS = 256;
 
 // One group of observations (same (sync, object, keypoint) key) per TRI_LANES lanes (8 for the 2-6 views of a
@@ -222,62 +260,27 @@ tri_dlt_kernel(const double* __restrict__ proj, int n_cams, int proj_in_smem, co
   double m[10];
 #pragma unroll
   for (int k = 0; k < 10; ++k) m[k] = 0.0;
-  unsigned long long h1 = 0, h2 = 0;
+  unsigned long long h[2] = {0, 0};
   for (int i = b + lane; i < e; i += TRI_LANES) {
     const int r = rows[i];
     const int c = obs_cam[r];
-    const double2 xy = reinterpret_cast<const double2*>(obs_xy)[r];
-    const double* Pc = P + (size_t)pstride * (size_t)c;
-    double a[4], bb[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const double p2 = Pc[8 + k];
-      a[k] = xy.x * p2 - Pc[k];
-      bb[k] = xy.y * p2 - Pc[4 + k];
-    }
-    int t = 0;
-#pragma unroll
-    for (int p = 0; p < 4; ++p)
-#pragma unroll
-      for (int q = p; q < 4; ++q) {
-        m[t] = fma(a[p], a[q], fma(bb[p], bb[q], m[t]));
-        ++t;
-      }
-    h1 += tri_mix((unsigned long long)(unsigned)c, 0x9e3779b97f4a7c15ULL);
-    h2 += tri_mix((unsigned long long)(unsigned)c, 0xd1b54a32d192ed03ULL);
+    dlt_accumulate(P + (size_t)pstride * (size_t)c, reinterpret_cast<const double2*>(obs_xy)[r], m);
+    h[0] += tri_mix((unsigned long long)(unsigned)c, 0x9e3779b97f4a7c15ULL);
+    h[1] += tri_mix((unsigned long long)(unsigned)c, 0xd1b54a32d192ed03ULL);
   }
-#pragma unroll
-  for (int s = TRI_LANES / 2; s > 0; s >>= 1) {
-#pragma unroll
-    for (int k = 0; k < 10; ++k) m[k] += __shfl_xor_sync(0xffffffffu, m[k], s);
-    h1 += __shfl_xor_sync(0xffffffffu, h1, s);
-    h2 += __shfl_xor_sync(0xffffffffu, h2, s);
-  }
+  group_sum<TRI_LANES>(m);
+  group_sum<TRI_LANES>(h);
   if (!live || lane != 0) return;
   const int n = e - b;
   count[g] = n;
   rep_row[g] = rows[b];
-  sig[2 * g] = h1;
-  sig[2 * g + 1] = h2;
+  sig[2 * g] = h[0];
+  sig[2 * g + 1] = h[1];
   if (n < 2) {
     xyz[3 * g] = xyz[3 * g + 1] = xyz[3 * g + 2] = __longlong_as_double(0x7ff8000000000000LL);
     return;
   }
-  double A[4][4];
-  int t = 0;
-#pragma unroll
-  for (int p = 0; p < 4; ++p)
-#pragma unroll
-    for (int q = p; q < 4; ++q) {
-      A[p][q] = m[t];
-      A[q][p] = m[t];
-      ++t;
-    }
-  double w[4];
-  sym4_min_eigvec(A, w);
-  xyz[3 * g + 0] = w[0] / w[3];
-  xyz[3 * g + 1] = w[1] / w[3];
-  xyz[3 * g + 2] = w[2] / w[3];
+  dlt_solve(m, xyz + 3 * g);
 }
 
 // ---- refinement to the reprojection optimum and point covariance (cb_triangulate_refine, DESIGN.md section 4.7) -------
@@ -332,7 +335,7 @@ __device__ __forceinline__ const double* tri_stage_camtab(const double* __restri
 template <int LANES>
 __device__ __forceinline__ void tri_normal_eq(const double* cams, int stride, const int* __restrict__ rows,
                                               const int* __restrict__ obs_cam, const double* __restrict__ obs_px, int b,
-                                              int e, int lane, bool on, const double* X, double acc[10]) {
+                                              int e, int lane, bool on, const double* X, double (&acc)[10]) {
 #pragma unroll
   for (int k = 0; k < 10; ++k) acc[k] = 0.0;
   if (on)
@@ -357,17 +360,68 @@ __device__ __forceinline__ void tri_normal_eq(const double* cams, int stride, co
       acc[8] = fma(J[2], r0, fma(J[5], r1, acc[8]));
       acc[9] = fma(r0, r0, fma(r1, r1, acc[9]));
     }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1)
-#pragma unroll
-    for (int k = 0; k < 10; ++k) acc[k] += __shfl_xor_sync(0xffffffffu, acc[k], s);
+  group_sum<LANES>(acc);
 }
 
-// Per group, Levenberg-Marquardt on the pixel reprojection cost from the DLT point xyz0 (oracle/triangulation_refine.py
-// refine_points states the same rule):  solve (H + lam diag H) d = -g;  accept when the cost drops (lam /= 10), else
-// lam *= 10;  stop when |d| <= xtol (|X| + xtol) or after max_iter steps.  Every lane of a group holds the same reduced
-// sums, so every lane solves the same 3x3 system and takes the same decision; the loop runs until no group of the warp
-// is active, because the shuffles need the whole warp.  Writes xyz (the DLT point when H is not positive definite),
+// Levenberg-Marquardt over the N parameters x of one group, from sums at x that the caller has formed and found positive
+// definite (active: the group takes steps):  solve (H + lam diag H) d = -g;  accept when the cost drops (lam /= 10),
+// else lam *= 10;  stop when |d| <= xtol (|x| + xtol) (st stays) or after max_iter steps (st = TRI_MAX_ITER).  Every lane
+// of a group holds the same reduced sums, so every lane takes the same decision; the loop runs until no group of the
+// warp is active, because the reductions need the whole warp.  The caller owns the sums, where they live and how the
+// damped system is solved, through
+//   step(lam, on, d)   d = the damped step at x when on (called on every lane);
+//   trial(xt, on)      forms the sums at xt (every lane; the rows' terms only when on) and returns whether their cost
+//                      is below x's;
+//   keep()             the trial's sums become x's (the group's accepting lanes);
+//   norm(v)            |v| of a parameter vector, in the caller's own arithmetic.
+template <int N, typename Step, typename Trial, typename Keep, typename Norm>
+__device__ __forceinline__ int lm_iterate(double* x, bool active, int st, int max_iter, double xtol, Step step,
+                                          Trial trial, Keep keep, Norm norm) {
+  double lam = TRI_LAMBDA0;
+  int it = 0;
+  while (__any_sync(0xffffffffu, active)) {
+    if (active && it == max_iter) {
+      st = TRI_MAX_ITER;
+      active = false;
+    }
+    double d[N], xt[N];
+#pragma unroll
+    for (int k = 0; k < N; ++k) d[k] = 0.0;
+    step(lam, active, d);
+#pragma unroll
+    for (int k = 0; k < N; ++k) xt[k] = x[k] + d[k];
+    const bool lower = trial(xt, active);
+    if (active) {
+      ++it;
+      const double dn = norm(d), xn = norm(x);
+      if (lower) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) x[k] = xt[k];
+        keep();
+        lam *= 0.1;
+      } else {
+        lam *= 10.0;
+      }
+      if (dn <= xtol * (xn + xtol)) active = false;
+    }
+  }
+  return st;
+}
+
+// TRI_BEHIND when st is TRI_OK and depth(i) > 0 fails for a row position i in [b, e) of the group (on: a live group),
+// else st; the same on every lane
+template <int LANES, typename Depth>
+__device__ __forceinline__ int status_behind(int st, bool on, int b, int e, int lane, Depth depth) {
+  int behind = 0;
+  if (on && st == TRI_OK)
+    for (int i = b + lane; i < e; i += LANES) behind |= !(depth(i) > 0.0);
+  behind = group_or<LANES>(behind);
+  return st == TRI_OK && behind ? TRI_BEHIND : st;
+}
+
+// Per group, Levenberg-Marquardt (lm_iterate) on the pixel reprojection cost from the DLT point xyz0
+// (oracle/triangulation_refine.py refine_points states the same rule), the sums in registers and the damped 3x3 system
+// solved by chol3.  Writes xyz (the DLT point when H is not positive definite),
 // the pixel RMSE and the status code.
 template <int LANES>
 __global__ void __launch_bounds__(TRI_THREADS)
@@ -391,53 +445,30 @@ tri_refine_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem
   tri_normal_eq<LANES>(cams, stride, rows, obs_cam, obs_px, b, e, lane, live && st == TRI_OK, X, acc);
   const double cost0 = acc[9];
   if (st == TRI_OK && !chol3(acc, TRI_PD_RTOL, L)) st = TRI_NOT_PD;
-  bool active = live && st == TRI_OK;
-  double lam = TRI_LAMBDA0;
-  int it = 0;
-  while (__any_sync(0xffffffffu, active)) {
-    if (active && it == max_iter) {
-      st = TRI_MAX_ITER;
-      active = false;
-    }
-    double d[3] = {0.0, 0.0, 0.0}, Xt[3];
-    if (active) {
-      double A[6] = {acc[0] * (1.0 + lam), acc[1], acc[2], acc[3] * (1.0 + lam), acc[4], acc[5] * (1.0 + lam)};
-      chol3(A, 0.0, L);
-      chol3_solve_neg(L, acc + 6, d);
-    }
-#pragma unroll
-    for (int k = 0; k < 3; ++k) Xt[k] = X[k] + d[k];
-    double tr[10];
-    tri_normal_eq<LANES>(cams, stride, rows, obs_cam, obs_px, b, e, lane, active, Xt, tr);
-    if (active) {
-      ++it;
-      const double dn = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
-      const double xn = sqrt(X[0] * X[0] + X[1] * X[1] + X[2] * X[2]);
-      if (tr[9] < acc[9]) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) X[k] = Xt[k];
+  double tr[10];  // the sums at the trial point
+  st = lm_iterate<3>(
+      X, live && st == TRI_OK, st, max_iter, xtol,
+      [&](double lam, bool on, double* d) {
+        if (!on) return;
+        double A[6] = {acc[0] * (1.0 + lam), acc[1], acc[2], acc[3] * (1.0 + lam), acc[4], acc[5] * (1.0 + lam)};
+        chol3(A, 0.0, L);
+        chol3_solve_neg(L, acc + 6, d);
+      },
+      [&](const double* xt, bool on) {
+        tri_normal_eq<LANES>(cams, stride, rows, obs_cam, obs_px, b, e, lane, on, xt, tr);
+        return tr[9] < acc[9];
+      },
+      [&] {
 #pragma unroll
         for (int k = 0; k < 10; ++k) acc[k] = tr[k];
-        lam *= 0.1;
-      } else {
-        lam *= 10.0;
-      }
-      if (dn <= xtol * (xn + xtol)) active = false;
-    }
-  }
+      },
+      [](const double* v) { return sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]); });
   if ((st == TRI_OK || st == TRI_MAX_ITER) && !chol3(acc, TRI_PD_RTOL, L)) st = TRI_NOT_PD;
-  // behind a camera at the solution
-  int behind = 0;
-  if (live && st == TRI_OK)
-    for (int i = b + lane; i < e; i += LANES) {
-      const double* cam = cams + (size_t)stride * obs_cam[rows[i]];
-      const double z = fma(cam[CT_R + 6], X[0], fma(cam[CT_R + 7], X[1], fma(cam[CT_R + 8], X[2], cam[CT_T + 2])));
-      behind |= !(z > 0.0);
-    }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) behind |= __shfl_xor_sync(0xffffffffu, behind, s);
+  st = status_behind<LANES>(st, live, b, e, lane, [&](int i) {
+    const double* cam = cams + (size_t)stride * obs_cam[rows[i]];
+    return fma(cam[CT_R + 6], X[0], fma(cam[CT_R + 7], X[1], fma(cam[CT_R + 8], X[2], cam[CT_T + 2])));
+  });
   if (!live || lane != 0) return;
-  if (st == TRI_OK && behind) st = TRI_BEHIND;
   const double nan = __longlong_as_double(0x7ff8000000000000LL);
   const bool at_start = st == TRI_FEW_ROWS || st == TRI_NOT_PD;
 #pragma unroll
@@ -534,15 +565,9 @@ tri_cov_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, c
         for (int c = 0; c < 3; ++c) m[a][c] += same ? x[a][c] : x[a][c] + x[c][a];
     }
   }
+  group_sum<LANES>(h);
 #pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) {
-#pragma unroll
-    for (int q = 0; q < 6; ++q) h[q] += __shfl_xor_sync(0xffffffffu, h[q], s);
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-#pragma unroll
-      for (int c = 0; c < 3; ++c) m[a][c] += __shfl_xor_sync(0xffffffffu, m[a][c], s);
-  }
+  for (int a = 0; a < 3; ++a) group_sum<LANES>(m[a]);
   if (!live || lane != 0) return;
   double* out = cov + 9 * (size_t)g;
   if (!on) {
@@ -604,6 +629,41 @@ __device__ __forceinline__ double tri_row_err2(const double* cam, const double* 
   return du * du + dv * dv;
 }
 
+// a row's MSAC cost: its squared error within tau in front of the camera, else tau^2 (also for a non-finite error)
+__device__ __forceinline__ double msac_term(bool front, double e2, double tau2) { return (front && e2 <= tau2) ? e2 : tau2; }
+
+// Classification at the winner of a group's consensus (found: there is one).  Each lane flags its rows in front of the
+// camera with e_r^2 <= tau^2 (err2(r, front): the squared pixel error of caller row r) into `pos_flag` (key-sorted
+// position) and `inlier` (caller row); both are cleared when fewer than min_inliers rows agree.  Returns whether the
+// group has consensus; nin is the count of agreeing rows, the same on every lane.
+template <int LANES, typename RowErr2>
+__device__ __forceinline__ bool consensus_classify(bool found, const int* __restrict__ rows, int b, int e, int lane,
+                                                   double tau2, int min_inliers, RowErr2 err2,
+                                                   unsigned char* __restrict__ pos_flag,
+                                                   unsigned char* __restrict__ inlier, int& nin) {
+  nin = 0;
+  for (int i = b + lane; i < e; i += LANES) {
+    const int r = rows[i];
+    bool in = false;
+    if (found) {
+      bool front;
+      const double e2 = err2(r, front);
+      in = front && e2 <= tau2;
+    }
+    pos_flag[i] = in ? 1 : 0;
+    inlier[r] = in ? 1 : 0;
+    nin += in ? 1 : 0;
+  }
+  nin = group_sum<LANES>(nin);
+  const bool ok = found && nin >= min_inliers;
+  if (!ok && nin > 0)
+    for (int i = b + lane; i < e; i += LANES) {
+      pos_flag[i] = 0;
+      inlier[rows[i]] = 0;
+    }
+  return ok;
+}
+
 // One group per LANES lanes (the lane choice of tri_dlt_kernel).  The lanes stride over the group's candidate pairs; each
 // builds its pair's DLT point (tri_dlt_kernel's normal matrix on the undistorted float32-rounded coordinates `obs_xy`,
 // then sym4_min_eigvec) and scores it by MSAC over all k rows, sum min(e_r^2, tau^2) in raw pixels (a row behind its camera
@@ -649,42 +709,12 @@ tri_consensus_kernel(const double* __restrict__ camtab, int cam_in_smem, const d
     const int ri = rows[b + i], rj = rows[b + j];
     const int ci = obs_cam[ri], cj = obs_cam[rj];
     if (ci == cj) continue;
-    double mm[10];
+    double mm[10], h[3];
 #pragma unroll
     for (int t = 0; t < 10; ++t) mm[t] = 0.0;
-#pragma unroll
-    for (int s = 0; s < 2; ++s) {
-      const int r = s ? rj : ri;
-      const double2 xy = reinterpret_cast<const double2*>(obs_xy)[r];
-      const double* Pc = Pt + (size_t)pstride * (size_t)(s ? cj : ci);
-      double a[4], bb[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const double p2 = Pc[8 + q];
-        a[q] = xy.x * p2 - Pc[q];
-        bb[q] = xy.y * p2 - Pc[4 + q];
-      }
-      int t = 0;
-#pragma unroll
-      for (int p = 0; p < 4; ++p)
-#pragma unroll
-        for (int q = p; q < 4; ++q) {
-          mm[t] = fma(a[p], a[q], fma(bb[p], bb[q], mm[t]));
-          ++t;
-        }
-    }
-    double A[4][4], w[4];
-    int t = 0;
-#pragma unroll
-    for (int p = 0; p < 4; ++p)
-#pragma unroll
-      for (int q = p; q < 4; ++q) {
-        A[p][q] = mm[t];
-        A[q][p] = mm[t];
-        ++t;
-      }
-    sym4_min_eigvec(A, w);
-    const double h[3] = {w[0] / w[3], w[1] / w[3], w[2] / w[3]};
+    dlt_accumulate(Pt + (size_t)pstride * (size_t)ci, reinterpret_cast<const double2*>(obs_xy)[ri], mm);
+    dlt_accumulate(Pt + (size_t)pstride * (size_t)cj, reinterpret_cast<const double2*>(obs_xy)[rj], mm);
+    dlt_solve(mm, h);
     if (!isfinite(h[0]) || !isfinite(h[1]) || !isfinite(h[2])) continue;
     const double* Ci = cams + (size_t)stride * ci;
     const double* Cj = cams + (size_t)stride * cj;
@@ -696,7 +726,7 @@ tri_consensus_kernel(const double* __restrict__ camtab, int cam_in_smem, const d
       const int r = rows[p];
       bool front;
       const double e2 = tri_row_err2(cams + (size_t)stride * obs_cam[r], h, reinterpret_cast<const double2*>(obs_px)[r], front);
-      score += (front && e2 <= tau2) ? e2 : tau2;
+      score += msac_term(front, e2, tau2);
     }
     if (score < best) {  // candidates of a lane come in increasing rank: the first of equal scores stays
       best = score;
@@ -705,40 +735,16 @@ tri_consensus_kernel(const double* __restrict__ camtab, int cam_in_smem, const d
       for (int q = 0; q < 3; ++q) X[q] = h[q];
     }
   }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) {
-    const double ob = __shfl_xor_sync(0xffffffffu, best, s);
-    const long long om = __shfl_xor_sync(0xffffffffu, best_m, s);
-    if (ob < best || (ob == best && om < best_m)) {
-      best = ob;
-      best_m = om;
-    }
-  }
+  group_argmin<LANES>(best, best_m);
   const bool found = best < inf;
-  const int owner = found ? (int)(best_m % LANES) : 0;
-#pragma unroll
-  for (int q = 0; q < 3; ++q) X[q] = __shfl_sync(0xffffffffu, X[q], owner, LANES);
-  int nin = 0;
-  for (int i = b + lane; i < e; i += LANES) {
-    const int r = rows[i];
-    bool in = false;
-    if (found) {
-      bool front;
-      const double e2 = tri_row_err2(cams + (size_t)stride * obs_cam[r], X, reinterpret_cast<const double2*>(obs_px)[r], front);
-      in = front && e2 <= tau2;
-    }
-    pos_flag[i] = in ? 1 : 0;
-    inlier[r] = in ? 1 : 0;
-    nin += in ? 1 : 0;
-  }
-#pragma unroll
-  for (int s = LANES / 2; s > 0; s >>= 1) nin += __shfl_xor_sync(0xffffffffu, nin, s);
-  const bool ok = found && nin >= min_inliers;
-  if (!ok && nin > 0)
-    for (int i = b + lane; i < e; i += LANES) {
-      pos_flag[i] = 0;
-      inlier[rows[i]] = 0;
-    }
+  group_bcast<LANES>(X, found ? (int)(best_m % LANES) : 0);
+  int nin;
+  const bool ok = consensus_classify<LANES>(
+      found, rows, b, e, lane, tau2, min_inliers,
+      [&](int r, bool& front) {
+        return tri_row_err2(cams + (size_t)stride * obs_cam[r], X, reinterpret_cast<const double2*>(obs_px)[r], front);
+      },
+      pos_flag, inlier, nin);
   if (!live || lane != 0) return;
   const double nan = __longlong_as_double(0x7ff8000000000000LL);
   count[g] = k;

@@ -1,6 +1,7 @@
 """Stage times of cb_resect_robust (DESIGN.md 4.9), one JSON line per (workload, point covariance) pair.
 
     python profiles/resect_robust_timing.py [rig64] [track] [--steps 5] [--warmup 2] [--cpu-groups 200]
+        [--dump-outputs DIR]
 
 rig64: cfg4's 64 cameras and 50 000 points (synthetic.make_rig(64, 50_000, 2_000_000)), key = camera: 64 groups of about
 31 000 rows (the long shape), 5 % of the rows moved by up to +-200 px, priors 0.02 rad / 2 cm off the truth; run without
@@ -11,7 +12,8 @@ events recorded inside the call (CbResectStats).  Scoring evaluations are counte
 (1 + 4 min(C(k, 3), max_samples)) x k, an upper bound (samples with fewer than 4 solutions score fewer hypotheses).
 The pose error against the truth is over the groups with status 0.  For context only, cv2.solvePnPRansac (P3P, then
 solvePnPRefineLM on its inliers) runs on a sample of the groups on one host core: a different algorithm on the CPU, not
-a baseline of the same computation.  The card's name and power limit are printed with the numbers.
+a baseline of the same computation.  The card's name and power limit are printed with the numbers.  --dump-outputs
+writes every output array of the last timed call of each variant to DIR/<workload>_<variant>.npz.
 """
 import argparse
 import json
@@ -25,6 +27,7 @@ import numpy as np
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from caliscope_b200 import synthetic  # noqa: E402
 from caliscope_b200.resection import ResectStats, resect_robust  # noqa: E402
+from dump_outputs import dump_outputs  # noqa: E402
 
 TAU = 4.0
 MAX_SAMPLES = 64
@@ -158,7 +161,7 @@ def cpu_context(args, n_groups_sample: int):
     return {"groups": int(len(pick)), "ms_per_group": 1e3 * (time.perf_counter() - t0) / len(pick)}
 
 
-def run(name: str, steps: int, warmup: int, cpu_groups: int):
+def run(name: str, steps: int, warmup: int, cpu_groups: int, dump_dir=None):
     args, truth, moved, kw = make(name)
     key = args[5]
     _, k = np.unique(key, return_counts=True)
@@ -180,6 +183,7 @@ def run(name: str, steps: int, warmup: int, cpu_groups: int):
             acc += [st.group_ms, st.consensus_ms, st.refine_ms, st.cov_ms, st.total_ms]
             launches = st.kernel_launches
         acc /= steps
+        dump_outputs(dump_dir, f"{name}_{'pcov' if cov is not None else 'nopcov'}", out)
         ok = out.status == 0
         print(json.dumps({
             "workload": name, "card": card(), "points_cov": cov is not None, "n_obs": int(len(key)),
@@ -199,9 +203,10 @@ def main():
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
     ap.add_argument("--cpu-groups", type=int, default=200)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     a = ap.parse_args()
     for w in a.workloads:
-        run(w, a.steps, a.warmup, a.cpu_groups)
+        run(w, a.steps, a.warmup, a.cpu_groups, a.dump_outputs)
 
 
 if __name__ == "__main__":

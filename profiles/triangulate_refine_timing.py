@@ -1,6 +1,6 @@
 """Stage times of cb_triangulate_refine (DESIGN.md 4.7), one JSON line per (workload, camera covariance) pair.
 
-    python profiles/triangulate_refine_timing.py [cfg4] [mocap] [--steps 5] [--warmup 2]
+    python profiles/triangulate_refine_timing.py [cfg4] [mocap] [--steps 5] [--warmup 2] [--dump-outputs DIR]
 
 cfg4: 64 cameras, 50 000 groups, 2 000 000 observations (synthetic.cfg4).  mocap: 8 cameras, 500 000 groups of 2-8 rows
 (make_rig with cams_per_point=8).  Cameras at the rig's true poses, noisy pixels.  Each workload runs without and with a
@@ -9,6 +9,7 @@ camera covariance (a seeded SPD matrix in x's camera layout).  Stage times are t
 up to rounding at the convergence floor); refine-stage row evaluations are (steps + 2) x rows per group: the start, one
 evaluation per step, and the behind-camera pass.  Covariance flops are counted from the shapes: pairs x 2 (3 P^2 + 9 P)
 over the unordered pairs of each group's distinct cameras.  The card's name and power limit are printed with the numbers.
+--dump-outputs writes every output array of the last timed call of each variant to DIR/<workload>_<variant>.npz.
 """
 import argparse
 import json
@@ -21,6 +22,7 @@ import numpy as np
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from caliscope_b200 import synthetic  # noqa: E402
 from caliscope_b200.triangulation import RefineStats, triangulate_refined  # noqa: E402
+from dump_outputs import dump_outputs  # noqa: E402
 
 
 def card() -> str:
@@ -53,7 +55,7 @@ def mean_steps(rig, ncp: int, sample: int = 2000) -> float:
     return float(steps[live].mean())
 
 
-def run(name: str, steps: int, warmup: int):
+def run(name: str, steps: int, warmup: int, dump_dir=None):
     import torch
 
     rig = make(name)
@@ -79,6 +81,7 @@ def run(name: str, steps: int, warmup: int):
                                       stats=st)  # fmt: skip
             acc += [st.group_ms, st.dlt_ms, st.refine_ms, st.cov_ms, st.total_ms]
         acc /= steps
+        dump_outputs(dump_dir, f"{name}_{'cov' if cov is not None else 'nocov'}", out)
         cov_flop = pairs * 2 * (3 * P * P + 9 * P) if cov is not None else 0.0
         row_evals = (m_steps + 2) * float(n_rows[live].sum())
         print(json.dumps({
@@ -98,9 +101,10 @@ def main() -> None:
     ap.add_argument("workloads", nargs="*", default=["cfg4", "mocap"])
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     for name in args.workloads:
-        run(name, args.steps, args.warmup)
+        run(name, args.steps, args.warmup, args.dump_outputs)
 
 
 if __name__ == "__main__":

@@ -1,7 +1,7 @@
 """Stage times of cb_triangulate_robust (DESIGN.md 4.8) next to cb_triangulate_refine on the same input, one JSON line per
 (workload, camera covariance) pair.
 
-    python profiles/triangulate_robust_timing.py [cfg4] [mocap] [--steps 5] [--warmup 2]
+    python profiles/triangulate_robust_timing.py [cfg4] [mocap] [--steps 5] [--warmup 2] [--dump-outputs DIR]
 
 cfg4: 64 cameras, 50 000 groups, 2 000 000 observations.  mocap: 8 cameras, 500 000 groups of 2-8 rows (make_rig with
 cams_per_point=8).  Cameras at the rig's true poses, noisy pixels, and 5 % of the rows moved by up to +-200 px in each
@@ -10,7 +10,8 @@ matrix in x's camera layout).  Stage times are the CUDA events recorded inside t
 CbTriRefineStats).  Consensus row evaluations are counted from the shapes: sum over the groups of min(T, max_pairs) x k
 (T = k (k - 1) / 2 pairs of a group of k rows; same-camera pairs are counted although they skip the scoring).  The
 distance to the true point is over the groups both calls report with status 0.  The card's name and power limit are
-printed with the numbers.
+printed with the numbers.  --dump-outputs writes every output array of the last timed call of each variant to
+DIR/<workload>_<call>_<variant>.npz.
 """
 import argparse
 import json
@@ -23,6 +24,7 @@ import numpy as np
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 from caliscope_b200 import synthetic  # noqa: E402
 from caliscope_b200.triangulation import RefineStats, RobustStats, triangulate_refined, triangulate_robust  # noqa: E402
+from dump_outputs import dump_outputs  # noqa: E402
 
 TAU = 4.0
 MAX_PAIRS = 64
@@ -51,7 +53,7 @@ def _err(xyz, truth, m):
     return {"median": float(np.median(d)), "p99": float(np.percentile(d, 99))} if len(d) else None
 
 
-def run(name: str, steps: int, warmup: int):
+def run(name: str, steps: int, warmup: int, dump_dir=None):
     import torch
 
     rig = make(name)
@@ -79,6 +81,9 @@ def run(name: str, steps: int, warmup: int):
             ref_acc += [rst.group_ms, rst.dlt_ms, rst.refine_ms, rst.cov_ms, rst.total_ms]
         acc /= steps
         ref_acc /= steps
+        variant = "cov" if cov is not None else "nocov"
+        dump_outputs(dump_dir, f"{name}_robust_{variant}", out)
+        dump_outputs(dump_dir, f"{name}_refined_{variant}", ref)
         both = (out.status == 0) & (ref.status == 0)
         print(json.dumps({
             "workload": name, "camera_cov": cov is not None, "card": card(), "n_cams": rig.n_cams,
@@ -103,9 +108,10 @@ def main() -> None:
     ap.add_argument("workloads", nargs="*", default=["cfg4", "mocap"])
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     args = ap.parse_args()
     for name in args.workloads:
-        run(name, args.steps, args.warmup)
+        run(name, args.steps, args.warmup, args.dump_outputs)
 
 
 if __name__ == "__main__":
