@@ -25,8 +25,19 @@ __device__ __forceinline__ float2 load_px(const double* p, long long i) {
 }
 __device__ __forceinline__ float2 load_px(const float* p, long long i) { return reinterpret_cast<const float2*>(p)[i]; }
 
-// float32 in -> double arithmetic -> float32 out, exactly the precision contract of the reference call.
+// Unfused fp64 arithmetic for the undistortion.  OpenCV's x86 build rounds every product and every sum; nvcc would
+// contract a * b + c into one fma, which moves the double by up to an ulp, and the float32 result shows that wherever
+// the sum cancels (a pixel near 0, x0 - dx near 0).  These three are never contracted.
+__device__ __forceinline__ double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double add_rn(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double sub_rn(double a, double b) { return __dsub_rn(a, b); }
+
+// float32 in -> double arithmetic -> float32 out, exactly the precision contract of the reference call.  OpenCV's
+// expressions in OpenCV's evaluation order, so the only operation that is not bit-exact is the fisheye model's tan().
 // TIN = double (caller's array, rounded to float32 here) or float (already rounded on the host while staging).
+// Edges as OpenCV has them: a fisheye point whose Newton iteration fails or flips theta's sign is (-1e6, -1e6) in
+// both outputs; a NaN theta_d clamps to -pi/2 and iterates (std::max keeps its first argument on NaN); pixel output
+// is the homography P [x y 1]^T over its third row, which is NaN in both coordinates when x or y is not finite.
 template <typename TIN>
 __global__ void undistort_kernel(const UndistCam* __restrict__ cams, const int* __restrict__ obs_cam,
                                  const TIN* __restrict__ xy_in, double* __restrict__ xy_out, long long n,
@@ -37,19 +48,24 @@ __global__ void undistort_kernel(const UndistCam* __restrict__ cams, const int* 
   const float2 in = load_px(xy_in, i);
   const double u = (double)in.x, v = (double)in.y;
   double x, y;
+  bool sentinel = false;
   if (c.fisheye) {
-    const double pwx = (u - c.cx) / c.fx, pwy = (v - c.cy) / c.fy;
-    double theta_d = sqrt(pwx * pwx + pwy * pwy);
+    const double pwx = sub_rn(u, c.cx) / c.fx, pwy = sub_rn(v, c.cy) / c.fy;
+    double theta_d = sqrt(add_rn(mul_rn(pwx, pwx), mul_rn(pwy, pwy)));
     const double half_pi = 1.5707963267948966;
-    theta_d = fmin(fmax(-half_pi, theta_d), half_pi);
+    theta_d = (-half_pi < theta_d) ? theta_d : -half_pi;  // std::min(std::max(-pi/2, theta_d), pi/2)
+    theta_d = (half_pi < theta_d) ? half_pi : theta_d;
     bool converged = false;
     double th = theta_d, scale = 0.0;
-    if (theta_d > 1e-8) {
+    if (fabs(theta_d) > 1e-8) {
       for (int j = 0; j < 10; ++j) {
-        const double t2 = th * th, t4 = t2 * t2, t6 = t4 * t2, t8 = t4 * t4;
-        const double k0 = c.d[0] * t2, k1 = c.d[1] * t4, k2 = c.d[2] * t6, k3 = c.d[3] * t8;
-        const double fix = (th * (1 + k0 + k1 + k2 + k3) - theta_d) / (1 + 3 * k0 + 5 * k1 + 7 * k2 + 9 * k3);
-        th -= fix;
+        const double t2 = mul_rn(th, th), t4 = mul_rn(t2, t2), t6 = mul_rn(t4, t2), t8 = mul_rn(t6, t2);
+        const double k0 = mul_rn(c.d[0], t2), k1 = mul_rn(c.d[1], t4), k2 = mul_rn(c.d[2], t6), k3 = mul_rn(c.d[3], t8);
+        const double num = sub_rn(mul_rn(th, add_rn(add_rn(add_rn(add_rn(1.0, k0), k1), k2), k3)), theta_d);
+        const double den = add_rn(add_rn(add_rn(add_rn(1.0, mul_rn(3.0, k0)), mul_rn(5.0, k1)), mul_rn(7.0, k2)),
+                                  mul_rn(9.0, k3));
+        const double fix = num / den;
+        th = sub_rn(th, fix);
         if (fabs(fix) < 1e-8) {
           converged = true;
           break;
@@ -61,36 +77,50 @@ __global__ void undistort_kernel(const UndistCam* __restrict__ cams, const int* 
     }
     const bool flipped = (theta_d < 0 && th > 0) || (theta_d > 0 && th < 0);
     if (converged && !flipped) {
-      x = pwx * scale;
-      y = pwy * scale;
+      x = mul_rn(pwx, scale);
+      y = mul_rn(pwy, scale);
     } else {
       x = -1000000.0;
       y = -1000000.0;
+      sentinel = true;
     }
   } else {
-    const double x0 = (u - c.cx) / c.fx, y0 = (v - c.cy) / c.fy;
+    // the reciprocals, as OpenCV scales by them (the fisheye model above divides)
+    const double ifx = 1.0 / c.fx, ify = 1.0 / c.fy;
+    const double x0 = mul_rn(sub_rn(u, c.cx), ifx), y0 = mul_rn(sub_rn(v, c.cy), ify);
+    const double* k = c.d;
     x = x0;
     y = y0;
 #pragma unroll 1
     for (int j = 0; j < 5; ++j) {
-      const double r2 = x * x + y * y;
-      const double icdist =
-          (1 + ((c.d[7] * r2 + c.d[6]) * r2 + c.d[5]) * r2) / (1 + ((c.d[4] * r2 + c.d[1]) * r2 + c.d[0]) * r2);
+      const double r2 = add_rn(mul_rn(x, x), mul_rn(y, y));
+      // (1 + ((k6 r2 + k5) r2 + k4) r2) / (1 + ((k3 r2 + k2) r2 + k1) r2)
+      const double icdist = add_rn(1.0, mul_rn(add_rn(mul_rn(add_rn(mul_rn(k[7], r2), k[6]), r2), k[5]), r2)) /
+                            add_rn(1.0, mul_rn(add_rn(mul_rn(add_rn(mul_rn(k[4], r2), k[1]), r2), k[0]), r2));
       if (icdist < 0) {
         x = x0;
         y = y0;
         break;
       }
-      const double dx = 2 * c.d[2] * x * y + c.d[3] * (r2 + 2 * x * x) + c.d[8] * r2 + c.d[9] * r2 * r2;
-      const double dy = c.d[2] * (r2 + 2 * y * y) + 2 * c.d[3] * x * y + c.d[10] * r2 + c.d[11] * r2 * r2;
-      x = (x0 - dx) * icdist;
-      y = (y0 - dy) * icdist;
+      // dx = 2 p1 x y + p2 (r2 + 2 x x) + s1 r2 + s2 r2 r2,  dy = p1 (r2 + 2 y y) + 2 p2 x y + s3 r2 + s4 r2 r2
+      const double dx = add_rn(add_rn(add_rn(mul_rn(mul_rn(2 * k[2], x), y), mul_rn(k[3], add_rn(r2, mul_rn(2 * x, x)))),
+                                      mul_rn(k[8], r2)),
+                               mul_rn(mul_rn(k[9], r2), r2));
+      const double dy = add_rn(add_rn(add_rn(mul_rn(k[2], add_rn(r2, mul_rn(2 * y, y))), mul_rn(mul_rn(2 * k[3], x), y)),
+                                      mul_rn(k[10], r2)),
+                               mul_rn(mul_rn(k[11], r2), r2));
+      x = mul_rn(sub_rn(x0, dx), icdist);
+      y = mul_rn(sub_rn(y0, dy), icdist);
     }
   }
-  if (to_pixels) {
-    const double px = c.fx * x + c.skew * y + c.cx, py = c.fy * y + c.cy;
-    x = px;
-    y = py;
+  if (to_pixels && !sentinel) {
+    if (isfinite(x) && isfinite(y)) {
+      const double px = add_rn(add_rn(mul_rn(c.fx, x), mul_rn(c.skew, y)), c.cx), py = add_rn(mul_rn(c.fy, y), c.cy);
+      x = px;
+      y = py;
+    } else {
+      x = y = __longlong_as_double(0x7ff8000000000000LL);
+    }
   }
   reinterpret_cast<double2*>(xy_out)[i] = make_double2((double)(float)x, (double)(float)y);
 }

@@ -264,7 +264,11 @@ int cb_debug_fp64_peak(int device, double* dmma_tflops, double* dfma_tflops);
  *   cam_fisheye[n_cams]; cam_k[n_cams][5] = fx,fy,cx,cy,skew; cam_dist[n_cams][12] = k1 k2 p1 p2 k3 k4 k5 k6 s1..s4
  *   (zero-padded; fisheye: k1..k4); obs_cam[n] camera row per point (NULL with a single camera);
  *   to_pixels: 0 = normalised image plane (P = I), 1 = pixels (P = K).
- *   on_device: xy_in / obs_cam / xy_out are device pointers. */
+ *   on_device: xy_in / obs_cam / xy_out are device pointers.
+ * Pinhole results are bit-exact with OpenCV; fisheye within one float32 ulp (device tan).  Edges as OpenCV:
+ *   a fisheye point whose Newton iteration does not converge or flips theta's sign is (-1e6, -1e6) in both outputs;
+ *   NaN / inf input: pinhole (NaN, NaN); fisheye normalised: a NaN theta_d is clamped to -pi/2 and iterated, so the
+ *   finite coordinate keeps a value (e.g. (NaN, 100) -> (NaN, y)); any non-finite result in pixel output is (NaN, NaN). */
 int cb_undistort_points(int32_t n_cams, const int32_t* cam_fisheye, const double* cam_k, const double* cam_dist,
                         int64_t n, const int32_t* obs_cam, const double* xy_in, int on_device, int to_pixels,
                         double* xy_out, int device, void* stream);

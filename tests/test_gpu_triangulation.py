@@ -1,8 +1,8 @@
 """GPU parity of the step in front of bundle adjustment (SURVEY.md §8(f) rank 3): lens undistortion
 and DLT triangulation through the C ABI, against the reference's golden vectors and the oracle.
 
-Tolerances: undistortion is float32-valued like the reference — bit-exact expected, one float32 ulp
-allowed (device tan() vs libm); triangulation 1e-9 m on well-posed groups (the kernel takes the
+Tolerances: undistortion is float32-valued like the reference — bit-exact for pinhole cameras, one
+float32 ulp allowed for fisheye (device tan() vs libm); triangulation 1e-9 m on well-posed groups (the kernel takes the
 smallest eigenvector of the 4x4 normal matrix in fp64, the reference an SVD of the 2k x 4 system)."""
 from __future__ import annotations
 
@@ -112,8 +112,11 @@ def test_undistort_points_matches_reference_golden(g):
             got = undistort_points(pts, None, K[None], [d], [fish], output=mode)
             ref = g[f"und_{tag}_{key}"]
             assert got.dtype == np.float32 and got.shape == ref.shape
-            assert _ulp32(got, ref) <= 1, (tag, mode)
-            assert np.mean(got.astype(np.float64) == ref) > 0.999
+            if fish:
+                assert _ulp32(got, ref) <= 1, (tag, mode)
+                assert np.mean(got.astype(np.float64) == ref) > 0.999
+            else:  # no tan(): OpenCV's arithmetic, unfused, gives OpenCV's bits
+                assert np.array_equal(got.astype(np.float64), ref), (tag, mode)
 
 
 def test_undistort_all_cameras_in_one_launch_matches_per_camera_reference(g):
@@ -122,7 +125,7 @@ def test_undistort_all_cameras_in_one_launch_matches_per_camera_reference(g):
 
     rows = np.searchsorted(g["s4_cam_ids"], g["s4_px_cam"])
     got = undistort_points(g["s4_px"], rows, g["s4_K"], list(g["s4_dist"]), np.zeros(len(g["s4_K"]), np.int32))
-    assert _ulp32(got, g["s4_px_undist"]) <= 1
+    assert np.array_equal(got.astype(np.float64), g["s4_px_undist"])  # pinhole cameras: bit-exact
     with pytest.raises(ValueError):
         undistort_points(g["s4_px"], rows, g["s4_K"], list(g["s4_dist"]), np.zeros(len(g["s4_K"]), np.int32), output="mm")
     with pytest.raises(ValueError):  # fisheye needs 4 coefficients (camera_array / reprojection.py:26-27 behaviour)
