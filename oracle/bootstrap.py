@@ -264,3 +264,95 @@ def reference_calls_cv2(cam_ids, cam_k, cam_dist, cam_fisheye, sync_index, obs_c
         err = np.vstack([na - pa.reshape(-1, 2), nb - pb.reshape(-1, 2)])
         out[(a, b)] = (R, t, float(np.sqrt(np.mean(np.sum(err**2, axis=1)))))
     return poses, out
+
+
+# ----------------------------------------------------------------------------------------------------------------
+# The same OpenCV calls stage by stage, on normalised coordinates the caller supplies (test infrastructure; needs cv2).
+# Given the device's own undistortion output, which is pinned to cv2.undistortPoints separately, a comparison with these
+# isolates the PnP and stereo kernels from the undistortion.
+# ----------------------------------------------------------------------------------------------------------------
+PNP_OK, PNP_TOO_FEW, PNP_DEGENERATE, PNP_OK_FALLBACK = 0, 1, 3, 4  # caliscope_b200.bootstrap's status codes
+
+
+def pnp_cv2(norm_xy, cam_id, sync_index, object_id, obj_xyz, min_points: int = 4):
+    """pose_network_builder.py:272-321 per (camera, sync, object) group, in sorted key order: cv2.solvePnP(IPPE) on
+    float32 normalised points and float32 model points (NaN z counted as 0), SOLVEPNP_ITERATIVE where IPPE fails, the
+    RMSE through cv2.projectPoints in float32.  Returns (keys (g, 3), R (g, 3, 3), t (g, 3), rmse (g,), status (g,)):
+    PNP_TOO_FEW below min_points (NaN pose), PNP_DEGENERATE for a non-finite pose, PNP_OK_FALLBACK where ITERATIVE ran."""
+    import cv2
+
+    cam_id, sync_index, object_id = (np.asarray(a, np.int64) for a in (cam_id, sync_index, object_id))
+    order = np.lexsort((object_id, sync_index, cam_id))
+    key = np.stack([cam_id[order], sync_index[order], object_id[order]], axis=1)
+    brk = np.flatnonzero(np.any(np.diff(key, axis=0) != 0, axis=1)) + 1
+    starts = np.concatenate([[0], brk, [len(order)]])
+    g = len(starts) - 1
+    R = np.full((g, 3, 3), np.nan)
+    t = np.full((g, 3), np.nan)
+    rmse = np.full(g, np.nan)
+    status = np.full(g, PNP_TOO_FEW, np.int32)
+    Kp, Dp = np.identity(3), np.zeros(5)
+    for i, (s, e) in enumerate(zip(starts[:-1], starts[1:])):
+        if e - s < min_points:
+            continue
+        rows = order[s:e]
+        obj = np.asarray(obj_xyz, np.float64)[rows].copy()
+        obj[:, 2] = np.nan_to_num(obj[:, 2], nan=0.0)
+        if not np.ptp(obj[:, 2]) < 1e-6:
+            raise NotImplementedError("non-planar PnP group (the reference switches to SQPNP)")
+        obj = obj.astype(np.float32)
+        img = np.ascontiguousarray(np.asarray(norm_xy)[rows], dtype=np.float32)
+        ok, rvec, tvec = cv2.solvePnP(obj, img, cameraMatrix=Kp, distCoeffs=Dp, flags=cv2.SOLVEPNP_IPPE)
+        status[i] = PNP_OK
+        if not ok:
+            ok, rvec, tvec = cv2.solvePnP(obj, img, cameraMatrix=Kp, distCoeffs=Dp, flags=cv2.SOLVEPNP_ITERATIVE)
+            status[i] = PNP_OK_FALLBACK
+        if not ok or not (np.isfinite(rvec).all() and np.isfinite(tvec).all()):
+            status[i] = PNP_DEGENERATE
+            continue
+        R[i] = cv2.Rodrigues(rvec)[0]
+        t[i] = tvec.ravel()
+        proj, _ = cv2.projectPoints(obj, rvec, tvec, Kp, Dp)
+        rmse[i] = float(np.sqrt(np.mean(np.sum((img - proj.reshape(-1, 2)) ** 2, axis=1))))
+    return key[starts[:-1]], R, t, rmse, status
+
+
+def stereo_rmse_cv2(pairs, R, t, cam_ids, cam_ignore, norm_xy, cam_id, sync_index, object_id, keypoint_id, min_common: int = 4):
+    """calculate_stereo_rmse_for_pair (:638-685) for each (a, b) pair with pose [R | t]: cv2.triangulatePoints on the
+    float32 normalised points of the common (sync, object, keypoint) observations, cv2.projectPoints into both views,
+    float32 RMSE over the 2N stacked residuals.  Returns (rmse (p,), common count (p,)).  The reference's lookup quirk
+    (:589-598 with :655) is kept: a pair whose cameras come in (b, a) order in the dict ``cam_ids``, or that includes an
+    ignored camera, has no common observations (count 0, NaN); fewer than ``min_common`` gives NaN with its count."""
+    import cv2
+
+    pos = {int(c): i for i, c in enumerate(cam_ids) if not cam_ignore[i]}
+    cam_id = np.asarray(cam_id, np.int64)
+    key = np.zeros(len(cam_id), np.int64)
+    for col in (sync_index, object_id, keypoint_id):  # one integer per (sync, object, keypoint)
+        col = np.asarray(col, np.int64) - int(np.min(col))
+        key = key * (int(col.max()) + 1) + col
+    by_cam = np.argsort(cam_id, kind="stable")
+    cams, first = np.unique(cam_id[by_cam], return_index=True)
+    bounds = dict(zip(cams.tolist(), zip(first.tolist(), np.append(first[1:], len(by_cam)).tolist())))
+    norm = np.asarray(norm_xy, np.float32)
+    p = len(pairs)
+    rmse = np.full(p, np.nan)
+    cnt = np.zeros(p, np.int64)
+    for i, (a, b) in enumerate(np.asarray(pairs, np.int64).reshape(-1, 2)):
+        a, b = int(a), int(b)
+        if a not in pos or b not in pos or not pos[a] < pos[b]:
+            continue
+        ia, ib = (by_cam[slice(*bounds.get(c, (0, 0)))] for c in (a, b))
+        _, xa, xb = np.intersect1d(key[ia], key[ib], return_indices=True)
+        cnt[i] = len(xa)
+        if len(xa) < min_common:
+            continue
+        na, nb = norm[ia[xa]], norm[ib[xb]]
+        Ri, ti = np.asarray(R[i], np.float64), np.asarray(t[i], np.float64).reshape(3)
+        p4 = cv2.triangulatePoints(np.eye(3, 4), np.hstack((Ri, ti.reshape(3, 1))), na.T, nb.T)
+        p3 = p4[:3] / p4[3]
+        pa, _ = cv2.projectPoints(p3.T, np.zeros(3), np.zeros(3), np.eye(3), np.zeros(5))
+        pb, _ = cv2.projectPoints(p3.T, cv2.Rodrigues(Ri)[0], ti, np.eye(3), np.zeros(5))
+        err = np.vstack([na - pa.reshape(-1, 2), nb - pb.reshape(-1, 2)])
+        rmse[i] = float(np.sqrt(np.mean(np.sum(err**2, axis=1))))
+    return rmse, cnt
