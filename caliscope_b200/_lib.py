@@ -158,6 +158,7 @@ SYMBOLS = {
     "cb_ba_problem_stat": (C.c_double, [_P, C.c_int]),
     "cb_ba_constraint_rows": (C.c_int, [_P, _P, _P, _P, _P]),
     "cb_ba_solve": (C.c_int, [_P, C.POINTER(Options), _P, C.POINTER(Result), _P]),
+    "cb_ba_solve_from": (C.c_int, [_P, C.POINTER(Options), _P, _P, C.POINTER(Result), _P]),
     "cb_ba_residuals": (C.c_int, [_P, _P, _P, _P]),
     "cb_ba_jacobian_blocks": (C.c_int, [_P, _P, _P, _P, _P]),
     "cb_ba_reproj_errors_px": (C.c_int, [_P, _P, _P, _P]),

@@ -534,6 +534,7 @@ struct CbBaProblem {
   CUtensorMap zt_map{};  // d_Zt for the product's dense-path feed (Zt is allocated once and never moves)
   unsigned char* d_active = nullptr;
   double *d_lo = nullptr, *d_hi = nullptr;
+  int bounds_for = -1;  // use_bounds value d_lo / d_hi hold (-1: not uploaded yet)
   // work buffers (index [2]: current / trial point, selected on the device by LmState::cur)
   double *d_x = nullptr, *d_xc[2] = {nullptr, nullptr}, *d_xp4[2] = {nullptr, nullptr};
   double *d_camtab[2] = {nullptr, nullptr}, *d_Upk[2] = {nullptr, nullptr}, *d_gc[2] = {nullptr, nullptr},
@@ -548,7 +549,6 @@ struct CbBaProblem {
   cb::LmState* h_state = nullptr;  // pinned, 4 slots
   cb::LmLogRow* d_log = nullptr;
   int log_cap = 4096;
-  double* h_x = nullptr;   // pinned staging for x
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr, ev_state[2] = {nullptr, nullptr};
   cudaEvent_t ev_pp[2][4] = {{nullptr, nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr, nullptr}};  // point-pass / Schur brackets (direct mode)
   cudaStream_t cap_stream = nullptr;
@@ -577,6 +577,8 @@ struct CbBaProblem {
   int *d_covRank = nullptr, *d_covFail = nullptr;
   unsigned char* d_covFree = nullptr;
   float cov_ms[3] = {0.f, 0.f, 0.f};  // last call: linearisation + Schur, dense inverse, point marginals
+  // last solve, host microseconds: bounds, start state, upload of x, LM loop and download of x up to the synchronisation
+  double solve_host_us[4] = {0.0, 0.0, 0.0, 0.0};
   size_t red_len() const { return (size_t)nP * nP + 3 * (size_t)nP + 1 + red_slots; }
   cb::CPtr2 c_camtab() const { return {{d_camtab[0], d_camtab[1]}}; }
   cb::Ptr2 m_camtab() const { return {{d_camtab[0], d_camtab[1]}}; }
@@ -1005,26 +1007,33 @@ int enqueue_trial(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const
   return CB_OK;
 }
 
-int upload_x(CbBaProblem* p, const double* x, cudaStream_t st) {
-  stream_copy(p->h_x, x, sizeof(double) * p->n_params);
-  CB_CUDA(cudaMemcpyAsync(p->d_x, p->h_x, sizeof(double) * p->n_params, cudaMemcpyHostToDevice, st));
-  const int n = std::max(p->n_cams * p->P, p->n_pts);
-  CB_LAUNCH(cb::unpack_x_kernel, cdiv(std::max(n, 1), 256), 256, 0, st, p->d_x, p->d_cam_xoff, p->d_cam_flags,
-            p->d_cam_const, p->n_cams, p->P, p->n_pts, p->ncp, p->d_xc[0], p->d_xp4[0]);
+// x (the caller's pageable array) -> buffer 0.  At the size of x (1.2 MB on cfg4) the driver's own staging of a pageable
+// copy is faster than a copy into a pinned block followed by its DMA (DESIGN 7, "The solve's host path"); the call returns
+// once x has been read.  fresh: the same launch clears the buffers a solve starts from zero (init_state), which must
+// precede it.
+int upload_x(CbBaProblem* p, const double* x, cudaStream_t st, bool fresh = false) {
+  CB_CUDA(cudaMemcpyAsync(p->d_x, x, sizeof(double) * p->n_params, cudaMemcpyHostToDevice, st));
+  const int n = std::max(std::max(p->n_cams * p->P, p->n_pts), fresh ? (int)cb::SC_COUNT : 1);
+  const cb::FreshState z = fresh ? cb::FreshState{p->d_gmax, p->d_counter, p->d_sc, p->d_Dc2, p->d_Dp2} : cb::FreshState{};
+  CB_LAUNCH(cb::unpack_x_kernel, cdiv(n, 256), 256, 0, st, p->d_x, p->d_cam_xoff, p->d_cam_flags, p->d_cam_const,
+            p->n_cams, p->P, p->n_pts, p->ncp, p->d_xc[0], p->d_xp4[0], z);
   return CB_OK;
 }
 
-int download_x(CbBaProblem* p, int cur, double* x, cudaStream_t st) {
+// the final point (LmState::cur) -> x (the caller's pageable array), queued right behind the LM loop; the copy into
+// pageable memory returns when x has been written, after everything queued before it
+int download_x(CbBaProblem* p, double* x, cudaStream_t st) {
   const int n = std::max(p->n_cams * p->P, p->n_pts);
   CB_LAUNCH(cb::pack_x_kernel, cdiv(std::max(n, 1), 256), 256, 0, st, p->d_x, p->d_cam_xoff, p->d_cam_flags, p->n_cams,
-            p->P, p->n_pts, p->ncp, p->d_xc[cur], p->d_xp4[cur]);
-  CB_CUDA(cudaMemcpyAsync(p->h_x, p->d_x, sizeof(double) * p->n_params, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaStreamSynchronize(st));
-  std::memcpy(x, p->h_x, sizeof(double) * p->n_params);
+            p->P, p->n_pts, p->ncp, (const cb::LmState*)p->d_state, cb::CPtr2{{p->d_xc[0], p->d_xc[1]}}, p->c_xp());
+  CB_CUDA(cudaMemcpyAsync(x, p->d_x, sizeof(double) * p->n_params, cudaMemcpyDeviceToHost, st));
   return CB_OK;
 }
 
+// lower / upper bounds of the camera parameters, uploaded when the problem's use_bounds value changes (they depend on
+// nothing else)
 int set_bounds(CbBaProblem* p, bool use_bounds, cudaStream_t st) {
+  if (p->bounds_for == (use_bounds ? 1 : 0)) return CB_OK;
   std::vector<double> lo((size_t)p->nP, -1e300), hi((size_t)p->nP, 1e300);
   if (use_bounds && p->P == 9) {
     for (int c = 0; c < p->n_cams; ++c)
@@ -1036,11 +1045,13 @@ int set_bounds(CbBaProblem* p, bool use_bounds, cudaStream_t st) {
   }
   CB_CUDA(cudaMemcpyAsync(p->d_lo, lo.data(), sizeof(double) * p->nP, cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaMemcpyAsync(p->d_hi, hi.data(), sizeof(double) * p->nP, cudaMemcpyHostToDevice, st));
-  CB_CUDA(cudaStreamSynchronize(st));
+  // a copy from pageable memory has read its source when it returns, so the vectors may go; no synchronisation
+  p->bounds_for = use_bounds ? 1 : 0;
   return CB_OK;
 }
 
-// fresh device state for a solve (or a diagnostic evaluation) starting at buffer 0
+// fresh device state for a solve (or a diagnostic evaluation) starting at buffer 0, in one copy from pinned memory.  The
+// buffers that start from zero are cleared by the upload of x that must follow (upload_x(..., fresh = true)).
 int init_state(CbBaProblem* p, const CbBaOptions* opt, double lam, long long max_nfev, cudaStream_t st) {
   cb::LmState& h = p->h_state[3];
   std::memset(&h, 0, sizeof(h));
@@ -1059,11 +1070,6 @@ int init_state(CbBaProblem* p, const CbBaOptions* opt, double lam, long long max
     h.epoch_big = g->epoch_big; h.epoch_small = g->epoch_small;
   }
   CB_CUDA(cudaMemcpyAsync(p->d_state, &h, sizeof(h), cudaMemcpyHostToDevice, st));
-  CB_CUDA(cudaMemsetAsync(p->d_gmax, 0, 2 * sizeof(unsigned long long), st));
-  CB_CUDA(cudaMemsetAsync(p->d_counter, 0, 4 * sizeof(unsigned int), st));
-  CB_CUDA(cudaMemsetAsync(p->d_sc, 0, sizeof(double) * cb::SC_COUNT, st));
-  CB_CUDA(cudaMemsetAsync(p->d_Dc2, 0, sizeof(double) * p->nP, st));
-  CB_CUDA(cudaMemsetAsync(p->d_Dp2, 0, sizeof(double) * 3 * (size_t)std::max(p->n_pts, 1), st));
   return CB_OK;
 }
 
@@ -1124,7 +1130,7 @@ int ensure_graph(CbBaProblem* p, const CbBaOptions* opt, bool loop) {
 // trial ahead and looks at the state of trial t-1 while trial t executes.
 // ------------------------------------------------------------------------------------------
 template <int P>
-int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult* res, cudaStream_t st) {
+int lm_solve(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x_out, CbBaResult* res, cudaStream_t st) {
   NvtxRange nvtx_solve("cb_ba_solve");
   const long long max_nfev = opt->max_nfev > 0 ? opt->max_nfev : 100ll * p->n_params;
   const bool verbose = opt->verbose >= 2 && opt->rank == 0;
@@ -1142,9 +1148,18 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
   bool use_graph = !direct && !use_loop;
   if (use_graph && ensure_graph<P>(p, opt, false) != CB_OK) { cudaGetLastError(); use_graph = false; }
 
+  auto t_mark = std::chrono::steady_clock::now();
+  auto host_span = [&](int i) {  // host time since the previous mark -> solve_host_us[i] (stat keys 14-17)
+    const auto now = std::chrono::steady_clock::now();
+    p->solve_host_us[i] = std::chrono::duration<double, std::micro>(now - t_mark).count();
+    t_mark = now;
+  };
   CB_TRY(set_bounds(p, opt->use_bounds != 0, st));
+  host_span(0);
   CB_TRY(init_state(p, opt, opt->lambda0 > 0 ? opt->lambda0 : 1e-4, max_nfev, st));
-  CB_TRY(upload_x(p, x_inout, st));
+  host_span(1);
+  CB_TRY(upload_x(p, x0, st, true));
+  host_span(2);
   CB_CUDA(cudaEventRecord(p->ev0, st));
   CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
   CB_TRY(camera_pass<P>(p, 0, 0, st));
@@ -1201,7 +1216,13 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
     }
     ++t;
   }
+  // the final point goes to the host right behind the loop, so the GPU never waits on the host in between
+  if (rc == CB_OK) {
+    cudaEventRecord(p->ev1, st);  // an error here is the stream's, and the synchronisation below reports it
+    rc = download_x(p, x_out, st);
+  }
   cudaError_t e = cudaStreamSynchronize(st);
+  host_span(3);
   if (rc == CB_OK && e != cudaSuccess) { g_last_error = std::string("LM solve: ") + cudaGetErrorString(e); rc = CB_E_CUDA; }
   if (rc != CB_OK) { if (p->peer) p->peer->poisoned = true; return rc; }
   const cb::LmState fin = p->h_state[(t - 1) & 1];   // trial t-1 ran predicated-off or finished: final either way
@@ -1231,8 +1252,6 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult
                    (long long)rows[i].nfev, rows[i].cost, rows[i].cost_new, rows[i].ratio, rows[i].lam, rows[i].step,
                    rows[i].gnorm, (int)rows[i].pcg);
   }
-  CB_CUDA(cudaEventRecord(p->ev1, st));
-  CB_TRY(download_x(p, fin.cur, x_inout, st));
   float ms = 0.f;
   CB_CUDA(cudaEventElapsedTime(&ms, p->ev0, p->ev1));
   res->status = fin.status;
@@ -1500,7 +1519,6 @@ int cb_ba_problem_destroy(CbBaProblem* p) {
   if (p->cap_stream) cudaStreamDestroy(p->cap_stream);
   for (void* a : p->allocs) cached_free(a);
   cached_free_host(p->h_state);
-  cached_free_host(p->h_x);
   for (cudaEvent_t e : {p->ev0, p->ev1, p->ev2, p->ev3, p->ev_state[0], p->ev_state[1], p->ev_pp[0][0], p->ev_pp[0][1],
                         p->ev_pp[0][2], p->ev_pp[0][3], p->ev_pp[1][0], p->ev_pp[1][1], p->ev_pp[1][2], p->ev_pp[1][3]})
     if (e) cudaEventDestroy(e);
@@ -1525,6 +1543,7 @@ double cb_ba_problem_stat(const CbBaProblem* p, int what) {
     case 11: return (double)p->pcg_cs;
     case 12: return p->pcg_mode == 2 ? (double)p->pcg_cl : 0.0;
     case 13: return p->order_identity ? 0.0 : 1.0;
+    case 14: case 15: case 16: case 17: return p->solve_host_us[what - 14];
     default: return -1.0;
   }
 }
@@ -2031,7 +2050,6 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   CB_CUDA(cudaMemsetAsync(p->d_red2, 0, sizeof(double) * 8, st));
   CB_CUDA(cudaMemsetAsync(p->d_Linv6, 0, sizeof(double) * 6 * npts, st));
   CB_TRY(cached_malloc_host((void**)&p->h_state, sizeof(cb::LmState) * 4));
-  CB_TRY(cached_malloc_host((void**)&p->h_x, sizeof(double) * ((size_t)p->n_params + 1)));
   for (cudaEvent_t* e : {&p->ev0, &p->ev1, &p->ev2, &p->ev3, &p->ev_pp[0][0], &p->ev_pp[0][1], &p->ev_pp[0][2], &p->ev_pp[0][3],
                          &p->ev_pp[1][0], &p->ev_pp[1][1], &p->ev_pp[1][2], &p->ev_pp[1][3]})
     CB_CUDA(cudaEventCreate(e));
@@ -2104,7 +2122,12 @@ int cb_ba_problem_create(const CbBaProblemDesc* d, int device, void* stream, CbB
 }
 
 int cb_ba_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult* result, void* stream) {
-  if (!p || !opt || !x_inout || !result) { g_last_error = "cb_ba_solve: null argument"; return CB_E_INVALID; }
+  return cb_ba_solve_from(p, opt, x_inout, x_inout, result, stream);
+}
+
+int cb_ba_solve_from(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x_out, CbBaResult* result,
+                     void* stream) {
+  if (!p || !opt || !x0 || !x_out || !result) { g_last_error = "cb_ba_solve: null argument"; return CB_E_INVALID; }
   if (opt->loss < 0 || opt->loss > CB_LOSS_ARCTAN) { g_last_error = "unknown loss id"; return CB_E_INVALID; }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -2130,7 +2153,7 @@ int cb_ba_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaRes
                    "CbBaProblemDesc.cam_order (the same on every rank)";
     return CB_E_INVALID;
   }
-  const int rc = p->P == 6 ? lm_solve<6>(p, opt, x_inout, result, st) : lm_solve<9>(p, opt, x_inout, result, st);
+  const int rc = p->P == 6 ? lm_solve<6>(p, opt, x0, x_out, result, st) : lm_solve<9>(p, opt, x0, x_out, result, st);
   p->peer = nullptr;
   return rc;
 }
@@ -2205,7 +2228,7 @@ int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss, double
   opt.ftol = opt.xtol = opt.gtol = 0.0;
   CB_TRY(set_bounds(p, false, st));
   CB_TRY(init_state(p, &opt, lam, 1ll << 40, st));
-  CB_TRY(upload_x(p, x, st));
+  CB_TRY(upload_x(p, x, st, true));
   CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
   CB_TRY(camera_pass<P>(p, 0, 0, st));
   CB_TRY(build_system<P>(p, &opt, st));
@@ -2322,7 +2345,7 @@ int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs, int n_
   const int big[2] = {INT32_MAX, INT32_MAX};
   CB_CUDA(cudaMemcpyAsync(p->d_covFail, big, sizeof(big), cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaMemcpyAsync(p->d_covFree, fr.data(), nP, cudaMemcpyHostToDevice, st));
-  CB_TRY(upload_x(p, x, st));
+  CB_TRY(upload_x(p, x, st, true));
   CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
   CB_TRY(camera_pass<P>(p, 0, 0, st));
   CB_TRY(build_system<P>(p, &opt, st, nullptr, true));
@@ -3059,7 +3082,7 @@ int tri_cams_upload(int32_t n_cams, const int32_t* cam_flags, const double* cam_
   CB_CUDA(cudaMemcpyAsync(d_const, cam_const, sizeof(double) * 9 * n_cams, cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaMemcpyAsync(d_x, cam_x, sizeof(double) * ncp, cudaMemcpyHostToDevice, st));
   CB_LAUNCH(cb::unpack_x_kernel, cdiv((long long)n_cams * P, 256), 256, 0, st, d_x, d_xoff, d_flags, d_const, n_cams, P,
-            0, ncp, d_xc, nullptr);
+            0, ncp, d_xc, nullptr, cb::FreshState{});
   CB_LAUNCH(cb::cam_prep_kernel, cdiv(n_cams, 64), 64, 0, st, d_xc, d_flags, d_const, n_cams, P, d_camtab);
   c->camtab = d_camtab;
   return CB_OK;

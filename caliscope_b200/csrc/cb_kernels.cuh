@@ -44,14 +44,31 @@ enum {
   SC_PCG_ITS, SC_PCG_REL, SC_PCG_FLAG, SC_GNORM_P, SC_PCG_T0 = 16, SC_COUNT = 24
 };
 
+// The buffers an LM solve starts from zero: gradient maxima (2), trial counters (4), scalar slots (SC_COUNT), Marquardt
+// scales of the cameras (n_cams P) and points (3 n_pts).  unpack_x_kernel clears them when `Dp2` is set, so that a
+// fresh state costs no launches of its own (threads: max(n_cams P, n_pts, SC_COUNT)).
+struct FreshState {
+  unsigned long long* gmax;
+  unsigned int* counter;
+  double *sc, *Dc2, *Dp2;
+};
+
 // ---------------------------------------------------------------------------------------------
 // x (BundleParameterization.pack layout, caller's camera order) <-> engine buffers.  Internal camera slot i holds the
 // caller's camera whose block starts at cam_xoff[i] (the engine may reorder cameras so that cameras that see the same
 // points share Schur tiles); its width is 9 with free intrinsics, else 6.
 __global__ void unpack_x_kernel(const double* __restrict__ x, const int* __restrict__ cam_xoff,
                                 const int* __restrict__ cam_flags, const double* __restrict__ cam_const,
-                                int n_cams, int P, int n_pts, int ncp, double* __restrict__ xc, double* __restrict__ xp4) {
+                                int n_cams, int P, int n_pts, int ncp, double* __restrict__ xc, double* __restrict__ xp4,
+                                FreshState z) {
   int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (z.Dp2 != nullptr) {
+    if (i < 2) z.gmax[i] = 0ull;
+    if (i < 4) z.counter[i] = 0u;
+    if (i < SC_COUNT) z.sc[i] = 0.0;
+    if (i < n_cams * P) z.Dc2[i] = 0.0;
+    if (i < n_pts) { z.Dp2[3 * (size_t)i] = 0.0; z.Dp2[3 * (size_t)i + 1] = 0.0; z.Dp2[3 * (size_t)i + 2] = 0.0; }
+  }
   if (i < n_cams * P) {
     int c = i / P, p = i % P;
     int w = (cam_flags[c] & 1) ? 9 : 6;
@@ -65,21 +82,6 @@ __global__ void unpack_x_kernel(const double* __restrict__ x, const int* __restr
     xp4[4 * (size_t)i + 1] = x[ncp + 3 * (size_t)i + 1];
     xp4[4 * (size_t)i + 2] = x[ncp + 3 * (size_t)i + 2];
     xp4[4 * (size_t)i + 3] = 0.0;
-  }
-}
-
-__global__ void pack_x_kernel(double* __restrict__ x, const int* __restrict__ cam_xoff, const int* __restrict__ cam_flags,
-                              int n_cams, int P, int n_pts, int ncp, const double* __restrict__ xc,
-                              const double* __restrict__ xp4) {
-  int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n_cams * P) {
-    int c = i / P, p = i % P;
-    if (p < ((cam_flags[c] & 1) ? 9 : 6)) x[cam_xoff[c] + p] = xc[i];
-  }
-  if (i < n_pts) {
-    x[ncp + 3 * (size_t)i + 0] = xp4[4 * (size_t)i + 0];
-    x[ncp + 3 * (size_t)i + 1] = xp4[4 * (size_t)i + 1];
-    x[ncp + 3 * (size_t)i + 2] = xp4[4 * (size_t)i + 2];
   }
 }
 
@@ -103,6 +105,25 @@ struct Ptr2 {
 struct CPtr2 {
   const double* p[2];
 };
+
+// engine buffers -> x, from the buffer pair's point LmState::cur (read on the device, so the download can be queued
+// behind the LM loop before its outcome is known on the host)
+__global__ void pack_x_kernel(double* __restrict__ x, const int* __restrict__ cam_xoff, const int* __restrict__ cam_flags,
+                              int n_cams, int P, int n_pts, int ncp, const LmState* __restrict__ st, CPtr2 xc2, CPtr2 xp2) {
+  const bool sel = st->cur != 0;  // a select, not a dynamic index into the parameter (that would go through the stack)
+  const double* __restrict__ xc = sel ? xc2.p[1] : xc2.p[0];
+  const double* __restrict__ xp4 = sel ? xp2.p[1] : xp2.p[0];
+  int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_cams * P) {
+    int c = i / P, p = i % P;
+    if (p < ((cam_flags[c] & 1) ? 9 : 6)) x[cam_xoff[c] + p] = xc[i];
+  }
+  if (i < n_pts) {
+    x[ncp + 3 * (size_t)i + 0] = xp4[4 * (size_t)i + 0];
+    x[ncp + 3 * (size_t)i + 1] = xp4[4 * (size_t)i + 1];
+    x[ncp + 3 * (size_t)i + 2] = xp4[4 * (size_t)i + 2];
+  }
+}
 
 // rotation half of a camera table entry: Rodrigues R(r) and the SO(3) right Jacobian (CT_R, CT_JR)
 __device__ __forceinline__ void cam_prep_rot(double r0, double r1, double r2, double* __restrict__ o) {

@@ -205,7 +205,8 @@ class BAProblem:
         3 Schur CTAs, 4-6 stage milliseconds of the last ``covariance`` call, 7 lanes per point (8 or 32), 8 repeated
         (camera, point) rows, 9 camera table in shared memory, 10 reduced solve (0 direct, 1 L2-streamed PCG, 2 register
         PCG), 11 PCG cluster CTAs, 12 register-PCG columns per lane (0 otherwise), 13 internal camera order differs from
-        the caller's numbering.  -1 for an unknown key."""
+        the caller's numbering, 14-17 host microseconds of the last ``solve`` in the bounds, the start state, the upload
+        of x, and the LM loop with the download of x up to its synchronisation.  -1 for an unknown key."""
         return float(self._lib.cb_ba_problem_stat(self._h, int(what)))
 
     def _x(self, x) -> np.ndarray:
@@ -381,7 +382,8 @@ class BAProblem:
     ) -> SolveResult:
         if loss not in L.LOSS_IDS:
             raise ValueError(f"`loss` must be one of {list(L.LOSS_IDS)}")
-        x = self._x(x0).copy()
+        x0 = self._x(x0)
+        x = np.empty_like(x0)  # the engine reads x0 and writes the result here: x0 stays untouched, x is a fresh array
         opt = L.Options()
         self._lib.cb_ba_default_options(C.byref(opt))
         opt.ftol, opt.xtol, opt.gtol = float(ftol), float(xtol), float(gtol)
@@ -404,7 +406,8 @@ class BAProblem:
         opt.time_kernels = 1 if time_kernels else 0
         res = L.Result()
         try:
-            L.check(self._lib.cb_ba_solve(self._h, C.byref(opt), _ptr(x), C.byref(res), C.c_void_p(stream)), "solve")
+            L.check(self._lib.cb_ba_solve_from(self._h, C.byref(opt), _ptr(x0), _ptr(x), C.byref(res), C.c_void_p(stream)),
+                    "solve")
         except Exception:
             # a sharded solve that fails part-way leaves the ranks' reduction sequence numbers out of step: the engine
             # refuses further solves on this peer group; make the Python cache re-create it (collectively) next time

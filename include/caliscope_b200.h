@@ -170,8 +170,9 @@ int64_t cb_ba_problem_n_params(const CbBaProblem* p);
  * 7: lanes per point in the point kernels (8, or 32 when points average more than 96 rows), 8: 1 if some (camera, point)
  * pair has repeated rows, 9: 1 if the point kernels stage the camera table in shared memory, 10: reduced solve (0 direct,
  * 1 PCG with the slab streamed from L2, 2 PCG with the slab in registers), 11: CTAs of the PCG cluster, 12: matrix
- * columns per lane of the register PCG (0 otherwise), 13: 1 if the internal camera order is not the caller's numbering.
- * -1 for an unknown key. */
+ * columns per lane of the register PCG (0 otherwise), 13: 1 if the internal camera order is not the caller's numbering,
+ * 14-17: host microseconds the last cb_ba_solve spent on the bounds, the start state, the upload of x, and the LM loop
+ * with the download of x up to its one synchronisation.  -1 for an unknown key. */
 double cb_ba_problem_stat(const CbBaProblem* p, int what);
 
 /* Constraint rows at x, n_c = CbBaProblemDesc.n_constraints: r_out (n_c) == the tail of joint_residuals; dir_out (n_c x 3,
@@ -180,8 +181,14 @@ double cb_ba_problem_stat(const CbBaProblem* p, int what);
 int cb_ba_constraint_rows(CbBaProblem* p, const double* x, double* r_out, double* dir_out, void* stream);
 
 /* Replaces least_squares(joint_residuals, x0, jac=joint_jacobian, method="trf", ...)
- * (capture_volume.py:387-411).  x_inout: host, n_params doubles, overwritten with result.x. */
+ * (capture_volume.py:387-411).  x_inout: host, n_params doubles, overwritten with result.x (after a failure: see
+ * cb_ba_solve_from). */
 int cb_ba_solve(CbBaProblem* p, const CbBaOptions* opt, double* x_inout, CbBaResult* result, void* stream);
+/* The same solve from x0 into x_out (host, n_params doubles each; they may be the same array), so that a caller who
+ * keeps x0 needs no copy of it.  x_out is written only by a solve that ran to its end (its content is unspecified after
+ * a failure reported by the device or by a peer rank). */
+int cb_ba_solve_from(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x_out, CbBaResult* result,
+                     void* stream);
 
 /* == joint_residuals (reprojection.py:75-119), reprojection rows only: r_out host, 2*n_obs,
  * interleaved (x, y) / fx_initial in the caller's observation order. */
