@@ -73,6 +73,14 @@ std::atomic<long long> g_launches{0};
 
 inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// f(L) with L a std::integral_constant of the lanes per group (32, else 8), for launching the kernel instantiated
+// for them
+template <typename F>
+void with_lanes(int lanes, F&& f) {
+  if (lanes == 32) f(std::integral_constant<int, 32>{});
+  else f(std::integral_constant<int, 8>{});
+}
+
 // ------------------------------------------------------------------------------------------
 // NCCL, resolved at run time from the libnccl the process already has loaded (torch's bundled copy):
 // no link-time dependency, no second NCCL in the address space.
@@ -501,6 +509,67 @@ struct TrialGraph {
   int n_kernels = 0;  // kernels of one trial
 };
 
+// The kernel instantiations one problem launches, and the sizes that follow from the same choice.  select_kernels
+// fills it once, at creation; every launch, shared-memory opt-in and buffer size goes through it.  A kernel's signature
+// does not depend on its template arguments, so one instantiation names the type.
+struct Kernels {
+  decltype(&cb::resjac_kernel<6, 0>) resjac[5] = {};  // by MODE; the host launches 0, 2, 3 and 4
+  decltype(&cb::jac_blocks_kernel<6>) jac_blocks = nullptr;
+  decltype(&cb::pt_pass_kernel<6, 8, false, false>) pt_pass = nullptr, pt_pass_cov = nullptr;
+  decltype(&cb::pt_backsub_kernel<6, 8, false>) pt_backsub = nullptr;
+  decltype(&cb::trial_reduce_kernel<6>) trial_reduce = nullptr;
+  decltype(&cb::schur_finalize_kernel<6>) schur_finalize = nullptr;
+  decltype(&cb::schur_finalize_peer_kernel<6>) schur_finalize_peer = nullptr;
+  decltype(&cb::reduced_prep_kernel<6>) reduced_prep = nullptr;
+  decltype(&cb::small_rig_step_kernel<6>) small_rig_step = nullptr;
+  decltype(&cb::comp_build_kernel<6>) comp_build = nullptr;
+  decltype(&cb::cov_point_kernel<6>) cov_point = nullptr;
+  decltype(&cb::pcg_cluster_kernel<1, 6, 1>) pcg = nullptr;
+  size_t pt_stage_bytes = 0;  // the point pass's Zt staging (variants without repeated rows)
+  int NACC = 0, NU = 0;       // RowT<P>: accumulators of a camera-major chunk, packed upper triangle of a camera block
+};
+
+// P: camera stride (6, or 9 with free intrinsics).  pt_lanes, dups, cam_in_smem: lanes per point, repeated (camera,
+// point) rows present, camera table staged in shared memory (point pass and back-substitution).  pcg_mode 1: slab
+// streamed from L2, 2: slab in registers with pcg_cl columns per lane.
+static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, int pcg_mode, int pcg_cl) {
+  Kernels k;
+  auto with_stride = [&](auto f) { if (P == 6) f(std::integral_constant<int, 6>{}); else f(std::integral_constant<int, 9>{}); };
+  auto with_bool = [](bool b, auto f) { if (b) f(std::true_type{}); else f(std::false_type{}); };
+  with_stride([&](auto stride) {
+    constexpr int S = decltype(stride)::value;
+    k.NACC = cb::RowT<S>::NACC; k.NU = cb::RowT<S>::NU;
+    k.resjac[0] = cb::resjac_kernel<S, 0>; k.resjac[2] = cb::resjac_kernel<S, 2>;
+    k.resjac[3] = cb::resjac_kernel<S, 3>; k.resjac[4] = cb::resjac_kernel<S, 4>;
+    k.jac_blocks = cb::jac_blocks_kernel<S>;
+    k.trial_reduce = cb::trial_reduce_kernel<S>;
+    k.schur_finalize = cb::schur_finalize_kernel<S>;
+    k.schur_finalize_peer = cb::schur_finalize_peer_kernel<S>;
+    k.reduced_prep = cb::reduced_prep_kernel<S>;
+    k.small_rig_step = cb::small_rig_step_kernel<S>;
+    k.comp_build = cb::comp_build_kernel<S>;
+    k.cov_point = cb::cov_point_kernel<S>;
+    with_lanes(pt_lanes, [&](auto lanes) {
+      constexpr int L = decltype(lanes)::value;
+      k.pt_stage_bytes = cb::pt_stage_bytes<S, L>();
+      with_bool(cam_in_smem, [&](auto sm) {
+        constexpr bool SM = decltype(sm)::value;
+        k.pt_backsub = cb::pt_backsub_kernel<S, L, SM>;
+        with_bool(dups, [&](auto d) {
+          constexpr bool D = decltype(d)::value;
+          k.pt_pass = cb::pt_pass_kernel<S, L, D, SM>;
+          k.pt_pass_cov = cb::pt_pass_kernel<S, L, D, SM, true>;
+        });
+      });
+    });
+    if (pcg_mode != 2) k.pcg = cb::pcg_cluster_kernel<1, S, 1>;
+    else
+      k.pcg = pcg_cl == 2 ? cb::pcg_cluster_kernel<2, S, 2> : pcg_cl == 6 ? cb::pcg_cluster_kernel<2, S, 6>
+            : pcg_cl == 12 ? cb::pcg_cluster_kernel<2, S, 12> : cb::pcg_cluster_kernel<2, S, 18>;
+  });
+  return k;
+}
+
 struct CbBaProblem {
   int device = 0, num_sms = 132;
   int n_cams = 0, n_pts = 0, P = 6, nP = 0, n_obs = 0, n_params = 0;
@@ -508,6 +577,7 @@ struct CbBaProblem {
   int n_chunks = 0, pt_grid = 0, pt_lanes = 32, n_dups = 0;
   int cam_in_smem = 0;
   size_t pt_smem = 0, bs_smem = 0;
+  Kernels k;  // chosen by choose_pcg_config from P, pt_lanes, n_dups, cam_in_smem and the PCG configuration
   std::vector<int> h_cam_off;   // caller's layout: x offset of caller camera c
   std::vector<int> h_perm, h_slot;  // internal slot i holds caller camera h_perm[i]; h_slot[c] = slot of caller camera c
   std::vector<int> h_iflags;    // flags by internal slot
@@ -822,61 +892,34 @@ int build_indices(CbBaProblem* p, const int* d_obs_cam, const int* d_obs_pt, con
 // ------------------------------------------------------------------------------------------
 // the kernels of one evaluation / one LM trial
 // ------------------------------------------------------------------------------------------
-template <int P>
 int run_cam_prep(CbBaProblem* p, const double* xc, double* camtab, cudaStream_t st) {
-  CB_LAUNCH(cb::cam_prep_kernel, cdiv(p->n_cams, 64), 64, 0, st, xc, p->d_cam_flags, p->d_cam_const, p->n_cams, P, camtab);
+  CB_LAUNCH(cb::cam_prep_kernel, cdiv(p->n_cams, 64), 64, 0, st, xc, p->d_cam_flags, p->d_cam_const, p->n_cams, p->P, camtab);
   return CB_OK;
 }
 
-// camera-major pass; st_dev == nullptr: stand-alone evaluation at buffer 0
-template <int P, int MODE>
-void launch_resjac(CbBaProblem* p, const cb::LmState* st_dev, int flip, int loss, double fscale, double* out2,
+// camera-major pass in the kernel's MODE `mode`; st_dev == nullptr: stand-alone evaluation at buffer 0
+void launch_resjac(CbBaProblem* p, int mode, const cb::LmState* st_dev, int flip, int loss, double fscale, double* out2,
                    cudaStream_t st) {
   if (p->n_chunks == 0) return;
-  CB_LAUNCH((cb::resjac_kernel<P, MODE>), p->n_chunks, cb::RJ_THREADS, 0, st, st_dev, flip, p->d_chunk_cam,
+  CB_LAUNCH(p->k.resjac[mode], p->n_chunks, cb::RJ_THREADS, 0, st, st_dev, flip, p->d_chunk_cam,
             p->d_chunk_begin, p->d_chunk_end, p->d_cm_xy, p->d_cm_pt, p->d_cm_orig, p->c_camtab(), p->c_xp(), loss,
             fscale, p->d_partial, out2);
 }
 
-// COV: the covariance variant (pseudo-inverse root of V into d_covR, rank into d_covRank)
-template <int P, bool COV = false>
-void launch_pt_pass(CbBaProblem* p, cudaStream_t st) {
-#define CB_PT_PASS(LANES, DUPS, SM)                                                                                   \
-  CB_LAUNCH((cb::pt_pass_kernel<P, LANES, DUPS, SM, COV>), p->pt_grid, cb::PT_WARPS * 32, p->pt_smem, st, p->d_state, \
-            p->d_pt_start, p->d_pm_cam, p->d_pm_xy, p->d_pt_comp, p->n_pts, p->n_cams, p->c_camtab(), p->c_xp(),       \
-            p->d_V6, p->d_gp, p->d_Dp2, COV ? p->d_covR : p->d_Linv6, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax,    \
-            COV ? p->d_covRank : nullptr)
-#define CB_PT_PASS2(LANES, DUPS) do { if (p->cam_in_smem) CB_PT_PASS(LANES, DUPS, true); else CB_PT_PASS(LANES, DUPS, false); } while (0)
-  if (p->pt_lanes == 8) { if (p->n_dups) CB_PT_PASS2(8, true); else CB_PT_PASS2(8, false); }
-  else { if (p->n_dups) CB_PT_PASS2(32, true); else CB_PT_PASS2(32, false); }
-#undef CB_PT_PASS2
-#undef CB_PT_PASS
+// cov: the covariance variant (pseudo-inverse root of V into d_covR, rank into d_covRank)
+void launch_pt_pass(CbBaProblem* p, bool cov, cudaStream_t st) {
+  const auto pt_pass = cov ? p->k.pt_pass_cov : p->k.pt_pass;
+  CB_LAUNCH(pt_pass, p->pt_grid, cb::PT_WARPS * 32, p->pt_smem, st, p->d_state,
+            p->d_pt_start, p->d_pm_cam, p->d_pm_xy, p->d_pt_comp, p->n_pts, p->n_cams, p->c_camtab(), p->c_xp(),
+            p->d_V6, p->d_gp, p->d_Dp2, cov ? p->d_covR : p->d_Linv6, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax,
+            cov ? p->d_covRank : nullptr);
 }
 
-template <int P>
 void launch_pt_backsub(CbBaProblem* p, double* dp_out, cudaStream_t st) {
   const int bstride = p->pt_grid + p->n_comp;
-#define CB_PT_BACK(LANES, SM)                                                                                         \
-  CB_LAUNCH((cb::pt_backsub_kernel<P, LANES, SM>), p->pt_grid, cb::PT_WARPS * 32, p->bs_smem, st, p->d_state,         \
-            p->d_pt_start, p->d_pm_cam, p->d_pm_xy, p->d_pt_comp, p->n_pts, p->n_cams, p->nP, p->c_camtab(),           \
-            p->m_xp(), p->d_dc, p->d_Linv6, p->d_tvec, p->d_gp, p->d_Dp2, dp_out, p->d_bpart, bstride)
-  if (p->pt_lanes == 8) { if (p->cam_in_smem) CB_PT_BACK(8, true); else CB_PT_BACK(8, false); }
-  else { if (p->cam_in_smem) CB_PT_BACK(32, true); else CB_PT_BACK(32, false); }
-#undef CB_PT_BACK
-}
-
-using PcgFn = void (*)(const cb::LmState*, const double*, const double*, const double*, int, int, int, double, int,
-                       double*, double*);
-// mode 1: slab streamed from L2, 2: slab in registers with cl columns per lane
-PcgFn pcg_fn(int mode, int P, int cl) {
-  if (mode == 2) {
-    if (P == 6)
-      return cl == 2 ? cb::pcg_cluster_kernel<2, 6, 2> : cl == 6 ? cb::pcg_cluster_kernel<2, 6, 6>
-           : cl == 12 ? cb::pcg_cluster_kernel<2, 6, 12> : cb::pcg_cluster_kernel<2, 6, 18>;
-    return cl == 2 ? cb::pcg_cluster_kernel<2, 9, 2> : cl == 6 ? cb::pcg_cluster_kernel<2, 9, 6>
-         : cl == 12 ? cb::pcg_cluster_kernel<2, 9, 12> : cb::pcg_cluster_kernel<2, 9, 18>;
-  }
-  return P == 6 ? cb::pcg_cluster_kernel<1, 6, 1> : cb::pcg_cluster_kernel<1, 9, 1>;
+  CB_LAUNCH(p->k.pt_backsub, p->pt_grid, cb::PT_WARPS * 32, p->bs_smem, st, p->d_state,
+            p->d_pt_start, p->d_pm_cam, p->d_pm_xy, p->d_pt_comp, p->n_pts, p->n_cams, p->nP, p->c_camtab(),
+            p->m_xp(), p->d_dc, p->d_Linv6, p->d_tvec, p->d_gp, p->d_Dp2, dp_out, p->d_bpart, bstride);
 }
 
 int launch_pcg(CbBaProblem* p, const cb::LmState* st_dev, double tol2, int max_iter, cudaStream_t st) {
@@ -894,23 +937,21 @@ int launch_pcg(CbBaProblem* p, const cb::LmState* st_dev, double tol2, int max_i
   cfg.numAttrs = 1;
   const double* S = p->d_red;
   const double* b = p->d_red + (size_t)p->nP * p->nP;
-  auto fn = pcg_fn(p->pcg_mode, p->P, p->pcg_cl);
-  CB_CUDA(cudaLaunchKernelEx(&cfg, fn, st_dev, S, b, (const double*)p->d_Minv, p->nP, p->pcg_npa, p->pcg_rows, tol2,
+  CB_CUDA(cudaLaunchKernelEx(&cfg, p->k.pcg, st_dev, S, b, (const double*)p->d_Minv, p->nP, p->pcg_npa, p->pcg_rows, tol2,
                              max_iter, p->d_dc, p->d_sc));
   g_launches.fetch_add(1);
   return CB_OK;
 }
 
 // camera-major pass at buffer (cur ^ flip) + reduction of its partials; mode as trial_reduce_kernel
-template <int P>
 int camera_pass(CbBaProblem* p, int flip, int mode, cudaStream_t st) {
   const int loss = 0;
   const double fscale = 1.0;  // the kernels take both from the device state
-  launch_resjac<P, 0>(p, p->d_state, flip, loss, fscale, nullptr, st);
+  launch_resjac(p, 0, p->d_state, flip, loss, fscale, nullptr, st);
   if (p->n_c)
     CB_LAUNCH((cb::constraint_eval_kernel<false>), p->n_cblk, cb::CC_THREADS, 0, st, (const cb::LmState*)p->d_state, flip,
               p->ct, p->c_xp(), loss, fscale, p->m_crs(), p->m_cdirw(), (double*)nullptr, p->d_camcost + p->n_cams);
-  CB_LAUNCH((cb::trial_reduce_kernel<P>), p->n_cams + 1, 64, 0, st, p->d_state, mode, p->n_cams, p->d_cam_chunk_start,
+  CB_LAUNCH(p->k.trial_reduce, p->n_cams + 1, 64, 0, st, p->d_state, mode, p->n_cams, p->d_cam_chunk_start,
             p->d_partial, p->m_Upk(), p->m_gc(), p->m_costsum(), p->d_camcost, p->n_cblk, p->d_bpart,
             p->pt_grid + p->n_comp, p->pt_grid + p->n_comp, p->d_red2, p->d_counter, p->d_sc, p->d_log);
   return CB_OK;
@@ -920,14 +961,12 @@ int camera_pass(CbBaProblem* p, int flip, int mode, cudaStream_t st) {
 // (the last at the head of small_rig_step_kernel on small rigs, see solve_step).  ev: nullptr, or four events that
 // bracket the point pass (0, 1) and the Schur product (2, 3).  cov: the undamped covariance linearisation (point pass with
 // the pseudo-inverse root of V, no reduced_prep_kernel), single rank only
-template <int P>
 int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const cudaEvent_t* ev = nullptr, bool cov = false) {
   if (ev) CB_CUDA(cudaEventRecord(ev[0], st));
-  if (cov) launch_pt_pass<P, true>(p, st);
-  else launch_pt_pass<P>(p, st);
+  launch_pt_pass(p, cov, st);
   if (ev) CB_CUDA(cudaEventRecord(ev[1], st));
   if (p->n_c)
-    CB_LAUNCH((cb::comp_build_kernel<P>), p->n_comp, cb::CC_THREADS, p->comp_build_smem, st, (const cb::LmState*)p->d_state,
+    CB_LAUNCH(p->k.comp_build, p->n_comp, cb::CC_THREADS, p->comp_build_smem, st, (const cb::LmState*)p->d_state,
               p->ct, p->d_pt_start, p->d_pm_cam, p->d_V6, p->d_gp, p->d_Dp2, p->d_gpt, p->c_crs(), p->c_cdirw(), p->n_cams,
               p->d_compL, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax);
   if (ev) CB_CUDA(cudaEventRecord(ev[2], st));
@@ -942,7 +981,7 @@ int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const 
     // finalize + all-reduce over NVLink peer memory in one COOPERATIVE launch (cb_peer.cuh)
     CbPeerGroup* g = (CbPeerGroup*)opt->peer_group;
     int nb = 0;
-    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, cb::schur_finalize_peer_kernel<P>, cb::PEER_THREADS, 0));
+    CB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, p->k.schur_finalize_peer, cb::PEER_THREADS, 0));
     const int grid = std::max(1, std::min(nb, 2)) * p->num_sms;
     const cb::LmState* sd = p->d_state;
     int nP = p->nP, n_blk = p->n_blk, red_slots = p->red_slots, rk = rank;
@@ -950,27 +989,26 @@ int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const 
     const double* gmax = (const double*)p->d_gmax;
     void* args[] = {&sd, &nP, &n_blk, &p->d_tile_of, &p->d_tile_slot_start, &p->d_tile_slots, &p->d_part, &p->d_tpart,
                     &upk, &gc, &cs, &gmax, &red_slots, &rk, &g->tab, &p->d_red};
-    CB_CUDA(cudaLaunchCooperativeKernel((const void*)cb::schur_finalize_peer_kernel<P>, dim3(grid), dim3(cb::PEER_THREADS),
+    CB_CUDA(cudaLaunchCooperativeKernel((const void*)p->k.schur_finalize_peer, dim3(grid), dim3(cb::PEER_THREADS),
                                         args, 0, st));
     g_launches.fetch_add(1);
   } else {
-    CB_LAUNCH((cb::schur_finalize_kernel<P>), cdiv((long long)std::max<size_t>(nfin, p->red_slots), 256), 256, 0, st,
+    CB_LAUNCH(p->k.schur_finalize, cdiv((long long)std::max<size_t>(nfin, p->red_slots), 256), 256, 0, st,
               (const cb::LmState*)p->d_state, p->nP, p->n_blk, p->d_tile_of, p->d_tile_slot_start, p->d_tile_slots,
               p->d_part, p->d_tpart, p->c_Upk(), p->c_gc(), p->c_costsum(), (const double*)p->d_gmax, p->red_slots, rank,
               p->d_red);
     if (sharded(opt)) CB_TRY(do_allreduce(opt, p->d_red, (long long)p->red_len(), st));
   }
   if (!p->direct_solve && !cov)
-    CB_LAUNCH((cb::reduced_prep_kernel<P>), 1, 256, 0, st, p->d_state, p->nP, p->n_cams, p->red_slots, p->d_red, p->d_Dc2,
+    CB_LAUNCH(p->k.reduced_prep, 1, 256, 0, st, p->d_state, p->nP, p->n_cams, p->red_slots, p->d_red, p->d_Dc2,
               p->d_active, p->d_Minv, p->d_gmax, p->d_sc);
   return CB_OK;
 }
 
-template <int P>
 int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st) {
   const size_t nn = (size_t)p->nP * p->nP;
   if (p->direct_solve) {
-    CB_LAUNCH((cb::small_rig_step_kernel<P>), 1, cb::DIRECT_THREADS, p->direct_smem, st, p->d_state, p->nP, p->n_cams,
+    CB_LAUNCH(p->k.small_rig_step, 1, cb::DIRECT_THREADS, p->direct_smem, st, p->d_state, p->nP, p->n_cams,
               p->red_slots, p->d_red, p->d_Dc2, p->d_active, p->d_gmax, p->d_sc, p->m_xc(), p->d_dc, p->d_lo, p->d_hi,
               p->d_cam_flags, p->d_cam_const, p->m_camtab());
   } else {
@@ -979,7 +1017,7 @@ int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st) {
               p->d_lo, p->d_hi, p->d_red + nn + p->nP, p->d_Dc2, p->d_active, p->d_cam_flags, p->d_cam_const, p->m_camtab(),
               p->d_sc);
   }
-  launch_pt_backsub<P>(p, dp_out, st);
+  launch_pt_backsub(p, dp_out, st);
   if (p->n_c)
     CB_LAUNCH(cb::comp_backsub_kernel, p->n_comp, cb::CC_THREADS, p->comp_back_smem, st, (const cb::LmState*)p->d_state,
               p->ct, p->nP, p->d_Zt, (size_t)p->LD, p->d_dc, p->d_compL, p->d_tvec, p->d_gpt, p->d_Dp2, p->m_xp(), dp_out,
@@ -988,12 +1026,11 @@ int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st) {
 }
 
 // one whole LM trial: the same launches every time, all decisions on the device
-template <int P>
 int enqueue_trial(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const cudaEvent_t* ev = nullptr) {
-  CB_TRY(build_system<P>(p, opt, st, ev));
-  CB_TRY(solve_step<P>(p, nullptr, st));
+  CB_TRY(build_system(p, opt, st, ev));
+  CB_TRY(solve_step(p, nullptr, st));
   const bool multi = sharded(opt);
-  CB_TRY(camera_pass<P>(p, 1, multi ? 2 : 1, st));
+  CB_TRY(camera_pass(p, 1, multi ? 2 : 1, st));
   if (multi) {
     cb::PeerTable none = {};
     if (opt->peer_group) {
@@ -1077,7 +1114,6 @@ int init_state(CbBaProblem* p, const CbBaOptions* opt, double lam, long long max
 // trial is the body of a WHILE conditional node (CUDA 12.4+) whose last kernel sets the loop condition from
 // LmState::done, so the whole solve is ONE graph launch and ONE host synchronisation, and no predicated-off trial is
 // ever queued.
-template <int P>
 int ensure_graph(CbBaProblem* p, const CbBaOptions* opt, bool loop) {
   TrialGraph& g = loop ? p->loop_graph : p->trial_graph;
   const TrialGraph::Key key{opt->nccl_comm, opt->peer_group, opt->rank, opt->world_size};
@@ -1114,7 +1150,7 @@ int ensure_graph(CbBaProblem* p, const CbBaOptions* opt, bool loop) {
   }
   if (e != cudaSuccess) return fail("begin capture");
   const long long l0 = g_launches.load();
-  int rc = enqueue_trial<P>(p, opt, p->cap_stream);
+  int rc = enqueue_trial(p, opt, p->cap_stream);
   if (loop && rc == CB_OK) CB_LAUNCH(cb::lm_loop_cond_kernel, 1, 1, 0, p->cap_stream, (const cb::LmState*)p->d_state, h);
   g.n_kernels = (int)(g_launches.load() - l0);
   g_launches.store(l0);  // capture launches nothing
@@ -1129,7 +1165,6 @@ int ensure_graph(CbBaProblem* p, const CbBaOptions* opt, bool loop) {
 // Levenberg-Marquardt driver: the loop itself runs on the device (cb_lm.cuh); the host only keeps the GPU fed one
 // trial ahead and looks at the state of trial t-1 while trial t executes.
 // ------------------------------------------------------------------------------------------
-template <int P>
 int lm_solve(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x_out, CbBaResult* res, cudaStream_t st) {
   NvtxRange nvtx_solve("cb_ba_solve");
   const long long max_nfev = opt->max_nfev > 0 ? opt->max_nfev : 100ll * p->n_params;
@@ -1144,9 +1179,9 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x
   // capture cannot be read back).  A graph that cannot be built falls back: device loop -> per-trial graph -> direct.
   const bool direct = opt->allreduce != nullptr || opt->time_kernels;
   bool use_loop = !direct && !sharded(opt);
-  if (use_loop && ensure_graph<P>(p, opt, true) != CB_OK) { cudaGetLastError(); use_loop = false; }
+  if (use_loop && ensure_graph(p, opt, true) != CB_OK) { cudaGetLastError(); use_loop = false; }
   bool use_graph = !direct && !use_loop;
-  if (use_graph && ensure_graph<P>(p, opt, false) != CB_OK) { cudaGetLastError(); use_graph = false; }
+  if (use_graph && ensure_graph(p, opt, false) != CB_OK) { cudaGetLastError(); use_graph = false; }
 
   auto t_mark = std::chrono::steady_clock::now();
   auto host_span = [&](int i) {  // host time since the previous mark -> solve_host_us[i] (stat keys 14-17)
@@ -1161,8 +1196,8 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x
   CB_TRY(upload_x(p, x0, st, true));
   host_span(2);
   CB_CUDA(cudaEventRecord(p->ev0, st));
-  CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
-  CB_TRY(camera_pass<P>(p, 0, 0, st));
+  CB_TRY(run_cam_prep(p, p->d_xc[0], p->d_camtab[0], st));
+  CB_TRY(camera_pass(p, 0, 0, st));
 
   double pp_ms_total = 0.0;
   long long pp_launches = 0, trials = 0;
@@ -1201,7 +1236,7 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x
       g_launches.fetch_add(p->trial_graph.n_kernels);
     } else {
       NvtxRange nvtx_trial("lm_trial (direct launches)");
-      rc = enqueue_trial<P>(p, opt, st, p->ev_pp[t & 1]);
+      rc = enqueue_trial(p, opt, st, p->ev_pp[t & 1]);
       if (rc != CB_OK) break;
     }
     cudaMemcpyAsync(&p->h_state[t & 1], p->d_state, sizeof(cb::LmState), cudaMemcpyDeviceToHost, st);
@@ -1286,8 +1321,29 @@ int lm_solve(CbBaProblem* p, const CbBaOptions* opt, const double* x0, double* x
   return CB_OK;
 }
 
+// The dynamic shared memory a kernel may be launched with.  The limit belongs to the function (per device), not to a
+// problem, and problems of different sizes share instantiations: it is set to the largest size any problem has asked for
+// and never lowered.  What was asked is remembered here, since the runtime reports 48 KB for a function nobody has asked
+// about, and the first request sets the limit even below that, as it always has.
+int reserve_smem(const void* kernel, size_t bytes) {
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> granted;
+  int dev = 0;
+  CB_CUDA(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lk(mu);
+  size_t& have = granted[{dev, kernel}];
+  if (bytes <= have) return CB_OK;
+  CB_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  have = bytes;
+  return CB_OK;
+}
+
+// The reduced solve's configuration and, with it, the problem's kernel table p->k (needs P, pt_lanes, n_dups and
+// cam_in_smem, i.e. build_indices)
 int choose_pcg_config(CbBaProblem* p) {
   const int nP = p->nP, P = p->P;
+  auto kernels = [&](int mode, int cl) { return select_kernels(P, p->pt_lanes, p->n_dups != 0, p->cam_in_smem != 0, mode, cl); };
+  p->k = kernels(p->pcg_mode, p->pcg_cl);  // the PCG variant is settled by try_config below
   int max_optin = 0;
   cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
   const size_t budget = (size_t)std::max(max_optin, 48 * 1024);
@@ -1299,9 +1355,10 @@ int choose_pcg_config(CbBaProblem* p) {
     const size_t smem = (9 * (size_t)npa + 2 * nw + 2 * 16 * nw + minv) * sizeof(double);
     if (smem > budget) return false;
     if (mode == 2 && rows > 3 * nw) return false;
-    const void* fn = (const void*)pcg_fn(mode, P, cl);
+    const Kernels k = kernels(mode, cl);
+    const void* fn = (const void*)k.pcg;
     cudaFuncSetAttribute(fn, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
-    if (cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
+    if (reserve_smem(fn, smem) != CB_OK) {
       cudaGetLastError();
       return false;
     }
@@ -1320,14 +1377,14 @@ int choose_pcg_config(CbBaProblem* p) {
       return false;
     }
     p->pcg_cs = cs; p->pcg_rows = rows; p->pcg_mode = mode; p->pcg_cl = cl; p->pcg_npa = npa; p->pcg_smem = smem;
+    p->k = k;
     return true;
   };
   // (0) small rigs: prep, direct LDL^T and camera step in one CTA (small_rig_step_kernel) when it fits
   p->direct_solve = false;
   if (nP <= cb::DIRECT_MAX_N) {
     const size_t smem = ((size_t)(nP + 1) * (nP | 1) + nP) * sizeof(double);
-    const void* fn = P == 6 ? (const void*)cb::small_rig_step_kernel<6> : (const void*)cb::small_rig_step_kernel<9>;
-    if (smem <= budget && cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess) {
+    if (smem <= budget && reserve_smem((const void*)p->k.small_rig_step, smem) == CB_OK) {
       p->direct_solve = true;
       p->direct_smem = smem;
     } else {
@@ -1345,6 +1402,55 @@ int choose_pcg_config(CbBaProblem* p) {
   if (try_config(1, 8, 1)) return CB_OK;
   g_last_error = "no feasible PCG cluster configuration for n_camera_params = " + std::to_string(nP);
   return CB_E_UNSUPPORTED;
+}
+
+// peak-rate kernels of the diagnostic cb_debug_fp64_peak
+template <int NT>
+__global__ void fp64_dmma_peak_kernel(double* out, int iters, double a0, double b0) {
+  double c[NT][2];
+#pragma unroll
+  for (int i = 0; i < NT; ++i) { c[i][0] = threadIdx.x; c[i][1] = i; }
+  double a = a0 + threadIdx.x * 1e-9, b = b0;
+  for (int it = 0; it < iters; ++it) {
+#pragma unroll
+    for (int i = 0; i < NT; ++i) cb::dmma884(c[i][0], c[i][1], a, b);
+  }
+  double s = 0;
+#pragma unroll
+  for (int i = 0; i < NT; ++i) s += c[i][0] + c[i][1];
+  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
+template <int NT>
+__global__ void fp64_dmma16816_peak_kernel(double* out, int iters, double a0, double b0) {
+  double c[NT][4], a[8], b[4];
+#pragma unroll
+  for (int i = 0; i < NT; ++i) { c[i][0] = threadIdx.x; c[i][1] = i; c[i][2] = 0.0; c[i][3] = 1.0; }
+#pragma unroll
+  for (int i = 0; i < 8; ++i) a[i] = a0 + threadIdx.x * 1e-9 + i * 1e-12;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) b[j] = b0;
+  for (int it = 0; it < iters; ++it) {
+#pragma unroll
+    for (int i = 0; i < NT; ++i) cb::dmma16816(c[i], a, b);
+  }
+  double s = 0;
+#pragma unroll
+  for (int i = 0; i < NT; ++i) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
+  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
+}
+template <int NACC>
+__global__ void fp64_dfma_peak_kernel(double* out, int iters, double a, double b) {
+  double acc[NACC];
+#pragma unroll
+  for (int i = 0; i < NACC; ++i) acc[i] = threadIdx.x * 1e-3 + i;
+  for (int it = 0; it < iters; ++it) {
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = fma(acc[i], a, b);
+  }
+  double s = 0;
+#pragma unroll
+  for (int i = 0; i < NACC; ++i) s += acc[i];
+  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
 }
 
 }  // namespace
@@ -1850,11 +1956,6 @@ static int build_components(CbBaProblem* p, const CbBaProblemDesc* d, cudaStream
   const int esm = std::min(ndmax, cb::CC_SMEM_DIM);
   p->comp_build_smem = sizeof(double) * ((size_t)ndmax * (1 + p->P) + (size_t)esm * esm) + 4 * ((size_t)(p->n_cams + 31) / 32 + 4);
   p->comp_back_smem = sizeof(double) * ((size_t)p->nP + ndmax);
-  if (p->P == 6)
-    CB_CUDA(cudaFuncSetAttribute(cb::comp_build_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_build_smem));
-  else
-    CB_CUDA(cudaFuncSetAttribute(cb::comp_build_kernel<9>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_build_smem));
-  CB_CUDA(cudaFuncSetAttribute(cb::comp_backsub_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->comp_back_smem));
   p->h_ga.assign(groups_a, groups_a + 4 * (size_t)nc); p->h_gb.assign(groups_b, groups_b + 4 * (size_t)nc);
   p->h_cdist.assign(distances, distances + nc); p->h_cw.assign(weights, weights + nc);
   return CB_OK;
@@ -1977,11 +2078,11 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   p->h_cam_const.assign(d->cam_const, d->cam_const + 9 * (size_t)p->n_cams);
   lap("alloc + staged upload");
   CB_TRY(build_indices(p, d_cam, d_pt, d_xy, d->cam_order, st, xy_up.started ? &xy_up : nullptr));
+  CB_TRY(choose_pcg_config(p));
+  lap("kernel table + pcg config");
   // the point pass's Zt staging per point group (cfg4: 18.9 KB of table + 44.8 KB, 2 CTAs per SM); the run-summed
   // variants store their pieces directly and get none, which leaves their register spills the L1 they had
-  if (!p->n_dups)
-    p->pt_smem += p->P == 6 ? (p->pt_lanes == 8 ? cb::pt_stage_bytes<6, 8>() : cb::pt_stage_bytes<6, 32>())
-                            : (p->pt_lanes == 8 ? cb::pt_stage_bytes<9, 8>() : cb::pt_stage_bytes<9, 32>());
+  if (!p->n_dups) p->pt_smem += p->k.pt_stage_bytes;
   // camera tables by internal slot
   {
     std::vector<int> xoff(p->n_cams);
@@ -2012,7 +2113,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   CB_TRY(palloc(p, &p->d_lo, p->nP)); CB_TRY(palloc(p, &p->d_hi, p->nP));
 
   // work buffers
-  const int NACC = (p->P == 6) ? 28 : 55, NU = (p->P == 6) ? 21 : 45;
+  const int NACC = p->k.NACC, NU = p->k.NU;
   const size_t npts = (size_t)std::max(p->n_pts, 1);
   CB_TRY(palloc(p, &p->d_x, (size_t)p->n_params + 1));
   for (int k = 0; k < 2; ++k) {
@@ -2054,41 +2155,14 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
                          &p->ev_pp[1][0], &p->ev_pp[1][1], &p->ev_pp[1][2], &p->ev_pp[1][3]})
     CB_CUDA(cudaEventCreate(e));
   for (cudaEvent_t* e : {&p->ev_state[0], &p->ev_state[1]}) CB_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-  CB_CUDA(cudaFuncSetAttribute(cb::schur_syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                               (int)sizeof(cb::SyrkSmem)));
-  if (p->pt_smem > 48 * 1024 || p->bs_smem > 48 * 1024) {
-    const int a = (int)p->pt_smem, b2 = (int)p->bs_smem;
-#define CB_SMEM_ATTR(PP)                                                                                           \
-    do {                                                                                                             \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a);  \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a);   \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a);  \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a);  \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 8, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, false, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_pass_kernel<PP, 32, true, false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, a); \
-      cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 8, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);     \
-      cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);    \
-      cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 8, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);    \
-      cudaFuncSetAttribute(cb::pt_backsub_kernel<PP, 32, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, b2);   \
-    } while (0)
-    if (p->P == 6) CB_SMEM_ATTR(6); else CB_SMEM_ATTR(9);
-#undef CB_SMEM_ATTR
-    CB_CUDA(cudaGetLastError());
-  }
-  lap("work buffers + memsets");
-  CB_TRY(choose_pcg_config(p));
+  CB_TRY(reserve_smem((const void*)cb::schur_syrk_kernel, sizeof(cb::SyrkSmem)));
+  CB_TRY(reserve_smem((const void*)p->k.pt_pass, p->pt_smem));
+  CB_TRY(reserve_smem((const void*)p->k.pt_pass_cov, p->pt_smem));
+  CB_TRY(reserve_smem((const void*)p->k.pt_backsub, p->bs_smem));
+  CB_TRY(reserve_smem((const void*)p->k.comp_build, p->comp_build_smem));
+  CB_TRY(reserve_smem((const void*)cb::comp_backsub_kernel, p->comp_back_smem));
   CB_CUDA(cudaStreamSynchronize(st));
-  lap("pcg config");
+  lap("work buffers + memsets");
   return CB_OK;
 }
 
@@ -2153,28 +2227,24 @@ int cb_ba_solve_from(CbBaProblem* p, const CbBaOptions* opt, const double* x0, d
                    "CbBaProblemDesc.cam_order (the same on every rank)";
     return CB_E_INVALID;
   }
-  const int rc = p->P == 6 ? lm_solve<6>(p, opt, x0, x_out, result, st) : lm_solve<9>(p, opt, x0, x_out, result, st);
+  const int rc = lm_solve(p, opt, x0, x_out, result, st);
   p->peer = nullptr;
   return rc;
 }
 
-}  // extern "C"
-namespace {
-template <int P, int MODE>
-int eval_mode(CbBaProblem* p, const double* x, cudaStream_t st) {
+// stand-alone camera-major evaluation at x in resjac_kernel's MODE `mode`, into d_out2
+static int eval_mode(CbBaProblem* p, int mode, const double* x, cudaStream_t st) {
   CB_TRY(upload_x(p, x, st));
-  CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
-  launch_resjac<P, MODE>(p, nullptr, 0, 0, 1.0, p->d_out2, st);
+  CB_TRY(run_cam_prep(p, p->d_xc[0], p->d_camtab[0], st));
+  launch_resjac(p, mode, nullptr, 0, 0, 1.0, p->d_out2, st);
   return CB_OK;
 }
-}  // namespace
-extern "C" {
 
 int cb_ba_residuals(CbBaProblem* p, const double* x, double* r_out, void* stream) {
   if (!p || !x || !r_out) { g_last_error = "cb_ba_residuals: null argument"; return CB_E_INVALID; }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
-  CB_TRY(p->P == 6 ? (eval_mode<6, 2>(p, x, st)) : (eval_mode<9, 2>(p, x, st)));
+  CB_TRY(eval_mode(p, 2, x, st));
   CB_CUDA(cudaMemcpyAsync(r_out, p->d_out2, sizeof(double) * 2 * (size_t)p->n_obs, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   return CB_OK;
@@ -2184,7 +2254,7 @@ int cb_ba_reproj_errors_px(CbBaProblem* p, const double* x, double* err_xy, void
   if (!p || !x || !err_xy) { g_last_error = "cb_ba_reproj_errors_px: null argument"; return CB_E_INVALID; }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
-  CB_TRY(p->P == 6 ? (eval_mode<6, 3>(p, x, st)) : (eval_mode<9, 3>(p, x, st)));
+  CB_TRY(eval_mode(p, 3, x, st));
   CB_CUDA(cudaMemcpyAsync(err_xy, p->d_out2, sizeof(double) * 2 * (size_t)p->n_obs, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   return CB_OK;
@@ -2200,28 +2270,19 @@ int cb_ba_jacobian_blocks(CbBaProblem* p, const double* x, double* Jc, double* J
   double *dJc, *dJp;
   CB_TRY(sf.alloc(&dJc, 18 * (size_t)std::max(n, 1)));
   CB_TRY(sf.alloc(&dJp, 6 * (size_t)std::max(n, 1)));
-  if (p->P == 6) {
-    CB_TRY(run_cam_prep<6>(p, p->d_xc[0], p->d_camtab[0], st));
-    if (n) CB_LAUNCH((cb::jac_blocks_kernel<6>), cdiv(n, 128), 128, 0, st, p->d_obs_cam, (const int*)p->d_cam_slot, p->d_obs_pt,
-                     reinterpret_cast<const double2*>(p->d_obs_xy), n, (const double*)p->d_camtab[0], (const double*)p->d_xp4[0], dJc, dJp);
-  } else {
-    CB_TRY(run_cam_prep<9>(p, p->d_xc[0], p->d_camtab[0], st));
-    if (n) CB_LAUNCH((cb::jac_blocks_kernel<9>), cdiv(n, 128), 128, 0, st, p->d_obs_cam, (const int*)p->d_cam_slot, p->d_obs_pt,
-                     reinterpret_cast<const double2*>(p->d_obs_xy), n, (const double*)p->d_camtab[0], (const double*)p->d_xp4[0], dJc, dJp);
-  }
+  CB_TRY(run_cam_prep(p, p->d_xc[0], p->d_camtab[0], st));
+  if (n) CB_LAUNCH(p->k.jac_blocks, cdiv(n, 128), 128, 0, st, p->d_obs_cam, (const int*)p->d_cam_slot, p->d_obs_pt,
+                   reinterpret_cast<const double2*>(p->d_obs_xy), n, (const double*)p->d_camtab[0], (const double*)p->d_xp4[0], dJc, dJp);
   CB_CUDA(cudaMemcpyAsync(Jc, dJc, sizeof(double) * 18 * (size_t)n, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(Jp, dJp, sizeof(double) * 6 * (size_t)n, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   return CB_OK;
 }
 
-}  // extern "C"
-namespace {
-template <int P>
-int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss, double fs, double* cost, double* U,
+static int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss, double fs, double* cost, double* U,
                           double* gc, double* V, double* gp, double* S, double* b, double* dc, double* dp,
                           cudaStream_t st) {
-  using RT = cb::RowT<P>;
+  const int P = p->P, NU = p->k.NU;
   CbBaOptions opt;
   cb_ba_default_options(&opt);
   opt.loss = loss; opt.f_scale = fs;
@@ -2229,15 +2290,15 @@ int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss, double
   CB_TRY(set_bounds(p, false, st));
   CB_TRY(init_state(p, &opt, lam, 1ll << 40, st));
   CB_TRY(upload_x(p, x, st, true));
-  CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
-  CB_TRY(camera_pass<P>(p, 0, 0, st));
-  CB_TRY(build_system<P>(p, &opt, st));
-  CB_TRY(solve_step<P>(p, p->d_dp, st));
+  CB_TRY(run_cam_prep(p, p->d_xc[0], p->d_camtab[0], st));
+  CB_TRY(camera_pass(p, 0, 0, st));
+  CB_TRY(build_system(p, &opt, st));
+  CB_TRY(solve_step(p, p->d_dp, st));
   // after solve_step: small rigs apply the damping in small_rig_step_kernel; nothing in solve_step writes d_red otherwise
   const size_t nn = (size_t)p->nP * p->nP;
   std::vector<double> hS(nn + 3 * (size_t)p->nP + 1);
   CB_CUDA(cudaMemcpyAsync(hS.data(), p->d_red, sizeof(double) * hS.size(), cudaMemcpyDeviceToHost, st));
-  std::vector<double> hU((size_t)p->n_cams * RT::NU), hV(6 * (size_t)std::max(p->n_pts, 1));
+  std::vector<double> hU((size_t)p->n_cams * NU), hV(6 * (size_t)std::max(p->n_pts, 1));
   CB_CUDA(cudaMemcpyAsync(hU.data(), p->d_Upk[0], sizeof(double) * hU.size(), cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaMemcpyAsync(hV.data(), p->d_V6, sizeof(double) * hV.size(), cudaMemcpyDeviceToHost, st));
   if (gc) CB_CUDA(cudaMemcpyAsync(gc, p->d_gc[0], sizeof(double) * p->nP, cudaMemcpyDeviceToHost, st));
@@ -2268,8 +2329,8 @@ int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss, double
       int u = 0;
       for (int a = 0; a < P; ++a)
         for (int bb = a; bb < P; ++bb, ++u) {
-          U[((size_t)c * P + a) * P + bb] = hU[(size_t)i * RT::NU + u];
-          U[((size_t)c * P + bb) * P + a] = hU[(size_t)i * RT::NU + u];
+          U[((size_t)c * P + a) * P + bb] = hU[(size_t)i * NU + u];
+          U[((size_t)c * P + bb) * P + a] = hU[(size_t)i * NU + u];
         }
     }
   if (V)
@@ -2280,8 +2341,6 @@ int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss, double
     }
   return CB_OK;
 }
-}  // namespace
-extern "C" {
 
 int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32_t loss, double f_scale, double* cost,
                            double* U, double* gc, double* V, double* gp, double* S, double* b, double* dc, double* dp,
@@ -2289,16 +2348,12 @@ int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32
   if (!p || !x) { g_last_error = "cb_ba_normal_equations: null argument"; return CB_E_INVALID; }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
-  return p->P == 6 ? normal_eq_impl<6>(p, x, lambda, loss, f_scale, cost, U, gc, V, gp, S, b, dc, dp, st)
-                   : normal_eq_impl<9>(p, x, lambda, loss, f_scale, cost, U, gc, V, gp, S, b, dc, dp, st);
+  return normal_eq_impl(p, x, lambda, loss, f_scale, cost, U, gc, V, gp, S, b, dc, dp, st);
 }
 
-}  // extern "C"
-namespace {
-template <int P>
-int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs, int n_fixed, const int32_t* fixed, double vf,
-                    double* cam_cov, double* pt_cov, double* s2_out, int64_t* dof_out, int32_t* pt_rank, cudaStream_t st) {
-  const int nP = p->nP, nc = p->n_cams, npts = std::max(p->n_pts, 1);
+static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs, int n_fixed, const int32_t* fixed, double vf,
+                           double* cam_cov, double* pt_cov, double* s2_out, int64_t* dof_out, int32_t* pt_rank, cudaStream_t st) {
+  const int P = p->P, nP = p->nP, nc = p->n_cams, npts = std::max(p->n_pts, 1);
   const size_t nn = (size_t)nP * nP;
   // free mask (internal slot order): the camera's own slots, camera observed, not fixed
   std::vector<int> cs(nc + 1);
@@ -2346,9 +2401,9 @@ int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs, int n_
   CB_CUDA(cudaMemcpyAsync(p->d_covFail, big, sizeof(big), cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaMemcpyAsync(p->d_covFree, fr.data(), nP, cudaMemcpyHostToDevice, st));
   CB_TRY(upload_x(p, x, st, true));
-  CB_TRY(run_cam_prep<P>(p, p->d_xc[0], p->d_camtab[0], st));
-  CB_TRY(camera_pass<P>(p, 0, 0, st));
-  CB_TRY(build_system<P>(p, &opt, st, nullptr, true));
+  CB_TRY(run_cam_prep(p, p->d_xc[0], p->d_camtab[0], st));
+  CB_TRY(camera_pass(p, 0, 0, st));
+  CB_TRY(build_system(p, &opt, st, nullptr, true));
   if (p->n_c) CB_LAUNCH(cb::comp_failed_kernel, cdiv(p->n_comp, 128), 128, 0, st, p->ct, (const double*)p->d_compL, p->d_covFail + 1);
   CB_CUDA(cudaEventRecord(p->ev1, st));
   // dense inverse of the gauge-fixed reduced system
@@ -2396,7 +2451,7 @@ int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs, int n_
   if (dof_out) *dof_out = dof;
   if (pt_rank) std::memcpy(pt_rank, rank.data(), sizeof(int) * p->n_pts);
   if (pt_cov && p->n_pts > 0) {
-    CB_LAUNCH((cb::cov_point_kernel<P>), 4 * p->num_sms, 256, 0, st, (const int*)p->d_pt_start, (const int*)p->d_pm_cam,
+    CB_LAUNCH(p->k.cov_point, 4 * p->num_sms, 256, 0, st, (const int*)p->d_pt_start, (const int*)p->d_pm_cam,
               p->n_pts, (const double*)p->d_Zt, (size_t)p->LD, (const double*)p->d_covS, nP, (const double*)p->d_covR,
               (const int*)p->d_covRank, s2, p->d_covPt);
   }
@@ -2431,8 +2486,6 @@ int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs, int n_
   }
   return CB_OK;
 }
-}  // namespace
-extern "C" {
 
 int cb_ba_covariance(CbBaProblem* p, const double* x, int32_t loss, double f_scale, int32_t n_fixed, const int32_t* fixed,
                      double variance_factor, double* cam_cov, double* pt_cov, double* s2_out, int64_t* dof_out,
@@ -2446,8 +2499,7 @@ int cb_ba_covariance(CbBaProblem* p, const double* x, int32_t loss, double f_sca
     }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
-  return p->P == 6 ? covariance_impl<6>(p, x, loss, f_scale, n_fixed, fixed, variance_factor, cam_cov, pt_cov, s2_out, dof_out, pt_rank, st)
-                   : covariance_impl<9>(p, x, loss, f_scale, n_fixed, fixed, variance_factor, cam_cov, pt_cov, s2_out, dof_out, pt_rank, st);
+  return covariance_impl(p, x, loss, f_scale, n_fixed, fixed, variance_factor, cam_cov, pt_cov, s2_out, dof_out, pt_rank, st);
 }
 
 // Diagnostic: time `reps` launches of the PCG kernel on the system left by the last
@@ -2472,58 +2524,6 @@ int cb_ba_debug_pcg_time(CbBaProblem* p, int max_iter, int reps, double* ms_per_
                t[cb::SC_PCG_T0 + 3] / max_iter, t[cb::SC_PCG_T0 + 4] / max_iter);
   return CB_OK;
 }
-
-}  // extern "C"
-namespace {
-template <int NT>
-__global__ void fp64_dmma_peak_kernel(double* out, int iters, double a0, double b0) {
-  double c[NT][2];
-#pragma unroll
-  for (int i = 0; i < NT; ++i) { c[i][0] = threadIdx.x; c[i][1] = i; }
-  double a = a0 + threadIdx.x * 1e-9, b = b0;
-  for (int it = 0; it < iters; ++it) {
-#pragma unroll
-    for (int i = 0; i < NT; ++i) cb::dmma884(c[i][0], c[i][1], a, b);
-  }
-  double s = 0;
-#pragma unroll
-  for (int i = 0; i < NT; ++i) s += c[i][0] + c[i][1];
-  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
-}
-template <int NT>
-__global__ void fp64_dmma16816_peak_kernel(double* out, int iters, double a0, double b0) {
-  double c[NT][4], a[8], b[4];
-#pragma unroll
-  for (int i = 0; i < NT; ++i) { c[i][0] = threadIdx.x; c[i][1] = i; c[i][2] = 0.0; c[i][3] = 1.0; }
-#pragma unroll
-  for (int i = 0; i < 8; ++i) a[i] = a0 + threadIdx.x * 1e-9 + i * 1e-12;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) b[j] = b0;
-  for (int it = 0; it < iters; ++it) {
-#pragma unroll
-    for (int i = 0; i < NT; ++i) cb::dmma16816(c[i], a, b);
-  }
-  double s = 0;
-#pragma unroll
-  for (int i = 0; i < NT; ++i) s += c[i][0] + c[i][1] + c[i][2] + c[i][3];
-  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
-}
-template <int NACC>
-__global__ void fp64_dfma_peak_kernel(double* out, int iters, double a, double b) {
-  double acc[NACC];
-#pragma unroll
-  for (int i = 0; i < NACC; ++i) acc[i] = threadIdx.x * 1e-3 + i;
-  for (int it = 0; it < iters; ++it) {
-#pragma unroll
-    for (int i = 0; i < NACC; ++i) acc[i] = fma(acc[i], a, b);
-  }
-  double s = 0;
-#pragma unroll
-  for (int i = 0; i < NACC; ++i) s += acc[i];
-  out[blockIdx.x * blockDim.x + threadIdx.x] = s;
-}
-}  // namespace
-extern "C" {
 
 int cb_debug_fp64_peak(int device, double* dmma_tflops, double* dfma_tflops) {
   if (!dmma_tflops || !dfma_tflops) { g_last_error = "cb_debug_fp64_peak: null argument"; return CB_E_INVALID; }
@@ -2571,7 +2571,7 @@ int cb_ba_error_order_stats(CbBaProblem* p, const double* x, double q_percent, d
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
   const int n = p->n_obs;
-  CB_TRY(p->P == 6 ? (eval_mode<6, 4>(p, x, st)) : (eval_mode<9, 4>(p, x, st)));
+  CB_TRY(eval_mode(p, 4, x, st));
   ScopedFree sf(st);
   double *d_lo, *d_hi;
   long long* d_cnt;
@@ -2620,7 +2620,7 @@ int cb_ba_rmse_px(CbBaProblem* p, const double* x, double* overall, double* per_
   if (!p || !x || !overall) { g_last_error = "cb_ba_rmse_px: null argument"; return CB_E_INVALID; }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
-  CB_TRY(p->P == 6 ? (eval_mode<6, 4>(p, x, st)) : (eval_mode<9, 4>(p, x, st)));
+  CB_TRY(eval_mode(p, 4, x, st));
   ScopedFree sf(st);
   double* d_ss;
   CB_TRY(sf.alloc(&d_ss, p->n_cams));
@@ -2652,7 +2652,7 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
   const int n = p->n_obs, nc = p->n_cams;
-  CB_TRY(p->P == 6 ? (eval_mode<6, 4>(p, x, st)) : (eval_mode<9, 4>(p, x, st)));
+  CB_TRY(eval_mode(p, 4, x, st));
   double *d_thr, *d_ss;
   long long* d_kept;
   unsigned char* d_flag;
@@ -2961,14 +2961,6 @@ int obs_group_stage(int32_t n_cams, const std::vector<cb::UndistCam>* undist, in
 // Lanes per group of the triangulation kernels.  8: the serial 4x4 eigen-solve of one lane per group, not the gather,
 // bounds the DLT kernel, so more groups per warp wins until groups get very long (more than 96 rows on average).
 int tri_lanes(int n, int n_groups) { return (n / std::max(n_groups, 1) > 96) ? 32 : 8; }
-
-// f(L) with L a std::integral_constant of the lanes per group (32, else 8), for launching the kernel instantiated
-// for them
-template <typename F>
-void with_lanes(int lanes, F&& f) {
-  if (lanes == 32) f(std::integral_constant<int, 32>{});
-  else f(std::integral_constant<int, 8>{});
-}
 
 // the DLT of every group (buffers held by the call's workspace)
 struct TriDlt {

@@ -1,7 +1,8 @@
 """Rigs that reach each shape-selected engine variant, with the variant the engine must report for them (test
 infrastructure).  The engine picks kernel instantiations and the reduced solve from the problem's shape alone, so a
-path is tested only if some rig has its shape; ``BAProblem.stat`` keys 7-13 say which path a problem took, and
-``check_stats`` pins them so that a moved threshold cannot silently send a case back to an already covered path."""
+path is tested only if some rig has its shape; ``BAProblem.stat`` keys 7-13 say which path a problem took (DESIGN.md §4,
+"Where the variants are chosen"), and ``check_stats`` pins them so that a moved threshold cannot silently send a case
+back to an already covered path."""
 from __future__ import annotations
 
 from dataclasses import dataclass, field
