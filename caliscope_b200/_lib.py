@@ -144,6 +144,18 @@ class ResectStats(C.Structure):
     ]
 
 
+class IntrinsicsStats(C.Structure):
+    _fields_ = [
+        ("group_ms", C.c_double),
+        ("start_ms", C.c_double),
+        ("lm_ms", C.c_double),
+        ("cov_ms", C.c_double),
+        ("total_ms", C.c_double),
+        ("iterations", C.c_int32),
+        ("kernel_launches", C.c_int32),
+    ]
+
+
 # every symbol include/caliscope_b200.h declares: name -> (restype, argtypes)
 _P = C.c_void_p
 _D = C.POINTER(C.c_double)
@@ -213,6 +225,13 @@ SYMBOLS = {
         [C.c_int32, _P, _P, _P, C.c_int32, _P, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32,
          C.c_int32, C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, _P, _P, _P, _P, _P,
          _P, C.POINTER(ResectStats), C.c_int, _P],
+    ),
+    "cb_calibrate_intrinsics": (
+        C.c_int,
+        [C.c_int32, _P, _P, _P, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+         C.c_int32,
+         C.POINTER(C.c_int32), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+         C.POINTER(IntrinsicsStats), C.c_int, _P],
     ),
     "cb_peer_create": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, C.POINTER(_P), _P]),
     "cb_peer_connect": (C.c_int, [_P, _P]),

@@ -17,6 +17,7 @@
 #include <atomic>
 #include <chrono>
 #include <cmath>
+#include <limits>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -38,6 +39,7 @@
 #include "cb_triangulate.cuh"
 #include "cb_resect.cuh"
 #include "cb_bootstrap.cuh"
+#include "cb_intrinsics.cuh"
 #include "cb_peer.cuh"
 
 namespace {
@@ -3634,6 +3636,317 @@ int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam
                      obs_px, obs_on_device, threshold_px, min_inliers, max_samples, use_prior ? 1 : 0, pixel_sigma,
                      max_iter, xtol, max_groups, n_groups_out, cam_out, pose_out, cov_out, rmse_px_out, count_out,
                      n_inliers_out, rep_row_out, status_out, inlier_out, stats, device, stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// one launch of an intrinsic-calibration cluster kernel: a cluster of cs CTAs per camera in A.cams
+int intr_launch(void (*kernel)(cb::IntrArgs), int n_active, int cs, size_t smem, const cb::IntrArgs& A, cudaStream_t st) {
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(n_active * cs);
+  cfg.blockDim = dim3(cb::INTR_THREADS);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeClusterDimension;
+  at[0].val.clusterDim.x = cs;
+  at[0].val.clusterDim.y = 1;
+  at[0].val.clusterDim.z = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  CB_CUDA(cudaLaunchKernelEx(&cfg, kernel, A));
+  g_launches.fetch_add(1);
+  return CB_OK;
+}
+
+int intrinsics_impl(int32_t n_cams, const int32_t* image_size, const int32_t* cam_flags, const int32_t* cam_fixed,
+                    const double* guess,
+                    int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const double* obs_obj,
+                    const double* obs_px, int obs_on_device, int32_t min_points, int32_t min_views, int32_t max_iter,
+                    double xtol, int32_t max_views, int32_t* n_views_out, double* params_out, double* std_out,
+                    double* cov_out, double* rms_out, double* sigma2_out, int32_t* used_views_out, int32_t* rows_out,
+                    int32_t* iterations_out, int32_t* status_out, int32_t* view_cam_out, double* view_pose_out,
+                    double* view_std_out, double* view_rmse_out, int32_t* view_count_out, int32_t* view_rep_out,
+                    int32_t* view_status_out, CbIntrinsicsStats* stats, int device, void* stream) {
+  const char* who = "cb_calibrate_intrinsics";
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  CB_TRY(select_device(device));
+  *n_views_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  for (int c = 0; c < n_cams; ++c) {
+    for (int k = 0; k < 9; ++k) params_out[9 * c + k] = std_out[9 * c + k] = nan;
+    if (cov_out)
+      for (int k = 0; k < 81; ++k) cov_out[81 * c + k] = nan;
+    rms_out[c] = sigma2_out[c] = nan;
+    used_views_out[c] = rows_out[c] = iterations_out[c] = 0;
+    status_out[c] = cb::IC_TOO_FEW_VIEWS;
+  }
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf(st);
+  const int n = (int)n_obs;
+  StageEvents<8> ev;
+  CB_TRY(ev.create());
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  const double* d_obj = nullptr;
+  CB_TRY(to_device(obs_obj, 3 * (size_t)n, obs_on_device, &d_obj, sf, st));
+  ObsGroups g;
+  CB_TRY(obs_group_stage(n_cams, nullptr, n, obs_cam, obs_key, obs_px, obs_on_device, max_views, n_views_out, who, ev[1],
+                         sf, st, &g));
+  const int V = g.n_groups;
+
+  // views: status and homography
+  int *d_vcam, *d_vcount, *d_vrep, *d_vstatus;
+  double* d_vH;
+  CB_TRY(sf.alloc(&d_vcam, (size_t)V));
+  CB_TRY(sf.alloc(&d_vcount, (size_t)V));
+  CB_TRY(sf.alloc(&d_vrep, (size_t)V));
+  CB_TRY(sf.alloc(&d_vstatus, (size_t)V));
+  CB_TRY(sf.alloc(&d_vH, 9 * (size_t)V));
+  CB_CUDA(cudaEventRecord(ev[2], st));
+  CB_LAUNCH(cb::intr_view_kernel, cdiv((long long)V * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, g.start, g.rows, g.cam,
+            d_obj, g.xy, V, (int)min_points, d_vcam, d_vcount, d_vrep, d_vstatus, d_vH);
+  CB_CUDA(cudaGetLastError());
+  std::vector<int> vcam(V), vstatus(V);
+  CB_CUDA(cudaMemcpyAsync(vcam.data(), d_vcam, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(vstatus.data(), d_vstatus, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  // per camera, its views of status 0 in key order (CSR)
+  auto camera_lists = [&](std::vector<int>& cstart, std::vector<int>& list) {
+    cstart.assign(n_cams + 1, 0);
+    for (int v = 0; v < V; ++v)
+      if (vstatus[v] == cb::IV_OK) ++cstart[vcam[v] + 1];
+    for (int c = 0; c < n_cams; ++c) cstart[c + 1] += cstart[c];
+    list.assign(std::max(cstart[n_cams], 1), 0);
+    std::vector<int> fill(cstart.begin(), cstart.end() - 1);
+    for (int v = 0; v < V; ++v)
+      if (vstatus[v] == cb::IV_OK) list[fill[vcam[v]]++] = v;
+  };
+  std::vector<int> hv_start, hv_list;
+  camera_lists(hv_start, hv_list);
+
+  // start: guess or Zhang, then the IPPE pose of every view on the pixels undistorted with the start
+  // the kernels' per-camera word: bits 0-8 fixed parameters, cb::INTR_USE_GUESS
+  std::vector<int> iflags(n_cams);
+  for (int c = 0; c < n_cams; ++c)
+    iflags[c] = (cam_fixed ? cam_fixed[c] : 0) | ((cam_flags[c] & CB_INTR_USE_GUESS) ? cb::INTR_USE_GUESS : 0);
+  const int *d_flags, *d_isize, *d_hvs, *d_hvl;
+  const double* d_guess = nullptr;
+  CB_TRY(to_device(iflags.data(), (size_t)n_cams, 0, &d_flags, sf, st));
+  CB_TRY(to_device(image_size, 2 * (size_t)n_cams, 0, &d_isize, sf, st));
+  CB_TRY(to_device(hv_start.data(), hv_start.size(), 0, &d_hvs, sf, st));
+  CB_TRY(to_device(hv_list.data(), hv_list.size(), 0, &d_hvl, sf, st));
+  if (guess) CB_TRY(to_device(guess, 9 * (size_t)n_cams, 0, &d_guess, sf, st));
+  double *d_theta, *d_q;
+  int* d_cstatus;
+  CB_TRY(sf.alloc(&d_theta, 9 * (size_t)n_cams));
+  CB_TRY(sf.alloc(&d_cstatus, (size_t)n_cams));
+  CB_TRY(sf.alloc(&d_q, 6 * (size_t)V));
+  CB_LAUNCH(cb::intr_zhang_kernel, cdiv(n_cams, 128), 128, 0, st, d_flags, d_guess, d_isize, d_hvs, d_hvl, d_vH, n_cams,
+            d_theta, d_cstatus);
+  std::vector<double> theta(9 * (size_t)n_cams);
+  std::vector<int> cstatus(n_cams);
+  CB_CUDA(cudaMemcpyAsync(theta.data(), d_theta, sizeof(double) * theta.size(), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(cstatus.data(), d_cstatus, sizeof(int) * n_cams, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  std::vector<cb::UndistCam> tab(n_cams);
+  for (int c = 0; c < n_cams; ++c) {
+    const double* t = &theta[9 * (size_t)c];
+    const bool ok = cstatus[c] == cb::IC_OK;
+    cb::UndistCam& u = tab[c];
+    std::memset(&u, 0, sizeof(u));
+    u.fx = ok ? t[0] : 1.0; u.fy = ok ? t[1] : 1.0; u.cx = ok ? t[2] : 0.0; u.cy = ok ? t[3] : 0.0;
+    for (int k = 0; k < 5; ++k) u.d[k] = ok ? t[4 + k] : 0.0;
+  }
+  const cb::UndistCam* d_tab = nullptr;
+  CB_TRY(upload_undist_table(tab, sf, st, &d_tab));
+  double *d_norm, *d_R, *d_t, *d_prmse;
+  int *d_pst, *d_pcnt, *d_prep;
+  CB_TRY(sf.alloc(&d_norm, 2 * (size_t)n));
+  CB_TRY(sf.alloc(&d_R, 9 * (size_t)V));
+  CB_TRY(sf.alloc(&d_t, 3 * (size_t)V));
+  CB_TRY(sf.alloc(&d_prmse, (size_t)V));
+  CB_TRY(sf.alloc(&d_pst, (size_t)V));
+  CB_TRY(sf.alloc(&d_pcnt, (size_t)V));
+  CB_TRY(sf.alloc(&d_prep, (size_t)V));
+  CB_LAUNCH(cb::undistort_kernel<double>, cdiv(n, 256), 256, 0, st, d_tab, g.cam, g.xy, d_norm, (long long)n, 0);
+  CB_LAUNCH(cb::pnp_ippe_kernel, cdiv((long long)V * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, g.start, g.rows, d_obj,
+            d_norm, V, (int)min_points, d_R, d_t, d_prmse, d_pst, d_pcnt, d_prep);
+  CB_LAUNCH(cb::intr_pose_kernel, cdiv(V, 128), 128, 0, st, d_vcam, d_cstatus, d_R, d_t, d_pst, V, d_vstatus, d_q);
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaMemcpyAsync(vstatus.data(), d_vstatus, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+
+  // the cameras to solve and their used views
+  std::vector<int> uv_start, uv_list, crows(n_cams, 0), active;
+  camera_lists(uv_start, uv_list);
+  std::vector<int> vcount(V);
+  CB_CUDA(cudaMemcpyAsync(vcount.data(), d_vcount, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  int max_nv = 0;
+  for (int c = 0; c < n_cams; ++c) {
+    const int nv = uv_start[c + 1] - uv_start[c];
+    if (nv < min_views) cstatus[c] = cb::IC_TOO_FEW_VIEWS;
+    if (cstatus[c] != cb::IC_OK) continue;
+    active.push_back(c);
+    max_nv = std::max(max_nv, nv);
+    for (int j = uv_start[c]; j < uv_start[c + 1]; ++j) crows[c] += vcount[uv_list[j]];
+    used_views_out[c] = nv;
+    rows_out[c] = crows[c];
+  }
+  CB_CUDA(cudaEventRecord(ev[3], st));
+  const int n_active = (int)active.size();
+  std::vector<double> sse(n_cams, nan);
+  std::vector<int> iters(n_cams, 0);
+  double *d_std = nullptr, *d_cov = nullptr, *d_sig = nullptr, *d_sse = nullptr, *d_vstd = nullptr, *d_vrmse = nullptr;
+  CB_TRY(sf.alloc(&d_vstd, 6 * (size_t)V));
+  CB_TRY(sf.alloc(&d_vrmse, (size_t)V));
+  if (n_active > 0) {
+    const int n_used = uv_start[n_cams];
+    const int *d_uvs, *d_uvl, *d_act, *d_crows;
+    CB_TRY(to_device(uv_start.data(), uv_start.size(), 0, &d_uvs, sf, st));
+    CB_TRY(to_device(uv_list.data(), uv_list.size(), 0, &d_uvl, sf, st));
+    CB_TRY(to_device(active.data(), active.size(), 0, &d_act, sf, st));
+    CB_TRY(to_device(crows.data(), crows.size(), 0, &d_crows, sf, st));
+    CB_CUDA(cudaMemcpyAsync(d_cstatus, cstatus.data(), sizeof(int) * n_cams, cudaMemcpyHostToDevice, st));
+    double *d_gram, *d_con, *d_trial;
+    int* d_iters;
+    CB_TRY(sf.alloc(&d_gram, (size_t)n_used * cb::INTR_G));
+    CB_TRY(sf.alloc(&d_con, (size_t)n_used * cb::INTR_CON));
+    CB_TRY(sf.alloc(&d_trial, (size_t)n_used * cb::INTR_TRIAL));
+    CB_TRY(sf.alloc(&d_iters, (size_t)n_cams));
+    CB_TRY(sf.alloc(&d_std, 9 * (size_t)n_cams));
+    CB_TRY(sf.alloc(&d_sig, (size_t)n_cams));
+    CB_TRY(sf.alloc(&d_sse, (size_t)n_cams));
+    if (cov_out) CB_TRY(sf.alloc(&d_cov, 81 * (size_t)n_cams));
+    cb::IntrArgs A{g.start, g.rows, d_obj, g.xy, d_act, d_uvs, d_uvl, d_flags, d_crows, d_theta, d_q, d_gram, d_con,
+                   d_trial, d_cstatus, d_iters, d_sse, d_std, d_cov, d_sig, d_vstd, d_vrmse, (int)max_iter, xtol};
+    // cluster size: about four views per warp, up to the portable limit of 8 CTAs
+    const int cs = std::max(1, std::min(cb::INTR_MAX_CLUSTER, cdiv(max_nv, 4 * cb::INTR_WARPS)));
+    CB_CUDA(cudaFuncSetAttribute(cb::intr_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb::INTR_SMEM));
+    CB_CUDA(cudaEventRecord(ev[4], st));
+    CB_TRY(intr_launch(cb::intr_lm_kernel, n_active, cs, cb::INTR_SMEM, A, st));
+    CB_CUDA(cudaEventRecord(ev[5], st));
+    CB_TRY(intr_launch(cb::intr_cov_kernel, n_active, cs, 0, A, st));
+    CB_CUDA(cudaEventRecord(ev[6], st));
+    CB_CUDA(cudaMemcpyAsync(theta.data(), d_theta, sizeof(double) * theta.size(), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(cstatus.data(), d_cstatus, sizeof(int) * n_cams, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(iters.data(), d_iters, sizeof(int) * n_cams, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(sse.data(), d_sse, sizeof(double) * n_cams, cudaMemcpyDeviceToHost, st));
+    std::vector<double> stdv(9 * (size_t)n_cams), sig(n_cams), cov(cov_out ? 81 * (size_t)n_cams : 0);
+    CB_CUDA(cudaMemcpyAsync(stdv.data(), d_std, sizeof(double) * stdv.size(), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(sig.data(), d_sig, sizeof(double) * n_cams, cudaMemcpyDeviceToHost, st));
+    if (cov_out) CB_CUDA(cudaMemcpyAsync(cov.data(), d_cov, sizeof(double) * cov.size(), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaStreamSynchronize(st));
+    for (int c : active) {
+      std::memcpy(std_out + 9 * (size_t)c, &stdv[9 * (size_t)c], sizeof(double) * 9);
+      if (cov_out) std::memcpy(cov_out + 81 * (size_t)c, &cov[81 * (size_t)c], sizeof(double) * 81);
+      sigma2_out[c] = sig[c];
+      rms_out[c] = std::sqrt(sse[c] / crows[c]);
+      iterations_out[c] = iters[c];
+    }
+  }
+  if (stats) CB_CUDA(cudaEventRecord(ev[7], st));
+  for (int c = 0; c < n_cams; ++c) {
+    status_out[c] = cstatus[c];
+    std::memcpy(params_out + 9 * (size_t)c, &theta[9 * (size_t)c], sizeof(double) * 9);
+  }
+  // per view, in key order
+  std::vector<double> q(6 * (size_t)V), vstd(6 * (size_t)V), vrmse(V);
+  CB_CUDA(cudaMemcpyAsync(q.data(), d_q, sizeof(double) * q.size(), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(vstd.data(), d_vstd, sizeof(double) * vstd.size(), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(vrmse.data(), d_vrmse, sizeof(double) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(view_cam_out, d_vcam, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(view_count_out, d_vcount, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(view_rep_out, d_vrep, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  for (int v = 0; v < V; ++v) {
+    view_status_out[v] = vstatus[v];
+    const bool solved = vstatus[v] == cb::IV_OK && (cstatus[vcam[v]] == cb::IC_OK || cstatus[vcam[v]] == cb::IC_MAX_ITER ||
+                                                    cstatus[vcam[v]] == cb::IC_NOT_PD);
+    for (int k = 0; k < 6; ++k) {
+      view_pose_out[6 * (size_t)v + k] = solved ? q[6 * (size_t)v + k] : nan;
+      view_std_out[6 * (size_t)v + k] = solved ? vstd[6 * (size_t)v + k] : nan;
+    }
+    view_rmse_out[v] = solved ? vrmse[v] : nan;
+  }
+  if (stats) {
+    stats->group_ms = ev.ms(0, 1);
+    stats->start_ms = ev.ms(2, 3);
+    if (n_active > 0) {
+      stats->lm_ms = ev.ms(4, 5);
+      stats->cov_ms = ev.ms(5, 6);
+    }
+    stats->total_ms = ev.ms(0, 7);
+    int it_max = 0;
+    for (int c = 0; c < n_cams; ++c) it_max = std::max(it_max, iterations_out[c]);
+    stats->iterations = it_max;
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cb_calibrate_intrinsics(int32_t n_cams, const int32_t* image_size, const int32_t* cam_flags,
+                            const int32_t* cam_fixed, const double* guess,
+                            int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const double* obs_obj,
+                            const double* obs_px, int obs_on_device, int32_t min_points, int32_t min_views,
+                            int32_t max_iter, double xtol, int32_t max_views, int32_t* n_views_out, double* params_out,
+                            double* std_out, double* cov_out, double* rms_out, double* sigma2_out,
+                            int32_t* used_views_out, int32_t* rows_out, int32_t* iterations_out, int32_t* status_out,
+                            int32_t* view_cam_out, double* view_pose_out, double* view_std_out, double* view_rmse_out,
+                            int32_t* view_count_out, int32_t* view_rep_out, int32_t* view_status_out,
+                            CbIntrinsicsStats* stats, int device, void* stream) {
+  const char* who = "cb_calibrate_intrinsics";
+  if (n_cams <= 0 || !image_size || !cam_flags || n_obs < 0 || n_obs > 0x7fffffffLL || !n_views_out || max_views < 0 ||
+      (n_obs > 0 && (!obs_cam || !obs_key || !obs_obj || !obs_px)) || !params_out || !std_out || !rms_out ||
+      !sigma2_out || !used_views_out || !rows_out || !iterations_out || !status_out ||
+      (max_views > 0 && (!view_cam_out || !view_pose_out || !view_std_out || !view_rmse_out || !view_count_out ||
+                         !view_rep_out || !view_status_out)) ||
+      min_points < 4 || min_views < 2 || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol))) {
+    g_last_error = std::string(who) + ": bad argument";
+    return CB_E_INVALID;
+  }
+  for (int c = 0; c < n_cams; ++c) {
+    const int f = cam_flags[c];
+    if (f & ~(CB_CAM_FREE_INTRINSICS | CB_INTR_USE_GUESS)) {
+      g_last_error = std::string(who) + ": camera " + std::to_string(c) +
+                     " asks for a model or flag this call does not implement (fisheye, fixed aspect ratio, ...)";
+      return CB_E_UNSUPPORTED;
+    }
+    if (cam_fixed && (cam_fixed[c] & ~CB_INTR_FIX_ALL)) {
+      g_last_error = std::string(who) + ": cam_fixed of camera " + std::to_string(c) + " has bits beyond the 9 parameters";
+      return CB_E_INVALID;
+    }
+    if (image_size[2 * c] <= 0 || image_size[2 * c + 1] <= 0) {
+      g_last_error = std::string(who) + ": image size of camera " + std::to_string(c) + " is not positive";
+      return CB_E_INVALID;
+    }
+    if (f & CB_INTR_USE_GUESS) {
+      if (!guess) {
+        g_last_error = std::string(who) + ": camera " + std::to_string(c) + " starts from a guess but guess is null";
+        return CB_E_INVALID;
+      }
+      const double* t = guess + 9 * (size_t)c;
+      bool ok = t[0] > 0.0 && t[1] > 0.0;
+      for (int k = 0; k < 9; ++k) ok = ok && std::isfinite(t[k]);
+      if (!ok) {
+        g_last_error = std::string(who) + ": guess of camera " + std::to_string(c) + " is not finite with fx, fy > 0";
+        return CB_E_INVALID;
+      }
+    }
+  }
+  return intrinsics_impl(n_cams, image_size, cam_flags, cam_fixed, guess, n_obs, obs_cam, obs_key, obs_obj, obs_px, obs_on_device,
+                         min_points, min_views, max_iter, xtol, max_views, n_views_out, params_out, std_out, cov_out,
+                         rms_out, sigma2_out, used_views_out, rows_out, iterations_out, status_out, view_cam_out,
+                         view_pose_out, view_std_out, view_rmse_out, view_count_out, view_rep_out, view_status_out, stats,
+                         device, stream);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -436,6 +436,68 @@ int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam
                      int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
                      CbResectStats* stats, int device, void* stream);
 
+typedef struct CbIntrinsicsStats {
+  double group_ms;  /* upload + validation + radix sort + view boundaries */
+  double start_ms;  /* view statuses, homographies, Zhang's start, undistortion, IPPE poses */
+  double lm_ms;     /* the Levenberg-Marquardt kernel */
+  double cov_ms;    /* the covariance kernel */
+  double total_ms;
+  int32_t iterations;  /* the most LM steps any camera took */
+  int32_t kernel_launches;
+} CbIntrinsicsStats;
+
+/* Per-camera words of cb_calibrate_intrinsics.  cam_flags is in the CB_CAM_* namespace of every other call:
+ * CB_CAM_FISHEYE (a fisheye lens: cv2.fisheye.calibrate is a different model and algorithm) is refused with
+ * CB_E_UNSUPPORTED, as is CB_INTR_FIX_ASPECT_RATIO and any bit not named here; CB_CAM_FREE_INTRINSICS is accepted and
+ * changes nothing (every parameter not in cam_fixed is free); CB_INTR_USE_GUESS starts the camera from guess[c].
+ * cam_fixed (nullable: nothing fixed): bit k (k = 0..8) keeps parameter k of (fx, fy, cx, cy, k1, k2, p1, p2, k3) at its
+ * start value; other bits are CB_E_INVALID. */
+#define CB_INTR_USE_GUESS 0x100
+#define CB_INTR_FIX_ASPECT_RATIO 0x200
+#define CB_INTR_FIX_ALL 0x1ff
+
+/* Intrinsic calibration of every camera from planar-board views: pinhole + Brown-Conrady (k1 k2 p1 p2 k3), the model
+ * and the optimum of cv2.calibrateCamera, with OpenCV's standard deviations (DESIGN.md section 4.10).
+ * Inputs: image_size[n_cams][2] (w, h), cam_flags[n_cams], cam_fixed[n_cams] (nullable), guess (nullable unless a
+ * camera sets CB_INTR_USE_GUESS)
+ * [n_cams][9]; rows obs_cam, obs_key (int64 >= 0: rows with equal key are one view), obs_obj[n][3] board coordinates,
+ * obs_px[n][2] raw pixels (float64, full precision) -- host arrays or, with obs_on_device, device pointers.
+ *   1. views, ascending key order, rows in caller order within a key; view status, first match wins: 6 rows from more
+ *      than one camera; 1 fewer than min_points rows; 2 non-planar (z spread >= 1e-6, or a non-finite z); 5 degenerate
+ *      Harker-O'Leary homography (board points collinear, ...) or a non-finite start pose; else 0.
+ *   2. start: the guess, or Zhang's closed form as cv2.initIntrinsicParams2D (no aspect ratio): principal point
+ *      ((w-1)/2, (h-1)/2), distortion 0, a = 1/fx^2 and b = 1/fy^2 by least squares from the two constraints of every
+ *      view with a homography (camera-major sums in view order); a or b <= 0 or not finite: camera status 2.  Each
+ *      view's start pose is cb_pnp_ippe's IPPE on its board points and its pixels undistorted with the start.
+ *   3. fixed parameters keep their start value and leave the system (no zero step).
+ *   4. Levenberg-Marquardt over the free intrinsics theta and every used view's q = (r, t), residuals in pixels
+ *      pi(X; theta, q) - u, unweighted: U, W_v, V_v, g; (H + lambda diag H) d = -g through S = U_lambda - sum_v W_v
+ *      V_v,lambda^-1 W_v^T on the free subset, back-substituted per view; lambda0 = 1e-3, a lower cost is accepted with
+ *      lambda / 10, else lambda * 10; r += dr additively; stop when |d| <= xtol (|(theta_free, q)| + xtol) or after
+ *      max_iter steps (status 4).  A step whose damped system is not positive definite is rejected without the
+ *      stopping test.
+ *   5. covariance at the solution (lambda = 0): sigma^2 = SSE / (2N - p), N rows, p = free intrinsics + 6 used views;
+ *      cov_theta = sigma^2 S^-1 (fixed rows / columns 0); per view cov_q = sigma^2 (V^-1 + V^-1 W^T S^-1 W V^-1).
+ *      S not positive definite (a Cholesky pivot <= 1e-12 of the Jacobi-scaled S): status 3, theta the last iterate,
+ *      std / cov NaN.
+ * A camera with fewer than min_views usable views is status 1.  Camera status, first match wins: 1, 2, 3, 4, else 0.
+ * Outputs per camera: params[9] (NaN without a start), std[9], cov[81] (nullable), rms = sqrt(SSE / N) (cv2's return
+ * value), sigma^2, used views, rows, iterations, status.  Per view in key order (room for max_views): camera (of its
+ * first row), pose[6] = (r, t), std[6], rmse_px (cv2's perViewErrors), count, rep_row (first caller row), status; pose,
+ * std and rmse are NaN for a view that was not solved.
+ * Arguments: min_points >= 4, min_views >= 2, max_iter >= 1, finite xtol >= 0, image sizes > 0, a guess finite with
+ * fx, fy > 0.  No floating-point atomics: repeated calls return bit-identical outputs. */
+int cb_calibrate_intrinsics(int32_t n_cams, const int32_t* image_size, const int32_t* cam_flags,
+                            const int32_t* cam_fixed, const double* guess,
+                            int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const double* obs_obj,
+                            const double* obs_px, int obs_on_device, int32_t min_points, int32_t min_views,
+                            int32_t max_iter, double xtol, int32_t max_views, int32_t* n_views_out, double* params_out,
+                            double* std_out, double* cov_out, double* rms_out, double* sigma2_out,
+                            int32_t* used_views_out, int32_t* rows_out, int32_t* iterations_out, int32_t* status_out,
+                            int32_t* view_cam_out, double* view_pose_out, double* view_std_out, double* view_rmse_out,
+                            int32_t* view_count_out, int32_t* view_rep_out, int32_t* view_status_out,
+                            CbIntrinsicsStats* stats, int device, void* stream);
+
 /* Optional NCCL transport owned by the engine (no host callback per all-reduce).  NCCL is resolved at run time from
  * the libnccl the process already has loaded (PyTorch's).  Rank 0 calls cb_nccl_unique_id and distributes the 128
  * bytes (e.g. torch.distributed.broadcast); every rank then calls cb_nccl_comm_create (collective). */
