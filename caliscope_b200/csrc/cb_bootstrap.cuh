@@ -157,6 +157,108 @@ __device__ __forceinline__ bool solve6(const double* Hp, const double* g, double
   return true;
 }
 
+// Harker-O'Leary homography (BMVC 2005) of the rows [b, e) of `rows`, one warp: img ~ H (x - mx, y - my, 1) with the
+// model points x = ax(r, 0..1) centred on their mean (mx, my) and the image points img(r, 0..1) (mean (mu, mv)).
+// Returns false when the points have no spread or the model points' 2x2 moment matrix is singular; det, a00 and a11
+// come back with H so that a caller can reject (nearly) collinear model points.  pnp_ippe_kernel (float32 model points)
+// and intr_view_kernel (full precision) both fit with it.
+struct HoFit {
+  double betaA, betaB, c1, c2, c3, c4, a00, a11, det, i00, i01, i11;
+  double H[9];
+};
+
+template <typename AX, typename IMG>
+__device__ __forceinline__ bool ho_fit(const int* __restrict__ rows, int b, int e, int lane, int n, double mx, double my,
+                                       double mu, double mv, AX ax, IMG img, HoFit& f) {
+  // ---- pass 1: isotropic scales
+  double ka = 0, kb = 0;
+  for (int i = b + lane; i < e; i += 32) {
+    const int r = rows[i];
+    const double ax0 = ax(r, 0) - mx, ay0 = ax(r, 1) - my, bu = img(r, 0) - mu, bv = img(r, 1) - mv;
+    ka += ax0 * ax0 + ay0 * ay0;
+    kb += bu * bu + bv * bv;
+  }
+  ka = warp_sum(ka); kb = warp_sum(kb);
+  if (!(ka > 0.0) || !(kb > 0.0)) return false;
+  const double betaA = sqrt(2.0 * n / ka), betaB = sqrt(2.0 * n / kb);
+  // normalised source A = betaA (obj - mean), target B = betaB (img - mean)
+#define HO_LOAD(r)                                                                                     \
+  const double A0 = betaA * (ax(r, 0) - mx), A1 = betaA * (ax(r, 1) - my);                             \
+  const double B0 = betaB * (img(r, 0) - mu), B1 = betaB * (img(r, 1) - mv)
+  // ---- pass 2: means of C1..C4, A A^T
+  double c1 = 0, c2 = 0, c3 = 0, c4 = 0, a00 = 0, a01 = 0, a11 = 0;
+  for (int i = b + lane; i < e; i += 32) {
+    const int r = rows[i];
+    HO_LOAD(r);
+    c1 += -B0 * A0; c2 += -B0 * A1; c3 += -B1 * A0; c4 += -B1 * A1;
+    a00 += A0 * A0; a01 += A0 * A1; a11 += A1 * A1;
+  }
+  c1 = warp_sum(c1) / n; c2 = warp_sum(c2) / n; c3 = warp_sum(c3) / n; c4 = warp_sum(c4) / n;
+  a00 = warp_sum(a00); a01 = warp_sum(a01); a11 = warp_sum(a11);
+  const double det = a00 * a11 - a01 * a01;
+  if (!(fabs(det) > 0.0)) return false;
+  const double i00 = a11 / det, i01 = -a01 / det, i11 = a00 / det;
+  // ---- pass 3: A Mx, A My (2x3 each)
+  double amx[6] = {0, 0, 0, 0, 0, 0}, amy[6] = {0, 0, 0, 0, 0, 0};
+  for (int i = b + lane; i < e; i += 32) {
+    const int r = rows[i];
+    HO_LOAD(r);
+    const double mxr[3] = {-B0 * A0 - c1, -B0 * A1 - c2, -B0}, myr[3] = {-B1 * A0 - c3, -B1 * A1 - c4, -B1};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      amx[k] += A0 * mxr[k]; amx[3 + k] += A1 * mxr[k];
+      amy[k] += A0 * myr[k]; amy[3 + k] += A1 * myr[k];
+    }
+  }
+  double Bx[6], By[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) { amx[k] = warp_sum(amx[k]); amy[k] = warp_sum(amy[k]); }
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    Bx[k] = i00 * amx[k] + i01 * amx[3 + k]; Bx[3 + k] = i01 * amx[k] + i11 * amx[3 + k];
+    By[k] = i00 * amy[k] + i01 * amy[3 + k]; By[3 + k] = i01 * amy[k] + i11 * amy[3 + k];
+  }
+  // ---- pass 4: D^T D with D rows = Mx_i - A_i^T Bx ; My_i - A_i^T By
+  double dd[6] = {0, 0, 0, 0, 0, 0};
+  for (int i = b + lane; i < e; i += 32) {
+    const int r = rows[i];
+    HO_LOAD(r);
+    double d1[3], d2[3];
+    const double mxr[3] = {-B0 * A0 - c1, -B0 * A1 - c2, -B0}, myr[3] = {-B1 * A0 - c3, -B1 * A1 - c4, -B1};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      d1[k] = mxr[k] - (A0 * Bx[k] + A1 * Bx[3 + k]);
+      d2[k] = myr[k] - (A0 * By[k] + A1 * By[3 + k]);
+    }
+    dd[0] += d1[0] * d1[0] + d2[0] * d2[0]; dd[1] += d1[0] * d1[1] + d2[0] * d2[1]; dd[2] += d1[0] * d1[2] + d2[0] * d2[2];
+    dd[3] += d1[1] * d1[1] + d2[1] * d2[1]; dd[4] += d1[1] * d1[2] + d2[1] * d2[2]; dd[5] += d1[2] * d1[2] + d2[2] * d2[2];
+  }
+#pragma unroll
+  for (int k = 0; k < 6; ++k) dd[k] = warp_sum(dd[k]);
+  double M[3][3] = {{dd[0], dd[1], dd[2]}, {dd[1], dd[3], dd[4]}, {dd[2], dd[4], dd[5]}};
+  double h789[3];
+  sym3_min_eigvec(M, h789);
+  // normalised-frame homography, then H = TB^-1 Hn TA
+  double Hn[9];
+  Hn[0] = -(Bx[0] * h789[0] + Bx[1] * h789[1] + Bx[2] * h789[2]);
+  Hn[1] = -(Bx[3] * h789[0] + Bx[4] * h789[1] + Bx[5] * h789[2]);
+  Hn[2] = -(c1 * h789[0] + c2 * h789[1]);
+  Hn[3] = -(By[0] * h789[0] + By[1] * h789[1] + By[2] * h789[2]);
+  Hn[4] = -(By[3] * h789[0] + By[4] * h789[1] + By[5] * h789[2]);
+  Hn[5] = -(c3 * h789[0] + c4 * h789[1]);
+  Hn[6] = h789[0]; Hn[7] = h789[1]; Hn[8] = h789[2];
+  // canonical source frame = centred object points (mean removed), so TA = diag(betaA, betaA, 1) there
+  const double TA[9] = {betaA, 0, 0, 0, betaA, 0, 0, 0, 1};
+  const double TBi[9] = {1.0 / betaB, 0, mu, 0, 1.0 / betaB, mv, 0, 0, 1};
+  double T1[9];
+  mat3_mul(Hn, TA, T1);
+  mat3_mul(TBi, T1, f.H);
+#undef HO_LOAD
+  f.betaA = betaA; f.betaB = betaB; f.c1 = c1; f.c2 = c2; f.c3 = c3; f.c4 = c4;
+  f.a00 = a00; f.a11 = a11; f.det = det; f.i00 = i00; f.i01 = i01; f.i11 = i11;
+  return true;
+}
+
 // status codes of a PnP group
 constexpr int PNP_OK = 0, PNP_TOO_FEW = 1, PNP_NON_PLANAR = 2, PNP_DEGENERATE = 3, PNP_OK_FALLBACK = 4;
 constexpr double IPPE_GAMMA_MIN = 1e-7;
@@ -206,92 +308,16 @@ pnp_ippe_kernel(const int* __restrict__ start, const int* __restrict__ rows, con
   if (!(zmax - zmin < 1e-6)) { fail(PNP_NON_PLANAR); return; }  // np.ptp(z) < 1e-6 (:279)
   if (n < min_points) { fail(PNP_TOO_FEW); return; }
   const double mx = sx / n, my = sy / n, mz = sz / n, mu = su / n, mv = sv / n;
-  // ---- pass 1: isotropic scales
-  double ka = 0, kb = 0;
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    const double ax = ox(r, 0) - mx, ay = ox(r, 1) - my, bu = img[2 * (size_t)r] - mu, bv = img[2 * (size_t)r + 1] - mv;
-    ka += ax * ax + ay * ay;
-    kb += bu * bu + bv * bv;
+  // ---- passes 1-4: the homography of the centred model plane
+  HoFit f;
+  if (!ho_fit(rows, b, e, lane, n, mx, my, mu, mv, ox, [&](int r, int k) { return img[2 * (size_t)r + k]; }, f)) {
+    fail(PNP_DEGENERATE);
+    return;
   }
-  ka = warp_sum(ka); kb = warp_sum(kb);
-  if (!(ka > 0.0) || !(kb > 0.0)) { fail(PNP_DEGENERATE); return; }
-  const double betaA = sqrt(2.0 * n / ka), betaB = sqrt(2.0 * n / kb);
-  // normalised source A = betaA (obj - mean), target B = betaB (img - mean)
-#define BS_LOAD(r)                                                                                     \
-  const double A0 = betaA * (ox(r, 0) - mx), A1 = betaA * (ox(r, 1) - my);                            \
-  const double B0 = betaB * (img[2 * (size_t)(r)] - mu), B1 = betaB * (img[2 * (size_t)(r) + 1] - mv)
-  // ---- pass 2: means of C1..C4, A A^T
-  double c1 = 0, c2 = 0, c3 = 0, c4 = 0, a00 = 0, a01 = 0, a11 = 0;
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    BS_LOAD(r);
-    c1 += -B0 * A0; c2 += -B0 * A1; c3 += -B1 * A0; c4 += -B1 * A1;
-    a00 += A0 * A0; a01 += A0 * A1; a11 += A1 * A1;
-  }
-  c1 = warp_sum(c1) / n; c2 = warp_sum(c2) / n; c3 = warp_sum(c3) / n; c4 = warp_sum(c4) / n;
-  a00 = warp_sum(a00); a01 = warp_sum(a01); a11 = warp_sum(a11);
-  const double det = a00 * a11 - a01 * a01;
-  if (!(fabs(det) > 0.0)) { fail(PNP_DEGENERATE); return; }
-  const double i00 = a11 / det, i01 = -a01 / det, i11 = a00 / det;
-  // ---- pass 3: A Mx, A My (2x3 each)
-  double amx[6] = {0, 0, 0, 0, 0, 0}, amy[6] = {0, 0, 0, 0, 0, 0};
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    BS_LOAD(r);
-    const double mxr[3] = {-B0 * A0 - c1, -B0 * A1 - c2, -B0}, myr[3] = {-B1 * A0 - c3, -B1 * A1 - c4, -B1};
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      amx[k] += A0 * mxr[k]; amx[3 + k] += A1 * mxr[k];
-      amy[k] += A0 * myr[k]; amy[3 + k] += A1 * myr[k];
-    }
-  }
-  double Bx[6], By[6];
-#pragma unroll
-  for (int k = 0; k < 6; ++k) { amx[k] = warp_sum(amx[k]); amy[k] = warp_sum(amy[k]); }
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    Bx[k] = i00 * amx[k] + i01 * amx[3 + k]; Bx[3 + k] = i01 * amx[k] + i11 * amx[3 + k];
-    By[k] = i00 * amy[k] + i01 * amy[3 + k]; By[3 + k] = i01 * amy[k] + i11 * amy[3 + k];
-  }
-  // ---- pass 4: D^T D with D rows = Mx_i - A_i^T Bx ; My_i - A_i^T By
-  double dd[6] = {0, 0, 0, 0, 0, 0};
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    BS_LOAD(r);
-    double d1[3], d2[3];
-    const double mxr[3] = {-B0 * A0 - c1, -B0 * A1 - c2, -B0}, myr[3] = {-B1 * A0 - c3, -B1 * A1 - c4, -B1};
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      d1[k] = mxr[k] - (A0 * Bx[k] + A1 * Bx[3 + k]);
-      d2[k] = myr[k] - (A0 * By[k] + A1 * By[3 + k]);
-    }
-    dd[0] += d1[0] * d1[0] + d2[0] * d2[0]; dd[1] += d1[0] * d1[1] + d2[0] * d2[1]; dd[2] += d1[0] * d1[2] + d2[0] * d2[2];
-    dd[3] += d1[1] * d1[1] + d2[1] * d2[1]; dd[4] += d1[1] * d1[2] + d2[1] * d2[2]; dd[5] += d1[2] * d1[2] + d2[2] * d2[2];
-  }
-#pragma unroll
-  for (int k = 0; k < 6; ++k) dd[k] = warp_sum(dd[k]);
-  double M[3][3] = {{dd[0], dd[1], dd[2]}, {dd[1], dd[3], dd[4]}, {dd[2], dd[4], dd[5]}};
-  double h789[3];
-  sym3_min_eigvec(M, h789);
-  // normalised-frame homography, then H = TB^-1 Hn TA
-  double Hn[9];
-  Hn[0] = -(Bx[0] * h789[0] + Bx[1] * h789[1] + Bx[2] * h789[2]);
-  Hn[1] = -(Bx[3] * h789[0] + Bx[4] * h789[1] + Bx[5] * h789[2]);
-  Hn[2] = -(c1 * h789[0] + c2 * h789[1]);
-  Hn[3] = -(By[0] * h789[0] + By[1] * h789[1] + By[2] * h789[2]);
-  Hn[4] = -(By[3] * h789[0] + By[4] * h789[1] + By[5] * h789[2]);
-  Hn[5] = -(c3 * h789[0] + c4 * h789[1]);
-  Hn[6] = h789[0]; Hn[7] = h789[1]; Hn[8] = h789[2];
-  // canonical source frame = centred object points (mean removed), so TA = diag(betaA, betaA, 1) there
-  const double TA[9] = {betaA, 0, 0, 0, betaA, 0, 0, 0, 1};
-  const double TBi[9] = {1.0 / betaB, 0, mu, 0, 1.0 / betaB, mv, 0, 0, 1};
-  double T1[9], H[9];
-  mat3_mul(Hn, TA, T1);
-  mat3_mul(TBi, T1, H);
+  double* H = f.H;
   // all model points on one line: no pose (cv2 reports success with a NaN pose; the reference keeps the group and its
   // NaN filter drops it later, pose_network_builder.py:364-367)
-  if (!(fabs(det) > 1e-12 * (a00 + a11) * (a00 + a11))) { fail(PNP_DEGENERATE); return; }
+  if (!(fabs(f.det) > 1e-12 * (f.a00 + f.a11) * (f.a00 + f.a11))) { fail(PNP_DEGENERATE); return; }
   double Rs[2][9], ts[2][3], err[2];
   double gamma = -1.0;
   if (fabs(H[8]) > 0.0) {
@@ -308,9 +334,9 @@ pnp_ippe_kernel(const int* __restrict__ start, const int* __restrict__ rows, con
   const bool fallback = !(gamma >= IPPE_GAMMA_MIN);
   if (fallback) {
     // affine fit in normalised coordinates: B ~ Mn A, Mn = (sum B A^T)(sum A A^T)^-1, sum B A^T = -n [c1 c2; c3 c4]
-    const double s00 = -n * c1, s01 = -n * c2, s10 = -n * c3, s11 = -n * c4, sc = betaA / betaB;
-    const double m00 = sc * (s00 * i00 + s01 * i01), m01 = sc * (s00 * i01 + s01 * i11);
-    const double m10 = sc * (s10 * i00 + s11 * i01), m11 = sc * (s10 * i01 + s11 * i11);
+    const double s00 = -n * f.c1, s01 = -n * f.c2, s10 = -n * f.c3, s11 = -n * f.c4, sc = f.betaA / f.betaB;
+    const double m00 = sc * (s00 * f.i00 + s01 * f.i01), m01 = sc * (s00 * f.i01 + s01 * f.i11);
+    const double m10 = sc * (s10 * f.i00 + s11 * f.i01), m11 = sc * (s10 * f.i01 + s11 * f.i11);
     gamma = ippe_rotations(m00, m01, m10, m11, mu, mv, Rs);
     if (!(gamma > 0.0)) { fail(PNP_DEGENERATE); return; }
   }
@@ -409,7 +435,6 @@ pnp_ippe_kernel(const int* __restrict__ start, const int* __restrict__ rows, con
     }
     err[0] = warp_sum(e0); err[1] = warp_sum(e1);
   }
-#undef BS_LOAD
   const int best = (err[1] < err[0]) ? 1 : 0;
   if (lane == 0) {
     const double* R = Rs[best];

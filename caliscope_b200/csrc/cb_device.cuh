@@ -31,6 +31,10 @@ constexpr int CT_SMEM = 37;
 
 constexpr double CB_EPS = 2.220446049250313e-16;
 
+// index of entry (i, j), i <= j, of a symmetric N x N matrix packed as its upper triangle row by row
+template <int N>
+__host__ __device__ constexpr int ut(int i, int j) { return i * N - i * (i - 1) / 2 + (j - i); }
+
 // ---------------------------------------------------------------------------------------------
 // one full 32-byte sector per thread (32-byte aligned): sm_90 has no 256-bit global access, so two 128-bit
 // accesses (LDG.E.128 / STG.E.128) to the two halves of the same sector

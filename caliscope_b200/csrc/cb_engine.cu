@@ -83,6 +83,26 @@ void with_lanes(int lanes, F&& f) {
   else f(std::integral_constant<int, 8>{});
 }
 
+// launch configuration (cfg) of `grid` CTAs of `block` threads in 1-D thread-block clusters of `cluster` CTAs
+struct ClusterConfig {
+  cudaLaunchConfig_t cfg = {};
+  cudaLaunchAttribute at[1] = {};
+  ClusterConfig(int grid, int block, int cluster, size_t smem, cudaStream_t st) {
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(block);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    at[0].id = cudaLaunchAttributeClusterDimension;
+    at[0].val.clusterDim.x = cluster;
+    at[0].val.clusterDim.y = 1;
+    at[0].val.clusterDim.z = 1;
+    cfg.attrs = at;
+    cfg.numAttrs = 1;
+  }
+  ClusterConfig(const ClusterConfig&) = delete;  // cfg points into this object
+  ClusterConfig& operator=(const ClusterConfig&) = delete;
+};
+
 // ------------------------------------------------------------------------------------------
 // NCCL, resolved at run time from the libnccl the process already has loaded (torch's bundled copy):
 // no link-time dependency, no second NCCL in the address space.
@@ -925,22 +945,11 @@ void launch_pt_backsub(CbBaProblem* p, double* dp_out, cudaStream_t st) {
 }
 
 int launch_pcg(CbBaProblem* p, const cb::LmState* st_dev, double tol2, int max_iter, cudaStream_t st) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(p->pcg_cs);
-  cfg.blockDim = dim3(cb::PCG_THREADS);
-  cfg.dynamicSmemBytes = p->pcg_smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = p->pcg_cs;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
+  const ClusterConfig c(p->pcg_cs, cb::PCG_THREADS, p->pcg_cs, p->pcg_smem, st);
   const double* S = p->d_red;
   const double* b = p->d_red + (size_t)p->nP * p->nP;
-  CB_CUDA(cudaLaunchKernelEx(&cfg, p->k.pcg, st_dev, S, b, (const double*)p->d_Minv, p->nP, p->pcg_npa, p->pcg_rows, tol2,
-                             max_iter, p->d_dc, p->d_sc));
+  CB_CUDA(cudaLaunchKernelEx(&c.cfg, p->k.pcg, st_dev, S, b, (const double*)p->d_Minv, p->nP, p->pcg_npa, p->pcg_rows,
+                             tol2, max_iter, p->d_dc, p->d_sc));
   g_launches.fetch_add(1);
   return CB_OK;
 }
@@ -1364,17 +1373,9 @@ int choose_pcg_config(CbBaProblem* p) {
       cudaGetLastError();
       return false;
     }
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(cs);
-    cfg.blockDim = dim3(cb::PCG_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cudaLaunchAttribute at[1];
-    at[0].id = cudaLaunchAttributeClusterDimension;
-    at[0].val.clusterDim.x = cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-    cfg.attrs = at;
-    cfg.numAttrs = 1;
+    const ClusterConfig c(cs, cb::PCG_THREADS, cs, smem, nullptr);
     int ncl = 0;
-    if (cudaOccupancyMaxActiveClusters(&ncl, fn, &cfg) != cudaSuccess || ncl < 1) {
+    if (cudaOccupancyMaxActiveClusters(&ncl, fn, &c.cfg) != cudaSuccess || ncl < 1) {
       cudaGetLastError();
       return false;
     }
@@ -2993,6 +2994,35 @@ int tri_dlt_launch(int32_t n_cams, const double* d_proj, const ObsGroups& g, int
   return CB_OK;
 }
 
+// the planar PnP of every group (buffers held by the call's workspace), pnp_ippe_kernel's outputs
+struct PnpPoses {
+  double* R = nullptr;
+  double* t = nullptr;
+  double* rmse = nullptr;
+  int* status = nullptr;
+  int* count = nullptr;
+  int* rep = nullptr;
+};
+
+// the planar PnP of every group of `g` from the object points d_obj (n, 3) and the undistorted normalised image points
+// d_norm (n, 2), ev_a / ev_b (when not null) around the kernel
+int pnp_launch(const ObsGroups& g, const double* d_obj, const double* d_norm, int min_points, cudaEvent_t ev_a,
+               cudaEvent_t ev_b, ScopedFree& sf, cudaStream_t st, PnpPoses* p) {
+  const int n_groups = g.n_groups;
+  CB_TRY(sf.alloc(&p->R, 9 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&p->t, 3 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&p->rmse, (size_t)n_groups));
+  CB_TRY(sf.alloc(&p->status, (size_t)n_groups));
+  CB_TRY(sf.alloc(&p->count, (size_t)n_groups));
+  CB_TRY(sf.alloc(&p->rep, (size_t)n_groups));
+  if (ev_a) CB_CUDA(cudaEventRecord(ev_a, st));
+  CB_LAUNCH(cb::pnp_ippe_kernel, cdiv((long long)n_groups * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, g.start, g.rows,
+            d_obj, d_norm, n_groups, min_points, p->R, p->t, p->rmse, p->status, p->count, p->rep);
+  CB_CUDA(cudaGetLastError());
+  if (ev_b) CB_CUDA(cudaEventRecord(ev_b, st));
+  return CB_OK;
+}
+
 // Cameras of the calibrated triangulation calls, given in the bundle-adjustment layout (x: [r t] or [r t s k1 k2] per
 // camera).  tri_cams_prepare validates them on the host and derives the DLT start's normalised projection matrices [R|t]
 // and undistortion tables (intrinsics as cam_prep_one forms them); tri_cams_upload builds the device camera table with
@@ -3642,25 +3672,6 @@ int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam
 
 namespace {
 
-// one launch of an intrinsic-calibration cluster kernel: a cluster of cs CTAs per camera in A.cams
-int intr_launch(void (*kernel)(cb::IntrArgs), int n_active, int cs, size_t smem, const cb::IntrArgs& A, cudaStream_t st) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(n_active * cs);
-  cfg.blockDim = dim3(cb::INTR_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeClusterDimension;
-  at[0].val.clusterDim.x = cs;
-  at[0].val.clusterDim.y = 1;
-  at[0].val.clusterDim.z = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  CB_CUDA(cudaLaunchKernelEx(&cfg, kernel, A));
-  g_launches.fetch_add(1);
-  return CB_OK;
-}
-
 int intrinsics_impl(int32_t n_cams, const int32_t* image_size, const int32_t* cam_flags, const int32_t* cam_fixed,
                     const double* guess,
                     int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const double* obs_obj,
@@ -3763,19 +3774,13 @@ int intrinsics_impl(int32_t n_cams, const int32_t* image_size, const int32_t* ca
   }
   const cb::UndistCam* d_tab = nullptr;
   CB_TRY(upload_undist_table(tab, sf, st, &d_tab));
-  double *d_norm, *d_R, *d_t, *d_prmse;
-  int *d_pst, *d_pcnt, *d_prep;
+  double* d_norm;
   CB_TRY(sf.alloc(&d_norm, 2 * (size_t)n));
-  CB_TRY(sf.alloc(&d_R, 9 * (size_t)V));
-  CB_TRY(sf.alloc(&d_t, 3 * (size_t)V));
-  CB_TRY(sf.alloc(&d_prmse, (size_t)V));
-  CB_TRY(sf.alloc(&d_pst, (size_t)V));
-  CB_TRY(sf.alloc(&d_pcnt, (size_t)V));
-  CB_TRY(sf.alloc(&d_prep, (size_t)V));
   CB_LAUNCH(cb::undistort_kernel<double>, cdiv(n, 256), 256, 0, st, d_tab, g.cam, g.xy, d_norm, (long long)n, 0);
-  CB_LAUNCH(cb::pnp_ippe_kernel, cdiv((long long)V * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, g.start, g.rows, d_obj,
-            d_norm, V, (int)min_points, d_R, d_t, d_prmse, d_pst, d_pcnt, d_prep);
-  CB_LAUNCH(cb::intr_pose_kernel, cdiv(V, 128), 128, 0, st, d_vcam, d_cstatus, d_R, d_t, d_pst, V, d_vstatus, d_q);
+  PnpPoses pnp;
+  CB_TRY(pnp_launch(g, d_obj, d_norm, (int)min_points, nullptr, nullptr, sf, st, &pnp));
+  CB_LAUNCH(cb::intr_pose_kernel, cdiv(V, 128), 128, 0, st, d_vcam, d_cstatus, pnp.R, pnp.t, pnp.status, V, d_vstatus,
+            d_q);
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaMemcpyAsync(vstatus.data(), d_vstatus, sizeof(int) * V, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
@@ -3824,13 +3829,17 @@ int intrinsics_impl(int32_t n_cams, const int32_t* image_size, const int32_t* ca
     if (cov_out) CB_TRY(sf.alloc(&d_cov, 81 * (size_t)n_cams));
     cb::IntrArgs A{g.start, g.rows, d_obj, g.xy, d_act, d_uvs, d_uvl, d_flags, d_crows, d_theta, d_q, d_gram, d_con,
                    d_trial, d_cstatus, d_iters, d_sse, d_std, d_cov, d_sig, d_vstd, d_vrmse, (int)max_iter, xtol};
-    // cluster size: about four views per warp, up to the portable limit of 8 CTAs
+    // a cluster of cs CTAs per camera; cs: about four views per warp, up to the portable limit of 8 CTAs
     const int cs = std::max(1, std::min(cb::INTR_MAX_CLUSTER, cdiv(max_nv, 4 * cb::INTR_WARPS)));
+    const ClusterConfig lm_cfg(n_active * cs, cb::INTR_THREADS, cs, cb::INTR_SMEM, st);
+    const ClusterConfig cov_cfg(n_active * cs, cb::INTR_THREADS, cs, 0, st);
     CB_CUDA(cudaFuncSetAttribute(cb::intr_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb::INTR_SMEM));
     CB_CUDA(cudaEventRecord(ev[4], st));
-    CB_TRY(intr_launch(cb::intr_lm_kernel, n_active, cs, cb::INTR_SMEM, A, st));
+    CB_CUDA(cudaLaunchKernelEx(&lm_cfg.cfg, cb::intr_lm_kernel, A));
+    g_launches.fetch_add(1);
     CB_CUDA(cudaEventRecord(ev[5], st));
-    CB_TRY(intr_launch(cb::intr_cov_kernel, n_active, cs, 0, A, st));
+    CB_CUDA(cudaLaunchKernelEx(&cov_cfg.cfg, cb::intr_cov_kernel, A));
+    g_launches.fetch_add(1);
     CB_CUDA(cudaEventRecord(ev[6], st));
     CB_CUDA(cudaMemcpyAsync(theta.data(), d_theta, sizeof(double) * theta.size(), cudaMemcpyDeviceToHost, st));
     CB_CUDA(cudaMemcpyAsync(cstatus.data(), d_cstatus, sizeof(int) * n_cams, cudaMemcpyDeviceToHost, st));
@@ -3983,25 +3992,14 @@ int cb_pnp_ippe(int32_t n_cams, const int32_t* cam_fisheye, const double* cam_k,
   CB_TRY(obs_group_stage(n_cams, &tab, n, obs_cam, obs_key, obs_px, 0, max_groups, n_groups_out, "cb_pnp_ippe", ev[1], sf,
                          st, &g));
   const int n_groups = g.n_groups;
-  double *d_R, *d_t, *d_rmse;
-  int *d_status, *d_count, *d_rep;
-  CB_TRY(sf.alloc(&d_R, 9 * (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_t, 3 * (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_rmse, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_status, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_count, (size_t)n_groups));
-  CB_TRY(sf.alloc(&d_rep, (size_t)n_groups));
-  CB_CUDA(cudaEventRecord(ev[2], st));
-  CB_LAUNCH(cb::pnp_ippe_kernel, cdiv((long long)n_groups * 32, cb::BS_THREADS), cb::BS_THREADS, 0, st, g.start, g.rows, d_obj,
-            g.xy, n_groups, (int)min_points, d_R, d_t, d_rmse, d_status, d_count, d_rep);
-  CB_CUDA(cudaGetLastError());
-  CB_CUDA(cudaEventRecord(ev[3], st));
-  CB_CUDA(cudaMemcpyAsync(R_out, d_R, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(t_out, d_t, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rmse_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(count_out, d_count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaMemcpyAsync(rep_row_out, d_rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  PnpPoses p;
+  CB_TRY(pnp_launch(g, d_obj, g.xy, (int)min_points, ev[2], ev[3], sf, st, &p));
+  CB_CUDA(cudaMemcpyAsync(R_out, p.R, sizeof(double) * 9 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(t_out, p.t, sizeof(double) * 3 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rmse_out, p.rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(status_out, p.status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, p.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, p.rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   if (stats) {
     stats->group_ms = ev.ms(0, 1);

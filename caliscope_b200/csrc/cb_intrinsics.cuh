@@ -2,7 +2,7 @@
 // pinhole + Brown-Conrady (k1 k2 p1 p2 k3), the model and optimum of cv2.calibrateCamera.
 //
 //   intr_view_kernel   one warp per view (rows of one key): view status and the Harker-O'Leary homography from the
-//                      board plane to the pixels (ho_fit: pnp_ippe_kernel's passes, on full-precision inputs)
+//                      board plane to the pixels (ho_fit, shared with pnp_ippe_kernel, on full-precision inputs)
 //   intr_zhang_kernel  one thread per camera: the guess, or Zhang's closed form from the homographies in view order
 //   intr_pose_kernel   one thread per view: the IPPE pose of pnp_ippe_kernel as (r, t), or status 5
 //   intr_lm_kernel     one thread-block cluster per camera: Levenberg-Marquardt over the free intrinsics and every view
@@ -35,113 +35,7 @@ constexpr int INTR_TRIAL = 9;  // per view: q + dq (6), trial cost, |dq|^2, |q|^
 constexpr int INTR_STAGE = 32 * 32;  // doubles of one warp's staging buffer: 32 rows x ([J_u r_u] [J_v r_v])
 constexpr size_t INTR_SMEM = sizeof(double) * INTR_WARPS * INTR_STAGE;
 
-__host__ __device__ constexpr int ut16(int i, int j) { return i * 16 - i * (i - 1) / 2 + (j - i); }  // i <= j
-__host__ __device__ constexpr int ut9(int i, int j) { return i * 9 - i * (i - 1) / 2 + (j - i); }    // i <= j
-
 // ---- views ---------------------------------------------------------------------------------------------------------
-// Harker-O'Leary homography (BMVC 2005) of the rows [b, e) of `rows`, one warp: img ~ H (x - mx, y - my, 1) with the
-// model points x = ax(r, 0..1) centred on their mean (mx, my) and the image points img(r, 0..1) (mean (mu, mv)).
-// Returns false when the points have no spread or the model points' 2x2 moment matrix is singular; det, a00 and a11
-// come back with H so that a caller can reject (nearly) collinear model points.  The steps are pnp_ippe_kernel's
-// passes 1-4 in the same order; that kernel keeps its inline copy because calling this function changes its SASS
-// (154 -> 159 registers).
-struct HoFit {
-  double betaA, betaB, c1, c2, c3, c4, a00, a11, det, i00, i01, i11;
-  double H[9];
-};
-
-template <typename AX, typename IMG>
-__device__ __forceinline__ bool ho_fit(const int* __restrict__ rows, int b, int e, int lane, int n, double mx, double my,
-                                       double mu, double mv, AX ax, IMG img, HoFit& f) {
-  // ---- pass 1: isotropic scales
-  double ka = 0, kb = 0;
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    const double ax0 = ax(r, 0) - mx, ay0 = ax(r, 1) - my, bu = img(r, 0) - mu, bv = img(r, 1) - mv;
-    ka += ax0 * ax0 + ay0 * ay0;
-    kb += bu * bu + bv * bv;
-  }
-  ka = warp_sum(ka); kb = warp_sum(kb);
-  if (!(ka > 0.0) || !(kb > 0.0)) return false;
-  const double betaA = sqrt(2.0 * n / ka), betaB = sqrt(2.0 * n / kb);
-  // normalised source A = betaA (obj - mean), target B = betaB (img - mean)
-#define INTR_LOAD(r)                                                                                     \
-  const double A0 = betaA * (ax(r, 0) - mx), A1 = betaA * (ax(r, 1) - my);                            \
-  const double B0 = betaB * (img(r, 0) - mu), B1 = betaB * (img(r, 1) - mv)
-  // ---- pass 2: means of C1..C4, A A^T
-  double c1 = 0, c2 = 0, c3 = 0, c4 = 0, a00 = 0, a01 = 0, a11 = 0;
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    INTR_LOAD(r);
-    c1 += -B0 * A0; c2 += -B0 * A1; c3 += -B1 * A0; c4 += -B1 * A1;
-    a00 += A0 * A0; a01 += A0 * A1; a11 += A1 * A1;
-  }
-  c1 = warp_sum(c1) / n; c2 = warp_sum(c2) / n; c3 = warp_sum(c3) / n; c4 = warp_sum(c4) / n;
-  a00 = warp_sum(a00); a01 = warp_sum(a01); a11 = warp_sum(a11);
-  const double det = a00 * a11 - a01 * a01;
-  if (!(fabs(det) > 0.0)) return false;
-  const double i00 = a11 / det, i01 = -a01 / det, i11 = a00 / det;
-  // ---- pass 3: A Mx, A My (2x3 each)
-  double amx[6] = {0, 0, 0, 0, 0, 0}, amy[6] = {0, 0, 0, 0, 0, 0};
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    INTR_LOAD(r);
-    const double mxr[3] = {-B0 * A0 - c1, -B0 * A1 - c2, -B0}, myr[3] = {-B1 * A0 - c3, -B1 * A1 - c4, -B1};
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      amx[k] += A0 * mxr[k]; amx[3 + k] += A1 * mxr[k];
-      amy[k] += A0 * myr[k]; amy[3 + k] += A1 * myr[k];
-    }
-  }
-  double Bx[6], By[6];
-#pragma unroll
-  for (int k = 0; k < 6; ++k) { amx[k] = warp_sum(amx[k]); amy[k] = warp_sum(amy[k]); }
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    Bx[k] = i00 * amx[k] + i01 * amx[3 + k]; Bx[3 + k] = i01 * amx[k] + i11 * amx[3 + k];
-    By[k] = i00 * amy[k] + i01 * amy[3 + k]; By[3 + k] = i01 * amy[k] + i11 * amy[3 + k];
-  }
-  // ---- pass 4: D^T D with D rows = Mx_i - A_i^T Bx ; My_i - A_i^T By
-  double dd[6] = {0, 0, 0, 0, 0, 0};
-  for (int i = b + lane; i < e; i += 32) {
-    const int r = rows[i];
-    INTR_LOAD(r);
-    double d1[3], d2[3];
-    const double mxr[3] = {-B0 * A0 - c1, -B0 * A1 - c2, -B0}, myr[3] = {-B1 * A0 - c3, -B1 * A1 - c4, -B1};
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      d1[k] = mxr[k] - (A0 * Bx[k] + A1 * Bx[3 + k]);
-      d2[k] = myr[k] - (A0 * By[k] + A1 * By[3 + k]);
-    }
-    dd[0] += d1[0] * d1[0] + d2[0] * d2[0]; dd[1] += d1[0] * d1[1] + d2[0] * d2[1]; dd[2] += d1[0] * d1[2] + d2[0] * d2[2];
-    dd[3] += d1[1] * d1[1] + d2[1] * d2[1]; dd[4] += d1[1] * d1[2] + d2[1] * d2[2]; dd[5] += d1[2] * d1[2] + d2[2] * d2[2];
-  }
-#pragma unroll
-  for (int k = 0; k < 6; ++k) dd[k] = warp_sum(dd[k]);
-  double M[3][3] = {{dd[0], dd[1], dd[2]}, {dd[1], dd[3], dd[4]}, {dd[2], dd[4], dd[5]}};
-  double h789[3];
-  sym3_min_eigvec(M, h789);
-  // normalised-frame homography, then H = TB^-1 Hn TA
-  double Hn[9];
-  Hn[0] = -(Bx[0] * h789[0] + Bx[1] * h789[1] + Bx[2] * h789[2]);
-  Hn[1] = -(Bx[3] * h789[0] + Bx[4] * h789[1] + Bx[5] * h789[2]);
-  Hn[2] = -(c1 * h789[0] + c2 * h789[1]);
-  Hn[3] = -(By[0] * h789[0] + By[1] * h789[1] + By[2] * h789[2]);
-  Hn[4] = -(By[3] * h789[0] + By[4] * h789[1] + By[5] * h789[2]);
-  Hn[5] = -(c3 * h789[0] + c4 * h789[1]);
-  Hn[6] = h789[0]; Hn[7] = h789[1]; Hn[8] = h789[2];
-  // canonical source frame = centred object points (mean removed), so TA = diag(betaA, betaA, 1) there
-  const double TA[9] = {betaA, 0, 0, 0, betaA, 0, 0, 0, 1};
-  const double TBi[9] = {1.0 / betaB, 0, mu, 0, 1.0 / betaB, mv, 0, 0, 1};
-  double T1[9];
-  mat3_mul(Hn, TA, T1);
-  mat3_mul(TBi, T1, f.H);
-#undef INTR_LOAD
-  f.betaA = betaA; f.betaB = betaB; f.c1 = c1; f.c2 = c2; f.c3 = c3; f.c4 = c4;
-  f.a00 = a00; f.a11 = a11; f.det = det; f.i00 = i00; f.i01 = i01; f.i11 = i11;
-  return true;
-}
-
 // Per view (rows start[v] .. start[v+1] of rows): camera (of the first row), count, rep_row, status (6, 1, 2, else 0)
 // and, for status 0, the homography pixels ~ H (X, Y, 1) with H[8] = 1 (status 5 when it is degenerate).
 __global__ void __launch_bounds__(BS_THREADS)
@@ -398,7 +292,7 @@ __device__ __forceinline__ bool intr_chol_v(const double* g, double lam, double 
 #pragma unroll
   for (int i = 0; i < 6; ++i)
 #pragma unroll
-    for (int j = i; j < 6; ++j) h[res_ut(i, j)] = g[ut16(9 + i, 9 + j)] * (i == j ? 1.0 + lam : 1.0);
+    for (int j = i; j < 6; ++j) h[ut<6>(i, j)] = g[ut<16>(9 + i, 9 + j)] * (i == j ? 1.0 + lam : 1.0);
   return res_chol6(h, 0.0, L);
 }
 
@@ -411,21 +305,21 @@ __device__ __forceinline__ void intr_schur(const double* g, double lam, double* 
     const bool ok = intr_chol_v(g, lam, L);
     double y[6];
 #pragma unroll
-    for (int k = 0; k < 6; ++k) y[k] = g[ut16(i, 9 + k)];
+    for (int k = 0; k < 6; ++k) y[k] = g[ut<16>(i, 9 + k)];
     res_chol6_solve(L, y);
     for (int j = i; j < 9; ++j) {
-      double s = g[ut16(i <= j ? i : j, j)];
+      double s = g[ut<16>(i <= j ? i : j, j)];
 #pragma unroll
-      for (int k = 0; k < 6; ++k) s -= y[k] * g[ut16(j, 9 + k)];
-      con[ut9(i, j)] = ok ? s : __longlong_as_double(0x7ff8000000000000LL);
+      for (int k = 0; k < 6; ++k) s -= y[k] * g[ut<16>(j, 9 + k)];
+      con[ut<9>(i, j)] = ok ? s : __longlong_as_double(0x7ff8000000000000LL);
     }
-    double rh = g[ut16(i, 15)];
+    double rh = g[ut<16>(i, 15)];
 #pragma unroll
-    for (int k = 0; k < 6; ++k) rh -= y[k] * g[ut16(9 + k, 15)];
-    con[45 + i] = g[ut16(i, i)];
+    for (int k = 0; k < 6; ++k) rh -= y[k] * g[ut<16>(9 + k, 15)];
+    con[45 + i] = g[ut<16>(i, i)];
     con[54 + i] = rh;
   }
-  if (lane == 0) con[63] = g[ut16(15, 15)];
+  if (lane == 0) con[63] = g[ut<16>(15, 15)];
   __syncwarp();
 }
 
@@ -461,18 +355,18 @@ __device__ __forceinline__ void intr_reduce(cg::cluster_group& cl, const double*
   __syncthreads();
 }
 
-// 9 x 9 S (packed ut9) restricted to the free parameters (fixed rows / columns become the identity); Cholesky factor
+// 9 x 9 S (packed ut<9>) restricted to the free parameters (fixed rows / columns become the identity); Cholesky factor
 // L (lower, row-major); pivots must exceed thr (of the Jacobi-scaled matrix when scaled)
 __device__ __forceinline__ bool intr_chol9(const double* Sp, int fixed, bool scaled, double thr, double L[9][9],
                                            double* d) {
 #pragma unroll 1
-  for (int i = 0; i < 9; ++i) d[i] = ((fixed >> i) & 1) ? 1.0 : (scaled ? 1.0 / sqrt(Sp[ut9(i, i)]) : 1.0);
+  for (int i = 0; i < 9; ++i) d[i] = ((fixed >> i) & 1) ? 1.0 : (scaled ? 1.0 / sqrt(Sp[ut<9>(i, i)]) : 1.0);
   bool ok = true;
 #pragma unroll 1
   for (int j = 0; j < 9; ++j) {
     for (int i = j; i < 9; ++i) {
       const bool fx = ((fixed >> i) & 1) || ((fixed >> j) & 1);
-      double v = fx ? (i == j ? 1.0 : 0.0) : Sp[ut9(j, i)] * d[i] * d[j];
+      double v = fx ? (i == j ? 1.0 : 0.0) : Sp[ut<9>(j, i)] * d[i] * d[j];
       for (int k = 0; k < j; ++k) v -= L[i][k] * L[j][k];
       if (i == j) {
         ok = ok && v > thr;
@@ -540,7 +434,7 @@ intr_lm_kernel(IntrArgs A) {
       cost = sh.tot[63];
       double Sp[45], L[9][9], dsc[9], x[9];
       for (int k = 0; k < 45; ++k) Sp[k] = sh.tot[k];
-      for (int i = 0; i < 9; ++i) Sp[ut9(i, i)] += lam * sh.tot[45 + i];
+      for (int i = 0; i < 9; ++i) Sp[ut<9>(i, i)] += lam * sh.tot[45 + i];
       const bool ok = intr_chol9(Sp, fixed, false, 0.0, L, dsc);
       for (int i = 0; i < 9; ++i) x[i] = ((fixed >> i) & 1) ? 0.0 : -sh.tot[54 + i];
       if (ok) intr_chol9_solve(L, x);
@@ -578,9 +472,9 @@ intr_lm_kernel(IntrArgs A) {
       intr_chol_v(g, lam, L);
 #pragma unroll
       for (int k = 0; k < 6; ++k) {
-        double s = g[ut16(9 + k, 15)];
+        double s = g[ut<16>(9 + k, 15)];
 #pragma unroll
-        for (int i = 0; i < 9; ++i) s += g[ut16(i, 9 + k)] * sh.dth[i];
+        for (int i = 0; i < 9; ++i) s += g[ut<16>(i, 9 + k)] * sh.dth[i];
         dq[k] = s;
       }
       res_chol6_solve(L, dq);
@@ -709,7 +603,7 @@ intr_cov_kernel(IntrArgs A) {
     if (lane < 15) {
       double y[6];
 #pragma unroll
-      for (int k = 0; k < 6; ++k) y[k] = lane < 6 ? (k == lane ? 1.0 : 0.0) : g[ut16(lane - 6, 9 + k)];
+      for (int k = 0; k < 6; ++k) y[k] = lane < 6 ? (k == lane ? 1.0 : 0.0) : g[ut<16>(lane - 6, 9 + k)];
       res_chol6_solve(L, y);
 #pragma unroll
       for (int k = 0; k < 6; ++k) {
@@ -727,7 +621,7 @@ intr_cov_kernel(IntrArgs A) {
       }
       A.vstd[6 * (size_t)v + lane] = sqrt(s2 * (vi[7 * lane] + s));
     }
-    if (lane == 0) A.vrmse[v] = sqrt(g[ut16(15, 15)] / (A.start[v + 1] - A.start[v]));
+    if (lane == 0) A.vrmse[v] = sqrt(g[ut<16>(15, 15)] / (A.start[v + 1] - A.start[v]));
     __syncwarp();
   }
   cl.sync();

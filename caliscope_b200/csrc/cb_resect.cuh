@@ -664,9 +664,6 @@ __device__ __forceinline__ void res_rot_log(const double* R, double* r) {
   r[0] = rx; r[1] = ry; r[2] = rz;
 }
 
-// packed upper-triangle index of a symmetric 6x6
-__host__ __device__ constexpr int res_ut(int i, int j) { return i <= j ? i * 6 - i * (i - 1) / 2 + (j - i) : j * 6 - j * (j - 1) / 2 + (i - j); }
-
 // camera table entry of pose q = (r, t) with the intrinsics of entry `cam`
 __device__ __forceinline__ void res_entry(const double* cam, const double* q, double* E) {
 #pragma unroll
@@ -707,7 +704,7 @@ __device__ __forceinline__ void res_normal_eq(const double* cam, const double* q
 #pragma unroll
       for (int a = 0; a < 6; ++a) {
 #pragma unroll
-        for (int c = a; c < 6; ++c) acc[res_ut(a, c)] = fma(J[a], J[c], fma(J[6 + a], J[6 + c], acc[res_ut(a, c)]));
+        for (int c = a; c < 6; ++c) acc[ut<6>(a, c)] = fma(J[a], J[c], fma(J[6 + a], J[6 + c], acc[ut<6>(a, c)]));
         acc[21 + a] = fma(J[a], rr[0], fma(J[6 + a], rr[1], acc[21 + a]));
       }
       acc[27] = fma(rr[0], rr[0], fma(rr[1], rr[1], acc[27]));
@@ -721,7 +718,7 @@ __device__ __forceinline__ bool res_chol6(const double* h, double thr, double L[
   bool ok = true;
 #pragma unroll
   for (int j = 0; j < 6; ++j) {
-    double d = h[res_ut(j, j)];
+    double d = h[ut<6>(j, j)];
 #pragma unroll
     for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k];
     ok = ok && d > thr;
@@ -729,7 +726,7 @@ __device__ __forceinline__ bool res_chol6(const double* h, double thr, double L[
     const double il = 1.0 / L[j][j];
 #pragma unroll
     for (int i = j + 1; i < 6; ++i) {
-      double v = h[res_ut(i, j)];
+      double v = h[ut<6>(j, i)];
 #pragma unroll
       for (int k = 0; k < j; ++k) v -= L[i][k] * L[j][k];
       L[i][j] = v * il;
@@ -745,11 +742,11 @@ __device__ __forceinline__ bool res_chol6(const double* h, double thr, double L[
 __device__ __forceinline__ bool res_pd6(const double* h) {
   double s[6], hs[21], L[6][6];
 #pragma unroll
-  for (int i = 0; i < 6; ++i) s[i] = 1.0 / sqrt(h[res_ut(i, i)]);
+  for (int i = 0; i < 6; ++i) s[i] = 1.0 / sqrt(h[ut<6>(i, i)]);
 #pragma unroll
   for (int i = 0; i < 6; ++i)
 #pragma unroll
-    for (int j = i; j < 6; ++j) hs[res_ut(i, j)] = h[res_ut(i, j)] * s[i] * s[j];
+    for (int j = i; j < 6; ++j) hs[ut<6>(i, j)] = h[ut<6>(i, j)] * s[i] * s[j];
   return res_chol6(hs, TRI_PD_RTOL, L);
 }
 
@@ -823,7 +820,7 @@ res_refine_kernel(const double* __restrict__ camtab, const int* __restrict__ sta
         for (int k = 0; k < 21; ++k) A[k] = sa[k];
 #pragma unroll
         for (int k = 0; k < 6; ++k) {
-          A[res_ut(k, k)] = sa[res_ut(k, k)] * (1.0 + lam);
+          A[ut<6>(k, k)] = sa[ut<6>(k, k)] * (1.0 + lam);
           d[k] = -sa[21 + k];
         }
         res_chol6(A, 0.0, L);
@@ -911,7 +908,7 @@ res_cov_kernel(const double* __restrict__ camtab, const int* __restrict__ start,
 #pragma unroll
           for (int a = 0; a < 6; ++a)
 #pragma unroll
-            for (int c = a; c < 6; ++c) h[res_ut(a, c)] = fma(J[a], J[c], fma(J[6 + a], J[6 + c], h[res_ut(a, c)]));
+            for (int c = a; c < 6; ++c) h[ut<6>(a, c)] = fma(J[a], J[c], fma(J[6 + a], J[6 + c], h[ut<6>(a, c)]));
         if (head)
 #pragma unroll
           for (int a = 0; a < 6; ++a)
@@ -928,7 +925,7 @@ res_cov_kernel(const double* __restrict__ camtab, const int* __restrict__ start,
 #pragma unroll
         for (int a = 0; a < 6; ++a)
 #pragma unroll
-          for (int c = a; c < 6; ++c) m[res_ut(a, c)] += GS[a][0] * G[c][0] + GS[a][1] * G[c][1] + GS[a][2] * G[c][2];
+          for (int c = a; c < 6; ++c) m[ut<6>(a, c)] += GS[a][0] * G[c][0] + GS[a][1] * G[c][1] + GS[a][2] * G[c][2];
       }
     }
   }
@@ -964,7 +961,7 @@ res_cov_kernel(const double* __restrict__ camtab, const int* __restrict__ start,
     for (int c = 0; c < 6; ++c) {
       double v = 0.0;
 #pragma unroll
-      for (int k = 0; k < 6; ++k) v += m[res_ut(a, k)] * Hi[k][c];
+      for (int k = 0; k < 6; ++k) v += m[a <= k ? ut<6>(a, k) : ut<6>(k, a)] * Hi[k][c];
       T[a][c] = v;
     }
 #pragma unroll

@@ -1,5 +1,5 @@
-"""--dump-outputs of the triangulation and resection timing scripts: every output array of one call to an .npz, so the
-outputs of two builds can be compared bit for bit."""
+"""--dump-outputs of the triangulation, resection and intrinsics timing scripts: every output array of one call to an
+.npz, so the outputs of two builds can be compared bit for bit."""
 import dataclasses
 from pathlib import Path
 

@@ -1,6 +1,7 @@
 """Stage times of cb_calibrate_intrinsics (DESIGN.md 4.10), one JSON line per workload.
 
     python profiles/intrinsics_timing.py [one3000] [eight1000] [sixtyfour300] [--steps 3] [--warmup 1] [--no-cpu]
+        [--dump-outputs DIR]
 
 Workloads, all of a 54-corner (9 x 6) chessboard seen with 0.5 px noise (tests/_intrinsics_cases.py): one3000 = one
 1920 x 1080 camera with 3000 views; eight1000 = 8 cameras (two lenses alternating) with 1000 views each;
@@ -8,7 +9,8 @@ sixtyfour300 = 64 cameras with 300 views each.  Times are the CUDA events record
 (CbIntrinsicsStats), the median over --steps timed calls after --warmup; the parameter error is |theta_hat - truth| /
 std, worst over cameras and parameters.  For context only, cv2.calibrateCamera runs on 30 / 100 / 300 views of the first
 camera on one host core (a CPU library, not a baseline of the same computation).  The card's name and power limit are
-read in the same run and printed with the numbers.
+read in the same run and printed with the numbers.  --dump-outputs writes every output array of the last timed call of
+each workload to DIR/<workload>.npz.
 """
 import argparse
 import json
@@ -23,6 +25,7 @@ import numpy as np
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT))
 from caliscope_b200.intrinsics import IntrinsicsStats, calibrate_cameras  # noqa: E402
+from dump_outputs import dump_outputs  # noqa: E402
 from tests._intrinsics_cases import STRONG, WEBCAM, cv2_views, make_case  # noqa: E402
 
 WORKLOADS = {"one3000": ([WEBCAM], 3000), "eight1000": ([WEBCAM, STRONG] * 4, 1000),
@@ -62,6 +65,7 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--no-cpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None)
     a = ap.parse_args()
     name = card()
     for w in a.workloads:
@@ -75,6 +79,7 @@ def main() -> None:
             wall = (time.perf_counter() - t) * 1e3
             if i >= a.warmup:
                 times.append((st.total_ms, st.group_ms, st.start_ms, st.lm_ms, st.cov_ms, wall))
+        dump_outputs(a.dump_outputs, w, res)
         med = np.median(np.array(times), axis=0)
         line = {"workload": w, "cameras": len(lenses), "views_per_camera": nv, "rows": int(len(case.obs_cam)),
                 "total_ms": round(med[0], 3), "group_ms": round(med[1], 3), "start_ms": round(med[2], 3),
