@@ -465,6 +465,21 @@ __global__ void stereo_slots_kernel(const int* __restrict__ start, int n_groups,
   nslots[g] = n * (n - 1) / 2;
 }
 
+// Slot k of a group of n rows from key-sorted position b: k -> (i, j), i < j, row-major over the strict upper triangle;
+// rows (ra, rb) and their cameras (ca, cb) swapped so that ca <= cb
+__device__ __forceinline__ void stereo_slot(long long k, int n, int b, const int* __restrict__ rows,
+                                            const int* __restrict__ obs_cam, int& ra, int& rb, int& ca, int& cb) {
+  int i = (int)((2.0 * n - 1.0 - sqrt((2.0 * n - 1.0) * (2.0 * n - 1.0) - 8.0 * (double)k)) * 0.5);
+  while ((long long)i * (2 * n - i - 1) / 2 > k) --i;
+  while ((long long)(i + 1) * (2 * n - i - 2) / 2 <= k) ++i;
+  const int j = (int)(k - (long long)i * (2 * n - i - 1) / 2) + i + 1;
+  ra = rows[b + i];
+  rb = rows[b + j];
+  ca = obs_cam[ra];
+  cb = obs_cam[rb];
+  if (ca > cb) { int t = ca; ca = cb; cb = t; t = ra; ra = rb; rb = t; }
+}
+
 __device__ __forceinline__ double sq_res_f32(double nx, double ny, double px, double py) {
   // the reference subtracts float32 projections from float32 points and squares in float32 (:678-679)
   const float ex = (float)nx - (float)px, ey = (float)ny - (float)py;
@@ -483,14 +498,8 @@ stereo_pairs_kernel(const int* __restrict__ start, const int* __restrict__ rows,
   const int b = start[g], n = start[g + 1] - b;
   const long long s0 = slot_start[g], np = (long long)n * (n - 1) / 2;
   for (long long k = lane; k < np; k += LANES) {
-    // k -> (i, j), i < j, row-major over the strict upper triangle
-    int i = (int)((2.0 * n - 1.0 - sqrt((2.0 * n - 1.0) * (2.0 * n - 1.0) - 8.0 * (double)k)) * 0.5);
-    while ((long long)i * (2 * n - i - 1) / 2 > k) --i;
-    while ((long long)(i + 1) * (2 * n - i - 2) / 2 <= k) ++i;
-    const int j = (int)(k - (long long)i * (2 * n - i - 1) / 2) + i + 1;
-    int ra = rows[b + i], rb = rows[b + j];
-    int ca = obs_cam[ra], cb = obs_cam[rb];
-    if (ca > cb) { int t = ca; ca = cb; cb = t; t = ra; ra = rb; rb = t; }
+    int ra, rb, ca, cb;
+    stereo_slot(k, n, b, rows, obs_cam, ra, rb, ca, cb);
     int pid = (ca != cb) ? pair_of[(size_t)ca * n_cams + cb] : -1;
     double val = 0.0;
     if (pid >= 0) {

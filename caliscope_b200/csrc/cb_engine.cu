@@ -39,6 +39,7 @@
 #include "cb_triangulate.cuh"
 #include "cb_resect.cuh"
 #include "cb_bootstrap.cuh"
+#include "cb_relpose.cuh"
 #include "cb_intrinsics.cuh"
 #include "cb_peer.cuh"
 
@@ -3666,6 +3667,224 @@ int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam
                      obs_px, obs_on_device, threshold_px, min_inliers, max_samples, use_prior ? 1 : 0, pixel_sigma,
                      max_iter, xtol, max_groups, n_groups_out, cam_out, pose_out, cov_out, rmse_px_out, count_out,
                      n_inliers_out, rep_row_out, status_out, inlier_out, stats, device, stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// cb_relative_pose_robust after its argument checks: grouping by key, the correspondence slots sorted by pair (stable),
+// the consensus stage over (chunk, hypothesis) tiles, the refinement and the covariance
+int relpose_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x, int64_t n_obs,
+                 const int32_t* obs_cam, const int64_t* obs_key, const double* obs_px, int obs_on_device, double tau,
+                 int32_t min_inliers, int32_t max_samples, double pixel_sigma, int32_t max_iter, double xtol,
+                 int32_t max_pairs, int32_t* n_pairs_out, int32_t* cam_a_out, int32_t* cam_b_out, double* pose_out,
+                 double* cov_out, double* rmse_px_out, double* parallax_deg_out, int32_t* count_out,
+                 int32_t* n_inliers_out, int32_t* status_out, CbRelPoseStats* stats, int device, void* stream) {
+  const char* who = "cb_relative_pose_robust";
+  TriCams cams;
+  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, who, &cams));
+  CB_TRY(select_device(device));
+  *n_pairs_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf(st);
+  const int n = (int)n_obs;
+  StageEvents<8> ev;
+  CB_TRY(ev.create());
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  std::vector<double> rp_cam((size_t)cb::RP_CAM * n_cams, 0.0);  // 1 / fx^2, 1 / fy^2, fisheye
+  for (int c = 0; c < n_cams; ++c) {
+    rp_cam[cb::RP_CAM * c] = 1.0 / (cams.tab[c].fx * cams.tab[c].fx);
+    rp_cam[cb::RP_CAM * c + 1] = 1.0 / (cams.tab[c].fy * cams.tab[c].fy);
+    rp_cam[cb::RP_CAM * c + 2] = cams.tab[c].fisheye;
+  }
+  const double* d_rpcam = nullptr;
+  CB_TRY(to_device(rp_cam.data(), rp_cam.size(), 0, &d_rpcam, sf, st));
+  ObsGroups g;
+  int32_t n_groups = 0;  // every group has room: the call's outputs are per camera pair
+  CB_TRY(obs_group_stage(n_cams, &cams.tab, n, obs_cam, obs_key, obs_px, obs_on_device, INT32_MAX, &n_groups, who,
+                         ev[1], sf, st, &g));
+
+  // correspondence slots of every key (cb_stereo_rmse's), sorted by pair (stable: key order, then (i, j))
+  long long *d_nslots = nullptr, *d_slot_start = nullptr;
+  CB_TRY(sf.alloc(&d_nslots, (size_t)n_groups + 1));
+  CB_TRY(sf.alloc(&d_slot_start, (size_t)n_groups + 1));
+  CB_CUDA(cudaMemsetAsync(d_nslots, 0, sizeof(long long) * ((size_t)n_groups + 1), st));
+  CB_LAUNCH(cb::stereo_slots_kernel, cdiv(n_groups, 256), 256, 0, st, g.start, n_groups, d_nslots);
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_nslots, d_slot_start, n_groups + 1, st);
+  g_launches.fetch_add(2);
+  long long total = 0;
+  CB_CUDA(cudaMemcpyAsync(&total, d_slot_start + n_groups, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (total > 0x7fffffffLL) {
+    g_last_error = std::string(who) + ": more than 2^31 - 1 row pairs within keys";
+    return CB_E_INVALID;
+  }
+  if (total == 0) return CB_OK;
+  const int m = (int)total;
+  unsigned int *d_k = nullptr, *d_ks = nullptr, *d_uk = nullptr;
+  unsigned long long *d_v = nullptr, *d_vs = nullptr;
+  int *d_len = nullptr, *d_nruns = nullptr;
+  CB_TRY(sf.alloc(&d_k, (size_t)m));
+  CB_TRY(sf.alloc(&d_ks, (size_t)m));
+  CB_TRY(sf.alloc(&d_v, (size_t)m));
+  CB_TRY(sf.alloc(&d_vs, (size_t)m));
+  with_lanes((n / std::max(n_groups, 1) > 12) ? 32 : 8, [&](auto L) {
+    CB_LAUNCH(cb::rp_slots_kernel<L.value>, cdiv((long long)n_groups * L.value, cb::BS_THREADS), cb::BS_THREADS, 0, st,
+              g.start, g.rows, g.cam, n_groups, (const long long*)d_slot_start, (int)n_cams, d_k, d_v);
+  });
+  CB_CUDA(cudaGetLastError());
+  const unsigned int none = (unsigned int)n_cams * (unsigned int)n_cams;
+  const int kbits = bits_for((unsigned long long)none);
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, d_v, d_vs, m, 0, kbits, st);
+  g_launches.fetch_add(2 * ((kbits + 7) / 8));
+  const size_t max_runs = std::min<size_t>((size_t)m, (size_t)none + 1);
+  CB_TRY(sf.alloc(&d_uk, max_runs));
+  CB_TRY(sf.alloc(&d_len, max_runs));
+  CB_TRY(sf.alloc(&d_nruns, 1));
+  CB_CUB(sf, cub::DeviceRunLengthEncode::Encode, d_ks, d_uk, d_len, d_nruns, m, st);
+  g_launches.fetch_add(2);
+  int nruns = 0;
+  CB_CUDA(cudaMemcpyAsync(&nruns, d_nruns, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  std::vector<unsigned int> uk(nruns);
+  std::vector<int> len(nruns);
+  CB_CUDA(cudaMemcpyAsync(uk.data(), d_uk, sizeof(unsigned int) * nruns, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(len.data(), d_len, sizeof(int) * nruns, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  const int n_pairs = (nruns > 0 && uk[nruns - 1] == none) ? nruns - 1 : nruns;  // the one-camera slots sort last
+  *n_pairs_out = n_pairs;
+  if (n_pairs > max_pairs) {
+    g_last_error = std::string(who) + ": " + std::to_string(n_pairs) + " pairs but room for " + std::to_string(max_pairs);
+    return CB_E_INVALID;
+  }
+  if (n_pairs == 0) return CB_OK;
+  std::vector<int> h_start(n_pairs + 1, 0), h_a(n_pairs), h_b(n_pairs);
+  for (int p = 0; p < n_pairs; ++p) {
+    h_start[p + 1] = h_start[p] + len[p];
+    h_a[p] = (int)(uk[p] / (unsigned int)n_cams);
+    h_b[p] = (int)(uk[p] % (unsigned int)n_cams);
+  }
+  const int nc = h_start[n_pairs];  // correspondences
+  const int *d_start = nullptr, *d_a = nullptr, *d_b = nullptr;
+  CB_TRY(to_device(h_start.data(), h_start.size(), 0, &d_start, sf, st));
+  CB_TRY(to_device(h_a.data(), h_a.size(), 0, &d_a, sf, st));
+  CB_TRY(to_device(h_b.data(), h_b.size(), 0, &d_b, sf, st));
+  double* d_xy4 = nullptr;
+  int* d_pos = nullptr;
+  CB_TRY(sf.alloc(&d_xy4, 4 * (size_t)nc));
+  CB_TRY(sf.alloc(&d_pos, (size_t)nc));
+  CB_LAUNCH(cb::rp_gather_kernel, cdiv(nc, 256), 256, 0, st, d_vs, g.cam, g.xy, d_rpcam, (long long)nc, d_xy4);
+  CB_LAUNCH(cb::tri_iota_kernel, cdiv(nc, 256), 256, 0, st, d_pos, (long long)nc);
+  CB_CUDA(cudaStreamSynchronize(st));  // the host vectors above are stack-lifetime uploads
+
+  // consensus: hypothesis table, (chunk, hypothesis) tiles, selection, classification, compaction
+  const int S = cb::RP_SLOTS_PER_SAMPLE * max_samples;
+  Consensus cs;
+  CB_TRY(consensus_alloc(n_pairs, nc, cb::RP_HYP, false, sf, st, &cs));
+  CB_CUDA(cudaEventRecord(ev[2], st));
+  double *d_tab = nullptr, *d_part = nullptr;
+  int *d_nchunk = nullptr, *d_choff = nullptr, *d_best = nullptr;
+  CB_TRY(sf.alloc(&d_tab, (size_t)n_pairs * S * cb::RP_HYP));
+  CB_TRY(sf.alloc(&d_nchunk, (size_t)n_pairs + 1));
+  CB_TRY(sf.alloc(&d_choff, (size_t)n_pairs + 1));
+  CB_TRY(sf.alloc(&d_best, (size_t)n_pairs));
+  CB_CUDA(cudaFuncSetAttribute(cb::rp_hyp_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, cb::RP_HYP_SMEM));
+  CB_LAUNCH(cb::rp_hyp_kernel, cdiv((long long)n_pairs * max_samples, cb::RP_HYP_THREADS), cb::RP_HYP_THREADS,
+            cb::RP_HYP_SMEM, st, d_start, d_xy4, n_pairs, max_samples, min_inliers, d_tab);
+  CB_LAUNCH(cb::res_chunks_kernel, cdiv(n_pairs + 1, 256), 256, 0, st, d_start, n_pairs, d_nchunk);
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_nchunk, d_choff, n_pairs + 1, st);
+  g_launches.fetch_add(2);
+  int n_chunks = 0;
+  CB_CUDA(cudaMemcpyAsync(&n_chunks, d_choff + n_pairs, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  CB_TRY(sf.alloc(&d_part, (size_t)n_chunks * S));
+  CB_LAUNCH(cb::rp_score_kernel, dim3(n_chunks, cdiv(S, cb::RES_SCORE_THREADS)), cb::RES_SCORE_THREADS, 0, st, d_start,
+            d_choff, d_xy4, d_a, d_b, d_rpcam, n_pairs, S, d_tab, tau, d_part);
+  CB_LAUNCH(cb::res_select_kernel, n_pairs, cb::RES_SCORE_THREADS, 0, st, d_choff, S, d_part, d_best);
+  CB_LAUNCH(cb::rp_classify_kernel, cdiv((long long)n_pairs * 32, cb::TRI_THREADS), cb::TRI_THREADS, 0, st, d_start,
+            d_pos, d_xy4, d_a, d_b, d_rpcam, n_pairs, S, d_tab, d_best, tau, min_inliers, cs.hyp, cs.count, cs.nin,
+            cs.status, cs.flag, cs.inl);
+  CB_CUDA(cudaGetLastError());
+  CB_TRY(consensus_compact(d_pos, nc, n_pairs, sf, st, &cs));
+  CB_CUDA(cudaEventRecord(ev[3], st));
+
+  // refinement on the consensus sets from the winners
+  const int lanes = tri_lanes(nc, n_pairs);
+  const int blocks = cdiv((long long)n_pairs * lanes, cb::TRI_THREADS);
+  double *d_pose = nullptr, *d_rmse = nullptr, *d_par = nullptr;
+  int* d_status = nullptr;
+  CB_TRY(sf.alloc(&d_pose, 6 * (size_t)n_pairs));
+  CB_TRY(sf.alloc(&d_rmse, (size_t)n_pairs));
+  CB_TRY(sf.alloc(&d_par, (size_t)n_pairs));
+  CB_TRY(sf.alloc(&d_status, (size_t)n_pairs));
+  CB_CUDA(cudaEventRecord(ev[4], st));
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::rp_refine_kernel<L.value>, blocks, cb::TRI_THREADS, 0, st, cs.start, cs.rows, d_xy4, d_a, d_b,
+              d_rpcam, n_pairs, cs.status, cs.hyp, max_iter, xtol, d_pose, d_rmse, d_par, d_status);
+  });
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaEventRecord(ev[5], st));
+  double* d_cov = nullptr;
+  if (cov_out) {
+    CB_TRY(sf.alloc(&d_cov, 36 * (size_t)n_pairs));
+    CB_CUDA(cudaEventRecord(ev[6], st));
+    with_lanes(lanes, [&](auto L) {
+      CB_LAUNCH(cb::rp_cov_kernel<L.value>, blocks, cb::TRI_THREADS, 0, st, cs.start, cs.rows, d_xy4, d_a, d_b, d_rpcam,
+                n_pairs, d_status, d_pose, pixel_sigma * pixel_sigma, d_cov);
+    });
+    CB_CUDA(cudaGetLastError());
+    CB_CUDA(cudaEventRecord(ev[7], st));
+  }
+  std::memcpy(cam_a_out, h_a.data(), sizeof(int) * n_pairs);
+  std::memcpy(cam_b_out, h_b.data(), sizeof(int) * n_pairs);
+  CB_CUDA(cudaMemcpyAsync(pose_out, d_pose, sizeof(double) * 6 * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(parallax_deg_out, d_par, sizeof(double) * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, cs.count, sizeof(int) * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(n_inliers_out, cs.nin, sizeof(int) * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
+  if (cov_out) CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 36 * (size_t)n_pairs, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (stats) {
+    stats->group_ms = ev.ms(0, 1);
+    stats->consensus_ms = ev.ms(2, 3);
+    stats->refine_ms = ev.ms(4, 5);
+    if (cov_out) stats->cov_ms = ev.ms(6, 7);
+    stats->total_ms = ev.ms(0, cov_out ? 7 : 5);
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cb_relative_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                            int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const double* obs_px,
+                            int obs_on_device, double threshold_px, int32_t min_inliers, int32_t max_samples,
+                            double pixel_sigma, int32_t max_iter, double xtol, int32_t max_pairs, int32_t* n_pairs_out,
+                            int32_t* cam_a_out, int32_t* cam_b_out, double* pose_out, double* cov_out,
+                            double* rmse_px_out, double* parallax_deg_out, int32_t* count_out, int32_t* n_inliers_out,
+                            int32_t* status_out, CbRelPoseStats* stats, int device, void* stream) {
+  if (n_cams <= 0 || n_cams > 46340 || !cam_flags || !cam_const || !cam_x || n_obs < 0 || n_obs > 0x7fffffffLL ||
+      !n_pairs_out || max_pairs < 0 || (n_obs > 0 && (!obs_cam || !obs_key || !obs_px)) ||
+      (max_pairs > 0 && (!cam_a_out || !cam_b_out || !pose_out || !rmse_px_out || !parallax_deg_out || !count_out ||
+                         !n_inliers_out || !status_out)) ||
+      !(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma)) || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol)) ||
+      !(threshold_px > 0.0 && std::isfinite(threshold_px)) || min_inliers < 5 || max_samples < 1 ||
+      max_samples > 4096) {
+    g_last_error = "cb_relative_pose_robust: bad argument";
+    return CB_E_INVALID;
+  }
+  return relpose_impl(n_cams, cam_flags, cam_const, cam_x, n_obs, obs_cam, obs_key, obs_px, obs_on_device, threshold_px,
+                      min_inliers, max_samples, pixel_sigma, max_iter, xtol, max_pairs, n_pairs_out, cam_a_out,
+                      cam_b_out, pose_out, cov_out, rmse_px_out, parallax_deg_out, count_out, n_inliers_out, status_out,
+                      stats, device, stream);
 }
 
 }  // extern "C"

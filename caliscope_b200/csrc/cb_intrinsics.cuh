@@ -293,7 +293,7 @@ __device__ __forceinline__ bool intr_chol_v(const double* g, double lam, double 
   for (int i = 0; i < 6; ++i)
 #pragma unroll
     for (int j = i; j < 6; ++j) h[ut<6>(i, j)] = g[ut<16>(9 + i, 9 + j)] * (i == j ? 1.0 + lam : 1.0);
-  return res_chol6(h, 0.0, L);
+  return res_chol<6>(h, 0.0, L);
 }
 
 // The view's Schur contribution at damping lam into con: row i of S_v = U_v - W_v V_lam^-1 W_v^T on lane i < 9, diag
@@ -306,7 +306,7 @@ __device__ __forceinline__ void intr_schur(const double* g, double lam, double* 
     double y[6];
 #pragma unroll
     for (int k = 0; k < 6; ++k) y[k] = g[ut<16>(i, 9 + k)];
-    res_chol6_solve(L, y);
+    res_chol_solve<6>(L, y);
     for (int j = i; j < 9; ++j) {
       double s = g[ut<16>(i <= j ? i : j, j)];
 #pragma unroll
@@ -477,7 +477,7 @@ intr_lm_kernel(IntrArgs A) {
         for (int i = 0; i < 9; ++i) s += g[ut<16>(i, 9 + k)] * sh.dth[i];
         dq[k] = s;
       }
-      res_chol6_solve(L, dq);
+      res_chol_solve<6>(L, dq);
       double dq2 = 0.0, q2 = 0.0;
 #pragma unroll
       for (int k = 0; k < 6; ++k) {
@@ -604,7 +604,7 @@ intr_cov_kernel(IntrArgs A) {
       double y[6];
 #pragma unroll
       for (int k = 0; k < 6; ++k) y[k] = lane < 6 ? (k == lane ? 1.0 : 0.0) : g[ut<16>(lane - 6, 9 + k)];
-      res_chol6_solve(L, y);
+      res_chol_solve<6>(L, y);
 #pragma unroll
       for (int k = 0; k < 6; ++k) {
         if (lane < 6) vi[6 * k + lane] = y[k];

@@ -33,43 +33,53 @@ __device__ __forceinline__ long long res_triples(int k) {
   return k >= (1 << 20) ? (1LL << 62) : (long long)k * (k - 1) * (k - 2) / 6;
 }
 
-// Positions i < j < l of candidate sample m of a group of k rows, T = C(k, 3): the lexicographic rank m when
-// T <= max_samples, else the first three distinct of splitmix64(m 2^32 + t) mod k, t = 0, 1, ..., sorted (false after
-// RES_DRAWS draws without three).  splitmix64(x) = mix(x + 0x9e3779b97f4a7c15), tri_mix's finaliser.
-__device__ __forceinline__ bool res_sample(long long m, long long T, int max_samples, int k, int& i, int& j, int& l) {
+// Positions p[0] < ... < p[S-1] of candidate sample m of a group of k rows, T = C(k, S): the lexicographic rank m when
+// T <= max_samples, else the first S distinct of splitmix64(m 2^32 + t) mod k, t = 0, 1, ..., sorted (false after
+// RES_DRAWS draws without S).  splitmix64(x) = mix(x + 0x9e3779b97f4a7c15), tri_mix's finaliser.  Resection samples
+// S = 3 rows, the relative pose S = 5 correspondences.
+template <int S>
+__device__ __forceinline__ bool res_sample(long long m, long long T, int max_samples, int k, int (&p)[S]) {
   if (T <= max_samples) {
     long long r = m;
-    for (i = 0;; ++i) {
-      const long long c = (long long)(k - 1 - i) * (k - 2 - i) / 2;
-      if (r < c) break;
-      r -= c;
+    int i = -1;
+#pragma unroll
+    for (int s = 0; s < S; ++s) {
+      for (i = i + 1;; ++i) {
+        long long c = 1;  // C(k - 1 - i, S - 1 - s): the subsets with p[s] = i
+#pragma unroll
+        for (int q = 0; q < S - 1 - s; ++q) c = c * (k - 1 - i - q) / (q + 1);
+        if (r < c) break;
+        r -= c;
+      }
+      p[s] = i;
     }
-    for (j = i + 1;; ++j) {
-      const long long c = k - 1 - j;
-      if (r < c) break;
-      r -= c;
-    }
-    l = j + 1 + (int)r;
     return true;
   }
-  int a = -1, b = -1, c = -1;
+  int got = 0;
 #pragma unroll 1
-  for (int t = 0; t < RES_DRAWS; ++t) {
+  for (int t = 0; t < RES_DRAWS && got < S; ++t) {
     const int v = (int)(tri_mix(((unsigned long long)m << 32) + (unsigned long long)t, 0x9e3779b97f4a7c15ULL) %
                         (unsigned long long)k);
-    if (a < 0) {
-      a = v;
-    } else if (v != a && b < 0) {
-      b = v;
-    } else if (v != a && v != b) {
-      c = v;
-      break;
+    bool dup = false;
+#pragma unroll
+    for (int q = 0; q < S; ++q) dup = dup || (q < got && p[q] == v);
+    if (!dup) {
+#pragma unroll
+      for (int q = 0; q < S; ++q)
+        if (q == got) p[q] = v;
+      ++got;
     }
   }
-  if (c < 0) return false;
-  i = min(a, min(b, c));
-  l = max(a, max(b, c));
-  j = a + b + c - i - l;
+  if (got < S) return false;
+#pragma unroll
+  for (int a = 1; a < S; ++a)
+#pragma unroll
+    for (int q = a; q > 0; --q)
+      if (p[q - 1] > p[q]) {
+        const int tmp = p[q];
+        p[q] = p[q - 1];
+        p[q - 1] = tmp;
+      }
   return true;
 }
 
@@ -430,10 +440,10 @@ res_consensus_kernel(const double* __restrict__ camtab, const int* __restrict__ 
       continue;
     }
     const long long m = task - 1;
-    int i, j, l;
-    if (!res_sample(m, T, max_samples, k, i, j, l)) continue;
+    int p[3];
+    if (!res_sample<3>(m, T, max_samples, k, p)) continue;
     double y[3][3], x[3][3];
-    if (!res_sample_inputs(rows, obs_pt, obs_xy, pts, b, i, j, l, y, x)) continue;
+    if (!res_sample_inputs(rows, obs_pt, obs_xy, pts, b, p[0], p[1], p[2], y, x)) continue;
     P3PDepths d;
     res_p3p_depths(y, x, d);
     double Xi[9];
@@ -493,10 +503,10 @@ __global__ void res_hyp_kernel(const double* __restrict__ camtab, const int* __r
   double* o = tab + (size_t)RES_HYP * (size_t)(g * S + 1 + RES_SLOTS_PER_SAMPLE * m);
   const long long T = res_triples(k);
   bool any = false;
-  int i, j, l;
+  int p[3];
   double y[3][3], x[3][3];
-  if (k >= 4 && m < T && res_sample(m, T, max_samples, k, i, j, l) &&
-      res_sample_inputs(rows, obs_pt, obs_xy, pts, b, i, j, l, y, x)) {
+  if (k >= 4 && m < T && res_sample<3>(m, T, max_samples, k, p) &&
+      res_sample_inputs(rows, obs_pt, obs_xy, pts, b, p[0], p[1], p[2], y, x)) {
     any = true;
     P3PDepths d;
     res_p3p_depths(y, x, d);
@@ -713,20 +723,21 @@ __device__ __forceinline__ void res_normal_eq(const double* cam, const double* q
   group_sum<LANES>(acc);
 }
 
-// Cholesky factor L (row-major lower, 6x6) of packed symmetric h; returns whether every pivot exceeds `thr`
-__device__ __forceinline__ bool res_chol6(const double* h, double thr, double L[6][6]) {
+// Cholesky factor L (row-major lower, N x N) of packed symmetric h; returns whether every pivot exceeds `thr`
+template <int N>
+__device__ __forceinline__ bool res_chol(const double* h, double thr, double L[N][N]) {
   bool ok = true;
 #pragma unroll
-  for (int j = 0; j < 6; ++j) {
-    double d = h[ut<6>(j, j)];
+  for (int j = 0; j < N; ++j) {
+    double d = h[ut<N>(j, j)];
 #pragma unroll
     for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k];
     ok = ok && d > thr;
     L[j][j] = sqrt(d);
     const double il = 1.0 / L[j][j];
 #pragma unroll
-    for (int i = j + 1; i < 6; ++i) {
-      double v = h[ut<6>(j, i)];
+    for (int i = j + 1; i < N; ++i) {
+      double v = h[ut<N>(j, i)];
 #pragma unroll
       for (int k = 0; k < j; ++k) v -= L[i][k] * L[j][k];
       L[i][j] = v * il;
@@ -739,31 +750,33 @@ __device__ __forceinline__ bool res_chol6(const double* h, double thr, double L[
 
 // H positive definite: every Cholesky pivot of the Jacobi-scaled D^-1/2 H D^-1/2 above TRI_PD_RTOL (radians and metres
 // mix in H, so the raw pivots have no common scale)
-__device__ __forceinline__ bool res_pd6(const double* h) {
-  double s[6], hs[21], L[6][6];
+template <int N>
+__device__ __forceinline__ bool res_pd(const double* h) {
+  double s[N], hs[N * (N + 1) / 2], L[N][N];
 #pragma unroll
-  for (int i = 0; i < 6; ++i) s[i] = 1.0 / sqrt(h[ut<6>(i, i)]);
+  for (int i = 0; i < N; ++i) s[i] = 1.0 / sqrt(h[ut<N>(i, i)]);
 #pragma unroll
-  for (int i = 0; i < 6; ++i)
+  for (int i = 0; i < N; ++i)
 #pragma unroll
-    for (int j = i; j < 6; ++j) hs[ut<6>(i, j)] = h[ut<6>(i, j)] * s[i] * s[j];
-  return res_chol6(hs, TRI_PD_RTOL, L);
+    for (int j = i; j < N; ++j) hs[ut<N>(i, j)] = h[ut<N>(i, j)] * s[i] * s[j];
+  return res_chol<N>(hs, TRI_PD_RTOL, L);
 }
 
 // (L L^T) x = v in place
-__device__ __forceinline__ void res_chol6_solve(const double L[6][6], double* v) {
+template <int N>
+__device__ __forceinline__ void res_chol_solve(const double L[N][N], double* v) {
 #pragma unroll
-  for (int i = 0; i < 6; ++i) {
+  for (int i = 0; i < N; ++i) {
     double a = v[i];
 #pragma unroll
     for (int k = 0; k < i; ++k) a -= L[i][k] * v[k];
     v[i] = a / L[i][i];
   }
 #pragma unroll
-  for (int i = 5; i >= 0; --i) {
+  for (int i = N - 1; i >= 0; --i) {
     double a = v[i];
 #pragma unroll
-    for (int k = i + 1; k < 6; ++k) a -= L[k][i] * v[k];
+    for (int k = i + 1; k < N; ++k) a -= L[k][i] * v[k];
     v[i] = a / L[i][i];
   }
 }
@@ -802,7 +815,7 @@ res_refine_kernel(const double* __restrict__ camtab, const int* __restrict__ sta
   {
     double acc[28];
     res_normal_eq<LANES>(ce, q, rows, obs_pt, obs_px, pts, b, e, lane, on, acc);
-    if (on && !res_pd6(acc)) st = TRI_NOT_PD;
+    if (on && !res_pd<6>(acc)) st = TRI_NOT_PD;
     if (lane == 0)
 #pragma unroll
       for (int k = 0; k < 28; ++k) sa[k] = acc[k];
@@ -823,8 +836,8 @@ res_refine_kernel(const double* __restrict__ camtab, const int* __restrict__ sta
           A[ut<6>(k, k)] = sa[ut<6>(k, k)] * (1.0 + lam);
           d[k] = -sa[21 + k];
         }
-        res_chol6(A, 0.0, L);
-        res_chol6_solve(L, d);
+        res_chol<6>(A, 0.0, L);
+        res_chol_solve<6>(L, d);
       },
       [&](const double* qt, bool on_) {
         res_normal_eq<LANES>(ce, qt, rows, obs_pt, obs_px, pts, b, e, lane, on_, tr);
@@ -848,7 +861,7 @@ res_refine_kernel(const double* __restrict__ camtab, const int* __restrict__ sta
     double h[21];
 #pragma unroll
     for (int k = 0; k < 21; ++k) h[k] = sa[k];
-    if (!res_pd6(h)) st = TRI_NOT_PD;
+    if (!res_pd<6>(h)) st = TRI_NOT_PD;
   }
   double E[CT_SIZE];
   if (live && st == TRI_OK) res_entry(ce, q, E);
@@ -944,13 +957,13 @@ res_cov_kernel(const double* __restrict__ camtab, const int* __restrict__ start,
   }
   // H^-1 column by column, then out = s2 H^-1 + H^-1 M H^-1 (symmetrised)
   double L[6][6], Hi[6][6];
-  res_chol6(h, 0.0, L);
+  res_chol<6>(h, 0.0, L);
 #pragma unroll
   for (int c = 0; c < 6; ++c) {
     double v[6];
 #pragma unroll
     for (int k = 0; k < 6; ++k) v[k] = k == c ? 1.0 : 0.0;
-    res_chol6_solve(L, v);
+    res_chol_solve<6>(L, v);
 #pragma unroll
     for (int k = 0; k < 6; ++k) Hi[k][c] = v[k];
   }

@@ -436,6 +436,63 @@ int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam
                      int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
                      CbResectStats* stats, int device, void* stream);
 
+typedef struct CbRelPoseStats {
+  double group_ms;      /* upload + undistortion + grouping by key, the correspondence slots and their sort by pair */
+  double consensus_ms;  /* five-point hypotheses, MSAC scoring, selection and the compaction of the consensus sets */
+  double refine_ms;     /* the Levenberg-Marquardt kernel on the consensus sets */
+  double cov_ms;        /* the covariance kernel (0 without cov_out) */
+  double total_ms;
+  int32_t kernel_launches;
+  int32_t pad_;
+} CbRelPoseStats;
+
+/* Robust relative pose of every camera pair from 2-D correspondences alone (DESIGN.md section 4.11).  Cameras in the
+ * bundle-adjustment layout as cb_triangulate_refine; only the intrinsics are read (s, k1, k2 of a free-intrinsics
+ * block), the extrinsics are ignored.  Observations (raw pixels) are host arrays or, with obs_on_device, device
+ * pointers (obs_cam, obs_key, obs_px); rows with equal obs_key (int64 >= 0) are one world point.  Pixels are undistorted
+ * as cv2.undistortPoints does (float32 rounding); a row whose coordinates are not finite, or a fisheye row at OpenCV's
+ * (-1e6, -1e6) failure sentinel, is unusable.
+ *   0. correspondences: rows i < j of one key (key-sorted, caller order within a key) from different cameras are one
+ *      correspondence of the pair (a, b), a < b (camera slots), its a-row camera a's.  A pair's correspondences are
+ *      ordered by key, then (i, j), k of them at positions 0..k-1 (cb_stereo_rmse's slot order).  Every pair with a
+ *      correspondence is reported, in ascending (a, b).  More than 2^31 - 1 row pairs within keys (the slots before
+ *      same-camera pairs are dropped; sum over keys of n (n - 1) / 2): CB_E_INVALID.
+ *   1. k < min_inliers: status 1.
+ *   2. candidate samples, T = C(k, 5): every 5-subset in lexicographic order when T <= max_samples; else sample m draws
+ *      splitmix64(m 2^32 + t) mod k, t = 0, 1, ..., keeps the first five distinct, sorted, gives up after 16 draws.
+ *   3. hypotheses of a sample of five usable correspondences: Nister's five-point solver on the normalised coordinates
+ *      (null space of the 5 x 9 epipolar system, the 10 x 20 cubic constraints, Gauss-Jordan, every real root of the
+ *      degree-10 polynomial by Sturm bisection and a Newton polish), up to 10 E.  Each E gives (R1, t), (R1, -t), (R2, t),
+ *      (R2, -t), |t| = 1; the first that puts the five points at positive depth in both cameras (least squares of
+ *      [R x_a, -x_b] (la, lb)^T = -t, la, lb > 0) is the hypothesis, slot 10 m + c.
+ *   4. score (MSAC): sum over all k correspondences of min(e^2, tau^2), e the Sampson distance in undistorted pixels,
+ *      e^2 = (x_b^T E x_a)^2 / ((E x_a)_1^2 / fx_b^2 + (E x_a)_2^2 / fy_b^2 + (E^T x_b)_1^2 / fx_a^2 + (E^T x_b)_2^2 / fy_a^2),
+ *      E = [t]x R (cv2.sampsonDistance with F = K_b^-T E K_a^-1); an unusable correspondence or a non-finite e adds
+ *      tau^2.  The lowest score wins, the lowest slot on a tie.
+ *   5. consensus set: the usable correspondences with e^2 <= tau^2 and positive depths at the winner.  No hypothesis or
+ *      fewer than min_inliers: status 5 (pose, cov, rmse, parallax NaN; n_inliers 0).
+ *   6. Levenberg-Marquardt over q = (r, alpha, beta) on the consensus set: r the winner's R as a rotation vector
+ *      (theta in [0, pi]), t = normalize(t0 + alpha u1 + beta u2), u1, u2 columns 1 and 2 of the Householder reflector
+ *      taking t0 to -+e3 (fixed at the start); residual the signed Sampson distance (x_b^T E x_a) / sqrt(den) in pixels;
+ *      cb_resect_robust's loop (lambda0 1e-3, / 10, * 10, |d| <= xtol (|q| + xtol), max_iter).
+ *   7. covariance at q*: the chart re-based at t*, cov5 = pixel_sigma^2 H^-1 over (r, du), returned as the 6 x 6
+ *      J cov5 J^T over (r, t) with J = diag(I3, [u1 u2](t*)) (rank 5).
+ *   8. status, first match wins: 1;  5;  2 H not positive definite at the start or at the solution (a Cholesky pivot
+ *      <= 1e-12 of the Jacobi-scaled H; pose = the hypothesis, cov NaN);  3 max_iter reached;  4 a consensus
+ *      correspondence has a non-positive depth at q*;  0 none.
+ * Arguments: threshold_px tau finite > 0, min_inliers >= 5, 1 <= max_samples <= 4096, max_iter >= 1, finite
+ * pixel_sigma >= 0 and xtol >= 0; obs_cam in [0, n_cams), obs_key >= 0.
+ * Outputs per pair (host, room for max_pairs): cam_a, cam_b, pose[6] = (r, t) with X_b = R X_a + t and |t| = 1,
+ * cov[36] (nullable), rmse_px (Sampson, consensus set), parallax_deg (mean angle between R x_a and x_b over the consensus
+ * set), count, n_inliers, status.  No floating-point atomics: repeated calls return bit-identical outputs. */
+int cb_relative_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                            int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const double* obs_px,
+                            int obs_on_device, double threshold_px, int32_t min_inliers, int32_t max_samples,
+                            double pixel_sigma, int32_t max_iter, double xtol, int32_t max_pairs, int32_t* n_pairs_out,
+                            int32_t* cam_a_out, int32_t* cam_b_out, double* pose_out, double* cov_out,
+                            double* rmse_px_out, double* parallax_deg_out, int32_t* count_out, int32_t* n_inliers_out,
+                            int32_t* status_out, CbRelPoseStats* stats, int device, void* stream);
+
 typedef struct CbIntrinsicsStats {
   double group_ms;  /* upload + validation + radix sort + view boundaries */
   double start_ms;  /* view statuses, homographies, Zhang's start, undistortion, IPPE poses */
