@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from oracle.relative_pose import relative_poses_robust as oracle_relpose
-from tests._relpose_cases import scene
+from tests._relpose_cases import assert_report, compare, scene
 
 pytestmark = pytest.mark.gpu
 
@@ -16,24 +16,6 @@ def _run(*a, **k):
     from caliscope_b200.epipolar import relative_poses_robust
 
     return relative_poses_robust(*a, **k)
-
-
-def _check(dev, orc):
-    assert (dev.cam_a == orc.cam_a).all() and (dev.cam_b == orc.cam_b).all()
-    assert (dev.count == orc.count).all()
-    for p in range(len(dev.status)):
-        tie = np.isfinite(orc.second[p]) and orc.second[p] - orc.best[p] <= 1e-9 * max(1.0, orc.best[p])
-        if tie:
-            continue
-        assert dev.status[p] == orc.status[p], p
-        assert dev.n_inliers[p] == orc.n_inliers[p], p
-        if orc.status[p] in (0, 2, 3, 4):
-            np.testing.assert_allclose(dev.pose[p], orc.pose[p], rtol=0, atol=1e-8)
-            np.testing.assert_allclose(dev.rmse_px[p], orc.rmse_px[p], rtol=1e-8, atol=1e-10)
-            np.testing.assert_allclose(dev.parallax_deg[p], orc.parallax_deg[p], rtol=1e-8, atol=1e-10)
-        if orc.status[p] in (0, 3, 4):
-            scale = np.abs(orc.cov[p]).max()
-            np.testing.assert_allclose(dev.cov[p], orc.cov[p], rtol=0, atol=1e-8 * scale)
 
 
 CASES = {
@@ -52,7 +34,7 @@ def test_device_matches_oracle(name):
     flags, const, x, cam, key, px, *_ = scene(**c)
     dev = _run(flags, const, cam, key, px, cam_x=x, threshold_px=3.0, **kw)
     orc = oracle_relpose(flags, const, x, cam, key, px, threshold_px=3.0, **kw)
-    _check(dev, orc)
+    assert_report(compare(dev, orc), name)
     if name == "below-min-inliers":
         assert (dev.status == 1).all()
     else:

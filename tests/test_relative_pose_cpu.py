@@ -154,3 +154,64 @@ def test_candidate_samples_are_sorted_distinct(k):
     for s in O.candidate_samples(k, 64):
         if s is not None:
             assert list(s) == sorted(set(s)) and len(s) == 5 and max(s) < k
+
+
+def _split_bank():
+    from tests._relpose_cases import pair_bank
+
+    fams = ["general", "sideways", "forward", "planar", "tiny", "rotation", "facing-y", "facing-oblique", "wild",
+            "general", "sideways", "general"]  # fmt: skip
+    lenses = ["pinhole", "fisheye", "sentinel", "free"]
+    specs = [dict(family=f, k=9 + 3 * i, noise_px=0.5 if i % 3 else 0.0, lens=lenses[i % 4], nan_rows=i % 2,
+                  outlier_frac=0.4 if f == "wild" else 0.0, sentinel=2) for i, f in enumerate(fams)]  # fmt: skip
+    return pair_bank(specs, seed=21)
+
+
+def test_bank_split_matches_the_whole_call():
+    """The oracle of every bank pair alone, cameras renumbered (0, 1) and run in a process pool, equals the oracle of
+    the whole call field for field: the pairs of a bank share no correspondence and their order does not matter."""
+    from tests._relpose_cases import oracle_bank
+
+    bank = _split_bank()
+    kw = dict(threshold_px=3.0, min_inliers=6, max_samples=8)
+    whole = O.relative_poses_robust(*bank.args(), **kw)
+    split = oracle_bank(bank, **kw)
+    assert len(whole.status) == len(bank.family) == 12
+    for f in ("cam_a", "cam_b", "pose", "cov", "cov5", "rmse_px", "parallax_deg", "count", "n_inliers", "status", "best",
+              "second"):  # fmt: skip
+        assert np.array_equal(getattr(whole, f), getattr(split, f), equal_nan=True), f
+    assert all(np.array_equal(a, b) for a, b in zip(whole.inlier, split.inlier, strict=True))
+    assert len(set(whole.status.tolist())) >= 2
+
+
+def test_bank_families_reach_their_edges():
+    """facing-y / facing-oblique: the five-point hypothesis nearest the truth takes rot_log's s < 1e-5 branch (rotation
+    at pi); sideways: the oracle's t_z takes both signs across seeds (the Householder chart's reflection flips);
+    sentinel: the planted rows are OpenCV's (-1e6, -1e6) before usable_coordinates and unusable (NaN) after it."""
+    from oracle.triangulation_robust import undistorted_coordinates
+    from tests._relpose_cases import pair_bank
+
+    for fam in ("facing-y", "facing-oblique"):
+        for seed in range(3):
+            bank = pair_bank([dict(family=fam, k=12)], seed=seed)
+            flags, const, x, cam, key, px = bank.args()
+            norm = O.usable_coordinates(flags, const, x, cam, px)
+            (ra, rb), = O.correspondences(cam, key).values()
+            hyps = [h for h in O.hypothesis(norm[ra[:5]], norm[rb[:5]]) if h is not None]
+            R = min(hyps, key=lambda h: np.abs(h[0] - bank.R[0]).max())[0]
+            assert np.abs(R - bank.R[0]).max() < 1e-5  # float32 coordinates, five points
+            s = np.linalg.norm([R[2, 1] - R[1, 2], R[0, 2] - R[2, 0], R[1, 0] - R[0, 1]]) / 2
+            assert s < 1e-5 and np.trace(R) < -0.99, (fam, seed, s)
+    tz = []
+    for seed in range(6):
+        bank = pair_bank([dict(family="sideways", k=30, noise_px=0.5)], seed=seed)
+        assert bank.t[0, 2] == 0.0
+        res = O.relative_poses_robust(*bank.args(), threshold_px=3.0, min_inliers=6, max_samples=8)
+        tz.append(res.pose[0, 5])
+    assert min(tz) < 0 < max(tz), tz
+    bank = pair_bank([dict(family="general", k=40, lens="sentinel", sentinel=5)], seed=4)
+    flags, const, x, cam, key, px = bank.args()
+    raw = undistorted_coordinates(flags, const, x, cam, px)
+    sent = (raw == -1e6).all(axis=1)
+    assert sent.sum() == 5 and (cam[sent] == 1).all() and (flags[1] & 2)
+    assert np.isnan(O.usable_coordinates(flags, const, x, cam, px)[sent]).all()
