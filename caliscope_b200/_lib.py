@@ -177,6 +177,10 @@ SYMBOLS = {
     "cb_ba_last_error": (C.c_char_p, []),
     "cb_ba_default_options": (None, [C.POINTER(Options)]),
     "cb_ba_problem_create": (C.c_int, [C.POINTER(ProblemDesc), C.c_int, _P, C.POINTER(_P)]),
+    "cb_ba_problem_create_fixed": (
+        C.c_int,
+        [C.POINTER(ProblemDesc), C.c_int32, _P, C.c_int32, _P, C.c_int, _P, C.POINTER(_P)],
+    ),
     "cb_ba_problem_destroy": (C.c_int, [_P]),
     "cb_ba_problem_n_params": (C.c_int64, [_P]),
     "cb_ba_problem_stat": (C.c_double, [_P, C.c_int]),

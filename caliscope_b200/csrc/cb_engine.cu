@@ -554,8 +554,10 @@ struct Kernels {
 
 // P: camera stride (6, or 9 with free intrinsics).  pt_lanes, dups, cam_in_smem: lanes per point, repeated (camera,
 // point) rows present, camera table staged in shared memory (point pass and back-substitution).  pcg_mode 1: slab
-// streamed from L2, 2: slab in registers with pcg_cl columns per lane.
-static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, int pcg_mode, int pcg_cl) {
+// streamed from L2, 2: slab in registers with pcg_cl columns per lane.  fixc, fixp: the problem holds camera parameters /
+// points fixed (DESIGN §4.12); without either, the problem runs exactly the kernels it ran before fixed sets existed.
+static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, int pcg_mode, int pcg_cl, bool fixc,
+                              bool fixp) {
   Kernels k;
   auto with_stride = [&](auto f) { if (P == 6) f(std::integral_constant<int, 6>{}); else f(std::integral_constant<int, 9>{}); };
   auto with_bool = [](bool b, auto f) { if (b) f(std::true_type{}); else f(std::false_type{}); };
@@ -568,8 +570,11 @@ static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, 
     k.trial_reduce = cb::trial_reduce_kernel<S>;
     k.schur_finalize = cb::schur_finalize_kernel<S>;
     k.schur_finalize_peer = cb::schur_finalize_peer_kernel<S>;
-    k.reduced_prep = cb::reduced_prep_kernel<S>;
-    k.small_rig_step = cb::small_rig_step_kernel<S>;
+    with_bool(fixc, [&](auto fc) {
+      constexpr bool FC = decltype(fc)::value;
+      k.reduced_prep = cb::reduced_prep_kernel<S, FC>;
+      k.small_rig_step = cb::small_rig_step_kernel<S, FC>;
+    });
     k.comp_build = cb::comp_build_kernel<S>;
     k.cov_point = cb::cov_point_kernel<S>;
     with_lanes(pt_lanes, [&](auto lanes) {
@@ -577,11 +582,14 @@ static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, 
       k.pt_stage_bytes = cb::pt_stage_bytes<S, L>();
       with_bool(cam_in_smem, [&](auto sm) {
         constexpr bool SM = decltype(sm)::value;
-        k.pt_backsub = cb::pt_backsub_kernel<S, L, SM>;
-        with_bool(dups, [&](auto d) {
-          constexpr bool D = decltype(d)::value;
-          k.pt_pass = cb::pt_pass_kernel<S, L, D, SM>;
-          k.pt_pass_cov = cb::pt_pass_kernel<S, L, D, SM, true>;
+        with_bool(fixp, [&](auto fp) {
+          constexpr bool FP = decltype(fp)::value;
+          k.pt_backsub = cb::pt_backsub_kernel<S, L, SM, FP>;
+          with_bool(dups, [&](auto d) {
+            constexpr bool D = decltype(d)::value;
+            k.pt_pass = cb::pt_pass_kernel<S, L, D, SM, false, FP>;
+            k.pt_pass_cov = cb::pt_pass_kernel<S, L, D, SM, true, FP>;
+          });
         });
       });
     });
@@ -626,6 +634,12 @@ struct CbBaProblem {
   int n_items = 0, n_slots = 0;
   CUtensorMap zt_map{};  // d_Zt for the product's dense-path feed (Zt is allocated once and never moves)
   unsigned char* d_active = nullptr;
+  // fixed camera parameters (caller's x indices, as given) and fixed points (DESIGN §4.12); d_fixc: the camera parameters
+  // as internal slot indices, d_fixp: the points
+  std::vector<int> h_fixc_x, h_fixp;
+  int *d_fixc = nullptr, *d_fixp = nullptr;
+  int n_fixc = 0;
+  bool has_fixed() const { return n_fixc > 0 || !h_fixp.empty(); }
   double *d_lo = nullptr, *d_hi = nullptr;
   int bounds_for = -1;  // use_bounds value d_lo / d_hi hold (-1: not uploaded yet)
   // work buffers (index [2]: current / trial point, selected on the device by LmState::cur)
@@ -1013,7 +1027,7 @@ int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const 
   }
   if (!p->direct_solve && !cov)
     CB_LAUNCH(p->k.reduced_prep, 1, 256, 0, st, p->d_state, p->nP, p->n_cams, p->red_slots, p->d_red, p->d_Dc2,
-              p->d_active, p->d_Minv, p->d_gmax, p->d_sc);
+              p->d_active, p->d_Minv, p->d_gmax, p->d_sc, (const int*)p->d_fixc, p->n_fixc);
   return CB_OK;
 }
 
@@ -1022,7 +1036,7 @@ int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st) {
   if (p->direct_solve) {
     CB_LAUNCH(p->k.small_rig_step, 1, cb::DIRECT_THREADS, p->direct_smem, st, p->d_state, p->nP, p->n_cams,
               p->red_slots, p->d_red, p->d_Dc2, p->d_active, p->d_gmax, p->d_sc, p->m_xc(), p->d_dc, p->d_lo, p->d_hi,
-              p->d_cam_flags, p->d_cam_const, p->m_camtab());
+              p->d_cam_flags, p->d_cam_const, p->m_camtab(), (const int*)p->d_fixc, p->n_fixc);
   } else {
     CB_TRY(launch_pcg(p, p->d_state, 0.0, 0, st));  // tolerance and iteration cap come from the device state
     CB_LAUNCH(cb::cam_step_kernel, 1, 256, 0, st, (const cb::LmState*)p->d_state, p->nP, p->n_cams, p->P, p->m_xc(), p->d_dc,
@@ -1066,6 +1080,9 @@ int upload_x(CbBaProblem* p, const double* x, cudaStream_t st, bool fresh = fals
   const cb::FreshState z = fresh ? cb::FreshState{p->d_gmax, p->d_counter, p->d_sc, p->d_Dc2, p->d_Dp2} : cb::FreshState{};
   CB_LAUNCH(cb::unpack_x_kernel, cdiv(n, 256), 256, 0, st, p->d_x, p->d_cam_xoff, p->d_cam_flags, p->d_cam_const,
             p->n_cams, p->P, p->n_pts, p->ncp, p->d_xc[0], p->d_xp4[0], z);
+  if (!p->h_fixp.empty())
+    CB_LAUNCH(cb::mark_fixed_points_kernel, cdiv((int)p->h_fixp.size(), 256), 256, 0, st, (const int*)p->d_fixp,
+              (int)p->h_fixp.size(), p->d_xp4[0]);
   return CB_OK;
 }
 
@@ -1354,7 +1371,9 @@ int reserve_smem(const void* kernel, size_t bytes) {
 // cam_in_smem, i.e. build_indices)
 int choose_pcg_config(CbBaProblem* p) {
   const int nP = p->nP, P = p->P;
-  auto kernels = [&](int mode, int cl) { return select_kernels(P, p->pt_lanes, p->n_dups != 0, p->cam_in_smem != 0, mode, cl); };
+  auto kernels = [&](int mode, int cl) {
+    return select_kernels(P, p->pt_lanes, p->n_dups != 0, p->cam_in_smem != 0, mode, cl, p->n_fixc > 0, !p->h_fixp.empty());
+  };
   p->k = kernels(p->pcg_mode, p->pcg_cl);  // the PCG variant is settled by try_config below
   int max_optin = 0;
   cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, p->device);
@@ -1965,7 +1984,9 @@ static int build_components(CbBaProblem* p, const CbBaProblemDesc* d, cudaStream
   return CB_OK;
 }
 
-static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_t st, CbBaProblem* p) {
+// fixc_x: fixed camera parameters (caller's x indices), fixp: fixed points; both checked by the caller
+static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_t st, CbBaProblem* p,
+                               const std::vector<int>& fixc_x, const std::vector<int>& fixp) {
   NvtxRange nvtx_create("cb_ba_problem_create (upload + index build)");
   // CB_PROFILE_CREATE=1: host wall-clock of the stages of problem creation on stderr (diagnostic)
   const bool prof = std::getenv("CB_PROFILE_CREATE") != nullptr;
@@ -2004,6 +2025,8 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   p->nP = p->n_cams * p->P;
   p->ncp = p->h_cam_off[p->n_cams];
   p->n_params = p->ncp + 3 * p->n_pts;
+  p->h_fixc_x = fixc_x; p->h_fixp = fixp;
+  p->n_fixc = (int)fixc_x.size();
   p->n_blk = cdiv(p->nP, cb::SY_TILE);
   p->LD = p->n_blk * cb::SY_TILE;
   p->n_tiles = p->n_blk * (p->n_blk + 1) / 2;
@@ -2111,6 +2134,20 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   std::vector<unsigned char> act((size_t)p->nP, 0);
   for (int c = 0; c < p->n_cams; ++c)
     for (int a = 0; a < ((p->h_iflags[c] & CB_CAM_FREE_INTRINSICS) ? 9 : 6); ++a) act[(size_t)c * p->P + a] = 1;
+  if (p->has_fixed()) {
+    std::vector<int> fc(p->n_fixc);
+    for (int i = 0; i < p->n_fixc; ++i) {  // caller's x index -> internal slot index
+      const int xi = p->h_fixc_x[i];
+      const int c = (int)(std::upper_bound(p->h_cam_off.begin(), p->h_cam_off.end(), xi) - p->h_cam_off.begin()) - 1;
+      fc[i] = p->h_slot[c] * p->P + (xi - p->h_cam_off[c]);
+      act[(size_t)fc[i]] = 0;
+    }
+    CB_TRY(palloc(p, &p->d_fixc, std::max(p->n_fixc, 1)));
+    CB_TRY(palloc(p, &p->d_fixp, std::max(p->h_fixp.size(), (size_t)1)));
+    if (p->n_fixc) CB_CUDA(cudaMemcpyAsync(p->d_fixc, fc.data(), sizeof(int) * fc.size(), cudaMemcpyHostToDevice, st));
+    if (!p->h_fixp.empty())
+      CB_CUDA(cudaMemcpyAsync(p->d_fixp, p->h_fixp.data(), sizeof(int) * p->h_fixp.size(), cudaMemcpyHostToDevice, st));
+  }
   CB_TRY(palloc(p, &p->d_active, p->nP));
   CB_CUDA(cudaMemcpyAsync(p->d_active, act.data(), p->nP, cudaMemcpyHostToDevice, st));
   CB_CUDA(cudaStreamSynchronize(st));
@@ -2171,6 +2208,12 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
 }
 
 int cb_ba_problem_create(const CbBaProblemDesc* d, int device, void* stream, CbBaProblem** out) {
+  return cb_ba_problem_create_fixed(d, 0, nullptr, 0, nullptr, device, stream, out);
+}
+
+int cb_ba_problem_create_fixed(const CbBaProblemDesc* d, int32_t n_fixed_cam_params, const int32_t* fixed_cam_params,
+                               int32_t n_fixed_pts, const int32_t* fixed_pts, int device, void* stream,
+                               CbBaProblem** out) {
   if (d && d->n_obs == 0) {
     // CaptureVolume._validate_geometry (capture_volume.py:97-98) rejects this before optimize() can run
     g_last_error = "No image observations provided";
@@ -2187,8 +2230,47 @@ int cb_ba_problem_create(const CbBaProblemDesc* d, int device, void* stream, CbB
     return CB_E_INVALID;
   }
   *out = nullptr;
+  // the fixed sets, checked on the host before any device work
+  if (n_fixed_cam_params < 0 || n_fixed_pts < 0 || (n_fixed_cam_params > 0 && !fixed_cam_params) ||
+      (n_fixed_pts > 0 && !fixed_pts)) {
+    g_last_error = "cb_ba_problem_create_fixed: bad fixed-parameter list";
+    return CB_E_INVALID;
+  }
+  long long ncp = 0;
+  for (int c = 0; c < d->n_cams; ++c) ncp += (d->cam_flags[c] & CB_CAM_FREE_INTRINSICS) ? 9 : 6;
+  auto check_set = [](const int32_t* v, int n, long long lim, const char* what) -> int {
+    std::vector<char> seen((size_t)lim, 0);
+    for (int i = 0; i < n; ++i) {
+      if (v[i] < 0 || v[i] >= lim || seen[(size_t)v[i]]) {
+        g_last_error = std::string("cb_ba_problem_create_fixed: ") + what + " index " + std::to_string(v[i]) +
+                       (v[i] < 0 || v[i] >= lim ? " is out of range" : " is repeated");
+        return CB_E_INVALID;
+      }
+      seen[(size_t)v[i]] = 1;
+    }
+    return CB_OK;
+  };
+  CB_TRY(check_set(fixed_cam_params, n_fixed_cam_params, ncp, "fixed camera parameter"));
+  CB_TRY(check_set(fixed_pts, n_fixed_pts, d->n_pts, "fixed point"));
+  if (n_fixed_cam_params == ncp && n_fixed_pts == d->n_pts) {
+    g_last_error = "cb_ba_problem_create_fixed: every parameter is fixed";
+    return CB_E_INVALID;
+  }
+  if (n_fixed_pts > 0 && d->n_constraints > 0) {
+    std::vector<char> fixed((size_t)d->n_pts, 0);
+    for (int i = 0; i < n_fixed_pts; ++i) fixed[fixed_pts[i]] = 1;
+    for (long long k = 0; k < 4ll * d->n_constraints; ++k)
+      for (const int32_t* g : {d->groups_a, d->groups_b})
+        if (g[k] >= 0 && g[k] < d->n_pts && fixed[g[k]]) {
+          g_last_error = "cb_ba_problem_create_fixed: fixed point " + std::to_string(g[k]) +
+                         " is in a rigid-distance constraint row (constraint components are eliminated jointly)";
+          return CB_E_UNSUPPORTED;
+        }
+  }
   CbBaProblem* p = new CbBaProblem();
-  int rc = problem_create_impl(d, device, (cudaStream_t)stream, p);
+  int rc = problem_create_impl(d, device, (cudaStream_t)stream, p,
+                               std::vector<int>(fixed_cam_params, fixed_cam_params + n_fixed_cam_params),
+                               std::vector<int>(fixed_pts, fixed_pts + n_fixed_pts));
   if (rc != CB_OK) {
     std::string keep = g_last_error;
     cb_ba_problem_destroy(p);
@@ -2207,6 +2289,10 @@ int cb_ba_solve_from(CbBaProblem* p, const CbBaOptions* opt, const double* x0, d
                      void* stream) {
   if (!p || !opt || !x0 || !x_out || !result) { g_last_error = "cb_ba_solve: null argument"; return CB_E_INVALID; }
   if (opt->loss < 0 || opt->loss > CB_LOSS_ARCTAN) { g_last_error = "unknown loss id"; return CB_E_INVALID; }
+  if (sharded(opt) && p->has_fixed()) {
+    g_last_error = "cb_ba_solve: fixed parameters are not supported in a sharded solve";
+    return CB_E_UNSUPPORTED;
+  }
   CB_CUDA(cudaSetDevice(p->device));
   cudaStream_t st = (cudaStream_t)stream;
   // with an all-reduce hook the caller shards by constraint component (distributed.shard_points), so every
@@ -2365,6 +2451,7 @@ static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs,
   CB_CUDA(cudaStreamSynchronize(st));
   std::vector<char> is_fixed((size_t)p->ncp, 0);
   for (int i = 0; i < n_fixed; ++i) is_fixed[fixed[i]] = 1;
+  for (int xi : p->h_fixc_x) is_fixed[xi] = 1;  // the problem's own fixed camera parameters
   std::vector<unsigned char> fr((size_t)nP, 0);
   std::vector<int> xidx((size_t)nP, -1);  // caller x index of each internal slot (-1: padding)
   long long n_masked = 0, n_fix = 0;
@@ -2448,7 +2535,7 @@ static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs,
   for (int j = 0; j < p->n_pts; ++j)
     if (rank[j] >= 0) null_pts += 3 - rank[j];
   const long long m = 2ll * p->n_obs + p->n_c;
-  const long long rk = (long long)p->n_params - n_fix - n_masked - null_pts;
+  const long long rk = (long long)p->n_params - n_fix - n_masked - null_pts - 3ll * (long long)p->h_fixp.size();
   const long long dof = m - rk;
   const double s2 = vf > 0.0 ? vf : (dof > 0 ? 2.0 * cost / (double)dof : std::nan(""));
   if (s2_out) *s2_out = s2;
@@ -2471,6 +2558,8 @@ static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs,
   CB_CUDA(cudaEventElapsedTime(&p->cov_ms[0], p->ev0, p->ev1));
   CB_CUDA(cudaEventElapsedTime(&p->cov_ms[1], p->ev1, p->ev2));
   CB_CUDA(cudaEventElapsedTime(&p->cov_ms[2], p->ev2, p->ev3));
+  if (pt_cov)  // fixed points (rank -2) are constants: zero covariance
+    for (int j : p->h_fixp) std::fill(pt_cov + 9 * (size_t)j, pt_cov + 9 * (size_t)j + 9, 0.0);
   if (cam_cov) {
     // caller layout: NaN rows / columns for the cameras without observations, zero for the fixed parameters
     const size_t ncp = (size_t)p->ncp;
@@ -2728,7 +2817,7 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
     d2.groups_a = p->h_ga.data(); d2.groups_b = p->h_gb.data(); d2.distances = p->h_cdist.data(); d2.weights = p->h_cw.data();
     CbBaProblem* q = new CbBaProblem();
     q->allocs.push_back(c_cam); q->allocs.push_back(c_pt); q->allocs.push_back(c_xy);  // owned by the new problem
-    rc = problem_create_impl(&d2, p->device, st, q);
+    rc = problem_create_impl(&d2, p->device, st, q, p->h_fixc_x, p->h_fixp);
     if (rc != CB_OK) {
       std::string keep = g_last_error;
       cb_ba_problem_destroy(q);

@@ -21,6 +21,10 @@
 //
 // The decision follows scipy's TRF bookkeeping (site-packages/scipy/optimize/_lsq/trf.py:465-560,
 // common.py:705-717): nfev / njev / nit count the same events, termination statuses 0..4 are scipy's.
+//
+// Fixed parameters (DESIGN.md §4.12) enter in two places, each behind a template flag chosen at creation: FIXC in
+// reduced_prep_body (unit rows / columns of S and zero b for fixed camera parameters, before the damping) and FIXP in
+// pt_pass_kernel / pt_backsub_kernel (a fixed point, flagged in the pad slot of xp4, has V^-1 := 0 and a zero step).
 #pragma once
 #include "cb_covariance.cuh"
 
@@ -47,6 +51,10 @@ struct LmLogRow {
 // COV: the covariance linearisation (cb_covariance.cuh).  The damping is ignored and the factor is the pseudo-inverse root R
 // of V (V^+ = R^T R, 9 values per point into Linv6, rank(V) into pt_rank, -1 for component points); Z = (Jc^T Jp) R^T,
 // t = 0, and neither Dp2 nor the gradient norm is touched.
+//
+// FIXP: the problem holds some points fixed (DESIGN §4.12); a fixed point carries 1.0 in the pad slot of xp4 (0.0
+// otherwise).  A fixed point is a constant: its factor is zero (V^-1 := 0, so Z = 0 and t = 0), its gradient is left out
+// of the gradient norm, and the covariance variant reports rank -2 for it.
 template <bool COV>
 __device__ __forceinline__ void pt_factor_rows(const double* JX, const double* Li, double& q00, double& q01, double& q02,
                                                double& q10, double& q11, double& q12) {
@@ -76,7 +84,7 @@ struct PtStage {
 template <int P, int LANES>
 constexpr size_t pt_stage_bytes() { return sizeof(PtStage<P, LANES>) * PT_WARPS * (32 / LANES); }
 
-template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false>
+template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false, bool FIXP = false>
 __global__ void __launch_bounds__(PT_WARPS * 32, 2)
 pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start, const int* __restrict__ pm_cam,
                const double2* __restrict__ pm_xy, const int* __restrict__ pt_comp, int n_pts, int n_cams,
@@ -153,11 +161,17 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
     constexpr int NL = COV ? 9 : 6;
     double Li[NL];
     int rank = -1;
+    // the flag is read again here rather than kept from the load above: live across the observation loop it costs spills
+    const bool fixed = FIXP && valid && xp4[4 * (size_t)j + 3] != 0.0;
     if (in_comp) {
 #pragma unroll
       for (int k = 0; k < NL; ++k) Li[k] = 0.0;
       if constexpr (COV) Li[0] = Li[4] = Li[8] = 1.0;
       else Li[0] = Li[2] = Li[5] = 1.0;
+    } else if (fixed) {
+#pragma unroll
+      for (int k = 0; k < NL; ++k) Li[k] = 0.0;
+      rank = -2;
     } else {
       if constexpr (COV) pinv_root3(v, Li, rank);
       else chol3_inv(v, D, lam, Li);
@@ -186,7 +200,7 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
         tvec[3 * (size_t)j + 0] = Li[0] * v[6];
         tvec[3 * (size_t)j + 1] = Li[1] * v[6] + Li[2] * v[7];
         tvec[3 * (size_t)j + 2] = Li[3] * v[6] + Li[4] * v[7] + Li[5] * v[8];
-        gm = fmax(gm, fmax(fabs(v[6]), fmax(fabs(v[7]), fabs(v[8]))));
+        if (!fixed) gm = fmax(gm, fmax(fabs(v[6]), fmax(fabs(v[7]), fabs(v[8]))));
       }
     }
     // ---- phase 2: Z = (Jc^T Jp) Linv^T per (camera, point) pair, rows 3j..3j+2 of the k-major factor.
@@ -344,8 +358,10 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
 //   dX_j = -L^-T (t_j + L^-1 u),  u = sum_obs Jp^T (Jc dc)
 // recomputed from the observation list (24 B / observation) instead of streaming the dense factor.
 // Per-CTA partial sums of the predicted reduction / step / x norms (fixed grid => deterministic).
+// FIXP: a fixed point (pad slot of xp4 non-zero) is copied to the trial buffer as it is, flag included, and adds nothing
+// to the three sums.
 // ---------------------------------------------------------------------------------------------
-template <int P, int LANES, bool CAMSM>
+template <int P, int LANES, bool CAMSM, bool FIXP = false>
 __global__ void __launch_bounds__(PT_WARPS * 32, 2)
 pt_backsub_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start, const int* __restrict__ pm_cam,
                   const double2* __restrict__ pm_xy, const int* __restrict__ pt_comp, int n_pts, int n_cams, int nP,
@@ -388,6 +404,8 @@ pt_backsub_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_sta
       ld256nc(xp4 + 4 * (size_t)j, X0, X1, X2, X3);
     }
     (void)X3;
+    const bool fixed = FIXP && valid && X3 != 0.0;
+    if (fixed) e = s;  // no observation to visit: the step is zero
     double u0 = 0.0, u1 = 0.0, u2 = 0.0;
     int cam_n = 0;
     double2 xy_n = make_double2(0.0, 0.0);
@@ -407,7 +425,11 @@ pt_backsub_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_sta
       u2 = fma(JX[2], s0, fma(JX[5], s1, u2));
     }
     u0 = group_sum<LANES>(u0); u1 = group_sum<LANES>(u1); u2 = group_sum<LANES>(u2);
-    if (valid && gl == 0) {
+    if (fixed && gl == 0) {
+      double* xn = xp4_new + 4 * (size_t)j;
+      xn[0] = X0; xn[1] = X1; xn[2] = X2; xn[3] = X3;
+      if (dp_out) { dp_out[3 * (size_t)j] = 0.0; dp_out[3 * (size_t)j + 1] = 0.0; dp_out[3 * (size_t)j + 2] = 0.0; }
+    } else if (valid && gl == 0) {
       const double* Li = Linv6 + (size_t)j * 6;
       const double w0 = Li[0] * u0, w1 = Li[1] * u0 + Li[2] * u1, w2 = Li[3] * u0 + Li[4] * u1 + Li[5] * u2;
       const double v0 = tvec[3 * (size_t)j] + w0, v1 = tvec[3 * (size_t)j + 1] + w1, v2 = tvec[3 * (size_t)j + 2] + w2;
@@ -480,14 +502,28 @@ __device__ __forceinline__ void block_inverse_one(const double* __restrict__ S, 
     }
 }
 
-template <int P, bool WANT_MINV>
+// FIXC: fixc[0..n_fixc) are fixed camera parameters (internal slot indices, DESIGN §4.12).  Before the damping their rows and
+// columns of S become unit vectors and their entries of b zero, so every solver returns a zero step for them; their active
+// bytes are clear, so the gradient norm, the step and the predicted reduction leave them out.
+template <int P, bool WANT_MINV, bool FIXC = false>
 __device__ __forceinline__ void reduced_prep_body(LmState* __restrict__ st, int nP, int n_cams, int red_slots,
                                                   double* __restrict__ red, double* __restrict__ Dc2,
                                                   const unsigned char* __restrict__ active, double* __restrict__ Minv,
-                                                  unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc) {
+                                                  unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc,
+                                                  const int* __restrict__ fixc, int n_fixc) {
   __shared__ double sh[32];
   const size_t nn = (size_t)nP * nP;
   const double lam = st->lam;
+  if constexpr (FIXC) {
+    for (int t = threadIdx.x; t < n_fixc * nP; t += blockDim.x) {
+      const int f = fixc[t / nP], i = t % nP;
+      const double v = i == f ? 1.0 : 0.0;
+      red[(size_t)f * nP + i] = v;
+      red[(size_t)i * nP + f] = v;
+    }
+    for (int t = threadIdx.x; t < n_fixc; t += blockDim.x) red[nn + fixc[t]] = 0.0;
+    __syncthreads();
+  }
   double gm = 0.0;
   for (int i = threadIdx.x; i < nP; i += blockDim.x) {
     double d = fmax(Dc2[i], red[nn + 2 * (size_t)nP + i]);  // running max; idempotent when the point is unchanged
@@ -526,13 +562,14 @@ __device__ __forceinline__ void reduced_prep_body(LmState* __restrict__ st, int 
   if constexpr (WANT_MINV)
     for (int c = threadIdx.x; c < n_cams; c += blockDim.x) block_inverse_one<P>(red, nP, c, Minv + (size_t)c * P * P);
 }
-template <int P>
+template <int P, bool FIXC = false>
 __global__ void __launch_bounds__(256)
 reduced_prep_kernel(LmState* __restrict__ st, int nP, int n_cams, int red_slots, double* __restrict__ red,
                     double* __restrict__ Dc2, const unsigned char* __restrict__ active, double* __restrict__ Minv,
-                    unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc) {
+                    unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc, const int* __restrict__ fixc,
+                    int n_fixc) {
   if (st->done) return;
-  reduced_prep_body<P, true>(st, nP, n_cams, red_slots, red, Dc2, active, Minv, gmax_bits, sc);
+  reduced_prep_body<P, true, FIXC>(st, nP, n_cams, red_slots, red, Dc2, active, Minv, gmax_bits, sc, fixc, n_fixc);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -590,16 +627,17 @@ cam_step_kernel(const LmState* __restrict__ st, int nP, int n_cams, int P, Ptr2 
 
 // Small rigs (n_camera_params <= DIRECT_MAX_N): damping + head-of-iteration tests, the direct reduced solve and the camera
 // step in ONE single-CTA kernel -- three launches and two kernel boundaries become one.
-template <int P>
+template <int P, bool FIXC = false>
 __global__ void __launch_bounds__(DIRECT_THREADS, 1)
 small_rig_step_kernel(LmState* __restrict__ st, int nP, int n_cams, int red_slots, double* __restrict__ red,
                       double* __restrict__ Dc2, const unsigned char* __restrict__ active,
                       unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc, Ptr2 xc2,
                       double* __restrict__ dc, const double* __restrict__ lo, const double* __restrict__ hi,
-                      const int* __restrict__ cam_flags, const double* __restrict__ cam_const, Ptr2 camtab2) {
+                      const int* __restrict__ cam_flags, const double* __restrict__ cam_const, Ptr2 camtab2,
+                      const int* __restrict__ fixc, int n_fixc) {
   extern __shared__ __align__(16) double dsm[];
   if (st->done) return;
-  reduced_prep_body<P, false>(st, nP, n_cams, red_slots, red, Dc2, active, nullptr, gmax_bits, sc);
+  reduced_prep_body<P, false, FIXC>(st, nP, n_cams, red_slots, red, Dc2, active, nullptr, gmax_bits, sc, fixc, n_fixc);
   __syncthreads();
   if (st->done) return;  // set by thread 0 before the barrier: gtol / max_nfev / non-finite start (uniform)
   const size_t nn = (size_t)nP * nP;

@@ -61,7 +61,8 @@ class Covariance:
 
     ``cameras``: (n_camera_params, n_camera_params) in x's camera layout; rows and columns of fixed parameters are 0,
     those of cameras without observations NaN.  ``points``: (n_pts, 3, 3), NaN where ``point_rank`` is not 3 (points
-    seen by one camera, unobserved points, points of rigid-constraint components, rank -1).  ``variance_factor``: the s2
+    seen by one camera, unobserved points, points of rigid-constraint components, rank -1); the problem's fixed points
+    have zero blocks and rank -2.  ``variance_factor``: the s2
     the inverse was scaled by; ``dof``: m - rank of the gauge-fixed Jacobian."""
 
     cameras: np.ndarray
@@ -121,9 +122,14 @@ class BAProblem:
     """
 
     def __init__(self, cam_flags, cam_const, n_pts, obs_cam, obs_pt, obs_xy, *, constraints=None, device: int = 0,
-                 stream: int = 0, cam_order=None):
+                 stream: int = 0, cam_order=None, fixed_cam_params=None, fixed_points=None):
         """``constraints``: optional ``(groups_a (n_c,4), groups_b (n_c,4), distances (n_c,), weights (n_c,))`` --
-        the rigid-distance rows of capture_volume.py:373-383 / reprojection.py:112-117."""
+        the rigid-distance rows of capture_volume.py:373-383 / reprojection.py:112-117.
+
+        ``fixed_cam_params``: indices into x's camera section (the layout ``covariance``'s ``fixed`` uses) and
+        ``fixed_points``: point indices, held at their values in x0 by every solve (DESIGN.md section 4.12): a solve is
+        the solve over the free parameters alone, and the fixed entries of its x are x0's, bit for bit.  A calibrated rig
+        held while a new camera is adjusted, surveyed points that set scale and frame, or partly known intrinsics."""
         lib = L.load()
         self._lib = lib
         self._h = None
@@ -177,8 +183,18 @@ class BAProblem:
             self.n_cams, self.n_pts, n_obs, _ptr(self.cam_flags), _ptr(self.cam_const), ptrs[0], ptrs[1], ptrs[2],
             1 if on_dev else 0, cam_bits, _ptr(order) if order is not None else None, self.n_constraints, *cons_ptrs,
         )  # fmt: skip
+        self.fixed_cam_params = np.unique(np.asarray([] if fixed_cam_params is None else fixed_cam_params, np.int64))
+        self.fixed_points = np.unique(np.asarray([] if fixed_points is None else fixed_points, np.int64))
+        fc = np.ascontiguousarray(fixed_cam_params if fixed_cam_params is not None else [], dtype=np.int32).ravel()
+        fp = np.ascontiguousarray(fixed_points if fixed_points is not None else [], dtype=np.int32).ravel()
         h = C.c_void_p()
-        L.check(lib.cb_ba_problem_create(C.byref(desc), self.device, C.c_void_p(stream), C.byref(h)), "problem_create")
+        if fixed_cam_params is None and fixed_points is None:
+            rc = lib.cb_ba_problem_create(C.byref(desc), self.device, C.c_void_p(stream), C.byref(h))
+        else:
+            rc = lib.cb_ba_problem_create_fixed(C.byref(desc), len(fc), _ptr(fc) if len(fc) else None, len(fp),
+                                                _ptr(fp) if len(fp) else None, self.device, C.c_void_p(stream),
+                                                C.byref(h))  # fmt: skip
+        L.check(rc, "problem_create")
         self._h = h
         self.cam_stride = int(lib.cb_ba_cam_stride(h))
 
@@ -285,6 +301,7 @@ class BAProblem:
         new.n_cams, new.n_pts, new.device, new.n_obs = self.n_cams, self.n_pts, self.device, int(n_kept.value)
         new.cam_offsets, new.n_camera_params, new.n_params = self.cam_offsets, self.n_camera_params, self.n_params
         new.cam_stride = self.cam_stride
+        new.fixed_cam_params, new.fixed_points = self.fixed_cam_params, self.fixed_points  # the engine keeps both sets
         new.n_constraints = self.n_constraints
         if self.n_constraints:
             new.constraints = self.constraints
@@ -314,7 +331,8 @@ class BAProblem:
     def covariance(self, x, *, loss: str = "linear", f_scale: float = 1.0, fixed=None, variance_factor=None,
                    points: bool = True, stream: int = 0) -> Covariance:
         """Covariance of the parameters at x (normally a solution of the same loss), ``cb_ba_covariance``.
-        ``fixed``: indices into x's camera section held fixed to remove the gauge; None: ``uncertainty.default_gauge``.
+        ``fixed``: indices into x's camera section held fixed to remove the gauge; None: ``uncertainty.default_gauge``,
+        or nothing on a problem with fixed parameters (``fixed_cam_params`` / ``fixed_points``), which join ``fixed``.
         ``variance_factor``: s2 (e.g. ``(pixel_sigma / fx) ** 2``); None: 2 cost / dof.  The problem must hold every
         observation (not one rank's shard)."""
         from . import uncertainty
@@ -322,7 +340,9 @@ class BAProblem:
         if loss not in L.LOSS_IDS:
             raise ValueError(f"`loss` must be one of {list(L.LOSS_IDS)}")
         x = self._x(x)
-        if fixed is None:
+        if fixed is None and (len(self.fixed_cam_params) or len(self.fixed_points)):
+            fixed = []  # the problem's own fixed parameters set the gauge; if they do not, the pivot check refuses
+        elif fixed is None:
             observed = self.error_order_stats(x, 50.0, stream, want_err=False)[3] > 0
             fixed = uncertainty.default_gauge(x, self.cam_offsets, observed, self.n_constraints > 0)
         fixed = np.ascontiguousarray(fixed, dtype=np.int32).ravel()

@@ -162,6 +162,21 @@ void cb_ba_default_options(CbBaOptions* opt);
 
 /* Upload + index build (sort by camera / by point, chunk and pair tables, constraint components). */
 int cb_ba_problem_create(const CbBaProblemDesc* desc, int device, void* stream, CbBaProblem** out);
+/* The same problem with some parameters held at their values in x0 (DESIGN.md section 4.12): every solve is the solve of
+ * the problem over the free parameters alone (scipy's least_squares on the free subvector), and the fixed entries of the
+ * returned x are bit-identical to x0.  cb_ba_problem_create is this call with both lists empty.
+ *   fixed_cam_params (host): n_fixed_cam_params indices into x's camera section, caller layout (as cb_ba_covariance's
+ *                    `fixed`).  A fixed camera parameter's rows and columns of the reduced system S are unit vectors and
+ *                    its entry of b is 0; observations still contribute to the camera's free parameters.
+ *   fixed_pts (host): n_fixed_pts point indices.  A fixed point is a known 3-D point: its observations contribute to the
+ *                    cost and the camera blocks, it has no Schur term, no step and no place in the gradient norm.
+ * CB_E_INVALID for an index out of range or repeated, or when no free parameter is left; CB_E_UNSUPPORTED for a fixed point
+ * in a rigid-distance constraint row.  All of these are refused before any device work.  cb_ba_cull's filtered problem
+ * keeps both sets; cb_ba_covariance treats the fixed camera parameters as part of its `fixed` and the fixed points as
+ * constants; a sharded cb_ba_solve (allreduce, nccl_comm or peer_group) on such a problem fails with CB_E_UNSUPPORTED. */
+int cb_ba_problem_create_fixed(const CbBaProblemDesc* desc, int32_t n_fixed_cam_params, const int32_t* fixed_cam_params,
+                               int32_t n_fixed_pts, const int32_t* fixed_pts, int device, void* stream,
+                               CbBaProblem** out);
 int cb_ba_problem_destroy(CbBaProblem* p);
 int64_t cb_ba_problem_n_params(const CbBaProblem* p);
 /* Facts about how the engine laid the problem out (measurement / diagnostics): what = 0: 1 if the Schur product walks
@@ -204,7 +219,9 @@ int cb_ba_reproj_errors_px(CbBaProblem* p, const double* x, double* err_xy, void
 
 /* Test/diagnostic access to one damped linearisation (all host outputs, any may be NULL):
  * U n_cams*P*P, gc n_cams*P, V n_pts*9, gp n_pts*3, S (n_cams*P)^2, b n_cams*P,
- * dc n_cams*P (PCG solution of S dc = -b), dp n_pts*3 (back-substituted), with P = cb_ba_cam_stride(). */
+ * dc n_cams*P (PCG solution of S dc = -b), dp n_pts*3 (back-substituted), with P = cb_ba_cam_stride().  On a problem
+ * with fixed parameters S, b, dc and dp are those the solve uses: fixed camera parameters have unit rows and columns of
+ * S before the damping, zero b and zero dc; fixed points have zero dp. */
 int cb_ba_cam_stride(const CbBaProblem* p);
 int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32_t loss, double f_scale,
                            double* cost, double* U, double* gc, double* V, double* gp, double* S, double* b,
@@ -216,7 +233,8 @@ int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32
  * through the Schur complement at lambda = 0 with the pseudo-inverse of every 3x3 point block V_j (a point seen by one
  * camera has rank(V_j) = 2, an unobserved point 0: their null directions are not parameters of F).
  *   fixed: n_fixed indices into x's camera section (caller layout), the gauge (caliscope_b200.uncertainty.default_gauge);
- *          their rows and columns of cam_cov are 0.
+ *          their rows and columns of cam_cov are 0.  The problem's own fixed camera parameters (cb_ba_problem_create_fixed)
+ *          join them; its fixed points are constants: pt_cov zero, pt_rank -2, and 3 parameters each fewer in the rank.
  *   masked: every parameter of a camera without observations; NaN rows and columns of cam_cov.
  *   variance_factor > 0: s2 as given (e.g. (pixel_sigma / fx)^2); <= 0: s2 = 2 cost / dof with dof = m - rank,
  *          m = 2 n_obs + n_c, rank = n_params - |fixed| - |masked| - sum_j (3 - rank V_j) over unconstrained points.
