@@ -10,6 +10,8 @@ import numpy as np
 import pytest
 
 from oracle.resection_robust import resect_robust as oracle_resect
+from tests._resect_bank import check as _check
+from tests._resect_bank import inlier_check as _inlier_check
 from tests._resect_cases import camera_offsets, make_rig, perturb_cameras, plant_outliers
 
 pytestmark = pytest.mark.gpu
@@ -19,41 +21,6 @@ def _resect():
     from caliscope_b200.resection import resect_robust
 
     return resect_robust
-
-
-def _check(dev, orc, *, near_tie_max=0.1):
-    """Exact count / rep_row / status / inlier equality away from near-tie scores; poses, rmse and cov to 1e-8."""
-    np.testing.assert_array_equal(dev.count, orc.count)
-    np.testing.assert_array_equal(dev.rep_row, orc.rep_row)
-    np.testing.assert_array_equal(dev.cam, orc.cam)
-    # near ties between hypotheses; a group without consensus (every hypothesis scoring k tau^2, say) has the same
-    # outputs whichever wins
-    with np.errstate(invalid="ignore"):
-        tie = np.isfinite(orc.second) & (np.abs(orc.second - orc.best) <= 1e-9 * np.maximum(1.0, np.abs(orc.best)))
-    tie &= ~np.isin(orc.status, (1, 5, 6))
-    assert tie.mean() <= near_tie_max
-    ok = ~tie
-    np.testing.assert_array_equal(dev.status[ok], orc.status[ok])
-    np.testing.assert_array_equal(dev.n_inliers[ok], orc.n_inliers[ok])
-    both = ok & np.isin(orc.status, (0, 3, 4)) & np.isin(dev.status, (0, 3, 4))
-    scale = np.maximum(1.0, np.abs(orc.pose[both]))
-    assert np.all(np.abs(dev.pose[both] - orc.pose[both]) <= 1e-8 * scale)
-    np.testing.assert_allclose(dev.rmse_px[both], orc.rmse_px[both], rtol=1e-8, atol=1e-12)
-    c_o, c_d = orc.cov[both], dev.cov[both]
-    np.testing.assert_array_equal(np.isnan(c_d), np.isnan(c_o))  # a NaN point covariance in the consensus set
-    fin = np.isfinite(c_o).all(axis=(1, 2))
-    c_o, c_d = c_o[fin], c_d[fin]
-    cs = np.maximum(np.abs(c_o).max(axis=(1, 2), keepdims=True), 1e-300)
-    assert np.all(np.abs(c_d - c_o) <= 1e-8 * cs)
-    nan_o = ~np.isin(orc.status, (0, 2, 3, 4)) & ok
-    assert np.isnan(dev.pose[nan_o]).all() and np.isnan(dev.cov[nan_o]).all()
-    return tie
-
-
-def _inlier_check(dev, orc, keys, tie):
-    _, grp = np.unique(keys, return_inverse=True)
-    rows_ok = ~tie[grp.ravel()]
-    np.testing.assert_array_equal(dev.inlier[rows_ok], orc.inlier[rows_ok])
 
 
 def _case(seed, *, n_cams=6, n_pts=40, fisheye=(), free=(), frac=0.15, frames=1, nan_pts=0, repeat=0):

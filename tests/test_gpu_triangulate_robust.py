@@ -1,6 +1,7 @@
 """cb_triangulate_robust against the NumPy oracle (oracle/triangulation_robust.py robust_points) at every shape-selected
 variant, with planted outliers: P = 6 and 9, fisheye, sampled pairs (dense groups), 8 and 32 lanes per group, same-camera
-pairs, and the camera table in and out of shared memory."""
+pairs, and the camera table in and out of shared memory; the pair table at T = max_pairs, groups with T above 2^31 and
+2^32, a long group under 8 lanes, and decisive rows at a group's first and last position."""
 import numpy as np
 import pytest
 
@@ -166,3 +167,134 @@ def test_bad_arguments_are_refused():
                                          ptr[5], ptr[6], ptr[7], None, 0, None)  # fmt: skip
         with pytest.raises(L.EngineError):
             L.check(code, "triangulate_robust")
+
+
+# ---- pair-table edges, huge groups, skewed lanes, decisive rows -------------------------------------------------------------
+def _ring(n_cams=64, seed=0):
+    """n_cams pinhole / fisheye cameras on a ring around the origin (tests/_resect_cases.make_rig's cameras)."""
+    from tests._resect_cases import make_rig
+
+    flags, const, cx, _, _, _, _ = make_rig(seed, n_cams, 1, fisheye=tuple(range(0, n_cams, 5)), free=(3, 7))
+    return flags, const, cx
+
+
+def _views(flags, const, cx, X, cams, noise, rng):
+    from oracle.ba_oracle import rodrigues
+    from oracle.resection_robust import cameras, project
+
+    cs = cameras(flags, const, cx)
+    px = np.empty((len(cams), 2))
+    for c in np.unique(cams):
+        m = cams == c
+        uv, _ = project(cs[c], rodrigues(cs[c].q[:3])[0], cs[c].q[3:6], X)
+        px[m] = uv + rng.normal(0, noise, (m.sum(), 2))
+    return px
+
+
+def _point_group(flags, const, cx, k, rng, *, noise=0.3, X=None):
+    X = rng.uniform(-0.5, 0.5, 3) if X is None else X
+    cams = np.sort(rng.choice(len(flags), k, replace=k > len(flags))).astype(np.int32)
+    rng.shuffle(cams)
+    return cams, _views(flags, const, cx, X, cams, noise, rng)
+
+
+def _lanes_of(cam):
+    return 32 if len(cam) // len(np.unique(cam)) > 96 else 8
+
+
+@pytest.mark.parametrize("k,max_pairs", [(12, 66), (12, 65), (2, 1)])
+def test_pair_table_edges(k, max_pairs):
+    """T = k (k - 1) / 2 against max_pairs: 66 at k = 12 (every pair, the table full), 65 (sampled ranks), and k = 2 at
+    max_pairs = 1; 40 groups each with 20 % outliers."""
+    flags, const, cx = _ring(16, 1)
+    rng = np.random.default_rng(k + max_pairs)
+    cam, key, px = [], [], []
+    for g in range(40):
+        c, p = _point_group(flags, const, cx, k, rng)
+        bad = rng.random(k) < 0.2
+        p[bad] += rng.uniform(20, 200, (bad.sum(), 2))
+        cam.append(c), key.append(np.full(k, g, np.int64)), px.append(p)
+    cam, key, px = np.concatenate(cam), np.concatenate(key), np.concatenate(px)
+    T = k * (k - 1) // 2
+    print(f"k {k}, max_pairs {max_pairs}: T {T}, {'every pair' if T <= max_pairs else 'sampled ranks'}, "
+          f"lanes {_lanes_of(key)}")  # fmt: skip
+    _check(flags, const, cx, cam, key, px, max_pairs=max_pairs, min_ok=0.0)
+
+
+@pytest.mark.parametrize("k", [65537, 100000])
+def test_huge_groups_rank_exactly(k):
+    """One point in k rows from 64 cameras: T = 2,147,516,416 (> 2^31 - 1) and 4,999,950,000 (> 2^32) pairs, ranks
+    floor(m T / 64).  With max_iter = 1 and 0.5 px of noise the output is one step from the selected pair's point, so
+    status, inliers and xyz show which rank won."""
+    flags, const, cx = _ring(64, 2)
+    rng = np.random.default_rng(k)
+    cam, px = _point_group(flags, const, cx, k, rng, noise=0.5)
+    bad = rng.random(k) < 0.1
+    px[bad] += rng.uniform(20, 200, (bad.sum(), 2))
+    key = np.zeros(k, np.int64)
+    T = k * (k - 1) // 2
+    assert T > (1 << 31) - 1 and (k < 100000 or T > 1 << 32)
+    out, st = _check(flags, const, cx, cam, key, px, max_pairs=64, max_iter=1, min_ok=-1.0)
+    print(f"k {k}: T {T}, sampled ranks, lanes {_lanes_of(key)}, launches {st.kernel_launches}, status {out.status}")
+    assert out.status[0] == 3
+
+
+def test_skewed_lanes():
+    """A 5000-row group among 300 two-view groups (mean ~ 18 rows: 8 lanes), and the same group alone (32 lanes)."""
+    flags, const, cx = _ring(64, 3)
+    rng = np.random.default_rng(7)
+    c0, p0 = _point_group(flags, const, cx, 5000, rng)
+    bad = rng.random(5000) < 0.15
+    p0[bad] += rng.uniform(20, 200, (bad.sum(), 2))
+    cam, key, px = [c0], [np.zeros(5000, np.int64)], [p0]
+    for g in range(300):
+        c, p = _point_group(flags, const, cx, 2, rng)
+        cam.append(c), key.append(np.full(2, g + 1, np.int64)), px.append(p)
+    cam, key, px = np.concatenate(cam), np.concatenate(key), np.concatenate(px)
+    mixed, _ = _check(flags, const, cx, cam, key, px, min_ok=0.5)
+    alone, _ = _check(flags, const, cx, c0, np.zeros(5000, np.int64), p0)
+    assert _lanes_of(key) == 8 and _lanes_of(np.zeros(5000)) == 32
+    print(f"skewed: lanes 8 with {len(np.unique(key))} groups, 32 alone; status {mixed.status[0]}, {mixed.n_inliers[0]} inliers")
+    np.testing.assert_array_equal(mixed.inlier[:5000], alone.inlier)
+    assert mixed.n_inliers[0] == alone.n_inliers[0] and mixed.status[0] == alone.status[0]
+
+
+def _decisive_group(flags, const, cx, k, at, rng):
+    """Rows of two points A and B 0.3 m apart, exact under their point (A's with 0.01 px of noise so that A's pairs do not
+    tie), A with one more row than B and A's rows at `at`: A's best pair wins by about tau^2; a score without one of A's
+    rows ties B at best, and B's exact pairs then win."""
+    XA = np.array([0.1, -0.05, 0.2])
+    XB = XA + np.array([0.0, 0.0, 0.3])
+    cam = (np.arange(k) % len(flags)).astype(np.int32)
+    rng.shuffle(cam)
+    n_a = k // 2 + 1
+    role = np.zeros(k, bool)
+    role[list(at)] = True
+    rest = np.flatnonzero(~role)
+    role[rng.choice(rest, n_a - role.sum(), replace=False)] = True
+    pa = _views(flags, const, cx, XA, cam, 0.01, rng)
+    pb = _views(flags, const, cx, XB, cam, 0.0, rng)
+    assert (np.linalg.norm(pa - pb, axis=1) > 4 * TAU).all()
+    return cam, np.where(role[:, None], pa, pb), role
+
+
+@pytest.mark.parametrize("lanes", [8, 32])
+def test_decisive_rows(lanes):
+    """The deciding row (one of A's) at the group's first and last position, in an 8-lane call (among two-view groups)
+    and a 32-lane call (alone)."""
+    flags, const, cx = _ring(64, 4)
+    rng = np.random.default_rng(lanes)
+    k = 21 if lanes == 8 else 201  # odd: A has (k + 1) / 2 rows, B one fewer
+    cam0, px0, role = _decisive_group(flags, const, cx, k, (0, k - 1), rng)
+    cam, key, px = [cam0], [np.zeros(k, np.int64)], [px0]
+    if lanes == 8:
+        for g in range(40):
+            c, p = _point_group(flags, const, cx, 2, rng)
+            cam.append(c), key.append(np.full(2, g + 1, np.int64)), px.append(p)
+    cam, key, px = np.concatenate(cam), np.concatenate(key), np.concatenate(px)
+    assert _lanes_of(key) == lanes
+    max_pairs = k * (k - 1) // 2 if lanes == 8 else 64
+    out, st = _check(flags, const, cx, cam, key, px, max_pairs=max_pairs, min_ok=0.0)
+    print(f"decisive rows: lanes {lanes}, k {k}, {'every pair' if lanes == 8 else 'sampled ranks'}, "
+          f"{out.n_inliers[0]} inliers")  # fmt: skip
+    np.testing.assert_array_equal(out.inlier[:k], role)
