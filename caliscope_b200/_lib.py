@@ -48,6 +48,19 @@ class ProblemDesc(C.Structure):
     ]
 
 
+class Priors(C.Structure):  # CbBaPriors
+    _fields_ = [
+        ("n_cams", C.c_int32),
+        ("cams", C.c_void_p),
+        ("cam_mean", C.c_void_p),
+        ("cam_info", C.c_void_p),
+        ("n_pts", C.c_int32),
+        ("pts", C.c_void_p),
+        ("pt_mean", C.c_void_p),
+        ("pt_info", C.c_void_p),
+    ]
+
+
 ALLREDUCE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p)
 
 
@@ -180,6 +193,10 @@ SYMBOLS = {
     "cb_ba_problem_create_fixed": (
         C.c_int,
         [C.POINTER(ProblemDesc), C.c_int32, _P, C.c_int32, _P, C.c_int, _P, C.POINTER(_P)],
+    ),
+    "cb_ba_problem_create_priors": (
+        C.c_int,
+        [C.POINTER(ProblemDesc), C.c_int32, _P, C.c_int32, _P, C.POINTER(Priors), C.c_int, _P, C.POINTER(_P)],
     ),
     "cb_ba_problem_destroy": (C.c_int, [_P]),
     "cb_ba_problem_n_params": (C.c_int64, [_P]),

@@ -25,8 +25,10 @@
 // Fixed parameters (DESIGN.md §4.12) enter in two places, each behind a template flag chosen at creation: FIXC in
 // reduced_prep_body (unit rows / columns of S and zero b for fixed camera parameters, before the damping) and FIXP in
 // pt_pass_kernel / pt_backsub_kernel (a fixed point, flagged in the pad slot of xp4, has V^-1 := 0 and a zero step).
+// Gaussian priors (DESIGN.md §4.13, cb_priors.cuh) enter behind PRIORC in reduced_prep_body and PRIORP in pt_pass_kernel.
 #pragma once
 #include "cb_covariance.cuh"
+#include "cb_priors.cuh"
 
 namespace cb {
 
@@ -55,6 +57,10 @@ struct LmLogRow {
 // FIXP: the problem holds some points fixed (DESIGN §4.12); a fixed point carries 1.0 in the pad slot of xp4 (0.0
 // otherwise).  A fixed point is a constant: its factor is zero (V^-1 := 0, so Z = 0 and t = 0), its gradient is left out
 // of the gradient norm, and the covariance variant reports rank -2 for it.
+//
+// PRIORP: the problem holds point priors (cb_priors.cuh); the prior of point j (pp.idx[j] >= 0) adds L_j to V_j and
+// L_j (X_j - m_j) to g_j before D, the damping and the factor are formed.  Only instantiated with FIXP (the two flags
+// combine: one more variant, not two).
 template <bool COV>
 __device__ __forceinline__ void pt_factor_rows(const double* JX, const double* Li, double& q00, double& q01, double& q02,
                                                double& q10, double& q11, double& q12) {
@@ -84,14 +90,14 @@ struct PtStage {
 template <int P, int LANES>
 constexpr size_t pt_stage_bytes() { return sizeof(PtStage<P, LANES>) * PT_WARPS * (32 / LANES); }
 
-template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false, bool FIXP = false>
+template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false, bool FIXP = false, bool PRIORP = false>
 __global__ void __launch_bounds__(PT_WARPS * 32, 2)
 pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start, const int* __restrict__ pm_cam,
                const double2* __restrict__ pm_xy, const int* __restrict__ pt_comp, int n_pts, int n_cams,
                CPtr2 camtab2, CPtr2 xp2, double* __restrict__ V6, double* __restrict__ gp,
                double* __restrict__ Dp2, double* __restrict__ Linv6, double* __restrict__ tvec,
                double* __restrict__ Zt, size_t LD, unsigned long long* __restrict__ gmax_bits,
-               int* __restrict__ pt_rank = nullptr) {
+               int* __restrict__ pt_rank, PointPriors pp) {
   extern __shared__ __align__(16) double pt_sm[];
   __shared__ double wmax[PT_WARPS];
   if (st->done) return;
@@ -151,6 +157,18 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
     }
 #pragma unroll
     for (int k = 0; k < 9; ++k) v[k] = group_sum<LANES>(v[k]);
+    if constexpr (PRIORP) {
+      const int q = valid ? pp.idx[j] : -1;
+      if (q >= 0) {
+        const double* L = pp.info + 9 * (size_t)q;
+        const double* m = pp.mean + 3 * (size_t)q;
+        const double d0 = X0 - m[0], d1 = X1 - m[1], d2 = X2 - m[2];
+        v[0] += L[0]; v[1] += L[1]; v[2] += L[2]; v[3] += L[4]; v[4] += L[5]; v[5] += L[8];
+        v[6] += fma(L[0], d0, fma(L[1], d1, L[2] * d2));
+        v[7] += fma(L[3], d0, fma(L[4], d1, L[5] * d2));
+        v[8] += fma(L[6], d0, fma(L[7], d1, L[8] * d2));
+      }
+    }
     bool pieces_only = false;
     if constexpr (!DUPS) pieces_only = ((__ballot_sync(0xffffffffu, unsorted) >> (grp * LANES)) & LMASK) != 0;
     double D[3] = {1.0, 1.0, 1.0};
@@ -505,15 +523,24 @@ __device__ __forceinline__ void block_inverse_one(const double* __restrict__ S, 
 // FIXC: fixc[0..n_fixc) are fixed camera parameters (internal slot indices, DESIGN §4.12).  Before the damping their rows and
 // columns of S become unit vectors and their entries of b zero, so every solver returns a zero step for them; their active
 // bytes are clear, so the gradient norm, the step and the predicted reduction leave them out.
-template <int P, bool WANT_MINV, bool FIXC = false>
+// PRIORC: the camera priors *cpp (cb_priors.cuh; a device pointer rather than a by-value parameter, which leaves the
+// kernels without priors their earlier SASS) at the current cameras enter S, b, the g_c slot and the diag-U slot first,
+// so a fixed parameter still ends up a unit row and its diagonal prior information still reaches Dc2.  Only instantiated
+// with FIXC (the two flags combine).
+template <int P, bool WANT_MINV, bool FIXC = false, bool PRIORC = false>
 __device__ __forceinline__ void reduced_prep_body(LmState* __restrict__ st, int nP, int n_cams, int red_slots,
                                                   double* __restrict__ red, double* __restrict__ Dc2,
                                                   const unsigned char* __restrict__ active, double* __restrict__ Minv,
                                                   unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc,
-                                                  const int* __restrict__ fixc, int n_fixc) {
+                                                  const int* __restrict__ fixc, int n_fixc, const CamPriors* __restrict__ cpp) {
   __shared__ double sh[32];
   const size_t nn = (size_t)nP * nP;
   const double lam = st->lam;
+  if constexpr (PRIORC) {
+    const CamPriors cp = *cpp;
+    add_cam_priors<P>(red, nP, cp.xc.p[st->cur], cp);
+    __syncthreads();
+  }
   if constexpr (FIXC) {
     for (int t = threadIdx.x; t < n_fixc * nP; t += blockDim.x) {
       const int f = fixc[t / nP], i = t % nP;
@@ -562,14 +589,15 @@ __device__ __forceinline__ void reduced_prep_body(LmState* __restrict__ st, int 
   if constexpr (WANT_MINV)
     for (int c = threadIdx.x; c < n_cams; c += blockDim.x) block_inverse_one<P>(red, nP, c, Minv + (size_t)c * P * P);
 }
-template <int P, bool FIXC = false>
+template <int P, bool FIXC = false, bool PRIORC = false>
 __global__ void __launch_bounds__(256)
 reduced_prep_kernel(LmState* __restrict__ st, int nP, int n_cams, int red_slots, double* __restrict__ red,
                     double* __restrict__ Dc2, const unsigned char* __restrict__ active, double* __restrict__ Minv,
                     unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc, const int* __restrict__ fixc,
-                    int n_fixc) {
+                    int n_fixc, const CamPriors* __restrict__ cp) {
   if (st->done) return;
-  reduced_prep_body<P, true, FIXC>(st, nP, n_cams, red_slots, red, Dc2, active, Minv, gmax_bits, sc, fixc, n_fixc);
+  reduced_prep_body<P, true, FIXC, PRIORC>(st, nP, n_cams, red_slots, red, Dc2, active, Minv, gmax_bits, sc, fixc, n_fixc,
+                                           cp);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -627,17 +655,18 @@ cam_step_kernel(const LmState* __restrict__ st, int nP, int n_cams, int P, Ptr2 
 
 // Small rigs (n_camera_params <= DIRECT_MAX_N): damping + head-of-iteration tests, the direct reduced solve and the camera
 // step in ONE single-CTA kernel -- three launches and two kernel boundaries become one.
-template <int P, bool FIXC = false>
+template <int P, bool FIXC = false, bool PRIORC = false>
 __global__ void __launch_bounds__(DIRECT_THREADS, 1)
 small_rig_step_kernel(LmState* __restrict__ st, int nP, int n_cams, int red_slots, double* __restrict__ red,
                       double* __restrict__ Dc2, const unsigned char* __restrict__ active,
                       unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc, Ptr2 xc2,
                       double* __restrict__ dc, const double* __restrict__ lo, const double* __restrict__ hi,
                       const int* __restrict__ cam_flags, const double* __restrict__ cam_const, Ptr2 camtab2,
-                      const int* __restrict__ fixc, int n_fixc) {
+                      const int* __restrict__ fixc, int n_fixc, const CamPriors* __restrict__ cp) {
   extern __shared__ __align__(16) double dsm[];
   if (st->done) return;
-  reduced_prep_body<P, false, FIXC>(st, nP, n_cams, red_slots, red, Dc2, active, nullptr, gmax_bits, sc, fixc, n_fixc);
+  reduced_prep_body<P, false, FIXC, PRIORC>(st, nP, n_cams, red_slots, red, Dc2, active, nullptr, gmax_bits, sc, fixc,
+                                            n_fixc, cp);
   __syncthreads();
   if (st->done) return;  // set by thread 0 before the barrier: gtol / max_nfev / non-finite start (uniform)
   const size_t nn = (size_t)nP * nP;

@@ -15,6 +15,21 @@ def _ptr(a: np.ndarray) -> int:
     return a.ctypes.data
 
 
+def _prior_arrays(priors, w: int, name: str) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """(index, mean, info) as contiguous int32 (k,), float64 (k, w), float64 (k, w, w); None: no priors."""
+    if priors is None:
+        return np.zeros(0, np.int32), np.zeros((0, w)), np.zeros((0, w, w))
+    idx, mean, info = priors
+    idx = np.ascontiguousarray(idx, dtype=np.int32).ravel()
+    mean = np.ascontiguousarray(mean, dtype=np.float64)
+    info = np.ascontiguousarray(info, dtype=np.float64)
+    k = len(idx)
+    if mean.shape != (k, w) or info.shape != (k, w, w):
+        raise ValueError(f"{name}: mean must have shape ({k}, {w}) and info ({k}, {w}, {w}), got {mean.shape} and "
+                         f"{info.shape}")  # fmt: skip
+    return idx, mean, info
+
+
 def _check_device_obs(obs_cam, obs_pt, obs_xy, device: int) -> int:
     """Validate a device-resident observation list, which the engine reads in place: CUDA tensors on ``device``,
     contiguous, equal lengths; obs_cam int32 or int16, obs_pt int32, obs_xy float64 (n, 2).  Returns obs_cam's width in
@@ -122,14 +137,21 @@ class BAProblem:
     """
 
     def __init__(self, cam_flags, cam_const, n_pts, obs_cam, obs_pt, obs_xy, *, constraints=None, device: int = 0,
-                 stream: int = 0, cam_order=None, fixed_cam_params=None, fixed_points=None):
+                 stream: int = 0, cam_order=None, fixed_cam_params=None, fixed_points=None, camera_priors=None,
+                 point_priors=None):
         """``constraints``: optional ``(groups_a (n_c,4), groups_b (n_c,4), distances (n_c,), weights (n_c,))`` --
         the rigid-distance rows of capture_volume.py:373-383 / reprojection.py:112-117.
 
         ``fixed_cam_params``: indices into x's camera section (the layout ``covariance``'s ``fixed`` uses) and
         ``fixed_points``: point indices, held at their values in x0 by every solve (DESIGN.md section 4.12): a solve is
         the solve over the free parameters alone, and the fixed entries of its x are x0's, bit for bit.  A calibrated rig
-        held while a new camera is adjusted, surveyed points that set scale and frame, or partly known intrinsics."""
+        held while a new camera is adjusted, surveyed points that set scale and frame, or partly known intrinsics.
+
+        ``camera_priors``: ``(cams (k,), mean (k, 9), info (k, 9, 9))`` and ``point_priors``: ``(points (k,), mean (k, 3),
+        info (k, 3, 3))``: Gaussian priors (DESIGN.md section 4.13), ``1/2 (x - mean)^T info (x - mean)`` added to the
+        objective whatever the loss.  A camera's mean is its slice of x (6 or 9 values, padded to 9); a 6-parameter
+        camera's info is zero outside its 6 x 6 block.  ``info`` is positive semi-definite, in the objective's units:
+        ``uncertainty.prior_information`` makes it from a covariance.  Fixed parameters and priors may share a camera."""
         lib = L.load()
         self._lib = lib
         self._h = None
@@ -187,8 +209,16 @@ class BAProblem:
         self.fixed_points = np.unique(np.asarray([] if fixed_points is None else fixed_points, np.int64))
         fc = np.ascontiguousarray(fixed_cam_params if fixed_cam_params is not None else [], dtype=np.int32).ravel()
         fp = np.ascontiguousarray(fixed_points if fixed_points is not None else [], dtype=np.int32).ravel()
+        self.camera_priors = _prior_arrays(camera_priors, 9, "camera_priors")
+        self.point_priors = _prior_arrays(point_priors, 3, "point_priors")
         h = C.c_void_p()
-        if fixed_cam_params is None and fixed_points is None:
+        if self.has_priors:
+            (ci, cm, cl), (pi, pm, pl) = self.camera_priors, self.point_priors
+            pri = L.Priors(len(ci), _ptr(ci), _ptr(cm), _ptr(cl), len(pi), _ptr(pi), _ptr(pm), _ptr(pl))
+            rc = lib.cb_ba_problem_create_priors(C.byref(desc), len(fc), _ptr(fc) if len(fc) else None, len(fp),
+                                                 _ptr(fp) if len(fp) else None, C.byref(pri), self.device,
+                                                 C.c_void_p(stream), C.byref(h))  # fmt: skip
+        elif fixed_cam_params is None and fixed_points is None:
             rc = lib.cb_ba_problem_create(C.byref(desc), self.device, C.c_void_p(stream), C.byref(h))
         else:
             rc = lib.cb_ba_problem_create_fixed(C.byref(desc), len(fc), _ptr(fc) if len(fc) else None, len(fp),
@@ -197,6 +227,10 @@ class BAProblem:
         L.check(rc, "problem_create")
         self._h = h
         self.cam_stride = int(lib.cb_ba_cam_stride(h))
+
+    @property
+    def has_priors(self) -> bool:
+        return len(self.camera_priors[0]) > 0 or len(self.point_priors[0]) > 0
 
     # -- lifetime -----------------------------------------------------------------------------
     def close(self) -> None:
@@ -302,6 +336,7 @@ class BAProblem:
         new.cam_offsets, new.n_camera_params, new.n_params = self.cam_offsets, self.n_camera_params, self.n_params
         new.cam_stride = self.cam_stride
         new.fixed_cam_params, new.fixed_points = self.fixed_cam_params, self.fixed_points  # the engine keeps both sets
+        new.camera_priors, new.point_priors = self.camera_priors, self.point_priors  # and the priors
         new.n_constraints = self.n_constraints
         if self.n_constraints:
             new.constraints = self.constraints
@@ -332,7 +367,8 @@ class BAProblem:
                    points: bool = True, stream: int = 0) -> Covariance:
         """Covariance of the parameters at x (normally a solution of the same loss), ``cb_ba_covariance``.
         ``fixed``: indices into x's camera section held fixed to remove the gauge; None: ``uncertainty.default_gauge``,
-        or nothing on a problem with fixed parameters (``fixed_cam_params`` / ``fixed_points``), which join ``fixed``.
+        or nothing on a problem with fixed parameters (``fixed_cam_params`` / ``fixed_points``), which join ``fixed``,
+        or with priors, whose information enters the inverse (the result is then the posterior covariance).
         ``variance_factor``: s2 (e.g. ``(pixel_sigma / fx) ** 2``); None: 2 cost / dof.  The problem must hold every
         observation (not one rank's shard)."""
         from . import uncertainty
@@ -340,8 +376,8 @@ class BAProblem:
         if loss not in L.LOSS_IDS:
             raise ValueError(f"`loss` must be one of {list(L.LOSS_IDS)}")
         x = self._x(x)
-        if fixed is None and (len(self.fixed_cam_params) or len(self.fixed_points)):
-            fixed = []  # the problem's own fixed parameters set the gauge; if they do not, the pivot check refuses
+        if fixed is None and (len(self.fixed_cam_params) or len(self.fixed_points) or self.has_priors):
+            fixed = []  # the problem's fixed parameters and priors set the gauge; if they do not, the pivot check refuses
         elif fixed is None:
             observed = self.error_order_stats(x, 50.0, stream, want_err=False)[3] > 0
             fixed = uncertainty.default_gauge(x, self.cam_offsets, observed, self.n_constraints > 0)

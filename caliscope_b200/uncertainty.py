@@ -112,3 +112,50 @@ def camera_poses(x, cam_offsets, cam_cov) -> list[PoseUncertainty | None]:
         blk = cam_cov[o : o + 6, o : o + 6]
         out.append(None if np.isnan(blk).any() else pose_from_extrinsics(x[o : o + 3], x[o + 3 : o + 6], blk))
     return out
+
+
+def prior_information(cov, pixel_sigma: float, fx: float) -> np.ndarray:
+    """Information matrix of a Gaussian prior (``BAProblem``'s ``camera_priors`` / ``point_priors``, DESIGN.md section
+    4.13) from a physical covariance ``cov`` (k, k): ``(pixel_sigma / fx) ** 2 * inv(cov)``, in the objective's units
+    (reprojection rows are pixels / fx_initial; exact when the cameras share one focal length).
+
+    A row and column whose variance is ``inf`` is unconstrained: its information is zero, and the rest is the inverse of
+    the remaining block.  A zero variance, or a finite block that is singular, would be an exactly known direction:
+    refused (ValueError), since that is ``fixed_cam_params`` / ``fixed_points``.  So is a ``cov`` that is not symmetric
+    to 1e-12 relative.
+
+    Intrinsics example.  x holds ``s`` with ``fx = s * fx_initial``, so from ``intrinsics.calibrate_cameras``' standard
+    deviations ``std`` (fx first) ``sigma_s = std[0] / fx_initial``; with ``k1``, ``k2`` from the same row and the pose
+    free (infinite variance)::
+
+        var = np.full(9, np.inf)
+        var[6:] = (std[0] / fx_initial) ** 2, std[4] ** 2, std[5] ** 2
+        info = prior_information(np.diag(var), pixel_sigma, fx_initial)   # (9, 9), zero outside s, k1, k2
+    """
+    cov = np.asarray(cov, dtype=np.float64)
+    if cov.ndim != 2 or cov.shape[0] != cov.shape[1]:
+        raise ValueError(f"cov must be square, got shape {cov.shape}")
+    if not (pixel_sigma > 0 and fx != 0 and np.isfinite(pixel_sigma) and np.isfinite(fx)):
+        raise ValueError("pixel_sigma must be positive and fx non-zero, both finite")
+    var = np.diag(cov)
+    if np.isnan(cov).any() or (var < 0).any() or (var == -np.inf).any():
+        raise ValueError("cov has NaN entries or negative variances")
+    if (var == 0).any():
+        raise ValueError("a zero variance is an exactly known parameter: use fixed_cam_params / fixed_points instead")
+    free = np.isfinite(var)
+    info = np.zeros_like(cov)
+    if not free.any():
+        return info
+    sub = cov[np.ix_(free, free)]
+    if not np.isfinite(sub).all():
+        raise ValueError("cov has an infinite entry outside the rows and columns of infinite variance")
+    scale = np.abs(sub).max()
+    if np.abs(sub - sub.T).max() > 1e-12 * scale:
+        raise ValueError("cov is not symmetric")
+    ev = np.linalg.eigvalsh(0.5 * (sub + sub.T))
+    if ev[0] <= 1e-12 * ev[-1]:
+        raise ValueError("cov is singular (or not positive definite) on its finite rows: an exactly known direction is "
+                         "a fixed parameter, not a prior")  # fmt: skip
+    inv = np.linalg.inv(0.5 * (sub + sub.T))
+    info[np.ix_(free, free)] = (pixel_sigma / fx) ** 2 * 0.5 * (inv + inv.T)
+    return info

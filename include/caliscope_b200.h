@@ -177,6 +177,40 @@ int cb_ba_problem_create(const CbBaProblemDesc* desc, int device, void* stream, 
 int cb_ba_problem_create_fixed(const CbBaProblemDesc* desc, int32_t n_fixed_cam_params, const int32_t* fixed_cam_params,
                                int32_t n_fixed_pts, const int32_t* fixed_pts, int device, void* stream,
                                CbBaProblem** out);
+/* Gaussian priors on chosen cameras and points (DESIGN.md section 4.13).  Each adds a quadratic term to the objective,
+ * whatever the loss:
+ *   F(x) = 1/2 sum rho(r_i^2) + 1/2 sum_c (x_c - m_c)^T L_c (x_c - m_c) + 1/2 sum_j (X_j - m_j)^T L_j (X_j - m_j),
+ * i.e. scipy's least_squares on the residuals extended by rows W (x - m) with W^T W = L that the loss leaves linear.  L
+ * is symmetric positive semi-definite (a singular L is a partial prior) and in the objective's units: reprojection rows
+ * are pixels / fx_initial, so a covariance Sigma under pixel noise sigma gives L = (sigma / fx)^2 Sigma^-1.  Host pointers,
+ * copied at creation:
+ *   cams: n_cams camera indices (caller numbering); cam_mean n_cams x 9: the camera's slice of x (6 or 9 values, the rest
+ *         ignored); cam_info n_cams x 9 x 9, row-major, zero outside the 6 x 6 block of a 6-parameter camera.
+ *   pts: n_pts point indices; pt_mean n_pts x 3; pt_info n_pts x 3 x 3, row-major. */
+typedef struct {
+  int32_t n_cams;
+  const int32_t* cams;
+  const double* cam_mean;
+  const double* cam_info;
+  int32_t n_pts;
+  const int32_t* pts;
+  const double* pt_mean;
+  const double* pt_info;
+} CbBaPriors;
+
+/* cb_ba_problem_create_fixed with Gaussian priors (priors may be NULL: cb_ba_problem_create_fixed is this call with
+ * priors = NULL).  A solve minimises F above over the free parameters; a fixed entry of a camera with a prior stays x0's,
+ * and the prior still pulls the camera's free entries through the off-diagonal of L.  Refused before any device work:
+ * CB_E_INVALID for an index out of range or repeated within its list, a non-finite mean or information entry, an L that
+ * is not symmetric to 1e-12 relative or has an eigenvalue below -1e-12 of its largest, non-zero information outside a
+ * 6-parameter camera's 6 x 6 block, or a point that is both fixed and has a prior; CB_E_UNSUPPORTED for a point prior on
+ * a point of a rigid-distance constraint row.  A sharded cb_ba_solve on a problem with priors fails with
+ * CB_E_UNSUPPORTED.  cb_ba_cull's filtered problem keeps the priors; cb_ba_normal_equations returns S, b, U, gc, V, gp
+ * and the cost with them; the cost, initial_cost and optimality of a solve include them; cb_ba_covariance inverts the
+ * reduced system with them and counts sum rank(L) more rows in m. */
+int cb_ba_problem_create_priors(const CbBaProblemDesc* desc, int32_t n_fixed_cam_params, const int32_t* fixed_cam_params,
+                                int32_t n_fixed_pts, const int32_t* fixed_pts, const CbBaPriors* priors, int device,
+                                void* stream, CbBaProblem** out);
 int cb_ba_problem_destroy(CbBaProblem* p);
 int64_t cb_ba_problem_n_params(const CbBaProblem* p);
 /* Facts about how the engine laid the problem out (measurement / diagnostics): what = 0: 1 if the Schur product walks
@@ -228,7 +262,8 @@ int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32
                            double* dc, double* dp, void* stream);
 
 /* Covariance of the parameters at x (normally a solution), DESIGN.md section 4.6.  With J the engine's residual Jacobian
- * (pixels / fx_initial, then the constraint rows) after the robust row rescaling at x:
+ * (pixels / fx_initial, then the constraint rows, then the rows W (x - m) of any priors) after the robust row rescaling
+ * at x:
  *   Sigma = s2 * (J_F^T J_F)^-1,  F = parameters neither fixed nor masked,
  * through the Schur complement at lambda = 0 with the pseudo-inverse of every 3x3 point block V_j (a point seen by one
  * camera has rank(V_j) = 2, an unobserved point 0: their null directions are not parameters of F).
@@ -237,7 +272,8 @@ int cb_ba_normal_equations(CbBaProblem* p, const double* x, double lambda, int32
  *          join them; its fixed points are constants: pt_cov zero, pt_rank -2, and 3 parameters each fewer in the rank.
  *   masked: every parameter of a camera without observations; NaN rows and columns of cam_cov.
  *   variance_factor > 0: s2 as given (e.g. (pixel_sigma / fx)^2); <= 0: s2 = 2 cost / dof with dof = m - rank,
- *          m = 2 n_obs + n_c, rank = n_params - |fixed| - |masked| - sum_j (3 - rank V_j) over unconstrained points.
+ *          m = 2 n_obs + n_c (+ sum rank(L) over the problem's priors, cb_ba_problem_create_priors),
+ *          rank = n_params - |fixed| - |masked| - sum_j (3 - rank V_j) over unconstrained points.
  *   cam_cov (nullable): n_camera_params^2, caller layout.  pt_cov (nullable): n_pts*9, NaN for points with a rank
  *          deficient V_j and for points of rigid-constraint components.  pt_rank (nullable): n_pts, rank of V_j, -1 for
  *          component points.  s2_out / dof_out nullable.
