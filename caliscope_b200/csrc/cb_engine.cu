@@ -532,12 +532,27 @@ struct TrialGraph {
   int n_kernels = 0;  // kernels of one trial
 };
 
-// A problem's Gaussian priors on the host (DESIGN §4.13), as cb_ba_problem_create_priors took them: caller camera
-// numbering, camera means n x 9 and information n x 81, point means n x 3 and information n x 9; rank: sum of rank(L).
-struct HostPriors {
+// The parameters a problem holds: fixed camera parameters and points (DESIGN §4.12) and Gaussian priors (§4.13).  The
+// host lists are as cb_ba_problem_create_priors took them: fixed camera parameters as caller's x indices, priors in caller
+// camera numbering, camera means n x 9 and information n x 81, point means n x 3 and information n x 9; rank: sum of
+// rank(L); n_prior_blk: the prior-cost partials, in extra cost slots after the constraint blocks.  upload_held fills the
+// device tables of a problem that holds anything: d_fixc the fixed camera parameters as internal slot indices, d_fixp
+// the fixed points, the prior tables (with n = 0 and an all -1 point index when there are only fixed sets, which the
+// HELD kernel variants read) and d_cpri, a device copy of cpri.
+struct HeldSet {
+  std::vector<int> fixc_x, fixp;
   std::vector<int> cam, pt;
   std::vector<double> cmean, cinfo, pmean, pinfo;
   long long rank = 0;
+  int n_prior_blk = 0;
+  int *d_fixc = nullptr, *d_fixp = nullptr;
+  cb::CamPriors cpri{};
+  cb::CamPriors* d_cpri = nullptr;
+  cb::PointPriors ppri{};
+  bool cams() const { return !fixc_x.empty() || !cam.empty(); }  // the camera side runs the HELD variants
+  bool points() const { return !fixp.empty() || !pt.empty(); }   // the point side does
+  bool priors() const { return !cam.empty() || !pt.empty(); }
+  bool any() const { return cams() || points(); }
 };
 
 // The kernel instantiations one problem launches, and the sizes that follow from the same choice.  select_kernels
@@ -562,12 +577,12 @@ struct Kernels {
 
 // P: camera stride (6, or 9 with free intrinsics).  pt_lanes, dups, cam_in_smem: lanes per point, repeated (camera,
 // point) rows present, camera table staged in shared memory (point pass and back-substitution).  pcg_mode 1: slab
-// streamed from L2, 2: slab in registers with pcg_cl columns per lane.  fixc, fixp: the problem holds camera parameters /
-// points fixed (DESIGN §4.12); priorc, priorp: it holds camera / point priors (§4.13), whose variants also handle the
-// fixed sets (one more variant per flag, not two).  Without any of these, the problem runs exactly the kernels it ran
-// before fixed sets and priors existed.
-static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, int pcg_mode, int pcg_cl, bool fixc,
-                              bool fixp, bool priorc, bool priorp) {
+// streamed from L2, 2: slab in registers with pcg_cl columns per lane.  held: the HELD variants of the camera side and
+// of the point pass where the problem holds camera parameters / points fixed or near a prior, the FIXP back-substitution
+// where it holds points fixed.  A problem that holds nothing runs exactly the kernels it ran before held parameters
+// existed.
+static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, int pcg_mode, int pcg_cl,
+                              const HeldSet& held) {
   Kernels k;
   auto with_stride = [&](auto f) { if (P == 6) f(std::integral_constant<int, 6>{}); else f(std::integral_constant<int, 9>{}); };
   auto with_bool = [](bool b, auto f) { if (b) f(std::true_type{}); else f(std::false_type{}); };
@@ -580,16 +595,11 @@ static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, 
     k.trial_reduce = cb::trial_reduce_kernel<S>;
     k.schur_finalize = cb::schur_finalize_kernel<S>;
     k.schur_finalize_peer = cb::schur_finalize_peer_kernel<S>;
-    if (priorc) {
-      k.reduced_prep = cb::reduced_prep_kernel<S, true, true>;
-      k.small_rig_step = cb::small_rig_step_kernel<S, true, true>;
-    } else {
-      with_bool(fixc, [&](auto fc) {
-        constexpr bool FC = decltype(fc)::value;
-        k.reduced_prep = cb::reduced_prep_kernel<S, FC>;
-        k.small_rig_step = cb::small_rig_step_kernel<S, FC>;
-      });
-    }
+    with_bool(held.cams(), [&](auto hc) {
+      constexpr bool HC = decltype(hc)::value;
+      k.reduced_prep = cb::reduced_prep_kernel<S, HC>;
+      k.small_rig_step = cb::small_rig_step_kernel<S, HC>;
+    });
     k.comp_build = cb::comp_build_kernel<S>;
     k.cov_point = cb::cov_point_kernel<S>;
     with_lanes(pt_lanes, [&](auto lanes) {
@@ -597,18 +607,15 @@ static Kernels select_kernels(int P, int pt_lanes, bool dups, bool cam_in_smem, 
       k.pt_stage_bytes = cb::pt_stage_bytes<S, L>();
       with_bool(cam_in_smem, [&](auto sm) {
         constexpr bool SM = decltype(sm)::value;
-        with_bool(fixp, [&](auto fp) {
-          constexpr bool FP = decltype(fp)::value;
-          k.pt_backsub = cb::pt_backsub_kernel<S, L, SM, FP>;
+        with_bool(!held.fixp.empty(), [&](auto fp) {
+          k.pt_backsub = cb::pt_backsub_kernel<S, L, SM, decltype(fp)::value>;
+        });
+        with_bool(held.points(), [&](auto hp) {
+          constexpr bool HP = decltype(hp)::value;
           with_bool(dups, [&](auto d) {
             constexpr bool D = decltype(d)::value;
-            if (priorp) {
-              k.pt_pass = cb::pt_pass_kernel<S, L, D, SM, false, true, true>;
-              k.pt_pass_cov = cb::pt_pass_kernel<S, L, D, SM, true, true, true>;
-            } else {
-              k.pt_pass = cb::pt_pass_kernel<S, L, D, SM, false, FP>;
-              k.pt_pass_cov = cb::pt_pass_kernel<S, L, D, SM, true, FP>;
-            }
+            k.pt_pass = cb::pt_pass_kernel<S, L, D, SM, false, HP>;
+            k.pt_pass_cov = cb::pt_pass_kernel<S, L, D, SM, true, HP>;
           });
         });
       });
@@ -654,20 +661,7 @@ struct CbBaProblem {
   int n_items = 0, n_slots = 0;
   CUtensorMap zt_map{};  // d_Zt for the product's dense-path feed (Zt is allocated once and never moves)
   unsigned char* d_active = nullptr;
-  // fixed camera parameters (caller's x indices, as given) and fixed points (DESIGN §4.12); d_fixc: the camera parameters
-  // as internal slot indices, d_fixp: the points
-  std::vector<int> h_fixc_x, h_fixp;
-  int *d_fixc = nullptr, *d_fixp = nullptr;
-  int n_fixc = 0;
-  bool has_fixed() const { return n_fixc > 0 || !h_fixp.empty(); }
-  // Gaussian priors (DESIGN §4.13): the host copy as given (caller numbering), the device tables (camera slots, d_pp_idx
-  // per point), the partial-cost slots after the constraint blocks in d_camcost, and sum rank(L) for the covariance's m
-  HostPriors pri;
-  cb::CamPriors cpri{};
-  cb::CamPriors* d_cpri = nullptr;  // a device copy of cpri, read by the PRIORC variants
-  cb::PointPriors ppri{};
-  int n_prior_blk = 0;
-  bool has_priors() const { return !pri.cam.empty() || !pri.pt.empty(); }
+  HeldSet held;  // fixed parameters and priors
   double *d_lo = nullptr, *d_hi = nullptr;
   int bounds_for = -1;  // use_bounds value d_lo / d_hi hold (-1: not uploaded yet)
   // work buffers (index [2]: current / trial point, selected on the device by LmState::cur)
@@ -977,7 +971,7 @@ void launch_pt_pass(CbBaProblem* p, bool cov, cudaStream_t st) {
   CB_LAUNCH(pt_pass, p->pt_grid, cb::PT_WARPS * 32, p->pt_smem, st, p->d_state,
             p->d_pt_start, p->d_pm_cam, p->d_pm_xy, p->d_pt_comp, p->n_pts, p->n_cams, p->c_camtab(), p->c_xp(),
             p->d_V6, p->d_gp, p->d_Dp2, cov ? p->d_covR : p->d_Linv6, p->d_tvec, p->d_Zt, (size_t)p->LD, p->d_gmax,
-            cov ? p->d_covRank : nullptr, p->ppri);
+            cov ? p->d_covRank : nullptr, p->held.ppri);
 }
 
 void launch_pt_backsub(CbBaProblem* p, double* dp_out, cudaStream_t st) {
@@ -1005,11 +999,12 @@ int camera_pass(CbBaProblem* p, int flip, int mode, cudaStream_t st) {
   if (p->n_c)
     CB_LAUNCH((cb::constraint_eval_kernel<false>), p->n_cblk, cb::CC_THREADS, 0, st, (const cb::LmState*)p->d_state, flip,
               p->ct, p->c_xp(), loss, fscale, p->m_crs(), p->m_cdirw(), (double*)nullptr, p->d_camcost + p->n_cams);
-  if (p->has_priors())
-    CB_LAUNCH(cb::prior_cost_kernel, p->n_prior_blk, cb::PRIOR_THREADS, 0, st, (const cb::LmState*)p->d_state, flip, p->P,
-              p->cpri, p->ppri, p->c_xp(), p->d_camcost + p->n_cams + p->n_cblk);
+  const HeldSet& h = p->held;
+  if (h.priors())
+    CB_LAUNCH(cb::prior_cost_kernel, h.n_prior_blk, cb::PRIOR_THREADS, 0, st, (const cb::LmState*)p->d_state, flip, p->P,
+              h.cpri, h.ppri, p->c_xp(), p->d_camcost + p->n_cams + p->n_cblk);
   CB_LAUNCH(p->k.trial_reduce, p->n_cams + 1, 64, 0, st, p->d_state, mode, p->n_cams, p->d_cam_chunk_start,
-            p->d_partial, p->m_Upk(), p->m_gc(), p->m_costsum(), p->d_camcost, p->n_cblk + p->n_prior_blk, p->d_bpart,
+            p->d_partial, p->m_Upk(), p->m_gc(), p->m_costsum(), p->d_camcost, p->n_cblk + h.n_prior_blk, p->d_bpart,
             p->pt_grid + p->n_comp, p->pt_grid + p->n_comp, p->d_red2, p->d_counter, p->d_sc, p->d_log);
   return CB_OK;
 }
@@ -1058,7 +1053,8 @@ int build_system(CbBaProblem* p, const CbBaOptions* opt, cudaStream_t st, const 
   }
   if (!p->direct_solve && !cov)
     CB_LAUNCH(p->k.reduced_prep, 1, 256, 0, st, p->d_state, p->nP, p->n_cams, p->red_slots, p->d_red, p->d_Dc2,
-              p->d_active, p->d_Minv, p->d_gmax, p->d_sc, (const int*)p->d_fixc, p->n_fixc, (const cb::CamPriors*)p->d_cpri);
+              p->d_active, p->d_Minv, p->d_gmax, p->d_sc, (const int*)p->held.d_fixc, (int)p->held.fixc_x.size(),
+              (const cb::CamPriors*)p->held.d_cpri);
   return CB_OK;
 }
 
@@ -1067,8 +1063,8 @@ int solve_step(CbBaProblem* p, double* dp_out, cudaStream_t st) {
   if (p->direct_solve) {
     CB_LAUNCH(p->k.small_rig_step, 1, cb::DIRECT_THREADS, p->direct_smem, st, p->d_state, p->nP, p->n_cams,
               p->red_slots, p->d_red, p->d_Dc2, p->d_active, p->d_gmax, p->d_sc, p->m_xc(), p->d_dc, p->d_lo, p->d_hi,
-              p->d_cam_flags, p->d_cam_const, p->m_camtab(), (const int*)p->d_fixc, p->n_fixc,
-              (const cb::CamPriors*)p->d_cpri);
+              p->d_cam_flags, p->d_cam_const, p->m_camtab(), (const int*)p->held.d_fixc, (int)p->held.fixc_x.size(),
+              (const cb::CamPriors*)p->held.d_cpri);
   } else {
     CB_TRY(launch_pcg(p, p->d_state, 0.0, 0, st));  // tolerance and iteration cap come from the device state
     CB_LAUNCH(cb::cam_step_kernel, 1, 256, 0, st, (const cb::LmState*)p->d_state, p->nP, p->n_cams, p->P, p->m_xc(), p->d_dc,
@@ -1112,9 +1108,10 @@ int upload_x(CbBaProblem* p, const double* x, cudaStream_t st, bool fresh = fals
   const cb::FreshState z = fresh ? cb::FreshState{p->d_gmax, p->d_counter, p->d_sc, p->d_Dc2, p->d_Dp2} : cb::FreshState{};
   CB_LAUNCH(cb::unpack_x_kernel, cdiv(n, 256), 256, 0, st, p->d_x, p->d_cam_xoff, p->d_cam_flags, p->d_cam_const,
             p->n_cams, p->P, p->n_pts, p->ncp, p->d_xc[0], p->d_xp4[0], z);
-  if (!p->h_fixp.empty())
-    CB_LAUNCH(cb::mark_fixed_points_kernel, cdiv((int)p->h_fixp.size(), 256), 256, 0, st, (const int*)p->d_fixp,
-              (int)p->h_fixp.size(), p->d_xp4[0]);
+  const std::vector<int>& fixp = p->held.fixp;
+  if (!fixp.empty())
+    CB_LAUNCH(cb::mark_fixed_points_kernel, cdiv((int)fixp.size(), 256), 256, 0, st, (const int*)p->held.d_fixp,
+              (int)fixp.size(), p->d_xp4[0]);
   return CB_OK;
 }
 
@@ -1404,8 +1401,7 @@ int reserve_smem(const void* kernel, size_t bytes) {
 int choose_pcg_config(CbBaProblem* p) {
   const int nP = p->nP, P = p->P;
   auto kernels = [&](int mode, int cl) {
-    return select_kernels(P, p->pt_lanes, p->n_dups != 0, p->cam_in_smem != 0, mode, cl, p->n_fixc > 0, !p->h_fixp.empty(),
-                          !p->pri.cam.empty(), !p->pri.pt.empty());
+    return select_kernels(P, p->pt_lanes, p->n_dups != 0, p->cam_in_smem != 0, mode, cl, p->held);
   };
   p->k = kernels(p->pcg_mode, p->pcg_cl);  // the PCG variant is settled by try_config below
   int max_optin = 0;
@@ -2017,13 +2013,19 @@ static int build_components(CbBaProblem* p, const CbBaProblemDesc* d, cudaStream
   return CB_OK;
 }
 
-// The priors' device tables (DESIGN §4.13): camera slots, widths, means and information; the per-point prior index; the
-// number of prior-cost partials.  Nothing is allocated for a problem without priors.
-static int upload_priors(CbBaProblem* p, cudaStream_t st) {
-  const HostPriors& h = p->pri;
-  const int nc = (int)h.cam.size(), np = (int)h.pt.size();
-  if (nc + np == 0) return CB_OK;
-  p->n_prior_blk = (int)cdiv(nc + np, cb::PRIOR_THREADS);
+// The held set's device tables (HeldSet), after the work buffers (the camera priors carry the camera buffers); clears
+// the active bytes of the fixed camera parameters in act.  Nothing is allocated for a problem that holds nothing.
+static int upload_held(CbBaProblem* p, std::vector<unsigned char>& act, cudaStream_t st) {
+  HeldSet& h = p->held;
+  if (!h.any()) return CB_OK;
+  const int nf = (int)h.fixc_x.size(), nc = (int)h.cam.size(), np = (int)h.pt.size();
+  std::vector<int> fc(std::max(nf, 1));
+  for (int i = 0; i < nf; ++i) {  // caller's x index -> internal slot index
+    const int xi = h.fixc_x[i];
+    const int c = (int)(std::upper_bound(p->h_cam_off.begin(), p->h_cam_off.end(), xi) - p->h_cam_off.begin()) - 1;
+    fc[i] = p->h_slot[c] * p->P + (xi - p->h_cam_off[c]);
+    act[(size_t)fc[i]] = 0;
+  }
   std::vector<int> slot(std::max(nc, 1)), width(std::max(nc, 1)), idx((size_t)p->n_pts, -1);
   for (int k = 0; k < nc; ++k) {
     slot[k] = p->h_slot[h.cam[k]];
@@ -2032,21 +2034,24 @@ static int upload_priors(CbBaProblem* p, cudaStream_t st) {
   for (int k = 0; k < np; ++k) idx[h.pt[k]] = k;
   int *d_slot, *d_width, *d_idx, *d_pt;
   double *d_cmean, *d_cinfo, *d_pmean, *d_pinfo;
+  CB_TRY(palloc(p, &h.d_fixc, fc.size())); CB_TRY(palloc(p, &h.d_fixp, std::max(h.fixp.size(), (size_t)1)));
   CB_TRY(palloc(p, &d_slot, slot.size())); CB_TRY(palloc(p, &d_width, width.size()));
   CB_TRY(palloc(p, &d_cmean, 9 * (size_t)std::max(nc, 1))); CB_TRY(palloc(p, &d_cinfo, 81 * (size_t)std::max(nc, 1)));
   CB_TRY(palloc(p, &d_idx, idx.size())); CB_TRY(palloc(p, &d_pt, (size_t)std::max(np, 1)));
   CB_TRY(palloc(p, &d_pmean, 3 * (size_t)std::max(np, 1))); CB_TRY(palloc(p, &d_pinfo, 9 * (size_t)std::max(np, 1)));
-  auto up = [&](auto* dst, const auto& src) -> int {
-    if (!src.empty()) CB_CUDA(cudaMemcpyAsync(dst, src.data(), sizeof(src[0]) * src.size(), cudaMemcpyHostToDevice, st));
+  CB_TRY(palloc(p, &h.d_cpri, 1));
+  h.cpri = cb::CamPriors{d_slot, d_width, d_cmean, d_cinfo, nc, {{p->d_xc[0], p->d_xc[1]}}};
+  h.ppri = cb::PointPriors{d_idx, d_pt, d_pmean, d_pinfo, np};
+  auto up = [&](auto* dst, const auto* src, size_t n) -> int {
+    if (n) CB_CUDA(cudaMemcpyAsync(dst, src, sizeof(src[0]) * n, cudaMemcpyHostToDevice, st));
     return CB_OK;
   };
-  if (nc) {
-    CB_TRY(up(d_slot, slot)); CB_TRY(up(d_width, width)); CB_TRY(up(d_cmean, h.cmean)); CB_TRY(up(d_cinfo, h.cinfo));
-  }
-  CB_TRY(up(d_idx, idx)); CB_TRY(up(d_pt, h.pt)); CB_TRY(up(d_pmean, h.pmean)); CB_TRY(up(d_pinfo, h.pinfo));
-  p->cpri.slot = d_slot; p->cpri.width = d_width; p->cpri.mean = d_cmean; p->cpri.info = d_cinfo; p->cpri.n = nc;
-  p->ppri = cb::PointPriors{d_idx, d_pt, d_pmean, d_pinfo, np};
-  return CB_OK;
+  CB_TRY(up(h.d_fixc, fc.data(), nf)); CB_TRY(up(h.d_fixp, h.fixp.data(), h.fixp.size()));
+  CB_TRY(up(d_slot, slot.data(), nc)); CB_TRY(up(d_width, width.data(), nc));
+  CB_TRY(up(d_cmean, h.cmean.data(), h.cmean.size())); CB_TRY(up(d_cinfo, h.cinfo.data(), h.cinfo.size()));
+  CB_TRY(up(d_idx, idx.data(), idx.size())); CB_TRY(up(d_pt, h.pt.data(), h.pt.size()));
+  CB_TRY(up(d_pmean, h.pmean.data(), h.pmean.size())); CB_TRY(up(d_pinfo, h.pinfo.data(), h.pinfo.size()));
+  return up(h.d_cpri, &h.cpri, 1);
 }
 
 // Eigenvalues of the symmetric n x n matrix A (row-major, n <= 9) by cyclic Jacobi rotations.
@@ -2111,77 +2116,114 @@ static int check_information(const double* L, int ld, int n, const double* mean,
   return CB_OK;
 }
 
-// The priors of cb_ba_problem_create_priors, checked on the host before any device work, into out.
-static int check_priors(const CbBaProblemDesc* d, const CbBaPriors* pr, int32_t n_fixed_pts, const int32_t* fixed_pts,
-                        HostPriors& out) {
-  if (!pr) return CB_OK;
-  if (pr->n_cams < 0 || pr->n_pts < 0 || (pr->n_cams > 0 && (!pr->cams || !pr->cam_mean || !pr->cam_info)) ||
-      (pr->n_pts > 0 && (!pr->pts || !pr->pt_mean || !pr->pt_info))) {
-    g_last_error = "cb_ba_problem_create_priors: bad prior list";
+// The fixed sets and priors of cb_ba_problem_create_priors, checked on the host before any device work, into out.
+static int check_held(const CbBaProblemDesc* d, int32_t n_fixed_cam_params, const int32_t* fixed_cam_params,
+                      int32_t n_fixed_pts, const int32_t* fixed_pts, const CbBaPriors* pr, HeldSet& out) {
+  if (n_fixed_cam_params < 0 || n_fixed_pts < 0 || (n_fixed_cam_params > 0 && !fixed_cam_params) ||
+      (n_fixed_pts > 0 && !fixed_pts)) {
+    g_last_error = "cb_ba_problem_create_fixed: bad fixed-parameter list";
     return CB_E_INVALID;
   }
-  std::vector<char> seen((size_t)d->n_cams, 0);
-  for (int k = 0; k < pr->n_cams; ++k) {
-    const int c = pr->cams[k];
-    if (c < 0 || c >= d->n_cams || seen[c]) {
-      g_last_error = "cb_ba_problem_create_priors: camera prior index " + std::to_string(c) +
-                     (c < 0 || c >= d->n_cams ? " is out of range" : " is repeated");
+  long long ncp = 0;
+  for (int c = 0; c < d->n_cams; ++c) ncp += (d->cam_flags[c] & CB_CAM_FREE_INTRINSICS) ? 9 : 6;
+  // held[j]: point j is fixed (1) or has a prior (2)
+  std::vector<char> seen_c((size_t)ncp, 0), held((size_t)d->n_pts, 0);
+  for (int i = 0; i < n_fixed_cam_params; ++i) {
+    const int v = fixed_cam_params[i];
+    if (v < 0 || v >= ncp || seen_c[v]) {
+      g_last_error = "cb_ba_problem_create_fixed: fixed camera parameter index " + std::to_string(v) +
+                     (v < 0 || v >= ncp ? " is out of range" : " is repeated");
       return CB_E_INVALID;
     }
-    seen[c] = 1;
-    const int w = (d->cam_flags[c] & CB_CAM_FREE_INTRINSICS) ? 9 : 6;
-    const double* L = pr->cam_info + 81 * (size_t)k;
-    for (int a = 0; a < 9; ++a)
-      for (int b = 0; b < 9; ++b)
-        if ((a >= w || b >= w) && L[9 * a + b] != 0.0) {
-          g_last_error = "cb_ba_problem_create_priors: camera " + std::to_string(c) +
-                         " has 6 parameters but non-zero prior information outside its 6 x 6 block";
-          return CB_E_INVALID;
-        }
-    int r = 0;
-    CB_TRY(check_information(L, 9, w, pr->cam_mean + 9 * (size_t)k, "the prior of camera " + std::to_string(c), r));
-    out.rank += r;
+    seen_c[v] = 1;
   }
-  std::vector<char> fixed((size_t)d->n_pts, 0), seenp((size_t)d->n_pts, 0);
-  for (int i = 0; i < n_fixed_pts; ++i) fixed[fixed_pts[i]] = 1;
-  for (int k = 0; k < pr->n_pts; ++k) {
-    const int j = pr->pts[k];
-    if (j < 0 || j >= d->n_pts || seenp[j]) {
-      g_last_error = "cb_ba_problem_create_priors: point prior index " + std::to_string(j) +
+  for (int i = 0; i < n_fixed_pts; ++i) {
+    const int j = fixed_pts[i];
+    if (j < 0 || j >= d->n_pts || held[j]) {
+      g_last_error = "cb_ba_problem_create_fixed: fixed point index " + std::to_string(j) +
                      (j < 0 || j >= d->n_pts ? " is out of range" : " is repeated");
       return CB_E_INVALID;
     }
-    seenp[j] = 1;
-    if (fixed[j]) {
-      g_last_error = "cb_ba_problem_create_priors: point " + std::to_string(j) + " is both fixed and has a prior";
+    held[j] = 1;
+  }
+  if (n_fixed_cam_params == ncp && n_fixed_pts == d->n_pts) {
+    g_last_error = "cb_ba_problem_create_fixed: every parameter is fixed";
+    return CB_E_INVALID;
+  }
+  out.fixc_x.assign(fixed_cam_params, fixed_cam_params + n_fixed_cam_params);
+  out.fixp.assign(fixed_pts, fixed_pts + n_fixed_pts);
+  if (pr) {
+    if (pr->n_cams < 0 || pr->n_pts < 0 || (pr->n_cams > 0 && (!pr->cams || !pr->cam_mean || !pr->cam_info)) ||
+        (pr->n_pts > 0 && (!pr->pts || !pr->pt_mean || !pr->pt_info))) {
+      g_last_error = "cb_ba_problem_create_priors: bad prior list";
       return CB_E_INVALID;
     }
-    int r = 0;
-    CB_TRY(check_information(pr->pt_info + 9 * (size_t)k, 3, 3, pr->pt_mean + 3 * (size_t)k,
-                             "the prior of point " + std::to_string(j), r));
-    out.rank += r;
+    std::vector<char> seen((size_t)d->n_cams, 0);
+    for (int k = 0; k < pr->n_cams; ++k) {
+      const int c = pr->cams[k];
+      if (c < 0 || c >= d->n_cams || seen[c]) {
+        g_last_error = "cb_ba_problem_create_priors: camera prior index " + std::to_string(c) +
+                       (c < 0 || c >= d->n_cams ? " is out of range" : " is repeated");
+        return CB_E_INVALID;
+      }
+      seen[c] = 1;
+      const int w = (d->cam_flags[c] & CB_CAM_FREE_INTRINSICS) ? 9 : 6;
+      const double* L = pr->cam_info + 81 * (size_t)k;
+      for (int a = 0; a < 9; ++a)
+        for (int b = 0; b < 9; ++b)
+          if ((a >= w || b >= w) && L[9 * a + b] != 0.0) {
+            g_last_error = "cb_ba_problem_create_priors: camera " + std::to_string(c) +
+                           " has 6 parameters but non-zero prior information outside its 6 x 6 block";
+            return CB_E_INVALID;
+          }
+      int r = 0;
+      CB_TRY(check_information(L, 9, w, pr->cam_mean + 9 * (size_t)k, "the prior of camera " + std::to_string(c), r));
+      out.rank += r;
+    }
+    for (int k = 0; k < pr->n_pts; ++k) {
+      const int j = pr->pts[k];
+      if (j < 0 || j >= d->n_pts || held[j] == 2) {
+        g_last_error = "cb_ba_problem_create_priors: point prior index " + std::to_string(j) +
+                       (j < 0 || j >= d->n_pts ? " is out of range" : " is repeated");
+        return CB_E_INVALID;
+      }
+      if (held[j] == 1) {
+        g_last_error = "cb_ba_problem_create_priors: point " + std::to_string(j) + " is both fixed and has a prior";
+        return CB_E_INVALID;
+      }
+      held[j] = 2;
+      int r = 0;
+      CB_TRY(check_information(pr->pt_info + 9 * (size_t)k, 3, 3, pr->pt_mean + 3 * (size_t)k,
+                               "the prior of point " + std::to_string(j), r));
+      out.rank += r;
+    }
+    out.cam.assign(pr->cams, pr->cams + pr->n_cams);
+    out.cmean.assign(pr->cam_mean, pr->cam_mean + 9 * (size_t)pr->n_cams);
+    out.cinfo.assign(pr->cam_info, pr->cam_info + 81 * (size_t)pr->n_cams);
+    out.pt.assign(pr->pts, pr->pts + pr->n_pts);
+    out.pmean.assign(pr->pt_mean, pr->pt_mean + 3 * (size_t)pr->n_pts);
+    out.pinfo.assign(pr->pt_info, pr->pt_info + 9 * (size_t)pr->n_pts);
+    out.n_prior_blk = (int)cdiv(pr->n_cams + pr->n_pts, cb::PRIOR_THREADS);
   }
-  if (pr->n_pts > 0 && d->n_constraints > 0)
-    for (long long k = 0; k < 4ll * d->n_constraints; ++k)
-      for (const int32_t* g : {d->groups_a, d->groups_b})
-        if (g[k] >= 0 && g[k] < d->n_pts && seenp[g[k]]) {
-          g_last_error = "cb_ba_problem_create_priors: point " + std::to_string(g[k]) +
-                         " has a prior and is in a rigid-distance constraint row (constraint components are eliminated "
-                         "jointly)";
-          return CB_E_UNSUPPORTED;
-        }
-  out.cam.assign(pr->cams, pr->cams + pr->n_cams);
-  out.cmean.assign(pr->cam_mean, pr->cam_mean + 9 * (size_t)pr->n_cams);
-  out.cinfo.assign(pr->cam_info, pr->cam_info + 81 * (size_t)pr->n_cams);
-  out.pt.assign(pr->pts, pr->pts + pr->n_pts);
-  out.pmean.assign(pr->pt_mean, pr->pt_mean + 3 * (size_t)pr->n_pts);
-  out.pinfo.assign(pr->pt_info, pr->pt_info + 9 * (size_t)pr->n_pts);
+  // constraint components are eliminated jointly: no held point in a rigid-distance constraint row
+  if (!out.points() || d->n_constraints == 0) return CB_OK;
+  for (long long k = 0; k < 4ll * d->n_constraints; ++k)
+    for (const int32_t* g : {d->groups_a, d->groups_b})
+      if (g[k] >= 0 && g[k] < d->n_pts && held[g[k]]) {
+        g_last_error = held[g[k]] == 1 ? "cb_ba_problem_create_fixed: fixed point " + std::to_string(g[k]) +
+                                             " is in a rigid-distance constraint row (constraint components are "
+                                             "eliminated jointly)"
+                                       : "cb_ba_problem_create_priors: point " + std::to_string(g[k]) +
+                                             " has a prior and is in a rigid-distance constraint row (constraint "
+                                             "components are eliminated jointly)";
+        return CB_E_UNSUPPORTED;
+      }
   return CB_OK;
 }
 
-// fixc_x: fixed camera parameters (caller's x indices), fixp: fixed points, pri: priors; all checked by the caller
+// held: the fixed sets and priors, checked by the caller
 static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_t st, CbBaProblem* p,
-                               const std::vector<int>& fixc_x, const std::vector<int>& fixp, const HostPriors& pri) {
+                               const HeldSet& held) {
   NvtxRange nvtx_create("cb_ba_problem_create (upload + index build)");
   // CB_PROFILE_CREATE=1: host wall-clock of the stages of problem creation on stderr (diagnostic)
   const bool prof = std::getenv("CB_PROFILE_CREATE") != nullptr;
@@ -2220,9 +2262,7 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   p->nP = p->n_cams * p->P;
   p->ncp = p->h_cam_off[p->n_cams];
   p->n_params = p->ncp + 3 * p->n_pts;
-  p->h_fixc_x = fixc_x; p->h_fixp = fixp;
-  p->n_fixc = (int)fixc_x.size();
-  p->pri = pri;
+  p->held = held;  // the host lists; upload_held replaces every device table
   p->n_blk = cdiv(p->nP, cb::SY_TILE);
   p->LD = p->n_blk * cb::SY_TILE;
   p->n_tiles = p->n_blk * (p->n_blk + 1) / 2;
@@ -2330,24 +2370,6 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   std::vector<unsigned char> act((size_t)p->nP, 0);
   for (int c = 0; c < p->n_cams; ++c)
     for (int a = 0; a < ((p->h_iflags[c] & CB_CAM_FREE_INTRINSICS) ? 9 : 6); ++a) act[(size_t)c * p->P + a] = 1;
-  if (p->has_fixed()) {
-    std::vector<int> fc(p->n_fixc);
-    for (int i = 0; i < p->n_fixc; ++i) {  // caller's x index -> internal slot index
-      const int xi = p->h_fixc_x[i];
-      const int c = (int)(std::upper_bound(p->h_cam_off.begin(), p->h_cam_off.end(), xi) - p->h_cam_off.begin()) - 1;
-      fc[i] = p->h_slot[c] * p->P + (xi - p->h_cam_off[c]);
-      act[(size_t)fc[i]] = 0;
-    }
-    CB_TRY(palloc(p, &p->d_fixc, std::max(p->n_fixc, 1)));
-    CB_TRY(palloc(p, &p->d_fixp, std::max(p->h_fixp.size(), (size_t)1)));
-    if (p->n_fixc) CB_CUDA(cudaMemcpyAsync(p->d_fixc, fc.data(), sizeof(int) * fc.size(), cudaMemcpyHostToDevice, st));
-    if (!p->h_fixp.empty())
-      CB_CUDA(cudaMemcpyAsync(p->d_fixp, p->h_fixp.data(), sizeof(int) * p->h_fixp.size(), cudaMemcpyHostToDevice, st));
-  }
-  CB_TRY(palloc(p, &p->d_active, p->nP));
-  CB_CUDA(cudaMemcpyAsync(p->d_active, act.data(), p->nP, cudaMemcpyHostToDevice, st));
-  CB_TRY(upload_priors(p, st));
-  CB_CUDA(cudaStreamSynchronize(st));
   CB_TRY(palloc(p, &p->d_lo, p->nP)); CB_TRY(palloc(p, &p->d_hi, p->nP));
 
   // work buffers
@@ -2356,14 +2378,13 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   CB_TRY(palloc(p, &p->d_x, (size_t)p->n_params + 1));
   for (int k = 0; k < 2; ++k) {
     CB_TRY(palloc(p, &p->d_xc[k], p->nP)); CB_TRY(palloc(p, &p->d_xp4[k], 4 * npts));
-    p->cpri.xc.p[k] = p->d_xc[k];
     CB_TRY(palloc(p, &p->d_camtab[k], (size_t)p->n_cams * cb::CT_SIZE));
     CB_TRY(palloc(p, &p->d_Upk[k], (size_t)p->n_cams * NU)); CB_TRY(palloc(p, &p->d_gc[k], p->nP));
     CB_TRY(palloc(p, &p->d_costsum[k], 4));
   }
   // the cost / step partial-sum arrays grow by the constraint blocks / components (by nothing without constraints)
   CB_TRY(palloc(p, &p->d_partial, (size_t)std::max(p->n_chunks, 1) * NACC + p->n_cblk));
-  CB_TRY(palloc(p, &p->d_camcost, (size_t)p->n_cams + p->n_cblk + p->n_prior_blk));
+  CB_TRY(palloc(p, &p->d_camcost, (size_t)p->n_cams + p->n_cblk + p->held.n_prior_blk));
   CB_TRY(palloc(p, &p->d_gpt, 3 * npts));
   CB_TRY(palloc(p, &p->d_V6, 6 * npts)); CB_TRY(palloc(p, &p->d_gp, 3 * npts)); CB_TRY(palloc(p, &p->d_Dp2, 3 * npts));
   CB_TRY(palloc(p, &p->d_Dc2, p->nP)); CB_TRY(palloc(p, &p->d_Linv6, 6 * npts));
@@ -2389,10 +2410,9 @@ static int problem_create_impl(const CbBaProblemDesc* d, int device, cudaStream_
   CB_CUDA(cudaMemsetAsync(p->d_part, 0, sizeof(double) * (size_t)p->n_slots * cb::SY_TILE * cb::SY_TILE, st));
   CB_CUDA(cudaMemsetAsync(p->d_red2, 0, sizeof(double) * 8, st));
   CB_CUDA(cudaMemsetAsync(p->d_Linv6, 0, sizeof(double) * 6 * npts, st));
-  if (p->cpri.n) {
-    CB_TRY(palloc(p, &p->d_cpri, 1));
-    CB_CUDA(cudaMemcpyAsync(p->d_cpri, &p->cpri, sizeof(cb::CamPriors), cudaMemcpyHostToDevice, st));
-  }
+  CB_TRY(upload_held(p, act, st));
+  CB_TRY(palloc(p, &p->d_active, p->nP));
+  CB_CUDA(cudaMemcpyAsync(p->d_active, act.data(), p->nP, cudaMemcpyHostToDevice, st));
   CB_TRY(cached_malloc_host((void**)&p->h_state, sizeof(cb::LmState) * 4));
   for (cudaEvent_t* e : {&p->ev0, &p->ev1, &p->ev2, &p->ev3, &p->ev_pp[0][0], &p->ev_pp[0][1], &p->ev_pp[0][2], &p->ev_pp[0][3],
                          &p->ev_pp[1][0], &p->ev_pp[1][1], &p->ev_pp[1][2], &p->ev_pp[1][3]})
@@ -2439,49 +2459,10 @@ int cb_ba_problem_create_priors(const CbBaProblemDesc* d, int32_t n_fixed_cam_pa
     return CB_E_INVALID;
   }
   *out = nullptr;
-  // the fixed sets, checked on the host before any device work
-  if (n_fixed_cam_params < 0 || n_fixed_pts < 0 || (n_fixed_cam_params > 0 && !fixed_cam_params) ||
-      (n_fixed_pts > 0 && !fixed_pts)) {
-    g_last_error = "cb_ba_problem_create_fixed: bad fixed-parameter list";
-    return CB_E_INVALID;
-  }
-  long long ncp = 0;
-  for (int c = 0; c < d->n_cams; ++c) ncp += (d->cam_flags[c] & CB_CAM_FREE_INTRINSICS) ? 9 : 6;
-  auto check_set = [](const int32_t* v, int n, long long lim, const char* what) -> int {
-    std::vector<char> seen((size_t)lim, 0);
-    for (int i = 0; i < n; ++i) {
-      if (v[i] < 0 || v[i] >= lim || seen[(size_t)v[i]]) {
-        g_last_error = std::string("cb_ba_problem_create_fixed: ") + what + " index " + std::to_string(v[i]) +
-                       (v[i] < 0 || v[i] >= lim ? " is out of range" : " is repeated");
-        return CB_E_INVALID;
-      }
-      seen[(size_t)v[i]] = 1;
-    }
-    return CB_OK;
-  };
-  CB_TRY(check_set(fixed_cam_params, n_fixed_cam_params, ncp, "fixed camera parameter"));
-  CB_TRY(check_set(fixed_pts, n_fixed_pts, d->n_pts, "fixed point"));
-  if (n_fixed_cam_params == ncp && n_fixed_pts == d->n_pts) {
-    g_last_error = "cb_ba_problem_create_fixed: every parameter is fixed";
-    return CB_E_INVALID;
-  }
-  if (n_fixed_pts > 0 && d->n_constraints > 0) {
-    std::vector<char> fixed((size_t)d->n_pts, 0);
-    for (int i = 0; i < n_fixed_pts; ++i) fixed[fixed_pts[i]] = 1;
-    for (long long k = 0; k < 4ll * d->n_constraints; ++k)
-      for (const int32_t* g : {d->groups_a, d->groups_b})
-        if (g[k] >= 0 && g[k] < d->n_pts && fixed[g[k]]) {
-          g_last_error = "cb_ba_problem_create_fixed: fixed point " + std::to_string(g[k]) +
-                         " is in a rigid-distance constraint row (constraint components are eliminated jointly)";
-          return CB_E_UNSUPPORTED;
-        }
-  }
-  HostPriors pri;
-  CB_TRY(check_priors(d, priors, n_fixed_pts, fixed_pts, pri));
+  HeldSet held;
+  CB_TRY(check_held(d, n_fixed_cam_params, fixed_cam_params, n_fixed_pts, fixed_pts, priors, held));
   CbBaProblem* p = new CbBaProblem();
-  int rc = problem_create_impl(d, device, (cudaStream_t)stream, p,
-                               std::vector<int>(fixed_cam_params, fixed_cam_params + n_fixed_cam_params),
-                               std::vector<int>(fixed_pts, fixed_pts + n_fixed_pts), pri);
+  int rc = problem_create_impl(d, device, (cudaStream_t)stream, p, held);
   if (rc != CB_OK) {
     std::string keep = g_last_error;
     cb_ba_problem_destroy(p);
@@ -2500,12 +2481,9 @@ int cb_ba_solve_from(CbBaProblem* p, const CbBaOptions* opt, const double* x0, d
                      void* stream) {
   if (!p || !opt || !x0 || !x_out || !result) { g_last_error = "cb_ba_solve: null argument"; return CB_E_INVALID; }
   if (opt->loss < 0 || opt->loss > CB_LOSS_ARCTAN) { g_last_error = "unknown loss id"; return CB_E_INVALID; }
-  if (sharded(opt) && p->has_fixed()) {
-    g_last_error = "cb_ba_solve: fixed parameters are not supported in a sharded solve";
-    return CB_E_UNSUPPORTED;
-  }
-  if (sharded(opt) && p->has_priors()) {
-    g_last_error = "cb_ba_solve: priors are not supported in a sharded solve";
+  if (sharded(opt) && p->held.any()) {
+    g_last_error = p->held.priors() ? "cb_ba_solve: priors are not supported in a sharded solve"
+                                    : "cb_ba_solve: fixed parameters are not supported in a sharded solve";
     return CB_E_UNSUPPORTED;
   }
   CB_CUDA(cudaSetDevice(p->device));
@@ -2612,7 +2590,7 @@ static int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss,
   if (dp) CB_CUDA(cudaMemcpyAsync(dp, p->d_dp, sizeof(double) * 3 * (size_t)p->n_pts, cudaMemcpyDeviceToHost, st));
   CB_CUDA(cudaStreamSynchronize(st));
   if (cost) *cost = hS[nn + 3 * (size_t)p->nP];
-  if (gc && p->has_priors()) std::memcpy(gc, &hS[nn + p->nP], sizeof(double) * p->nP);  // the g_c slot: with L_c (x_c - m_c)
+  if (gc && p->held.priors()) std::memcpy(gc, &hS[nn + p->nP], sizeof(double) * p->nP);  // the g_c slot: with L_c (x_c - m_c)
   // reduced system back in the caller's camera order
   const int nP = p->nP;
   if (S)
@@ -2640,10 +2618,10 @@ static int normal_eq_impl(CbBaProblem* p, const double* x, double lam, int loss,
         }
     }
   if (U)  // U as the solve sees it: with the camera priors' information
-    for (size_t k = 0; k < p->pri.cam.size(); ++k) {
-      const int c = p->pri.cam[k], w = p->h_cam_off[c + 1] - p->h_cam_off[c];
+    for (size_t k = 0; k < p->held.cam.size(); ++k) {
+      const int c = p->held.cam[k], w = p->h_cam_off[c + 1] - p->h_cam_off[c];
       for (int a = 0; a < w; ++a)
-        for (int bb = 0; bb < w; ++bb) U[((size_t)c * P + a) * P + bb] += p->pri.cinfo[81 * k + 9 * a + bb];
+        for (int bb = 0; bb < w; ++bb) U[((size_t)c * P + a) * P + bb] += p->held.cinfo[81 * k + 9 * a + bb];
     }
   if (V)
     for (int j = 0; j < p->n_pts; ++j) {
@@ -2673,7 +2651,8 @@ static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs,
   CB_CUDA(cudaStreamSynchronize(st));
   std::vector<char> is_fixed((size_t)p->ncp, 0);
   for (int i = 0; i < n_fixed; ++i) is_fixed[fixed[i]] = 1;
-  for (int xi : p->h_fixc_x) is_fixed[xi] = 1;  // the problem's own fixed camera parameters
+  const HeldSet& h = p->held;
+  for (int xi : h.fixc_x) is_fixed[xi] = 1;  // the problem's own fixed camera parameters
   std::vector<unsigned char> fr((size_t)nP, 0);
   std::vector<int> xidx((size_t)nP, -1);  // caller x index of each internal slot (-1: padding)
   long long n_masked = 0, n_fix = 0;
@@ -2718,9 +2697,9 @@ static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs,
   CB_TRY(camera_pass(p, 0, 0, st));
   CB_TRY(build_system(p, &opt, st, nullptr, true));
   if (p->n_c) CB_LAUNCH(cb::comp_failed_kernel, cdiv(p->n_comp, 128), 128, 0, st, p->ct, (const double*)p->d_compL, p->d_covFail + 1);
-  if (!p->pri.cam.empty()) {
-    if (P == 6) CB_LAUNCH(cb::prior_cam_kernel<6>, 1, 256, 0, st, p->d_red, nP, p->cpri);
-    else CB_LAUNCH(cb::prior_cam_kernel<9>, 1, 256, 0, st, p->d_red, nP, p->cpri);
+  if (!h.cam.empty()) {
+    if (P == 6) CB_LAUNCH(cb::prior_cam_kernel<6>, 1, 256, 0, st, p->d_red, nP, h.cpri);
+    else CB_LAUNCH(cb::prior_cam_kernel<9>, 1, 256, 0, st, p->d_red, nP, h.cpri);
   }
   CB_CUDA(cudaEventRecord(p->ev1, st));
   // dense inverse of the gauge-fixed reduced system
@@ -2760,8 +2739,8 @@ static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs,
   long long null_pts = 0;
   for (int j = 0; j < p->n_pts; ++j)
     if (rank[j] >= 0) null_pts += 3 - rank[j];
-  const long long m = 2ll * p->n_obs + p->n_c + p->pri.rank;  // each prior adds rank(L) rows W (x - m)
-  const long long rk = (long long)p->n_params - n_fix - n_masked - null_pts - 3ll * (long long)p->h_fixp.size();
+  const long long m = 2ll * p->n_obs + p->n_c + h.rank;  // each prior adds rank(L) rows W (x - m)
+  const long long rk = (long long)p->n_params - n_fix - n_masked - null_pts - 3ll * (long long)h.fixp.size();
   const long long dof = m - rk;
   const double s2 = vf > 0.0 ? vf : (dof > 0 ? 2.0 * cost / (double)dof : std::nan(""));
   if (s2_out) *s2_out = s2;
@@ -2785,7 +2764,7 @@ static int covariance_impl(CbBaProblem* p, const double* x, int loss, double fs,
   CB_CUDA(cudaEventElapsedTime(&p->cov_ms[1], p->ev1, p->ev2));
   CB_CUDA(cudaEventElapsedTime(&p->cov_ms[2], p->ev2, p->ev3));
   if (pt_cov)  // fixed points (rank -2) are constants: zero covariance
-    for (int j : p->h_fixp) std::fill(pt_cov + 9 * (size_t)j, pt_cov + 9 * (size_t)j + 9, 0.0);
+    for (int j : h.fixp) std::fill(pt_cov + 9 * (size_t)j, pt_cov + 9 * (size_t)j + 9, 0.0);
   if (cam_cov) {
     // caller layout: NaN rows / columns for the cameras without observations, zero for the fixed parameters
     const size_t ncp = (size_t)p->ncp;
@@ -3043,7 +3022,7 @@ int cb_ba_cull(CbBaProblem* p, const double* x, const double* thresholds, int32_
     d2.groups_a = p->h_ga.data(); d2.groups_b = p->h_gb.data(); d2.distances = p->h_cdist.data(); d2.weights = p->h_cw.data();
     CbBaProblem* q = new CbBaProblem();
     q->allocs.push_back(c_cam); q->allocs.push_back(c_pt); q->allocs.push_back(c_xy);  // owned by the new problem
-    rc = problem_create_impl(&d2, p->device, st, q, p->h_fixc_x, p->h_fixp, p->pri);
+    rc = problem_create_impl(&d2, p->device, st, q, p->held);
     if (rc != CB_OK) {
       std::string keep = g_last_error;
       cb_ba_problem_destroy(q);

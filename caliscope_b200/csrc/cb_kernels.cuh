@@ -86,7 +86,7 @@ __global__ void unpack_x_kernel(const double* __restrict__ x, const int* __restr
 }
 
 // The fixed points of a problem that holds some (DESIGN §4.12): 1.0 in the pad slot of their xp4 entry, which the point
-// kernels' FIXP variants read beside the coordinates (no extra traffic) and the back-substitution carries into the trial
+// kernels' HELD / FIXP variants read beside the coordinates (no extra traffic) and the back-substitution carries into the trial
 // buffer.
 __global__ void mark_fixed_points_kernel(const int* __restrict__ pts, int n, double* __restrict__ xp4) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;

@@ -22,10 +22,10 @@
 // The decision follows scipy's TRF bookkeeping (site-packages/scipy/optimize/_lsq/trf.py:465-560,
 // common.py:705-717): nfev / njev / nit count the same events, termination statuses 0..4 are scipy's.
 //
-// Fixed parameters (DESIGN.md §4.12) enter in two places, each behind a template flag chosen at creation: FIXC in
-// reduced_prep_body (unit rows / columns of S and zero b for fixed camera parameters, before the damping) and FIXP in
-// pt_pass_kernel / pt_backsub_kernel (a fixed point, flagged in the pad slot of xp4, has V^-1 := 0 and a zero step).
-// Gaussian priors (DESIGN.md §4.13, cb_priors.cuh) enter behind PRIORC in reduced_prep_body and PRIORP in pt_pass_kernel.
+// Held parameters -- fixed sets (DESIGN.md §4.12) and Gaussian priors (§4.13, cb_priors.cuh) -- enter behind one template
+// flag per side, chosen at creation: HELD in reduced_prep_body (camera priors into S and b, then unit rows / columns of S
+// and zero b for fixed camera parameters, before the damping) and HELD in pt_pass_kernel (point priors into V and g, and
+// V^-1 := 0 for a fixed point, flagged in the pad slot of xp4).  pt_backsub_kernel's FIXP gives a fixed point a zero step.
 #pragma once
 #include "cb_covariance.cuh"
 #include "cb_priors.cuh"
@@ -54,13 +54,11 @@ struct LmLogRow {
 // of V (V^+ = R^T R, 9 values per point into Linv6, rank(V) into pt_rank, -1 for component points); Z = (Jc^T Jp) R^T,
 // t = 0, and neither Dp2 nor the gradient norm is touched.
 //
-// FIXP: the problem holds some points fixed (DESIGN §4.12); a fixed point carries 1.0 in the pad slot of xp4 (0.0
-// otherwise).  A fixed point is a constant: its factor is zero (V^-1 := 0, so Z = 0 and t = 0), its gradient is left out
-// of the gradient norm, and the covariance variant reports rank -2 for it.
-//
-// PRIORP: the problem holds point priors (cb_priors.cuh); the prior of point j (pp.idx[j] >= 0) adds L_j to V_j and
-// L_j (X_j - m_j) to g_j before D, the damping and the factor are formed.  Only instantiated with FIXP (the two flags
-// combine: one more variant, not two).
+// HELD: the problem holds some points fixed (DESIGN §4.12) or near a prior (§4.13).  A fixed point carries 1.0 in the pad
+// slot of xp4 (0.0 otherwise) and is a constant: its factor is zero (V^-1 := 0, so Z = 0 and t = 0), its gradient is left
+// out of the gradient norm, and the covariance variant reports rank -2 for it.  The prior of point j (pp.idx[j] >= 0;
+// every entry is -1 in a problem with fixed points only) adds L_j to V_j and L_j (X_j - m_j) to g_j before D, the damping
+// and the factor are formed.
 template <bool COV>
 __device__ __forceinline__ void pt_factor_rows(const double* JX, const double* Li, double& q00, double& q01, double& q02,
                                                double& q10, double& q11, double& q12) {
@@ -90,7 +88,7 @@ struct PtStage {
 template <int P, int LANES>
 constexpr size_t pt_stage_bytes() { return sizeof(PtStage<P, LANES>) * PT_WARPS * (32 / LANES); }
 
-template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false, bool FIXP = false, bool PRIORP = false>
+template <int P, int LANES, bool DUPS, bool CAMSM, bool COV = false, bool HELD = false>
 __global__ void __launch_bounds__(PT_WARPS * 32, 2)
 pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start, const int* __restrict__ pm_cam,
                const double2* __restrict__ pm_xy, const int* __restrict__ pt_comp, int n_pts, int n_cams,
@@ -157,7 +155,7 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
     }
 #pragma unroll
     for (int k = 0; k < 9; ++k) v[k] = group_sum<LANES>(v[k]);
-    if constexpr (PRIORP) {
+    if constexpr (HELD) {
       const int q = valid ? pp.idx[j] : -1;
       if (q >= 0) {
         const double* L = pp.info + 9 * (size_t)q;
@@ -180,7 +178,7 @@ pt_pass_kernel(const LmState* __restrict__ st, const int* __restrict__ pt_start,
     double Li[NL];
     int rank = -1;
     // the flag is read again here rather than kept from the load above: live across the observation loop it costs spills
-    const bool fixed = FIXP && valid && xp4[4 * (size_t)j + 3] != 0.0;
+    const bool fixed = HELD && valid && xp4[4 * (size_t)j + 3] != 0.0;
     if (in_comp) {
 #pragma unroll
       for (int k = 0; k < NL; ++k) Li[k] = 0.0;
@@ -520,14 +518,14 @@ __device__ __forceinline__ void block_inverse_one(const double* __restrict__ S, 
     }
 }
 
-// FIXC: fixc[0..n_fixc) are fixed camera parameters (internal slot indices, DESIGN §4.12).  Before the damping their rows and
-// columns of S become unit vectors and their entries of b zero, so every solver returns a zero step for them; their active
-// bytes are clear, so the gradient norm, the step and the predicted reduction leave them out.
-// PRIORC: the camera priors *cpp (cb_priors.cuh; a device pointer rather than a by-value parameter, which leaves the
-// kernels without priors their earlier SASS) at the current cameras enter S, b, the g_c slot and the diag-U slot first,
-// so a fixed parameter still ends up a unit row and its diagonal prior information still reaches Dc2.  Only instantiated
-// with FIXC (the two flags combine).
-template <int P, bool WANT_MINV, bool FIXC = false, bool PRIORC = false>
+// HELD: the problem holds camera parameters fixed (DESIGN §4.12) or near a prior (§4.13).  The camera priors *cpp
+// (cb_priors.cuh; a device pointer rather than a by-value parameter, which leaves the kernels without held parameters
+// their own SASS; cpp->n = 0 with fixed parameters only) at the current cameras enter S, b, the g_c slot and the diag-U
+// slot first.  Then fixc[0..n_fixc), the fixed camera parameters (internal slot indices), get unit rows and columns of S
+// and zero entries of b before the damping, so every solver returns a zero step for them, while their diagonal prior
+// information still reaches Dc2; their active bytes are clear, so the gradient norm, the step and the predicted
+// reduction leave them out.
+template <int P, bool WANT_MINV, bool HELD = false>
 __device__ __forceinline__ void reduced_prep_body(LmState* __restrict__ st, int nP, int n_cams, int red_slots,
                                                   double* __restrict__ red, double* __restrict__ Dc2,
                                                   const unsigned char* __restrict__ active, double* __restrict__ Minv,
@@ -536,12 +534,10 @@ __device__ __forceinline__ void reduced_prep_body(LmState* __restrict__ st, int 
   __shared__ double sh[32];
   const size_t nn = (size_t)nP * nP;
   const double lam = st->lam;
-  if constexpr (PRIORC) {
+  if constexpr (HELD) {
     const CamPriors cp = *cpp;
     add_cam_priors<P>(red, nP, cp.xc.p[st->cur], cp);
     __syncthreads();
-  }
-  if constexpr (FIXC) {
     for (int t = threadIdx.x; t < n_fixc * nP; t += blockDim.x) {
       const int f = fixc[t / nP], i = t % nP;
       const double v = i == f ? 1.0 : 0.0;
@@ -589,15 +585,14 @@ __device__ __forceinline__ void reduced_prep_body(LmState* __restrict__ st, int 
   if constexpr (WANT_MINV)
     for (int c = threadIdx.x; c < n_cams; c += blockDim.x) block_inverse_one<P>(red, nP, c, Minv + (size_t)c * P * P);
 }
-template <int P, bool FIXC = false, bool PRIORC = false>
+template <int P, bool HELD = false>
 __global__ void __launch_bounds__(256)
 reduced_prep_kernel(LmState* __restrict__ st, int nP, int n_cams, int red_slots, double* __restrict__ red,
                     double* __restrict__ Dc2, const unsigned char* __restrict__ active, double* __restrict__ Minv,
                     unsigned long long* __restrict__ gmax_bits, double* __restrict__ sc, const int* __restrict__ fixc,
                     int n_fixc, const CamPriors* __restrict__ cp) {
   if (st->done) return;
-  reduced_prep_body<P, true, FIXC, PRIORC>(st, nP, n_cams, red_slots, red, Dc2, active, Minv, gmax_bits, sc, fixc, n_fixc,
-                                           cp);
+  reduced_prep_body<P, true, HELD>(st, nP, n_cams, red_slots, red, Dc2, active, Minv, gmax_bits, sc, fixc, n_fixc, cp);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -655,7 +650,7 @@ cam_step_kernel(const LmState* __restrict__ st, int nP, int n_cams, int P, Ptr2 
 
 // Small rigs (n_camera_params <= DIRECT_MAX_N): damping + head-of-iteration tests, the direct reduced solve and the camera
 // step in ONE single-CTA kernel -- three launches and two kernel boundaries become one.
-template <int P, bool FIXC = false, bool PRIORC = false>
+template <int P, bool HELD = false>
 __global__ void __launch_bounds__(DIRECT_THREADS, 1)
 small_rig_step_kernel(LmState* __restrict__ st, int nP, int n_cams, int red_slots, double* __restrict__ red,
                       double* __restrict__ Dc2, const unsigned char* __restrict__ active,
@@ -665,8 +660,8 @@ small_rig_step_kernel(LmState* __restrict__ st, int nP, int n_cams, int red_slot
                       const int* __restrict__ fixc, int n_fixc, const CamPriors* __restrict__ cp) {
   extern __shared__ __align__(16) double dsm[];
   if (st->done) return;
-  reduced_prep_body<P, false, FIXC, PRIORC>(st, nP, n_cams, red_slots, red, Dc2, active, nullptr, gmax_bits, sc, fixc,
-                                            n_fixc, cp);
+  reduced_prep_body<P, false, HELD>(st, nP, n_cams, red_slots, red, Dc2, active, nullptr, gmax_bits, sc, fixc, n_fixc,
+                                    cp);
   __syncthreads();
   if (st->done) return;  // set by thread 0 before the barrier: gtol / max_nfev / non-finite start (uniform)
   const size_t nn = (size_t)nP * nP;

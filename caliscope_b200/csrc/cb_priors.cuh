@@ -2,10 +2,10 @@
 //   1/2 (x_c - m_c)^T L_c (x_c - m_c)   or   1/2 (X_j - m_j)^T L_j (X_j - m_j)
 // to the objective, always quadratic whatever the loss: the rows W (x - m) with W^T W = L of the augmented least-squares
 // problem.  Each term enters where its parameter's blocks are already formed:
-//   camera priors   add_cam_priors, called by reduced_prep_body (PRIORC, after the (all-)reduce, before the FIXC mask)
+//   camera priors   add_cam_priors, called by reduced_prep_body (HELD, after the (all-)reduce, before the fixed mask)
 //                   and by prior_cam_kernel on the covariance path: L_c into the camera's diagonal block of S,
 //                   L_c (x_c - m_c) into b and the g_c slot, diag L_c into the diag-U slot that feeds the scaling Dc2;
-//   point priors    pt_pass_kernel (PRIORP): L_j into V_j, L_j (X_j - m_j) into g_j, before D, the damping and the
+//   point priors    pt_pass_kernel (HELD): L_j into V_j, L_j (X_j - m_j) into g_j, before D, the damping and the
 //                   factor (the covariance variant: before the pseudo-inverse);
 //   prior cost      prior_cost_kernel, one partial per CTA into the extra cost slots trial_reduce_kernel sums.
 #pragma once
@@ -27,7 +27,7 @@ struct CamPriors {
 };
 
 // n point priors: pt the point of each, mean n x 3, info n x 9 (row-major 3 x 3); idx[j]: the prior of point j or -1
-// (read only by the PRIORP point-pass variants).
+// (read only by the HELD point-pass variants).
 struct PointPriors {
   const int* idx;
   const int* pt;

@@ -212,18 +212,13 @@ class BAProblem:
         self.camera_priors = _prior_arrays(camera_priors, 9, "camera_priors")
         self.point_priors = _prior_arrays(point_priors, 3, "point_priors")
         h = C.c_void_p()
+        pri = None
         if self.has_priors:
             (ci, cm, cl), (pi, pm, pl) = self.camera_priors, self.point_priors
-            pri = L.Priors(len(ci), _ptr(ci), _ptr(cm), _ptr(cl), len(pi), _ptr(pi), _ptr(pm), _ptr(pl))
-            rc = lib.cb_ba_problem_create_priors(C.byref(desc), len(fc), _ptr(fc) if len(fc) else None, len(fp),
-                                                 _ptr(fp) if len(fp) else None, C.byref(pri), self.device,
-                                                 C.c_void_p(stream), C.byref(h))  # fmt: skip
-        elif fixed_cam_params is None and fixed_points is None:
-            rc = lib.cb_ba_problem_create(C.byref(desc), self.device, C.c_void_p(stream), C.byref(h))
-        else:
-            rc = lib.cb_ba_problem_create_fixed(C.byref(desc), len(fc), _ptr(fc) if len(fc) else None, len(fp),
-                                                _ptr(fp) if len(fp) else None, self.device, C.c_void_p(stream),
-                                                C.byref(h))  # fmt: skip
+            pri = C.byref(L.Priors(len(ci), _ptr(ci), _ptr(cm), _ptr(cl), len(pi), _ptr(pi), _ptr(pm), _ptr(pl)))
+        rc = lib.cb_ba_problem_create_priors(C.byref(desc), len(fc), _ptr(fc) if len(fc) else None, len(fp),
+                                             _ptr(fp) if len(fp) else None, pri, self.device, C.c_void_p(stream),
+                                             C.byref(h))  # fmt: skip
         L.check(rc, "problem_create")
         self._h = h
         self.cam_stride = int(lib.cb_ba_cam_stride(h))

@@ -6,7 +6,9 @@
 
 ``dump`` writes one .npz per rig of ``tests/_engine_cases.CASES`` and one rig with rigid-distance constraints: the solve (x,
 cost, nfev, kernel_launches), every array of ``normal_equations`` and, where ``COVARIANCE_CASES`` lists the rig, the
-covariance.  ``compare`` exits non-zero unless every array of every file is equal (NaNs in the same places)."""
+covariance.  Each rig of ``CASES`` is dumped twice more with held parameters, as ``tests/test_gpu_priors.py`` holds them:
+its fixed sets alone (``-fixed``) and its priors beside fixed sets (``-priors+fixed``), from the start vector with the
+true values at the fixed entries.  ``compare`` exits non-zero unless every array of every file is equal (NaNs in the same places)."""
 import sys
 from pathlib import Path
 
@@ -31,17 +33,35 @@ def outputs(p, x0, covariance: bool) -> dict:
     return out
 
 
+def held_problems(rig, x0, xt):
+    """(suffix, priors, BAProblem keywords, start vector) of the rig's two held problems."""
+    from tests import _engine_cases as EC
+    from tests.test_gpu_priors import _case_fixed_sets, _case_priors
+
+    fc, fp = _case_fixed_sets(rig)
+    pr, pfc, pfp = _case_priors(rig, x0)
+    out = []
+    for suffix, pri, c, p in (("-fixed", None, fc, fp), ("-priors+fixed", pr, pfc, pfp)):
+        x = np.where(EC.free_mask(rig, c, p), x0, xt)
+        out.append((suffix, pri, dict(fixed_cam_params=c, fixed_points=p), x))
+    return out
+
+
 def dump(out_dir: Path) -> None:
-    import caliscope_b200 as cb
     from tests import _constraint_cases as CCS
     from tests import _engine_cases as EC
 
     out_dir.mkdir(parents=True, exist_ok=True)
-    rigs = [(c.id, EC.oracle_rig(r), r.x0, None, c.id in EC.COVARIANCE_CASES) for c in EC.CASES.values() for r in [c.make()]]
+    rigs = []
+    for c in EC.CASES.values():
+        r = c.make()
+        rig, cov = EC.oracle_rig(r), c.id in EC.COVARIANCE_CASES
+        rigs.append((c.id, rig, r.x0, None, {}, cov))
+        rigs += [(c.id + s, rig, x, pr, kw, cov) for s, pr, kw, x in held_problems(rig, r.x0, r.x_true)]
     r, rig, _ = CCS.CASES[CONSTRAINED].make()
-    rigs.append(("constrained-" + CONSTRAINED, rig, r.x0, CCS.constraints_of(rig), False))
-    for name, rig, x0, cons, cov in rigs:
-        with cb.BAProblem(rig.cam_flags, rig.cam_const, rig.n_pts, rig.obs_cam, rig.obs_pt, rig.obs_xy, constraints=cons) as p:
+    rigs.append(("constrained-" + CONSTRAINED, rig, r.x0, None, {}, False))
+    for name, rig, x0, pr, kw, cov in rigs:
+        with EC.problem(rig, pr, **kw) as p:
             out = outputs(p, x0, cov)
         np.savez(out_dir / f"{name}.npz", **out)
         print(f"{name}: nfev {out['nfev']} cost {out['cost']:.15e} launches {out['kernel_launches']}" + (", covariance" if cov else ""))

@@ -72,6 +72,45 @@ def oracle_rig(r, keep=None) -> O.Rig:
     return O.Rig(r.cam_flags, r.cam_const, r.n_pts, r.obs_cam[keep], r.obs_pt[keep], r.obs_xy[keep])
 
 
+def problem(rig: O.Rig, pr=None, **kw):
+    """The engine's BAProblem of an oracle rig, with its constraints, the priors ``pr`` (``_held_oracle.Priors``) and
+    BAProblem's keywords ``kw``."""
+    import caliscope_b200 as cb
+
+    cons = (rig.groups_a, rig.groups_b, rig.distances, rig.weights) if rig.n_constraints else None
+    kw.update(pr.kwargs() if pr is not None else {})
+    return cb.BAProblem(rig.cam_flags, rig.cam_const, rig.n_pts, rig.obs_cam, rig.obs_pt, rig.obs_xy, constraints=cons,
+                        **kw)  # fmt: skip
+
+
+def free_mask(rig: O.Rig, cam_params=(), points=()) -> np.ndarray:
+    """Boolean over x: False at the camera-parameter indices and the coordinates of the points given."""
+    free = np.ones(rig.n_params, bool)
+    free[np.asarray(cam_params, np.int64)] = False
+    for j in points:
+        free[rig.n_camera_params + 3 * j : rig.n_camera_params + 3 * j + 3] = False
+    return free
+
+
+def relabelled_sparse_case():
+    """48 cameras with local visibility, two in three with free intrinsics: compacted Schur lists, a camera order the
+    engine chooses itself (test_gpu_engine_paths.py's rig) and 6-parameter cameras inside a P = 9 problem.  Returns the
+    rig, its start vector and its true x."""
+    from caliscope_b200 import synthetic
+
+    r = synthetic.make_rig(48, 4000, 24000, seed=7, cams_per_point=6, refine_intrinsics=True)
+    wide = np.arange(r.n_cams) % 3 != 0
+    const = r.cam_const.copy()
+    const[~wide, :2] = synthetic.WEBCAM_F
+
+    def layout(x):
+        blocks = x[: 9 * r.n_cams].reshape(r.n_cams, 9)
+        return np.concatenate([blocks[c] if wide[c] else blocks[c, :6] for c in range(r.n_cams)] + [x[9 * r.n_cams :]])
+
+    rig = O.Rig(wide.astype(np.int32), const, r.n_pts, r.obs_cam, r.obs_pt, r.obs_xy)
+    return rig, layout(r.x0), layout(r.x_true)
+
+
 def stats(p) -> dict:
     return {k: int(p.stat(k)) for k in (LANES, DUPS, CAM_SMEM, SOLVE, PCG_CTAS, PCG_CL, REORDERED)}
 

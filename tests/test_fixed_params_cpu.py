@@ -9,7 +9,7 @@ import pytest
 from oracle import ba_oracle as O
 from oracle import lm_schur as LS
 from tests import _engine_cases as EC
-from tests import _fixed_oracle as FO
+from tests import _held_oracle as HO
 
 
 def _rig(refine: bool, seed: int = 4):
@@ -51,8 +51,8 @@ def test_masked_dense_lm_reaches_free_subvector_scipy(refine, loss, kind):
     r, rig = _rig(refine)
     free = _free(rig, **_fixed_sets(rig, kind))
     fs = 2e-4
-    ref = FO.solve_scipy_fixed(rig, r.x0, free, loss=loss, f_scale=fs)
-    got = FO.lm_solve_dense(rig, r.x0, free, loss=loss, f_scale=fs)
+    ref = HO.solve_scipy(rig, r.x0, free, loss=loss, f_scale=fs)
+    got = HO.lm_solve_dense(rig, r.x0, free, loss=loss, f_scale=fs)
     print(f"{kind} P{'9' if refine else '6'} {loss}: dense status {got['status']} nfev {got['nfev']} cost "
           f"{got['cost']:.12e} | scipy status {ref.status} nfev {ref.nfev} cost {ref.cost:.12e}")  # fmt: skip
     assert np.array_equal(got["x"][~free], r.x0[~free]) and np.array_equal(ref.x[~free], r.x0[~free])
@@ -70,7 +70,7 @@ def test_masked_dense_lm_reaches_free_subvector_scipy(refine, loss, kind):
 def test_dense_lm_with_every_parameter_free_is_the_oracles():
     r, rig = _rig(False)
     a = LS.lm_solve_dense(rig, r.x0)
-    b = FO.lm_solve_dense(rig, r.x0, np.ones(rig.n_params, bool))
+    b = HO.lm_solve_dense(rig, r.x0, np.ones(rig.n_params, bool))
     assert np.array_equal(a["x"], b["x"]) and a["cost"] == b["cost"] and a["nfev"] == b["nfev"]
 
 
@@ -87,11 +87,11 @@ def test_masked_reduced_system_gives_the_free_subvector_step(refine):
     lin = LS.linearize(r.x0, rig)
     Dc2 = np.where(np.einsum("cii->ci", lin.U) > 0, np.einsum("cii->ci", lin.U), 1.0)
     Dp2 = np.where(np.einsum("jii->ji", lin.V) > 0, np.einsum("jii->ji", lin.V), 1.0)
-    fc, fp = FO.free_slots(free, rig, P)
+    fc, fp = HO.free_slots(free, rig, P)
     active = np.zeros(rig.n_cams * P, bool)
     for c in range(rig.n_cams):
         active[c * P : c * P + rig.cam_offsets[c + 1] - rig.cam_offsets[c]] = True
-    S, b, Einv, Wd = FO.schur_system(lin, rig, lam, Dc2, Dp2, fixed_slots=active & ~fc, fixed_pts=~fp)
+    S, b, Einv, Wd = HO.schur_system(lin, rig, lam, Dc2, Dp2, fixed_slots=active & ~fc, fixed_pts=~fp)
     dc = np.linalg.solve(S, -b).reshape(rig.n_cams, P)
     dp = -np.einsum("jab,jb->ja", Einv, lin.gp + np.einsum("jcpa,cp->ja", Wd, dc))
     # the same step from the full dense system over the free parameters
@@ -109,7 +109,7 @@ def test_masked_reduced_system_gives_the_free_subvector_step(refine):
     assert np.abs(dp.ravel() - d[ncp:]).max() <= 1e-9 * np.abs(d[ncp:]).max()
     assert np.all(dc.ravel()[active & ~fc] == 0.0) and np.all(dp[~fp] == 0.0)
     # linearize's own mask: the Jacobian of the free parameters, fixed columns zero
-    lin_f = FO.linearize(r.x0, rig, free)
+    lin_f = HO.linearize(r.x0, rig, free)
     assert np.all(lin_f.gc.ravel()[active & ~fc] == 0.0) and np.all(lin_f.V[~fp] == 0.0)
 
 
@@ -123,7 +123,7 @@ def test_masked_dense_covariance_is_that_of_the_free_columns():
     x = O.solve_scipy(rig, r.x0).x
     fixed_pts = np.array([2, 11, 23, 40])
     fixed = np.arange(6, 12)  # camera 1
-    ref = FO.dense_covariance(x, rig, fixed, fixed_pts)
+    ref = HO.dense_covariance(x, rig, fixed, fixed_pts)
     free = _free(rig, cams=(1,), points=fixed_pts)
     J = O.jacobian(x, rig).toarray()[:, free]
     assert np.linalg.matrix_rank(J) == J.shape[1]  # every point is seen twice or more: nothing to deflate

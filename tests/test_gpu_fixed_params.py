@@ -1,34 +1,16 @@
 """Fixed camera parameters and fixed points in the engine (DESIGN.md section 4.12): a solve is scipy's least_squares on
-the free subvector, the fixed entries of x come back bit for bit, every shape-selected variant applies the masks, and the
-refused inputs are refused before any device work."""
+the free subvector, the fixed entries of x come back bit for bit, and the refused inputs are refused before any device
+work.  Every shape-selected variant is tested with the priors, in test_gpu_priors.py."""
 from __future__ import annotations
 
 import numpy as np
 import pytest
 
 from oracle import ba_oracle as O
-from oracle import lm_schur as LS
 from tests import _engine_cases as EC
-from tests import _fixed_oracle as FO
+from tests import _held_oracle as HO
 
 pytestmark = pytest.mark.gpu
-
-
-def _problem(rig, **kw):
-    import caliscope_b200 as cb
-
-    cons = (rig.groups_a, rig.groups_b, rig.distances, rig.weights) if rig.n_constraints else None
-    return cb.BAProblem(rig.cam_flags, rig.cam_const, rig.n_pts, rig.obs_cam, rig.obs_pt, rig.obs_xy, constraints=cons,
-                        **kw)  # fmt: skip
-
-
-def _free(rig, cam_params=(), points=()):
-    """Boolean over x: False at the camera-parameter indices and the coordinates of the points given."""
-    free = np.ones(rig.n_params, bool)
-    free[np.asarray(cam_params, np.int64)] = False
-    for j in points:
-        free[rig.n_camera_params + 3 * j : rig.n_camera_params + 3 * j + 3] = False
-    return free
 
 
 def _whole_camera(rig, c):
@@ -66,13 +48,13 @@ def test_solve_matches_scipy_on_the_free_subvector(n_cams, n_pts, n_obs, fixed, 
         fc, fp = _whole_camera(rig, 1), list(range(0, n_pts, 10))
     else:
         fc, fp = _intrinsics_of(rig, range(0, n_cams, 2)), []
-    free = _free(rig, fc, fp)
+    free = EC.free_mask(rig, fc, fp)
     x0 = _known(r.x0, r.x_true, free)
     fs = 2.0 / synthetic.WEBCAM_F
-    ref = FO.solve_scipy_fixed(rig, x0, free, loss=loss, f_scale=fs)
+    ref = HO.solve_scipy(rig, x0, free, loss=loss, f_scale=fs)
     # tolerances 1e-15 never trigger here: 200 evaluations stand for "run to convergence"
-    tight = FO.solve_scipy_fixed(rig, x0, free, loss=loss, f_scale=fs, ftol=1e-15, xtol=1e-15, gtol=1e-15, max_nfev=200)
-    with _problem(rig, fixed_cam_params=fc, fixed_points=fp) as p:
+    tight = HO.solve_scipy(rig, x0, free, loss=loss, f_scale=fs, ftol=1e-15, xtol=1e-15, gtol=1e-15, max_nfev=200)
+    with EC.problem(rig, fixed_cam_params=fc, fixed_points=fp) as p:
         res = p.solve(x0, loss=loss, f_scale=fs)
         rm = p.overall_rmse_px(res.x)
     rm_ref, rm_tight = O.overall_rmse_px(ref.x, rig), O.overall_rmse_px(tight.x, rig)
@@ -111,10 +93,10 @@ def test_fixed_intrinsics_equal_a_camera_without_free_intrinsics():
     rig_a = O.Rig(a_flags, r.cam_const, r.n_pts, r.obs_cam, r.obs_pt, r.obs_xy)
     rig_b = O.Rig(b_flags, r.cam_const, r.n_pts, r.obs_cam, r.obs_pt, r.obs_xy)
     fc = _intrinsics_of(rig_a, [k])
-    with _problem(rig_a, fixed_cam_params=fc) as p:
+    with EC.problem(rig_a, fixed_cam_params=fc) as p:
         assert p.cam_stride == 9
         ra = p.solve(xa)
-    with _problem(rig_b) as p:
+    with EC.problem(rig_b) as p:
         rb = p.solve(xb)
     keep = np.ones(len(xa), bool)
     keep[fc] = False
@@ -126,84 +108,7 @@ def test_fixed_intrinsics_equal_a_camera_without_free_intrinsics():
 
 
 # ---------------------------------------------------------------------------------------------
-# 3. every shape-selected variant
-# ---------------------------------------------------------------------------------------------
-def _relabelled_sparse_case():
-    """48 cameras with local visibility, two in three with free intrinsics: compacted Schur lists and a camera order the
-    engine chooses itself (test_gpu_engine_paths.py's rig).  Returns the rig, its start vector and its true x."""
-    from caliscope_b200 import synthetic
-
-    r = synthetic.make_rig(48, 4000, 24000, seed=7, cams_per_point=6, refine_intrinsics=True)
-    free = np.arange(r.n_cams) % 3 != 0
-    const = r.cam_const.copy()
-    const[~free, :2] = synthetic.WEBCAM_F
-
-    def layout(x):
-        blocks = x[: 9 * r.n_cams].reshape(r.n_cams, 9)
-        return np.concatenate([blocks[c] if free[c] else blocks[c, :6] for c in range(r.n_cams)] + [x[9 * r.n_cams :]])
-
-    rig = O.Rig(free.astype(np.int32), const, r.n_pts, r.obs_cam, r.obs_pt, r.obs_xy)
-    return rig, layout(r.x0), layout(r.x_true)
-
-
-def _case_fixed_sets(rig):
-    """Camera 0 whole, s, k1, k2 of the first other camera with free intrinsics (if any), every seventh point."""
-    fc = _whole_camera(rig, 0)
-    wide = [c for c in range(1, rig.n_cams) if rig.cam_offsets[c + 1] - rig.cam_offsets[c] == 9]
-    if wide:
-        fc += _intrinsics_of(rig, wide[:1])
-    return fc, list(range(3, rig.n_pts, 7))
-
-
-@pytest.mark.parametrize("case", list(EC.CASES) + ["relabelled-sparse-lists"])
-def test_every_variant_applies_the_masks(case):
-    if case == "relabelled-sparse-lists":
-        rig, x0, xt = _relabelled_sparse_case()
-        c = None
-    else:
-        c = EC.CASES[case]
-        r = c.make()
-        rig, x0, xt = EC.oracle_rig(r), r.x0, r.x_true
-    fc, fp = _case_fixed_sets(rig)
-    free = _free(rig, fc, fp)
-    x0 = _known(x0, xt, free)
-    lam = 1e-3
-    with _problem(rig, fixed_cam_params=fc, fixed_points=fp) as p:
-        if c is not None and c.stats:
-            EC.check_stats(p, c)
-        if c is None:
-            print(f"{case}: compacted Schur lists {int(p.stat(0))}")
-            assert p.stat(EC.REORDERED) == 1 and p.stat(0) == 1  # relabelled, compacted lists
-        mode = int(p.stat(EC.SOLVE))
-        P = p.cam_stride
-        ne = p.normal_equations(x0, lam)
-        res = p.solve(x0)
-    lin = LS.linearize(x0, rig)
-    Dc2 = np.einsum("cii->ci", lin.U)
-    Dp2 = np.einsum("jii->ji", lin.V)
-    fcs, fps = FO.free_slots(free, rig, P)
-    active = np.zeros(rig.n_cams * P, bool)
-    for k in range(rig.n_cams):
-        active[k * P : k * P + rig.cam_offsets[k + 1] - rig.cam_offsets[k]] = True
-    S, b, Einv, Wd = FO.schur_system(lin, rig, lam, np.where(Dc2 > 0, Dc2, 1.0), np.where(Dp2 > 0, Dp2, 1.0),
-                                     fixed_slots=active & ~fcs, fixed_pts=~fps)  # fmt: skip
-    scale = np.abs(S).max()
-    assert np.abs(ne["S"] - S).max() < 1e-9 * scale
-    assert np.abs(ne["b"] - b).max() < 1e-9 * np.abs(b).max()
-    EC.check_step(ne["S"], ne["b"], ne["dc"], mode, case)
-    assert np.all(ne["dc"].ravel()[active & ~fcs] == 0.0) and np.all(ne["dp"][~fps] == 0.0)
-    dp = -np.einsum("jab,jb->ja", Einv, lin.gp + np.einsum("jcpa,cp->ja", Wd, ne["dc"]))
-    assert np.abs(ne["dp"] - dp).max() < 1e-9 * np.abs(dp).max()
-    ref = FO.solve_scipy_fixed(rig, x0, free)
-    print(f"{case}: gpu status {res.status} nfev {res.nfev} cost {res.cost:.15e} | scipy nfev {ref.nfev} "
-          f"cost {ref.cost:.15e}")  # fmt: skip
-    assert res.status in (1, 2, 3, 4)
-    assert np.array_equal(res.x[~free], x0[~free])
-    assert res.cost <= ref.cost * (1 + 1e-8)
-
-
-# ---------------------------------------------------------------------------------------------
-# 4. surveyed points: scale and frame from the solve, and a covariance without a gauge argument
+# 3. surveyed points: scale and frame from the solve, and a covariance without a gauge argument
 # ---------------------------------------------------------------------------------------------
 def _centres(x, rig):
     out = []
@@ -229,7 +134,7 @@ def test_surveyed_points_set_scale_and_frame():
     x0 = r.x0.copy()
     for j in picks:
         x0[ncp + 3 * j : ncp + 3 * j + 3] = X[j]
-    with _problem(rig, fixed_points=picks) as p:
+    with EC.problem(rig, fixed_points=picks) as p:
         res = p.solve(x0)
         cov = p.covariance(res.x)
     ct, c0, c1 = _centres(r.x_true, rig), _centres(r.x0, rig), _centres(res.x, rig)
@@ -238,7 +143,7 @@ def test_surveyed_points_set_scale_and_frame():
           f"status {res.status} nfev {res.nfev}")  # fmt: skip
     assert res.status in (1, 2, 3, 4)
     assert e1 < 0.01 and e1 < 0.5 * e0  # the start's translation noise is 0.01 m per axis
-    ref = FO.dense_covariance(res.x, rig, [], picks)
+    ref = HO.dense_covariance(res.x, rig, [], picks)
     e_cam = np.linalg.norm(cov.cameras - ref["cameras"]) / np.linalg.norm(ref["cameras"])
     ok = np.isfinite(ref["points"][:, 0, 0]) & (ref["point_rank"] == 3)
     e_pt = np.linalg.norm(cov.points[ok] - ref["points"][ok]) / np.linalg.norm(ref["points"][ok])
@@ -252,7 +157,7 @@ def test_surveyed_points_set_scale_and_frame():
 
 
 # ---------------------------------------------------------------------------------------------
-# 5. adding a camera to a calibrated rig
+# 4. adding a camera to a calibrated rig
 # ---------------------------------------------------------------------------------------------
 def test_adding_a_camera_keeps_the_calibrated_rig():
     from caliscope_b200 import resection, synthetic
@@ -262,7 +167,7 @@ def test_adding_a_camera_keeps_the_calibrated_rig():
     new = 8
     old_rows = rig.obs_cam != new
     rig_old = EC.oracle_rig(r, old_rows)
-    with _problem(rig_old) as p:
+    with EC.problem(rig_old) as p:
         x_old = p.solve(r.x0).x
     ncp = rig.n_camera_params
     X = x_old[ncp:].reshape(-1, 3)
@@ -275,7 +180,7 @@ def test_adding_a_camera_keeps_the_calibrated_rig():
     o = rig.cam_offsets[new]
     x1[o : o + 6] = poses.pose[0]
     fc = list(range(rig.cam_offsets[new]))  # every old camera
-    with _problem(rig, fixed_cam_params=fc) as p:
+    with EC.problem(rig, fixed_cam_params=fc) as p:
         rm0 = p.overall_rmse_px(x1)
         res = p.solve(x1)
         rm1 = p.overall_rmse_px(res.x)
@@ -288,7 +193,7 @@ def test_adding_a_camera_keeps_the_calibrated_rig():
 
 
 # ---------------------------------------------------------------------------------------------
-# 6. carry-over and repeatability
+# 5. carry-over and repeatability
 # ---------------------------------------------------------------------------------------------
 def test_cull_keeps_the_fixed_sets_and_solves_repeat():
     from caliscope_b200 import filtering, synthetic
@@ -296,8 +201,8 @@ def test_cull_keeps_the_fixed_sets_and_solves_repeat():
     r = synthetic.make_rig(10, 600, 7000, seed=10, outlier_frac=0.02)
     rig = EC.oracle_rig(r)
     fc, fp = _whole_camera(rig, 2) + [3, 4], list(range(0, rig.n_pts, 9))
-    free = _free(rig, fc, fp)
-    with _problem(rig, fixed_cam_params=fc, fixed_points=fp) as p:
+    free = EC.free_mask(rig, fc, fp)
+    with EC.problem(rig, fixed_cam_params=fc, fixed_points=fp) as p:
         a = p.solve(r.x0)
         b = p.solve(r.x0)
         assert np.array_equal(a.x, b.x) and a.cost == b.cost and a.nfev == b.nfev and a.nit == b.nit
@@ -308,7 +213,7 @@ def test_cull_keeps_the_fixed_sets_and_solves_repeat():
             c = p2.solve(a.x)
     assert not keep.all()
     assert np.array_equal(a.x[~free], r.x0[~free]) and np.array_equal(c.x[~free], r.x0[~free])
-    ref = FO.solve_scipy_fixed(EC.oracle_rig(r, keep), a.x, free)
+    ref = HO.solve_scipy(EC.oracle_rig(r, keep), a.x, free)
     print(f"after cull: gpu cost {c.cost:.15e} nfev {c.nfev} | scipy cost {ref.cost:.15e}")
     assert c.status in (1, 2, 3, 4) and c.cost <= ref.cost * (1 + 1e-8)
 
@@ -319,15 +224,15 @@ def test_empty_fixed_lists_equal_the_plain_problem():
     for refine in (False, True):
         r = synthetic.make_rig(12, 700, 9000, seed=3, refine_intrinsics=refine)
         rig = EC.oracle_rig(r)
-        with _problem(rig) as p:
+        with EC.problem(rig) as p:
             a = p.solve(r.x0)
-        with _problem(rig, fixed_cam_params=[], fixed_points=[]) as p:
+        with EC.problem(rig, fixed_cam_params=[], fixed_points=[]) as p:
             b = p.solve(r.x0)
         assert np.array_equal(a.x, b.x) and a.cost == b.cost and a.nfev == b.nfev and a.nit == b.nit, refine
 
 
 # ---------------------------------------------------------------------------------------------
-# 7. refusals
+# 6. refusals
 # ---------------------------------------------------------------------------------------------
 def test_refused_inputs_launch_nothing():
     import caliscope_b200 as cb
@@ -362,7 +267,7 @@ def test_refused_inputs_launch_nothing():
                       fixed_points=[7]) as p:  # fmt: skip
         assert p.solve(r.x0).status in (1, 2, 3, 4)
     # a sharded solve (here the all-reduce callback, on one GPU) is refused
-    with _problem(rig, fixed_points=[7]) as p:
+    with EC.problem(rig, fixed_points=[7]) as p:
         called = []
         n0 = lib.cb_ba_launch_count()
         with pytest.raises(cb.EngineError, match="sharded") as ei:

@@ -1,5 +1,5 @@
 """Gaussian priors on cameras and points in the engine (DESIGN.md section 4.13): every shape-selected variant forms the
-oracle's augmented system, a solve is scipy's least_squares on the augmented residuals, zero information changes
+oracle's system with fixed sets (section 4.12) alone and with priors beside them, a solve is scipy's least_squares on the augmented residuals, zero information changes
 nothing, stiff information approaches the fixed solve, the covariance is the posterior, and the refused inputs are
 refused before any device work."""
 from __future__ import annotations
@@ -10,19 +10,9 @@ import pytest
 from oracle import ba_oracle as O
 from oracle import lm_schur as LS
 from tests import _engine_cases as EC
-from tests import _fixed_oracle as FO
-from tests import _prior_oracle as PO
+from tests import _held_oracle as HO
 
 pytestmark = pytest.mark.gpu
-
-
-def _problem(rig, pr=None, **kw):
-    import caliscope_b200 as cb
-
-    cons = (rig.groups_a, rig.groups_b, rig.distances, rig.weights) if rig.n_constraints else None
-    kw.update(pr.kwargs() if pr is not None else {})
-    return cb.BAProblem(rig.cam_flags, rig.cam_const, rig.n_pts, rig.obs_cam, rig.obs_pt, rig.obs_xy, constraints=cons,
-                        **kw)  # fmt: skip
 
 
 def _width(rig, c):
@@ -66,7 +56,7 @@ def _case_priors(rig, x, seed=0):
     lin = LS.linearize(x, rig)
     u = float(np.median(np.einsum("cii->ci", lin.U)[lin.U[:, 0, 0] > 0]))
     v = float(np.median(np.einsum("jii->ji", lin.V)))
-    pr = PO.Priors()
+    pr = HO.Priors()
     ncp = rig.n_camera_params
 
     def cam_mean(c):
@@ -93,66 +83,58 @@ def _case_priors(rig, x, seed=0):
     return pr, fc, fp
 
 
-def _free(rig, cam_params=(), points=()):
-    free = np.ones(rig.n_params, bool)
-    free[np.asarray(cam_params, np.int64)] = False
-    for j in points:
-        free[rig.n_camera_params + 3 * j : rig.n_camera_params + 3 * j + 3] = False
-    return free
-
-
-def _relabelled_sparse_case():
-    """48 cameras with local visibility, two in three with free intrinsics: compacted Schur lists and a camera order the
-    engine chooses itself (test_gpu_fixed_params.py's rig); 6-parameter cameras inside a P = 9 problem."""
-    from caliscope_b200 import synthetic
-
-    r = synthetic.make_rig(48, 4000, 24000, seed=7, cams_per_point=6, refine_intrinsics=True)
-    wide = np.arange(r.n_cams) % 3 != 0
-    const = r.cam_const.copy()
-    const[~wide, :2] = synthetic.WEBCAM_F
-
-    def layout(x):
-        blocks = x[: 9 * r.n_cams].reshape(r.n_cams, 9)
-        return np.concatenate([blocks[c] if wide[c] else blocks[c, :6] for c in range(r.n_cams)] + [x[9 * r.n_cams :]])
-
-    rig = O.Rig(wide.astype(np.int32), const, r.n_pts, r.obs_cam, r.obs_pt, r.obs_xy)
-    return rig, layout(r.x0), layout(r.x_true)
+def _case_fixed_sets(rig):
+    """Camera 0 whole, s, k1, k2 of the first other camera with free intrinsics (if any), every seventh point."""
+    fc = list(range(rig.cam_offsets[0], rig.cam_offsets[1]))
+    wide = [c for c in range(1, rig.n_cams) if _width(rig, c) == 9]
+    fc += [int(rig.cam_offsets[c]) + a for c in wide[:1] for a in (6, 7, 8)]
+    return fc, list(range(3, rig.n_pts, 7))
 
 
 # ---------------------------------------------------------------------------------------------
-# 1. every shape-selected variant forms the oracle's augmented system
+# 1. every shape-selected variant forms the oracle's system, with fixed sets alone and with priors beside them
 # ---------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("held", ["fixed", "priors+fixed"])
 @pytest.mark.parametrize("case", list(EC.CASES) + ["relabelled-sparse-lists"])
-def test_every_variant_forms_the_augmented_system(case):
+def test_every_variant_forms_the_held_system(case, held):
+    """The engine's U, g_c, V, g_p and cost, its masked reduced system and step, and a solve: the fixed entries come back
+    bit for bit and the cost is at or below scipy's on the free subvector."""
     if case == "relabelled-sparse-lists":
-        rig, x0, xt = _relabelled_sparse_case()
+        rig, x0, xt = EC.relabelled_sparse_case()
         c = None
     else:
         c = EC.CASES[case]
         r = c.make()
         rig, x0, xt = EC.oracle_rig(r), r.x0, r.x_true
-    pr, fc, fp = _case_priors(rig, x0)
-    free = _free(rig, fc, fp)
-    x0 = np.where(free, x0, xt)  # known values at the fixed entries, as test_gpu_fixed_params does
+    if held == "fixed":
+        pr, (fc, fp) = None, _case_fixed_sets(rig)
+    else:
+        pr, fc, fp = _case_priors(rig, x0)
+    free = EC.free_mask(rig, fc, fp)
+    # known values at the fixed entries, as a caller's are: held at a noisy start, a fixed camera or point contradicts
+    # the observations, and the solve crawls along a flat valley where the termination tests stop at scattered points
+    x0 = np.where(free, x0, xt)
     lam = 1e-3
-    with _problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
+    with EC.problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
         if c is not None and c.stats:
             EC.check_stats(p, c)
         if c is None:
+            print(f"{case}: compacted Schur lists {int(p.stat(0))}")
             assert p.stat(EC.REORDERED) == 1 and p.stat(0) == 1  # relabelled, compacted lists
         mode = int(p.stat(EC.SOLVE))
         P = p.cam_stride
         ne = p.normal_equations(x0, lam)
         res = p.solve(x0)
-    whole = PO.linearize(x0, rig, pr)  # what the engine's U, g_c slot, V, g_p hold: every observation, plus the priors
-    lin = PO.linearize(x0, rig, pr, free)
-    Dc2, Dp2 = PO.scaling(x0, rig, pr)
-    fcs, fps = FO.free_slots(free, rig, P)
+    whole = HO.linearize(x0, rig, None, pr)  # what the engine's U, g_c slot, V, g_p hold: every observation, the priors
+    lin = HO.linearize(x0, rig, free, pr)
+    Dc2, Dp2 = HO.scaling(x0, rig, pr)
+    fcs, fps = HO.free_slots(free, rig, P)
     active = np.zeros(rig.n_cams * P, bool)
     for k in range(rig.n_cams):
         active[k * P : k * P + _width(rig, k)] = True
-    S, b, Einv, Wd = PO.schur_system(lin, rig, lam, Dc2, Dp2, active & ~fcs, ~fps)
-    print(f"{case}: P {P} solve mode {mode}, {len(pr.cams)} camera and {len(pr.pts)} point priors")
+    S, b, Einv, Wd = HO.schur_system(lin, rig, lam, Dc2, Dp2, active & ~fcs, ~fps)
+    n_cp, n_pp = (0, 0) if pr is None else (len(pr.cams), len(pr.pts))
+    print(f"{case} {held}: P {P} solve mode {mode}, {n_cp} camera and {n_pp} point priors")
     assert abs(ne["cost"] - whole.cost) <= 1e-12 * whole.cost
     for k, ref in (("U", whole.U), ("gc", whole.gc), ("V", whole.V), ("gp", whole.gp)):
         err = np.abs(ne[k] - ref).max() / np.abs(ref).max()
@@ -163,8 +145,8 @@ def test_every_variant_forms_the_augmented_system(case):
     assert np.all(ne["dc"].ravel()[active & ~fcs] == 0.0) and np.all(ne["dp"][~fps] == 0.0)
     dp = -np.einsum("jab,jb->ja", Einv, lin.gp + np.einsum("jcpa,cp->ja", Wd, ne["dc"]))
     assert np.abs(ne["dp"] - dp).max() < 1e-9 * np.abs(dp).max()
-    ref = PO.solve_scipy_prior(rig, x0, pr, free)
-    print(f"{case}: gpu status {res.status} nfev {res.nfev} cost {res.cost:.15e} | scipy nfev {ref.nfev} "
+    ref = HO.solve_scipy(rig, x0, free, pr)
+    print(f"{case} {held}: gpu status {res.status} nfev {res.nfev} cost {res.cost:.15e} | scipy nfev {ref.nfev} "
           f"cost {ref.cost:.15e}")  # fmt: skip
     assert res.status in (1, 2, 3, 4)
     assert np.array_equal(res.x[~free], x0[~free])
@@ -182,23 +164,23 @@ def test_prior_point_without_observations():
     x0 = np.concatenate([r.x0, [0.3, -0.2, 2.0]])
     mean = np.array([0.31, -0.18, 2.05])
     info = np.array([[4e3, 1e3, 0.0], [1e3, 3e3, 5e2], [0.0, 5e2, 2e3]])
-    pr = PO.Priors()
+    pr = HO.Priors()
     _add_pt(pr, j, mean, info)
-    pr_s = PO.Priors()
+    pr_s = HO.Priors()
     for jj, m in ((j, mean), (0, x0[rig.n_camera_params : rig.n_camera_params + 3]), (1, x0[rig.n_camera_params + 3 :][:3]),
                   (2, x0[rig.n_camera_params + 6 :][:3])):  # fmt: skip
         _add_pt(pr_s, jj, m, info)  # three more priors on seen points fix the gauge for the covariance
-    with _problem(rig, pr) as p:
+    with EC.problem(rig, pr) as p:
         ne = p.normal_equations(x0, 1e-3)
         assert np.array_equal(ne["V"][j], info)
         assert np.allclose(ne["gp"][j], info @ (x0[-3:] - mean), rtol=1e-14)
         res = p.solve(x0)
     assert res.status in (1, 2, 3, 4)
     assert np.abs(res.x[-3:] - mean).max() < 1e-6  # where ftol stops the approach
-    with _problem(rig, pr_s) as p:
+    with EC.problem(rig, pr_s) as p:
         res = p.solve(x0)
         cov = p.covariance(res.x)
-    ref = PO.dense_covariance(res.x, rig, pr_s)
+    ref = HO.dense_covariance(res.x, rig, priors=pr_s)
     assert cov.point_rank[j] == 3 and ref["point_rank"][j] == 3
     want = cov.variance_factor * np.linalg.inv(info)
     assert np.allclose(cov.points[j], want, rtol=1e-9)
@@ -222,7 +204,7 @@ def _pulled_case(n_cams, n_pts, n_obs, seed):
     seen = np.bincount(rig.obs_pt, minlength=rig.n_pts)
     anchor = int(np.argmax(seen))
     fc, fp = list(range(rig.cam_offsets[0], rig.cam_offsets[1])), [anchor]
-    pr = PO.Priors()
+    pr = HO.Priors()
     for c in (3, 5):
         o, w = rig.cam_offsets[c], _width(rig, c)
         L = np.diag(np.einsum("ii->i", lin.U[c])[:w])
@@ -231,7 +213,7 @@ def _pulled_case(n_cams, n_pts, n_obs, seed):
     for j in range(1, rig.n_pts, 9):
         if j != anchor:
             _add_pt(pr, j, X[j] + 5e-3 * rng.standard_normal(3), lin.V[j] + 1e-3 * np.eye(3))
-    free = _free(rig, fc, fp)
+    free = EC.free_mask(rig, fc, fp)
     x0 = np.where(free, r.x0, r.x_true)
     return rig, x0, free, pr, fc, fp
 
@@ -249,10 +231,9 @@ def test_solve_matches_scipy_with_priors(n_cams, n_pts, n_obs, loss, with_fixed)
     if not with_fixed:
         free, fc, fp = np.ones(rig.n_params, bool), [], []
     fs = 2.0 / synthetic.WEBCAM_F
-    ref = PO.solve_scipy_prior(rig, x0, pr, free, loss=loss, f_scale=fs)
-    tight = PO.solve_scipy_prior(rig, x0, pr, free, loss=loss, f_scale=fs, ftol=1e-15, xtol=1e-15, gtol=1e-15,
-                                 max_nfev=200)  # fmt: skip
-    with _problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
+    ref = HO.solve_scipy(rig, x0, free, pr, loss=loss, f_scale=fs)
+    tight = HO.solve_scipy(rig, x0, free, pr, loss=loss, f_scale=fs, ftol=1e-15, xtol=1e-15, gtol=1e-15, max_nfev=200)
+    with EC.problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
         res = p.solve(x0, loss=loss, f_scale=fs)
         rm = p.overall_rmse_px(res.x)
     rm_ref, rm_tight = O.overall_rmse_px(ref.x, rig), O.overall_rmse_px(tight.x, rig)
@@ -267,7 +248,7 @@ def test_solve_matches_scipy_with_priors(n_cams, n_pts, n_obs, loss, with_fixed)
     else:
         assert abs(res.cost - tight.cost) < 1e-6 * tight.cost
     for x, c in ((res.x, res.cost), (x0, res.initial_cost)):
-        want = O.robust_cost(O.residuals(x, rig), loss, fs) + PO.prior_cost(x, rig, pr)
+        want = O.robust_cost(O.residuals(x, rig), loss, fs) + HO.prior_cost(x, rig, pr)
         assert abs(c - want) <= 1e-10 * want
 
 
@@ -280,18 +261,18 @@ def test_huber_and_cauchy_match_scipy_with_priors():
 
     rig, x0, free, pr, fc, fp = _pulled_case(8, 300, 3000, 77)
     fs = 2.0 / synthetic.WEBCAM_F
-    with _problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
+    with EC.problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
         xs = p.solve(x0).x
         for loss in ("huber", "cauchy"):
             res = p.solve(xs, loss=loss, f_scale=fs)
-            ref = PO.solve_scipy_prior(rig, xs, pr, free, loss=loss, f_scale=fs)
+            ref = HO.solve_scipy(rig, xs, free, pr, loss=loss, f_scale=fs)
             print(f"{loss}: gpu status {res.status} nfev {res.nfev} cost {res.cost:.15e} | scipy nfev {ref.nfev} "
                   f"{ref.cost:.15e}")  # fmt: skip
             # scipy crawls here (huber: some 1800 evaluations to stop at a cost 2e-8 above the engine's); the engine's
             # cost is checked to be the augmented objective at its x, so lower is better, not different
             assert res.status in (1, 2, 3, 4)
             assert res.cost <= ref.cost * (1 + 1e-8)
-            want = O.robust_cost(O.residuals(res.x, rig), loss, fs) + PO.prior_cost(res.x, rig, pr)
+            want = O.robust_cost(O.residuals(res.x, rig), loss, fs) + HO.prior_cost(res.x, rig, pr)
             assert abs(res.cost - want) <= 1e-10 * want
 
 
@@ -303,12 +284,12 @@ def test_cost_and_optimality_include_the_priors():
     o = rig.cam_offsets[c]
     u = LS.linearize(x0, rig).U[c]
     _add_cam(pr, rig, c, x0[o : o + 9] + np.r_[0.0, 0.0, 0.0, 1.0, 1.0, 1.0, 0.0, 0.0, 0.0], np.diag(np.diag(u)))
-    lin = PO.linearize(x0, rig, pr, free)
+    lin = HO.linearize(x0, rig, free, pr)
     g = LS.join_x(lin.gc, lin.gp, rig)
     gmax = np.abs(g[free]).max()
-    lin0 = FO.linearize(x0, rig, free)
+    lin0 = HO.linearize(x0, rig, free)
     g0 = np.abs(LS.join_x(lin0.gc, lin0.gp, rig)[free]).max()
-    with _problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
+    with EC.problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
         res = p.solve(x0, gtol=2 * max(gmax, g0))
     print(f"optimality {res.optimality:.12e} (augmented {gmax:.12e}, prior-free {g0:.12e}); cost {res.cost:.12e} "
           f"(augmented {lin.cost:.12e}, prior-free {lin0.cost:.12e})")  # fmt: skip
@@ -322,11 +303,11 @@ def test_prior_pulls_between_the_free_solve_and_the_mean():
     """A camera and points whose prior means sit off the free solution, with information of the data's size: the
     solution lies between the free solve and the mean (on the segment's interior, in both distances)."""
     rig, x0, free, _, fc, fp = _pulled_case(8, 300, 3000, 51)
-    with _problem(rig, fixed_cam_params=fc, fixed_points=fp) as p:
+    with EC.problem(rig, fixed_cam_params=fc, fixed_points=fp) as p:
         xf = p.solve(x0, ftol=1e-12, xtol=1e-12, gtol=1e-12).x
     rng = np.random.default_rng(5)
     lin = LS.linearize(xf, rig)
-    pr = PO.Priors()
+    pr = HO.Priors()
     c = 4
     o, w = rig.cam_offsets[c], _width(rig, c)
     # isotropic information a I: to second order the solution is a + (H + a I)^-1 a (m - a), whose matrix is symmetric
@@ -336,9 +317,9 @@ def test_prior_pulls_between_the_free_solve_and_the_mean():
     pts = [j for j in range(2, rig.n_pts, 23) if j not in fp][:8]
     for j in pts:
         _add_pt(pr, j, xf[ncp + 3 * j : ncp + 3 * j + 3] + 0.01 * rng.standard_normal(3), np.trace(lin.V[j]) / 3 * np.eye(3))
-    with _problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
+    with EC.problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
         xp = p.solve(x0, ftol=1e-12, xtol=1e-12, gtol=1e-12).x
-    for cols, mean, _ in PO.blocks(rig, pr):
+    for cols, mean, _ in HO.blocks(rig, pr):
         a, m, b = xf[cols], mean, xp[cols]
         t = (b - a) @ (m - a) / ((m - a) @ (m - a))
         print(f"x{cols[0]}..: pulled {t:.3f} of the way to the mean")
@@ -356,14 +337,14 @@ def test_zero_information_is_bit_identical(case):
     exact zero (x + 0.0, fma(0, d, v)), so the solve is the prior-free one bit for bit."""
     r = EC.CASES[case].make()
     rig = EC.oracle_rig(r)
-    pr = PO.Priors()
+    pr = HO.Priors()
     for c in range(rig.n_cams):
         _add_cam(pr, rig, c, r.x0[rig.cam_offsets[c] : rig.cam_offsets[c + 1]] + 0.01, np.zeros((6, 6)), slots=range(6))
     for j in range(rig.n_pts):
         _add_pt(pr, j, r.x0[rig.n_camera_params + 3 * j :][:3] - 0.02, np.zeros((3, 3)))
-    with _problem(rig) as p:
+    with EC.problem(rig) as p:
         a = p.solve(r.x0)
-    with _problem(rig, pr) as p:
+    with EC.problem(rig, pr) as p:
         b = p.solve(r.x0)
     print(f"{case}: nfev {a.nfev} / {b.nfev}, cost {a.cost!r} / {b.cost!r}")
     assert np.array_equal(a.x, b.x) and a.cost == b.cost and a.nfev == b.nfev and a.njev == b.njev
@@ -386,14 +367,14 @@ def test_stiff_priors_approach_fixed():
     c = 3
     fc = list(range(rig.cam_offsets[c], rig.cam_offsets[c + 1]))
     x0[fc] = r.x_true[fc]
-    pr = PO.Priors()
+    pr = HO.Priors()
     _add_cam(pr, rig, c, x0[fc], 1e12 * np.eye(6))
     for j in picks:
         _add_pt(pr, j, x0[ncp + 3 * j : ncp + 3 * j + 3], 1e12 * np.eye(3))
     tight = dict(ftol=1e-12, xtol=1e-12, gtol=1e-12)
-    with _problem(rig, fixed_cam_params=fc, fixed_points=picks) as p:
+    with EC.problem(rig, fixed_cam_params=fc, fixed_points=picks) as p:
         a = p.solve(x0, **tight)
-    with _problem(rig, pr) as p:
+    with EC.problem(rig, pr) as p:
         b = p.solve(x0, **tight)
     err = np.abs(a.x - b.x).max()
     print(f"stiff priors vs fixed: max |dx| {err:.2e}, cost {a.cost:.12e} / {b.cost:.12e}, nfev {a.nfev} / {b.nfev}")
@@ -422,7 +403,7 @@ def test_covariance_is_the_posterior(refine):
     pixel_sigma, fx = 0.5, float(rig.cam_const[0, 0])
     vf = (pixel_sigma / fx) ** 2
     rng = np.random.default_rng(61)
-    pr = PO.Priors()
+    pr = HO.Priors()
     sig = {}
     for j in surveyed + [7, 19, 44]:
         S = np.diag([1e-6, 2e-6, 4e-6]) if j in surveyed else np.diag([1e-4, 1e-4, 1e-4])
@@ -435,11 +416,11 @@ def test_covariance_is_the_posterior(refine):
     _add_cam(pr, rig, c, r.x_true[o : o + w] + rng.multivariate_normal(np.zeros(w), Sc),
              uncertainty.prior_information(Sc, pixel_sigma, fx))  # fmt: skip
     x0 = r.x0.copy()
-    with _problem(rig, pr) as p:
+    with EC.problem(rig, pr) as p:
         res = p.solve(x0)
         cov = p.covariance(res.x)
         cov_vf = p.covariance(res.x, variance_factor=vf)
-    ref = PO.dense_covariance(res.x, rig, pr)
+    ref = HO.dense_covariance(res.x, rig, priors=pr)
     e_cam = np.linalg.norm(cov.cameras - ref["cameras"]) / np.linalg.norm(ref["cameras"])
     ok = ref["point_rank"] == 3
     e_pt = np.linalg.norm(cov.points[ok] - ref["points"][ok]) / np.linalg.norm(ref["points"][ok])
@@ -468,8 +449,8 @@ def test_cull_keeps_the_priors():
     r = synthetic.make_rig(10, 600, 7000, seed=10, outlier_frac=0.02)
     rig = EC.oracle_rig(r)
     pr, fc, fp = _case_priors(rig, r.x0, seed=3)
-    free = _free(rig, fc, fp)
-    with _problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
+    free = EC.free_mask(rig, fc, fp)
+    with EC.problem(rig, pr, fixed_cam_params=fc, fixed_points=fp) as p:
         a = p.solve(r.x0)
         _, thr = filtering.percentile_thresholds(p, a.x, 95.0, want_err=False)
         p2, keep = p.cull(a.x, thr, 10)
@@ -479,10 +460,10 @@ def test_cull_keeps_the_priors():
             c = p2.solve(a.x)
     assert not keep.all()
     rig2 = EC.oracle_rig(r, keep)
-    whole = PO.linearize(a.x, rig2, pr)
+    whole = HO.linearize(a.x, rig2, None, pr)
     assert abs(ne["cost"] - whole.cost) <= 1e-12 * whole.cost
     assert np.abs(ne["gc"] - whole.gc).max() <= 1e-10 * np.abs(whole.gc).max()
-    ref = PO.solve_scipy_prior(rig2, a.x, pr, free)
+    ref = HO.solve_scipy(rig2, a.x, free, pr)
     print(f"after cull: gpu cost {c.cost:.15e} nfev {c.nfev} | scipy cost {ref.cost:.15e}")
     assert c.status in (1, 2, 3, 4) and c.cost <= ref.cost * (1 + 1e-8)
     assert np.array_equal(c.x[~free], r.x0[~free])
@@ -556,7 +537,7 @@ def test_refused_inputs_launch_nothing():
                       **cams([1], info=ok[None]), **pts([7], info=tiny_neg[None])) as p:  # fmt: skip
         assert p.solve(r.x0).status in (1, 2, 3, 4)
     # a sharded solve (here the all-reduce callback, on one GPU) is refused
-    with _problem(rig, **pts([7])) as p:
+    with EC.problem(rig, **pts([7])) as p:
         called = []
         n0 = lib.cb_ba_launch_count()
         with pytest.raises(cb.EngineError, match="sharded") as ei:

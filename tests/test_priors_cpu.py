@@ -12,8 +12,7 @@ from caliscope_b200 import uncertainty
 from oracle import ba_oracle as O
 from oracle import lm_schur as LS
 from tests import _engine_cases as EC
-from tests import _fixed_oracle as FO
-from tests import _prior_oracle as PO
+from tests import _held_oracle as HO
 
 
 def _rig(refine: bool, seed: int = 4):
@@ -30,7 +29,7 @@ def _spd(rng, n, scale=1.0):
 
 def _priors(rig, x, rng, zero=False, scale=1e6):
     """Full priors on cameras 0 and 2 and every fifth point, means the start values plus noise."""
-    pr = PO.Priors()
+    pr = HO.Priors()
     cams = [0, 2]
     pr.cams = np.array(cams)
     pr.cam_mean = np.zeros((2, 9))
@@ -52,7 +51,7 @@ def test_zero_information_is_the_prior_free_reference(refine, loss):
     pr = _priors(rig, r.x0, np.random.default_rng(1), zero=True)
     fs = 2e-3  # a scale at which the robust solves converge in a few steps instead of crawling
     ref = O.solve_scipy(rig, r.x0, loss=loss, f_scale=fs)
-    got = PO.solve_scipy_prior(rig, r.x0, pr, loss=loss, f_scale=fs)
+    got = HO.solve_scipy(rig, r.x0, priors=pr, loss=loss, f_scale=fs)
     print(f"P{'9' if refine else '6'} {loss}: prior-oracle nfev {got.nfev} cost {got.cost:.15e} | scipy nfev {ref.nfev} "
           f"cost {ref.cost:.15e}")  # fmt: skip
     # a robust loss goes through scipy's callable-loss path in the one and its named path in the other: the same rho in
@@ -67,8 +66,8 @@ def test_zero_information_is_the_prior_free_reference(refine, loss):
     free = np.ones(rig.n_params, bool)
     free[rig.cam_offsets[1] : rig.cam_offsets[2]] = False
     free[rig.n_camera_params : rig.n_camera_params + 6] = False
-    ref = FO.solve_scipy_fixed(rig, r.x0, free, loss=loss, f_scale=fs)
-    got = PO.solve_scipy_prior(rig, r.x0, pr, free, loss=loss, f_scale=fs)
+    ref = HO.solve_scipy(rig, r.x0, free, loss=loss, f_scale=fs)
+    got = HO.solve_scipy(rig, r.x0, free, pr, loss=loss, f_scale=fs)
     if loss == "linear":
         assert got.nfev == ref.nfev
         # scipy's iterative (lsmr) trust-region solve rounds x further than the cost
@@ -85,19 +84,19 @@ def test_mixed_loss_is_the_named_loss_without_prior_rows(loss):
     f = rng.standard_normal(50) * 3.0
     fs = 0.7
     named = construct_loss_function(len(f), loss, fs)
-    mixed = construct_loss_function(len(f), PO.mixed_loss(len(f), loss, fs), fs)
+    mixed = construct_loss_function(len(f), HO.mixed_loss(len(f), loss, fs), fs)
     want = named(f) if named is not None else np.stack([f * f, np.ones_like(f), np.zeros_like(f)])
     assert np.allclose(mixed(f), want, rtol=1e-14, atol=0.0)
     # prior rows after them are linear whatever the loss: rho = f^2, rho' = 1, rho'' = 0 after scipy's scaling
     g = np.concatenate([f, rng.standard_normal(7)])
-    got = construct_loss_function(len(g), PO.mixed_loss(len(f), loss, fs), fs)(g)
+    got = construct_loss_function(len(g), HO.mixed_loss(len(f), loss, fs), fs)(g)
     assert np.allclose(got[:, : len(f)], want, rtol=1e-14, atol=0.0)
     assert np.allclose(got[0, len(f) :], g[len(f) :] ** 2, rtol=1e-14) and np.all(got[1, len(f) :] == 1.0)
     assert np.all(got[2, len(f) :] == 0.0)
     # and the whole solve without priors is oracle.ba_oracle.solve_scipy's
     r, rig = _rig(False, seed=6)
     ref = O.solve_scipy(rig, r.x0, loss=loss, f_scale=2e-4)
-    got = PO.solve_scipy_prior(rig, r.x0, PO.Priors(), loss=loss, f_scale=2e-4)
+    got = HO.solve_scipy(rig, r.x0, priors=HO.Priors(), loss=loss, f_scale=2e-4)
     assert abs(got.cost - ref.cost) <= 1e-9 * ref.cost
 
 
@@ -113,21 +112,21 @@ def test_prior_reduced_system_gives_the_dense_augmented_step(refine, fixed):
         free[rig.cam_offsets[2] + 6 : rig.cam_offsets[2] + 9] = False  # s, k1, k2 of a camera with a prior
         free[rig.n_camera_params + 3 : rig.n_camera_params + 6] = False  # point 1 (no prior)
     lam = 1e-3
-    lin = PO.linearize(r.x0, rig, pr, free)
-    Dc2, Dp2 = PO.scaling(r.x0, rig, pr)
-    fcs, fps = FO.free_slots(free, rig, P)
+    lin = HO.linearize(r.x0, rig, free, pr)
+    Dc2, Dp2 = HO.scaling(r.x0, rig, pr)
+    fcs, fps = HO.free_slots(free, rig, P)
     active = np.zeros(rig.n_cams * P, bool)
     for k in range(rig.n_cams):
         active[k * P : k * P + rig.cam_offsets[k + 1] - rig.cam_offsets[k]] = True
-    S, b, Einv, Wd = PO.schur_system(lin, rig, lam, Dc2, Dp2, active & ~fcs, ~fps)
+    S, b, Einv, Wd = HO.schur_system(lin, rig, lam, Dc2, Dp2, active & ~fcs, ~fps)
     sl = np.nonzero(active)[0]
     dc = np.zeros(rig.n_cams * P)
     dc[sl] = np.linalg.solve(S[np.ix_(sl, sl)], -b[sl])
     dp = -np.einsum("jab,jb->ja", Einv, lin.gp + np.einsum("jcpa,cp->ja", Wd, dc.reshape(rig.n_cams, P)))
     # dense: H = J^T J + info over the free parameters, damped by lam * D (D from the unmasked blocks)
     J = O.jacobian(r.x0, rig).toarray()
-    H = J.T @ J + PO.info_matrix(rig, pr)
-    g = J.T @ O.residuals(r.x0, rig) + PO.info_matrix(rig, pr) @ (r.x0 - _mean_vector(rig, pr, r.x0))
+    H = J.T @ J + HO.info_matrix(rig, pr)
+    g = J.T @ O.residuals(r.x0, rig) + HO.info_matrix(rig, pr) @ (r.x0 - _mean_vector(rig, pr, r.x0))
     D = np.concatenate([LS.join_x(Dc2, np.zeros((rig.n_pts, 3)), rig)[: rig.n_camera_params], Dp2.ravel()])
     fi = np.nonzero(free)[0]
     d = np.zeros(rig.n_params)
@@ -135,12 +134,12 @@ def test_prior_reduced_system_gives_the_dense_augmented_step(refine, fixed):
     got = LS.join_x(dc.reshape(rig.n_cams, P), dp, rig)
     assert np.abs(got - d).max() <= 1e-8 * np.abs(d).max()
     assert np.all(got[~free] == 0.0)
-    assert abs(lin.cost - (0.5 * O.residuals(r.x0, rig) @ O.residuals(r.x0, rig) + PO.prior_cost(r.x0, rig, pr))) < 1e-12
+    assert abs(lin.cost - (0.5 * O.residuals(r.x0, rig) @ O.residuals(r.x0, rig) + HO.prior_cost(r.x0, rig, pr))) < 1e-12
 
 
 def _mean_vector(rig, pr, x):
     m = np.array(x, dtype=np.float64)
-    for c, mu, _ in PO.blocks(rig, pr):
+    for c, mu, _ in HO.blocks(rig, pr):
         m[c] = mu
     return m
 
@@ -155,11 +154,11 @@ def test_dense_covariance_is_the_inverse_of_the_augmented_normal_matrix():
     pr.cam_mean = np.concatenate([r.x0[: rig.n_camera_params].reshape(-1, 6), np.zeros((rig.n_cams, 3))], axis=1)
     pr.cam_info = np.zeros((rig.n_cams, 9, 9))
     pr.cam_info[:, :6, :6] = _spd(rng, 6, 1e2)
-    cov = PO.dense_covariance(r.x0, rig, pr)
+    cov = HO.dense_covariance(r.x0, rig, priors=pr)
     J = O.jacobian(r.x0, rig).toarray()
-    H = J.T @ J + PO.info_matrix(rig, pr)
+    H = J.T @ J + HO.info_matrix(rig, pr)
     f = O.residuals(r.x0, rig)
-    cost = 0.5 * f @ f + PO.prior_cost(r.x0, rig, pr)
+    cost = 0.5 * f @ f + HO.prior_cost(r.x0, rig, pr)
     m = 2 * rig.n_obs + 6 * rig.n_cams + 3 * len(pr.pts)
     assert cov["dof"] == m - rig.n_params
     s2 = 2 * cost / cov["dof"]
