@@ -157,6 +157,19 @@ class ResectStats(C.Structure):
     ]
 
 
+class RigidStats(C.Structure):
+    _fields_ = [
+        ("group_ms", C.c_double),
+        ("points_ms", C.c_double),
+        ("consensus_ms", C.c_double),
+        ("refine_ms", C.c_double),
+        ("cov_ms", C.c_double),
+        ("total_ms", C.c_double),
+        ("kernel_launches", C.c_int32),
+        ("pad_", C.c_int32),
+    ]
+
+
 class RelPoseStats(C.Structure):
     _fields_ = [
         ("group_ms", C.c_double),
@@ -258,6 +271,12 @@ SYMBOLS = {
         [C.c_int32, _P, _P, _P, C.c_int32, _P, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32,
          C.c_int32, C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, _P, _P, _P, _P, _P,
          _P, C.POINTER(ResectStats), C.c_int, _P],
+    ),
+    "cb_rigid_pose_robust": (
+        C.c_int,
+        [C.c_int32, _P, _P, _P, _P, C.c_int32, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32,
+         C.c_int32, C.c_int32, _P, _P, C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P,
+         _P, _P, _P, _P, _P, _P, C.POINTER(RigidStats), C.c_int, _P],
     ),
     "cb_relative_pose_robust": (
         C.c_int,

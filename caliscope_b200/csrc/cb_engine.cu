@@ -38,6 +38,7 @@
 #include "cb_constraints.cuh"
 #include "cb_triangulate.cuh"
 #include "cb_resect.cuh"
+#include "cb_rigid.cuh"
 #include "cb_bootstrap.cuh"
 #include "cb_relpose.cuh"
 #include "cb_intrinsics.cuh"
@@ -3164,17 +3165,32 @@ int cb_undistort_points(int32_t n_cams, const int32_t* cam_fisheye, const double
 
 namespace {
 
+// the boundaries of the runs of equal keys in the sorted k_sorted (n > 0): d_start (n_groups + 1)
+int sorted_key_bounds(const unsigned long long* k_sorted, int n, cudaStream_t st, ScopedFree& sf, int** d_start,
+                      int* n_groups) {
+  const int TB = 256, G = cdiv(n, TB);
+  int *d_head = nullptr, *d_gid = nullptr, *dstart = nullptr;
+  CB_TRY(sf.alloc(&d_head, (size_t)n));
+  CB_TRY(sf.alloc(&d_gid, (size_t)n));
+  CB_TRY(sf.alloc(&dstart, (size_t)n + 1));
+  CB_LAUNCH(cb::tri_heads_kernel, G, TB, 0, st, k_sorted, (long long)n, d_head);
+  CB_CUB(sf, cub::DeviceScan::InclusiveSum, d_head, d_gid, n, st);
+  g_launches.fetch_add(2);
+  CB_LAUNCH(cb::tri_starts_kernel, G, TB, 0, st, d_head, d_gid, (long long)n, dstart);
+  CB_CUDA(cudaMemcpyAsync(n_groups, d_gid + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  *d_start = dstart;
+  return CB_OK;
+}
+
 // stable sort of the rows by key, group boundaries: d_rows (n), d_start (n_groups + 1)
 int group_by_key(const long long* d_key, int n, cudaStream_t st, ScopedFree& sf, int** d_rows, int** d_start, int* n_groups) {
   const int TB = 256, G = cdiv(n, TB);
   unsigned long long* k_out = nullptr;
-  int *v_in = nullptr, *v_out = nullptr, *d_head = nullptr, *d_gid = nullptr, *dstart = nullptr;
+  int *v_in = nullptr, *v_out = nullptr;
   CB_TRY(sf.alloc(&k_out, (size_t)n));
   CB_TRY(sf.alloc(&v_in, (size_t)n));
   CB_TRY(sf.alloc(&v_out, (size_t)n));
-  CB_TRY(sf.alloc(&d_head, (size_t)n));
-  CB_TRY(sf.alloc(&d_gid, (size_t)n));
-  CB_TRY(sf.alloc(&dstart, (size_t)n + 1));
   CB_LAUNCH(cb::tri_iota_kernel, G, TB, 0, st, v_in, (long long)n);
   // radix passes only over the key's significant bits (a packed (sync, object, keypoint) key of a 50k-point rig has 16)
   unsigned long long* d_max = nullptr;
@@ -3186,14 +3202,8 @@ int group_by_key(const long long* d_key, int n, cudaStream_t st, ScopedFree& sf,
   const int key_bits = std::min(63, bits_for(h_max));
   CB_CUB(sf, cub::DeviceRadixSort::SortPairs, (const unsigned long long*)d_key, k_out, v_in, v_out, n, 0, key_bits, st);
   g_launches.fetch_add(2 + 2 * ((key_bits + 7) / 8));
-  CB_LAUNCH(cb::tri_heads_kernel, G, TB, 0, st, k_out, (long long)n, d_head);
-  CB_CUB(sf, cub::DeviceScan::InclusiveSum, d_head, d_gid, n, st);
-  g_launches.fetch_add(2);
-  CB_LAUNCH(cb::tri_starts_kernel, G, TB, 0, st, d_head, d_gid, (long long)n, dstart);
-  CB_CUDA(cudaMemcpyAsync(n_groups, d_gid + (n - 1), sizeof(int), cudaMemcpyDeviceToHost, st));
-  CB_CUDA(cudaStreamSynchronize(st));
+  CB_TRY(sorted_key_bounds(k_out, n, st, sf, d_start, n_groups));
   *d_rows = v_out;
-  *d_start = dstart;
   return CB_OK;
 }
 
@@ -3504,30 +3514,38 @@ int tri_refine_launch(int32_t n_cams, const TriCams& c, int lanes, const int* st
   return CB_OK;
 }
 
+// The camera covariance cam_cov (x's camera layout) on the device at a uniform stride P (fixed / absent slots 0)
+int tri_cam_cov_upload(int32_t n_cams, const TriCams& c, const double* cam_cov, ScopedFree& sf, cudaStream_t st,
+                       double** d_sig) {
+  const int P = c.P, ncp = c.ncp;
+  const std::vector<int>& xoff = c.xoff;
+  const size_t nP = (size_t)n_cams * P;
+  std::vector<double> sig(nP * nP, 0.0);
+  for (int a = 0; a < n_cams; ++a)
+    for (int p = 0; p < xoff[a + 1] - xoff[a]; ++p)
+      for (int d = 0; d < n_cams; ++d)
+        for (int q = 0; q < xoff[d + 1] - xoff[d]; ++q)
+          sig[((size_t)a * P + p) * nP + (size_t)d * P + q] = cam_cov[(size_t)(xoff[a] + p) * ncp + xoff[d] + q];
+  CB_TRY(sf.alloc(d_sig, nP * nP));
+  CB_CUDA(cudaMemcpyAsync(*d_sig, sig.data(), sizeof(double) * nP * nP, cudaMemcpyHostToDevice, st));
+  CB_CUDA(cudaStreamSynchronize(st));  // `sig` is a stack-lifetime upload
+  return CB_OK;
+}
+
 // tri_cov_kernel over the row list (start, rows; n rows at most), recorded between ev_a and ev_b.  The camera covariance
 // (nullable) goes from x's layout to a uniform stride P (fixed / absent slots 0) and is uploaded once.
 int tri_cov_launch(int32_t n_cams, const TriCams& c, const double* cam_cov, double pixel_sigma, int lanes,
                    const int* start, const int* rows, const int* cam, const double* px, int n, int n_groups,
                    const double* xyz, const int* status, cudaEvent_t ev_a, cudaEvent_t ev_b, ScopedFree& sf,
                    cudaStream_t st, double** d_cov_out) {
-  const int P = c.P, ncp = c.ncp;
-  const std::vector<int>& xoff = c.xoff;
+  const int P = c.P;
   double* d_sig = nullptr;
   double* d_B = nullptr;
   int* d_first = nullptr;
   if (cam_cov) {
-    const size_t nP = (size_t)n_cams * P;
-    std::vector<double> sig(nP * nP, 0.0);
-    for (int a = 0; a < n_cams; ++a)
-      for (int p = 0; p < xoff[a + 1] - xoff[a]; ++p)
-        for (int d = 0; d < n_cams; ++d)
-          for (int q = 0; q < xoff[d + 1] - xoff[d]; ++q)
-            sig[((size_t)a * P + p) * nP + (size_t)d * P + q] = cam_cov[(size_t)(xoff[a] + p) * ncp + xoff[d] + q];
-    CB_TRY(sf.alloc(&d_sig, nP * nP));
-    CB_CUDA(cudaMemcpyAsync(d_sig, sig.data(), sizeof(double) * nP * nP, cudaMemcpyHostToDevice, st));
+    CB_TRY(tri_cam_cov_upload(n_cams, c, cam_cov, sf, st, &d_sig));
     CB_TRY(sf.alloc(&d_B, 3 * (size_t)P * n));
     CB_TRY(sf.alloc(&d_first, (size_t)n));
-    CB_CUDA(cudaStreamSynchronize(st));  // `sig` is a stack-lifetime upload
   }
   double* d_cov = nullptr;
   CB_TRY(sf.alloc(&d_cov, 9 * (size_t)n_groups));
@@ -3961,6 +3979,259 @@ int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam
                      obs_px, obs_on_device, threshold_px, min_inliers, max_samples, use_prior ? 1 : 0, pixel_sigma,
                      max_iter, xtol, max_groups, n_groups_out, cam_out, pose_out, cov_out, rmse_px_out, count_out,
                      n_inliers_out, rep_row_out, status_out, inlier_out, stats, device, stream);
+}
+
+}  // extern "C"
+
+namespace {
+
+// cb_rigid_pose_robust after its argument checks: upload and point validation, grouping by key, the (group, point)
+// sub-groups and their point consensus (tri_consensus_kernel unchanged), the qualified points and priors of every
+// group, the pose consensus, the refinement and the covariance.
+int rigid_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+               const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs, const int32_t* obs_cam,
+               const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px, int obs_on_device, double tau,
+               int32_t min_inliers, int32_t max_pairs, int32_t max_samples, int32_t n_prior, const int64_t* prior_key,
+               const double* prior_pose, double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups,
+               int32_t* n_groups_out, double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
+               int32_t* n_inliers_out, int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out,
+               uint8_t* inlier_out, CbRigidStats* stats, int device, void* stream) {
+  const char* who = "cb_rigid_pose_robust";
+  TriCams cams;
+  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, who, &cams));
+  CB_TRY(select_device(device));
+  *n_groups_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf(st);
+  const int n = (int)n_obs;
+  StageEvents<12> ev;  // 10, 11: around the point consensus inside the points stage
+  CB_TRY(ev.create());
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  const int *d_cam = nullptr, *d_pt = nullptr;
+  const long long* d_key = nullptr;
+  const double *d_px = nullptr, *d_model = nullptr, *d_proj = nullptr;
+  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
+  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
+  CB_TRY(to_device(obs_pt, (size_t)n, obs_on_device, &d_pt, sf, st));
+  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
+  CB_TRY(to_device(model_xyz, 3 * (size_t)n_model, 0, &d_model, sf, st));
+  CB_TRY(to_device(cams.proj.data(), cams.proj.size(), 0, &d_proj, sf, st));
+  {  // model indices in range (tri_validate_kernel's count with the model table as the "cameras")
+    int* d_bad = nullptr;
+    CB_TRY(sf.alloc(&d_bad, 1));
+    CB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+    CB_LAUNCH(cb::tri_validate_kernel, cdiv(n, 256), 256, 0, st, d_pt, nullptr, (long long)n, n_model, d_bad);
+    int bad = 0;
+    CB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaStreamSynchronize(st));
+    if (bad) {
+      g_last_error = std::string(who) + ": model point index out of range in " + std::to_string(bad) + " rows";
+      return CB_E_INVALID;
+    }
+  }
+  ObsGroups g;
+  CB_TRY(obs_group_stage(n_cams, &cams.tab, n, d_cam, (const int64_t*)d_key, d_px, 1, max_groups, n_groups_out, who,
+                         ev[1], sf, st, &g));
+  CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
+  const int n_groups = g.n_groups, lanes = tri_lanes(n, n_groups);
+  const int blocks = cdiv((long long)n_groups * lanes, cb::TRI_THREADS);
+  const size_t cam_smem = tri_camtab_smem(n_cams);
+  const int cam_in_smem = cam_smem ? 1 : 0;
+
+  // point hypotheses: the rows sorted by (group, model point) (stable) into sub-groups, the view-pair consensus of each
+  CB_CUDA(cudaEventRecord(ev[2], st));
+  const int pt_bits = std::max(1, bits_for((unsigned long long)std::max(n_model - 1, 0)));
+  const int key_bits = std::min(64, pt_bits + bits_for((unsigned long long)n_groups));
+  unsigned long long *d_k = nullptr, *d_ks = nullptr;
+  int *d_srows = nullptr, *d_sstart = nullptr, n_sub = 0;
+  CB_TRY(sf.alloc(&d_k, (size_t)n));
+  CB_TRY(sf.alloc(&d_ks, (size_t)n));
+  CB_TRY(sf.alloc(&d_srows, (size_t)n));
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::res_pt_key_kernel<L.value>, blocks, cb::TRI_THREADS, 0, st, g.start, g.rows, d_pt, n_groups, pt_bits,
+              d_k);
+  });
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, g.rows, d_srows, n, 0, key_bits, st);
+  g_launches.fetch_add(2 * ((key_bits + 7) / 8));
+  CB_TRY(sorted_key_bounds(d_ks, n, st, sf, &d_sstart, &n_sub));
+  ObsGroups sg;
+  sg.cam = g.cam; sg.xy = g.xy; sg.rows = d_srows; sg.start = d_sstart; sg.n_groups = n_sub;
+  Consensus pcs;
+  const TriConsensusArgs pargs = {tau, 2, max_pairs, nullptr, nullptr};
+  CB_TRY(tri_consensus_launch(n_cams, cams, d_proj, sg, tri_lanes(n, n_sub), n, d_px, pargs, ev[10], ev[11], sf, st,
+                              &pcs));
+  // the qualified points in (group, point) order, each group's range of them and its prior
+  int *d_qflag = nullptr, *d_qpos = nullptr, *d_qM = nullptr, *d_qG = nullptr, *d_qstart = nullptr, *d_pidx = nullptr;
+  double* d_qX = nullptr;
+  CB_TRY(sf.alloc(&d_qflag, (size_t)n_sub + 1));
+  CB_TRY(sf.alloc(&d_qpos, (size_t)n_sub + 1));
+  CB_LAUNCH(cb::rig_qual_flag_kernel, cdiv(n_sub + 1, 256), 256, 0, st, pcs.status, n_sub, d_qflag);
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_qflag, d_qpos, n_sub + 1, st);
+  g_launches.fetch_add(2);
+  int n_q = 0;
+  CB_CUDA(cudaMemcpyAsync(&n_q, d_qpos + n_sub, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  CB_TRY(sf.alloc(&d_qX, 3 * (size_t)std::max(n_q, 1)));
+  CB_TRY(sf.alloc(&d_qM, (size_t)std::max(n_q, 1)));
+  CB_TRY(sf.alloc(&d_qG, (size_t)std::max(n_q, 1)));
+  CB_LAUNCH(cb::rig_qual_kernel, cdiv(n_sub, 256), 256, 0, st, d_sstart, d_ks, pcs.status, pcs.hyp, n_sub, pt_bits,
+            d_qpos, d_qX, d_qM, d_qG);
+  const long long* d_pkey = nullptr;
+  const double* d_ppose = nullptr;
+  if (n_prior > 0) {
+    CB_TRY(to_device((const long long*)prior_key, (size_t)n_prior, 0, &d_pkey, sf, st));
+    CB_TRY(to_device(prior_pose, 6 * (size_t)n_prior, 0, &d_ppose, sf, st));
+  }
+  CB_TRY(sf.alloc(&d_qstart, (size_t)n_groups + 1));
+  CB_TRY(sf.alloc(&d_pidx, (size_t)n_groups));
+  CB_LAUNCH(cb::rig_group_kernel, cdiv(n_groups + 1, 256), 256, 0, st, g.start, g.rows, d_key, n_groups, d_qG, n_q,
+            d_pkey, n_prior, d_qstart, d_pidx);
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaEventRecord(ev[3], st));
+
+  // pose consensus: winner, count, rep_row, n_inliers, n_points, status 0 / 1 / 5, flags
+  Consensus cs;
+  int* d_npts = nullptr;
+  CB_TRY(consensus_alloc(n_groups, n, cb::RES_HYP, false, sf, st, &cs));
+  CB_TRY(sf.alloc(&d_npts, (size_t)n_groups));
+  CB_CUDA(cudaEventRecord(ev[4], st));
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::rig_consensus_kernel<L.value>, blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
+              cam_in_smem, g.start, g.rows, g.cam, d_pt, d_px, d_model, d_qstart, d_qX, d_qM, d_pidx, d_ppose, n_groups,
+              tau, min_inliers, max_samples, cs.hyp, cs.count, cs.rep, cs.nin, d_npts, cs.status, cs.flag, cs.inl);
+  });
+  CB_CUDA(cudaGetLastError());
+  CB_TRY(consensus_compact(g.rows, n, n_groups, sf, st, &cs));
+  CB_CUDA(cudaEventRecord(ev[5], st));
+
+  // refinement on the consensus rows from the winners
+  double *d_pose = nullptr, *d_rmse = nullptr;
+  int* d_status = nullptr;
+  CB_TRY(sf.alloc(&d_pose, 6 * (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_rmse, (size_t)n_groups));
+  CB_TRY(sf.alloc(&d_status, (size_t)n_groups));
+  CB_CUDA(cudaEventRecord(ev[6], st));
+  with_lanes(lanes, [&](auto L) {
+    CB_LAUNCH(cb::rig_refine_kernel<L.value>, blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams, cam_in_smem,
+              cs.start, cs.rows, g.cam, d_pt, d_px, d_model, n_groups, cs.status, cs.hyp, max_iter, xtol, d_pose,
+              d_rmse, d_status);
+  });
+  CB_CUDA(cudaGetLastError());
+  CB_CUDA(cudaEventRecord(ev[7], st));
+
+  // covariance: with a camera covariance, the consensus rows of each group sorted by camera (stable) so that each
+  // camera's rows are adjacent
+  double* d_cov = nullptr;
+  if (cov_out) {
+    CB_TRY(sf.alloc(&d_cov, 36 * (size_t)n_groups));
+    CB_CUDA(cudaEventRecord(ev[8], st));
+    const int P = cams.P;
+    double* d_M = nullptr;  // the camera term per group
+    if (cam_cov) {
+      double *d_sig = nullptr, *d_B = nullptr;
+      int *d_first = nullptr, *d_crow = nullptr, *d_hpos = nullptr;
+      CB_TRY(tri_cam_cov_upload(n_cams, cams, cam_cov, sf, st, &d_sig));
+      int n_cons = 0;
+      CB_CUDA(cudaMemcpyAsync(&n_cons, cs.n_rows, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CB_CUDA(cudaStreamSynchronize(st));
+      const int cam_bits = std::max(1, bits_for((unsigned long long)(n_cams - 1)));
+      const int ckey_bits = std::min(64, cam_bits + bits_for((unsigned long long)n_groups));
+      CB_TRY(sf.alloc(&d_crow, (size_t)std::max(n_cons, 1)));
+      CB_TRY(sf.alloc(&d_B, 6 * (size_t)P * std::max(n_cons, 1)));
+      CB_TRY(sf.alloc(&d_first, (size_t)std::max(n_cons, 1)));
+      CB_TRY(sf.alloc(&d_hpos, (size_t)std::max(n_cons, 1)));
+      CB_TRY(sf.alloc(&d_M, 21 * (size_t)n_groups));
+      if (n_cons > 0) {
+        with_lanes(lanes, [&](auto L) {
+          CB_LAUNCH(cb::res_pt_key_kernel<L.value>, blocks, cb::TRI_THREADS, 0, st, cs.start, cs.rows, g.cam, n_groups,
+                    cam_bits, d_k);
+        });
+        CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, cs.rows, d_crow, n_cons, 0, ckey_bits, st);
+        g_launches.fetch_add(2 * ((ckey_bits + 7) / 8));
+      }
+      with_lanes(lanes, [&](auto L) {
+        if (P == 9)
+          CB_LAUNCH((cb::rig_camterm_kernel<9, L.value>), blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
+                    cam_in_smem, cs.start, d_crow, g.cam, d_pt, d_px, d_model, n_groups, d_pose, d_status, d_sig, d_B,
+                    d_first, d_hpos, d_M);
+        else
+          CB_LAUNCH((cb::rig_camterm_kernel<6, L.value>), blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
+                    cam_in_smem, cs.start, d_crow, g.cam, d_pt, d_px, d_model, n_groups, d_pose, d_status, d_sig, d_B,
+                    d_first, d_hpos, d_M);
+      });
+    }
+    with_lanes(lanes, [&](auto L) {
+      CB_LAUNCH(cb::rig_cov_kernel<L.value>, blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams, cam_in_smem,
+                cs.start, cs.rows, g.cam, d_pt, d_px, d_model, n_groups, d_pose, d_status, d_M,
+                pixel_sigma * pixel_sigma, d_cov);
+    });
+    CB_CUDA(cudaGetLastError());
+    CB_CUDA(cudaEventRecord(ev[9], st));
+  }
+  CB_CUDA(cudaMemcpyAsync(pose_out, d_pose, sizeof(double) * 6 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rmse_px_out, d_rmse, sizeof(double) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(count_out, cs.count, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(n_inliers_out, cs.nin, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(n_points_out, d_npts, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rep_row_out, cs.rep, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(status_out, d_status, sizeof(int) * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(inlier_out, cs.inl, (size_t)n, cudaMemcpyDeviceToHost, st));
+  if (cov_out) CB_CUDA(cudaMemcpyAsync(cov_out, d_cov, sizeof(double) * 36 * (size_t)n_groups, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (stats) {
+    stats->group_ms = ev.ms(0, 1);
+    stats->points_ms = ev.ms(2, 3);
+    stats->consensus_ms = ev.ms(4, 5);
+    stats->refine_ms = ev.ms(6, 7);
+    if (cov_out) stats->cov_ms = ev.ms(8, 9);
+    stats->total_ms = ev.ms(0, cov_out ? 9 : 7);
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cb_rigid_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                         const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs,
+                         const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px,
+                         int obs_on_device, double threshold_px, int32_t min_inliers, int32_t max_pairs,
+                         int32_t max_samples, int32_t n_prior, const int64_t* prior_key, const double* prior_pose,
+                         double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups, int32_t* n_groups_out,
+                         double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
+                         int32_t* n_inliers_out, int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out,
+                         uint8_t* inlier_out, CbRigidStats* stats, int device, void* stream) {
+  if (n_cams <= 0 || !cam_flags || !cam_const || !cam_x || n_model < 0 || (n_model > 0 && !model_xyz) || n_obs < 0 ||
+      n_obs > 0x7fffffffLL || !n_groups_out || max_groups < 0 ||
+      (n_obs > 0 && (!obs_cam || !obs_key || !obs_pt || !obs_px || !inlier_out || n_model == 0)) ||
+      (max_groups > 0 && (!pose_out || !rmse_px_out || !count_out || !n_inliers_out || !n_points_out || !rep_row_out ||
+                          !status_out)) ||
+      !(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma)) || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol)) ||
+      !(threshold_px > 0.0 && std::isfinite(threshold_px)) || min_inliers < 4 || max_pairs < 1 || max_samples < 1 ||
+      max_samples > 4096 || n_prior < 0 || (n_prior > 0 && (!prior_key || !prior_pose))) {
+    g_last_error = "cb_rigid_pose_robust: bad argument";
+    return CB_E_INVALID;
+  }
+  for (int i = 0; i < n_prior; ++i) {
+    if (i > 0 && !(prior_key[i] > prior_key[i - 1])) {
+      g_last_error = "cb_rigid_pose_robust: prior keys must be strictly ascending";
+      return CB_E_INVALID;
+    }
+    for (int k = 0; k < 6; ++k)
+      if (!std::isfinite(prior_pose[6 * (size_t)i + k])) {
+        g_last_error = "cb_rigid_pose_robust: prior pose " + std::to_string(i) + " is not finite";
+        return CB_E_INVALID;
+      }
+  }
+  return rigid_impl(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_model, model_xyz, n_obs, obs_cam, obs_key, obs_pt,
+                    obs_px, obs_on_device, threshold_px, min_inliers, max_pairs, max_samples, n_prior, prior_key,
+                    prior_pose, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, pose_out, cov_out, rmse_px_out,
+                    count_out, n_inliers_out, n_points_out, rep_row_out, status_out, inlier_out, stats, device, stream);
 }
 
 }  // extern "C"

@@ -1,0 +1,612 @@
+// Robust pose of a rigid body seen by a calibrated rig (cb_rigid_pose_robust, DESIGN.md section 4.14): per group (the
+// rows of one body at one moment, every camera's), Horn poses of triples of triangulated model points scored by MSAC
+// over all rows, the consensus rows, then Levenberg-Marquardt over the body pose (r, t) with X_w = R(r) M + t and its
+// first-order covariance with the rig's camera term.  oracle/rigid_pose_robust.py states the rule.
+//
+// The point hypotheses come from tri_consensus_kernel run unchanged on the (group, model point) sub-groups; the kernels
+// here take the qualified points of each group (qX, qM: ascending model index) and follow the short shape of
+// cb_resect_robust: LANES (8 or 32) lanes per group, the camera table staged in shared memory when it fits.
+// No floating-point atomics: every sum has a fixed order, so repeated calls give bit-identical outputs.
+#pragma once
+#include <cstdint>
+
+#include "cb_device.cuh"
+#include "cb_kernels.cuh"
+#include "cb_resect.cuh"
+#include "cb_triangulate.cuh"
+
+namespace cb {
+
+constexpr double RIG_DEGENERATE = 1e-9;  // |u x v| <= this |u| |v|: a model triangle without a rotation
+
+// Horn's closed-form absolute orientation (JOSA A 4(4), 1987) without scale of three model points M against their
+// world points X: q the eigenvector of the largest eigenvalue of Horn's N (sym4_min_eigvec of -N), R = R(q),
+// t = mean(X) - R mean(M).  False when the model triangle is degenerate or R, t are not finite.
+__device__ __forceinline__ bool rig_horn(const double M[3][3], const double X[3][3], double* R, double* t) {
+  double u[3], v[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    u[a] = M[1][a] - M[0][a];
+    v[a] = M[2][a] - M[0][a];
+  }
+  const double c0 = u[1] * v[2] - u[2] * v[1], c1 = u[2] * v[0] - u[0] * v[2], c2 = u[0] * v[1] - u[1] * v[0];
+  const double nc = sqrt(c0 * c0 + c1 * c1 + c2 * c2);
+  const double nu = sqrt(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]), nv = sqrt(v[0] * v[0] + v[1] * v[1] + v[2] * v[2]);
+  if (!(nc > RIG_DEGENERATE * nu * nv)) return false;
+  double mb[3], xb[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    mb[a] = (M[0][a] + M[1][a] + M[2][a]) / 3.0;
+    xb[a] = (X[0][a] + X[1][a] + X[2][a]) / 3.0;
+  }
+  double S[3][3];  // sum_i (M_i - mean M)(X_i - mean X)^T
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      double s = 0.0;
+#pragma unroll
+      for (int i = 0; i < 3; ++i) s += (M[i][a] - mb[a]) * (X[i][b] - xb[b]);
+      S[a][b] = s;
+    }
+  // -N
+  double A[4][4];
+  A[0][0] = -(S[0][0] + S[1][1] + S[2][2]);
+  A[0][1] = A[1][0] = -(S[1][2] - S[2][1]);
+  A[0][2] = A[2][0] = -(S[2][0] - S[0][2]);
+  A[0][3] = A[3][0] = -(S[0][1] - S[1][0]);
+  A[1][1] = -(S[0][0] - S[1][1] - S[2][2]);
+  A[1][2] = A[2][1] = -(S[0][1] + S[1][0]);
+  A[1][3] = A[3][1] = -(S[2][0] + S[0][2]);
+  A[2][2] = -(-S[0][0] + S[1][1] - S[2][2]);
+  A[2][3] = A[3][2] = -(S[1][2] + S[2][1]);
+  A[3][3] = -(-S[0][0] - S[1][1] + S[2][2]);
+  double q[4];
+  sym4_min_eigvec(A, q);
+  const double w = q[0], x = q[1], y = q[2], z = q[3];
+  R[0] = w * w + x * x - y * y - z * z; R[1] = 2.0 * (x * y - w * z);         R[2] = 2.0 * (x * z + w * y);
+  R[3] = 2.0 * (x * y + w * z);         R[4] = w * w - x * x + y * y - z * z; R[5] = 2.0 * (y * z - w * x);
+  R[6] = 2.0 * (x * z - w * y);         R[7] = 2.0 * (y * z + w * x);         R[8] = w * w - x * x - y * y + z * z;
+  bool ok = true;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    t[a] = xb[a] - (R[3 * a] * mb[0] + R[3 * a + 1] * mb[1] + R[3 * a + 2] * mb[2]);
+    ok = ok && isfinite(t[a]);
+  }
+#pragma unroll
+  for (int k = 0; k < 9; ++k) ok = ok && isfinite(R[k]);
+  return ok;
+}
+
+// squared pixel error of caller row r at body pose (R, t) in its own camera, and whether it is in front of it
+__device__ __forceinline__ double rig_row_err2(const double* cams, int stride, const double* R, const double* t, int r,
+                                               const int* __restrict__ obs_cam, const int* __restrict__ obs_pt,
+                                               const double* __restrict__ obs_px, const double* __restrict__ model,
+                                               bool& front) {
+  const double* M = model + 3 * (size_t)obs_pt[r];
+  double X[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) X[a] = fma(R[3 * a], M[0], fma(R[3 * a + 1], M[1], fma(R[3 * a + 2], M[2], t[a])));
+  return tri_row_err2(cams + (size_t)stride * obs_cam[r], X, reinterpret_cast<const double2*>(obs_px)[r], front);
+}
+
+// Per group, the first qualified point qstart[g] (qG: the group of each qualified point, ascending; qstart[n_groups] =
+// n_q) and the prior row of the group's key (-1: none) by binary searches
+__global__ void rig_group_kernel(const int* __restrict__ start, const int* __restrict__ rows,
+                                 const long long* __restrict__ obs_key, int n_groups, const int* __restrict__ qG, int n_q,
+                                 const long long* __restrict__ prior_key, int n_prior, int* __restrict__ qstart,
+                                 int* __restrict__ prior_idx) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g > n_groups) return;
+  int lo = 0, hi = n_q;  // first qualified point of a group >= g
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (qG[mid] < g) lo = mid + 1;
+    else hi = mid;
+  }
+  qstart[g] = lo;
+  if (g == n_groups) return;
+  const long long key = obs_key[rows[start[g]]];
+  lo = 0;
+  hi = n_prior;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (prior_key[mid] < key) lo = mid + 1;
+    else hi = mid;
+  }
+  prior_idx[g] = (lo < n_prior && prior_key[lo] == key) ? lo : -1;
+}
+
+// 1 for a sub-group with a point hypothesis (consensus status 0), and a zero past the end for the scan
+__global__ void rig_qual_flag_kernel(const int* __restrict__ cstatus, int n_sub, int* __restrict__ flag) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s < n_sub) flag[s] = cstatus[s] == TRI_OK ? 1 : 0;
+  if (s == n_sub) flag[s] = 0;
+}
+
+// The qualified points in (group, model point) order: qX the point hypothesis, qM the model point, qG the group, at
+// position qpos[s] (exclusive scan of the flags) of sub-group s; the sub-group's (group, point) comes from its sorted key
+__global__ void rig_qual_kernel(const int* __restrict__ sstart, const unsigned long long* __restrict__ skey,
+                                const int* __restrict__ cstatus, const double* __restrict__ xyz0, int n_sub, int pt_bits,
+                                const int* __restrict__ qpos, double* __restrict__ qX, int* __restrict__ qM,
+                                int* __restrict__ qG) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= n_sub || cstatus[s] != TRI_OK) return;
+  const int j = qpos[s];
+  const unsigned long long k = skey[sstart[s]];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) qX[3 * (size_t)j + a] = xyz0[3 * (size_t)s + a];
+  qM[j] = (int)(k & ((1ULL << pt_bits) - 1));
+  qG[j] = (int)(k >> pt_bits);
+}
+
+// One group per LANES lanes.  Task 0 is the group's prior pose (prior_idx >= 0), task 1 + m sample m of the group's
+// n_q qualified points (res_sample<3>); the lanes stride over the tasks, each builds its task's Horn pose and scores it
+// over all k rows (slots increase along a lane's tasks, so the first of equal scores stays).  group_argmin picks the
+// winner, which reaches the group's lanes from the lane that owns its task; then consensus_classify.  Writes hyp
+// (R row-major, t; NaN without consensus), count, rep_row, n_inliers, n_points (n_q), status (1, 5 or 0) and the flags.
+template <int LANES>
+__global__ void __launch_bounds__(TRI_THREADS)
+rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
+                     const int* __restrict__ rows, const int* __restrict__ obs_cam, const int* __restrict__ obs_pt,
+                     const double* __restrict__ obs_px, const double* __restrict__ model, const int* __restrict__ qstart,
+                     const double* __restrict__ qX, const int* __restrict__ qM, const int* __restrict__ prior_idx,
+                     const double* __restrict__ prior_pose, int n_groups, double tau, int min_inliers, int max_samples,
+                     double* __restrict__ hyp, int* __restrict__ count, int* __restrict__ rep_row,
+                     int* __restrict__ n_inliers, int* __restrict__ n_points, int* __restrict__ status,
+                     unsigned char* __restrict__ pos_flag, unsigned char* __restrict__ inlier) {
+  extern __shared__ double s_cam[];
+  int stride;
+  const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
+  const int lane = threadIdx.x & (LANES - 1);
+  const long long g = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LANES;
+  const bool live = g < n_groups;
+  const int b = live ? start[g] : 0, e = live ? start[g + 1] : 0, k = e - b;
+  const int q0 = live ? qstart[g] : 0, nq = live ? qstart[g + 1] - q0 : 0;
+  const int pi = live ? prior_idx[g] : -1;
+  const int st = k < 4 ? TRI_FEW_ROWS : TRI_OK;
+  const double tau2 = tau * tau;
+  const double inf = __longlong_as_double(0x7ff0000000000000LL);
+  const long long T = res_triples(nq);
+  const long long ntask = (live && st == TRI_OK) ? 1 + (T < max_samples ? T : (long long)max_samples) : 0;
+  double best = inf, bR[9], bt[3];
+#pragma unroll
+  for (int a = 0; a < 9; ++a) bR[a] = 0.0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) bt[a] = 0.0;
+  long long best_s = 0x7fffffffffffffffLL;
+  for (long long task = lane; task < ntask; task += LANES) {
+    double R[9], t[3];
+    if (task == 0) {
+      if (pi < 0) continue;
+      const double* p = prior_pose + 6 * (size_t)pi;
+      double E[CT_JR + 9];
+      cam_prep_rot(p[0], p[1], p[2], E);
+#pragma unroll
+      for (int a = 0; a < 9; ++a) R[a] = E[CT_R + a];
+#pragma unroll
+      for (int a = 0; a < 3; ++a) t[a] = p[3 + a];
+    } else {
+      int p[3];
+      if (!res_sample<3>(task - 1, T, max_samples, nq, p)) continue;
+      double M[3][3], X[3][3];
+#pragma unroll
+      for (int s = 0; s < 3; ++s) {
+        const int j = q0 + p[s];
+        const double* m = model + 3 * (size_t)qM[j];
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+          M[s][a] = m[a];
+          X[s][a] = qX[3 * (size_t)j + a];
+        }
+      }
+      if (!rig_horn(M, X, R, t)) continue;
+    }
+    double sc = 0.0;
+    for (int i = b; i < e; ++i) {
+      bool front;
+      const double e2 = rig_row_err2(cams, stride, R, t, rows[i], obs_cam, obs_pt, obs_px, model, front);
+      sc += msac_term(front, e2, tau2);
+    }
+    if (sc < best) {
+      best = sc;
+      best_s = task;
+#pragma unroll
+      for (int a = 0; a < 9; ++a) bR[a] = R[a];
+#pragma unroll
+      for (int a = 0; a < 3; ++a) bt[a] = t[a];
+    }
+  }
+  group_argmin<LANES>(best, best_s);
+  const bool found = best < inf;
+  const int owner = found ? (int)(best_s % LANES) : 0;
+  group_bcast<LANES>(bR, owner);
+  group_bcast<LANES>(bt, owner);
+  int nin;
+  const bool ok = consensus_classify<LANES>(
+      found && st == TRI_OK, rows, b, e, lane, tau2, min_inliers,
+      [&](int r, bool& front) { return rig_row_err2(cams, stride, bR, bt, r, obs_cam, obs_pt, obs_px, model, front); },
+      pos_flag, inlier, nin);
+  if (!live || lane != 0) return;
+  count[g] = k;
+  rep_row[g] = rows[b];
+  n_inliers[g] = ok ? nin : 0;
+  n_points[g] = nq;
+  status[g] = st != TRI_OK ? st : ok ? TRI_OK : TRI_NO_CONSENSUS;
+#pragma unroll
+  for (int a = 0; a < 9; ++a) hyp[RES_HYP * g + a] = ok ? bR[a] : res_nan();
+#pragma unroll
+  for (int a = 0; a < 3; ++a) hyp[RES_HYP * g + 9 + a] = ok ? bt[a] : res_nan();
+}
+
+// J = d pi / d (r, t) of the body pose (2 x 6, pixels) from the row's J_X (normalised, 2 x 3) at B (R(r) and its right
+// Jacobian, cam_prep_rot's layout): X_w = R M + t, d X_w / d r = -R [M]x Jr, so row i of J_r is -((J_X,i R) x M) Jr
+__device__ __forceinline__ void rig_jq(const double* B, const double* M, const double* JX, double fx0, double* J) {
+  const double* R = B + CT_R;
+  const double* Jr = B + CT_JR;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    double w[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) w[a] = (JX[3 * i] * R[a] + JX[3 * i + 1] * R[3 + a] + JX[3 * i + 2] * R[6 + a]) * fx0;
+    const double c0 = w[1] * M[2] - w[2] * M[1], c1 = w[2] * M[0] - w[0] * M[2], c2 = w[0] * M[1] - w[1] * M[0];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      J[6 * i + a] = -(c0 * Jr[a] + c1 * Jr[3 + a] + c2 * Jr[6 + a]);
+      J[6 * i + 3 + a] = JX[3 * i + a] * fx0;
+    }
+  }
+}
+
+// X_w = R M + t at B (cam_prep_rot's layout)
+__device__ __forceinline__ void rig_world(const double* B, const double* t, const double* M, double* X) {
+  const double* R = B + CT_R;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) X[a] = fma(R[3 * a], M[0], fma(R[3 * a + 1], M[1], fma(R[3 * a + 2], M[2], t[a])));
+}
+
+// one row's pixel residual rr (2) and J (rig_jq) at body pose B, t
+__device__ __forceinline__ void rig_row_jac(const double* cam, const double* B, const double* t, const double* M,
+                                            double2 px, double* rr, double* J) {
+  double X[3], f[2], JX[6];
+  rig_world(B, t, M, X);
+  obs_res_jx(cam, X[0], X[1], X[2], px.x, px.y, 0, 1.0, f, JX);
+  const double fx0 = cam[CT_FX0];
+  rr[0] = f[0] * fx0;
+  rr[1] = f[1] * fx0;
+  rig_jq(B, M, JX, fx0, J);
+}
+
+// Cost, H = J^T J (packed, 21) and g = J^T r (6) of a group's rows [b, e) at body pose q, summed over the LANES lanes
+template <int LANES>
+__device__ __forceinline__ void rig_normal_eq(const double* cams, int stride, const double* q,
+                                              const int* __restrict__ rows, const int* __restrict__ obs_cam,
+                                              const int* __restrict__ obs_pt, const double* __restrict__ obs_px,
+                                              const double* __restrict__ model, int b, int e, int lane, bool on,
+                                              double (&acc)[28]) {
+#pragma unroll
+  for (int k = 0; k < 28; ++k) acc[k] = 0.0;
+  if (on) {
+    double B[CT_JR + 9];
+    cam_prep_rot(q[0], q[1], q[2], B);
+    for (int i = b + lane; i < e; i += LANES) {
+      const int r = rows[i];
+      double rr[2], J[12];
+      rig_row_jac(cams + (size_t)stride * obs_cam[r], B, q + 3, model + 3 * (size_t)obs_pt[r],
+                  reinterpret_cast<const double2*>(obs_px)[r], rr, J);
+#pragma unroll
+      for (int a = 0; a < 6; ++a) {
+#pragma unroll
+        for (int c = a; c < 6; ++c) acc[ut<6>(a, c)] = fma(J[a], J[c], fma(J[6 + a], J[6 + c], acc[ut<6>(a, c)]));
+        acc[21 + a] = fma(J[a], rr[0], fma(J[6 + a], rr[1], acc[21 + a]));
+      }
+      acc[27] = fma(rr[0], rr[0], fma(rr[1], rr[1], acc[27]));
+    }
+  }
+  group_sum<LANES>(acc);
+}
+
+// Per group with consensus (status 0 from the consensus stage), Levenberg-Marquardt (lm_iterate) over q = (r, t) on the
+// consensus rows (start, rows) from the winner hyp (R to a rotation vector by res_rot_log): res_refine_kernel's loop
+// with every row in its own camera.  Writes pose (the hypothesis for status 2, NaN without consensus), rmse over the
+// consensus rows and status (the consensus stage's 1 and 5, else 2, 3, 4 or 0).
+template <int LANES>
+__global__ void __launch_bounds__(TRI_THREADS)
+rig_refine_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
+                  const int* __restrict__ rows, const int* __restrict__ obs_cam, const int* __restrict__ obs_pt,
+                  const double* __restrict__ obs_px, const double* __restrict__ model, int n_groups,
+                  const int* __restrict__ cstatus, const double* __restrict__ hyp, int max_iter, double xtol,
+                  double* __restrict__ pose, double* __restrict__ rmse, int* __restrict__ status) {
+  extern __shared__ double s_cam[];
+  int stride;
+  const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
+  const int lane = threadIdx.x & (LANES - 1);
+  const long long g = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LANES;
+  const bool live = g < n_groups;
+  int st = live ? cstatus[g] : TRI_FEW_ROWS;
+  const bool on = st == TRI_OK;
+  const int b = on ? start[g] : 0, e = on ? start[g + 1] : 0, n = e - b;
+  double q0[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  if (on) {
+    res_rot_log(hyp + RES_HYP * g, q0);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) q0[3 + k] = hyp[RES_HYP * g + 9 + k];
+  }
+  double q[6];
+#pragma unroll
+  for (int k = 0; k < 6; ++k) q[k] = q0[k];
+  // the sums at the current q live in shared memory, one copy per group, as in res_refine_kernel
+  __shared__ double s_acc[TRI_THREADS / LANES][28];
+  double* sa = s_acc[threadIdx.x / LANES];
+  double cost;
+  {
+    double acc[28];
+    rig_normal_eq<LANES>(cams, stride, q, rows, obs_cam, obs_pt, obs_px, model, b, e, lane, on, acc);
+    if (on && !res_pd<6>(acc)) st = TRI_NOT_PD;
+    if (lane == 0)
+#pragma unroll
+      for (int k = 0; k < 28; ++k) sa[k] = acc[k];
+    cost = acc[27];
+  }
+  const double cost0 = cost;
+  double tr[28];
+  st = lm_iterate<6>(
+      q, on && st == TRI_OK, st, max_iter, xtol,
+      [&](double lam, bool on_, double* d) {
+        __syncwarp();  // lane 0's last write of sa is visible
+        if (!on_) return;
+        double A[21], L[6][6];
+#pragma unroll
+        for (int k = 0; k < 21; ++k) A[k] = sa[k];
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+          A[ut<6>(k, k)] = sa[ut<6>(k, k)] * (1.0 + lam);
+          d[k] = -sa[21 + k];
+        }
+        res_chol<6>(A, 0.0, L);
+        res_chol_solve<6>(L, d);
+      },
+      [&](const double* qt, bool on_) {
+        rig_normal_eq<LANES>(cams, stride, qt, rows, obs_cam, obs_pt, obs_px, model, b, e, lane, on_, tr);
+        __syncwarp();  // every lane has read sa
+        return tr[27] < cost;
+      },
+      [&] {
+        if (lane == 0)
+#pragma unroll
+          for (int k = 0; k < 28; ++k) sa[k] = tr[k];
+        cost = tr[27];
+      },
+      [](const double* v) {
+        double s2 = 0.0;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) s2 += v[k] * v[k];
+        return sqrt(s2);
+      });
+  __syncwarp();  // lane 0's last write of sa is visible
+  if (st == TRI_OK || st == TRI_MAX_ITER) {
+    double h[21];
+#pragma unroll
+    for (int k = 0; k < 21; ++k) h[k] = sa[k];
+    if (!res_pd<6>(h)) st = TRI_NOT_PD;
+  }
+  double B[CT_JR + 9];
+  if (live && st == TRI_OK) cam_prep_rot(q[0], q[1], q[2], B);
+  st = status_behind<LANES>(st, live, b, e, lane, [&](int i) {
+    const int r = rows[i];
+    bool front;
+    rig_row_err2(cams, stride, B + CT_R, q + 3, r, obs_cam, obs_pt, obs_px, model, front);
+    return front ? 1.0 : 0.0;
+  });
+  if (!live || lane != 0) return;
+  const double nan = res_nan();
+  const bool at_start = st == TRI_NOT_PD;
+#pragma unroll
+  for (int k = 0; k < 6; ++k) pose[6 * g + k] = !on ? nan : at_start ? q0[k] : q[k];
+  rmse[g] = !on ? nan : sqrt((at_start ? cost0 : cost) / n);
+  status[g] = st;
+}
+
+// The body pose of group g for the covariance kernels: q = pose[g] and B = cam_prep_rot(q) when `on`, zeros otherwise
+__device__ __forceinline__ void rig_cov_pose(const double* __restrict__ pose, long long g, bool on, double* q,
+                                             double* B) {
+#pragma unroll
+  for (int a = 0; a < 6; ++a) q[a] = on ? pose[6 * g + a] : 0.0;
+  cam_prep_rot(q[0], q[1], q[2], B);
+}
+
+// The camera term of the covariance, per group with status 0, 3 or 4 at the refined pose q* (zero otherwise):
+//   M = sum_{c,d} B_c Sigma_cd B_d^T (packed, 21 per group),  B_c = sum over the consensus rows of camera c of J_q^T J_c
+//   (6 x P, pixels),  Sigma = the camera covariance at a uniform stride P.
+// `rows` are the group's consensus rows sorted by camera within the group (stable), so each camera's rows are adjacent:
+// the lane holding the first row of a run sums the run's B_c into Bs at that position (first = 1), three rows of it at a
+// time (tri_cov_kernel's register budget); the run heads are compacted (hpos), and the lanes gather the unordered pairs
+// of runs with cov_pair_gather over the 3-row halves of each B.
+template <int P, int LANES>
+__global__ void __launch_bounds__(TRI_THREADS)
+rig_camterm_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
+                   const int* __restrict__ rows, const int* __restrict__ obs_cam, const int* __restrict__ obs_pt,
+                   const double* __restrict__ obs_px, const double* __restrict__ model, int n_groups,
+                   const double* __restrict__ pose, const int* __restrict__ status, const double* __restrict__ Sig,
+                   double* __restrict__ Bs, int* __restrict__ first, int* __restrict__ hpos,
+                   double* __restrict__ Mout) {
+  extern __shared__ double s_cam[];
+  int stride;
+  const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
+  const int lane = threadIdx.x & (LANES - 1);
+  const long long g = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LANES;
+  const bool live = g < n_groups;
+  const int st = live ? status[g] : TRI_FEW_ROWS;
+  const bool on = st == TRI_OK || st == TRI_MAX_ITER || st == TRI_BEHIND;
+  const int b = on ? start[g] : 0, e = on ? start[g + 1] : 0;
+  const int nP = n_cams * P;
+  double q[6], B[CT_JR + 9];
+  rig_cov_pose(pose, g, on, q, B);
+  for (int i = b + lane; i < e; i += LANES) {
+    const int c = obs_cam[rows[i]];
+    const bool head = i == b || obs_cam[rows[i - 1]] != c;
+    first[i] = head ? 1 : 0;
+    if (!head) continue;
+    const double* cam = cams + (size_t)stride * c;
+    const double fx0 = cam[CT_FX0];
+#pragma unroll 1
+    for (int hh = 0; hh < 2; ++hh) {
+      double Bc[3][P];
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int p = 0; p < P; ++p) Bc[a][p] = 0.0;
+      for (int j = i; j < e && (j == i || obs_cam[rows[j]] == c); ++j) {
+        const int rj = rows[j];
+        const double* M = model + 3 * (size_t)obs_pt[rj];
+        const double2 px = reinterpret_cast<const double2*>(obs_px)[rj];
+        double X[3], f[2], JX[6], Jc[2 * P], J[12];
+        rig_world(B, q + 3, M, X);
+        obs_jac<P>(cam, X[0], X[1], X[2], px.x, px.y, 0, 1.0, f, JX, Jc);
+        rig_jq(B, M, JX, fx0, J);
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+          const double j0 = hh ? J[3 + a] : J[a], j1 = hh ? J[9 + a] : J[6 + a];
+#pragma unroll
+          for (int p = 0; p < P; ++p) Bc[a][p] = fma(j0, Jc[p] * fx0, fma(j1, Jc[P + p] * fx0, Bc[a][p]));
+        }
+      }
+#pragma unroll
+      for (int a = 0; a < 3; ++a)
+#pragma unroll
+        for (int p = 0; p < P; ++p) Bs[(size_t)i * 6 * P + (3 * hh + a) * P + p] = Bc[a][p];
+    }
+  }
+  __syncwarp();
+  // the positions of the runs' first rows, compacted per group into hpos[b ..], nh of them (the same on every lane)
+  const int wl = threadIdx.x & 31;
+  const unsigned gmask = LANES == 32 ? 0xffffffffu : ((1u << LANES) - 1) << (wl & ~(LANES - 1));
+  int nh = 0;
+  for (int base = b; __any_sync(0xffffffffu, base < e); base += LANES) {
+    const int i = base + lane;
+    const bool hd = i < e && first[i];
+    const unsigned hm = __ballot_sync(0xffffffffu, hd) & gmask;
+    if (hd) hpos[b + nh + __popc(hm & ((1u << wl) - 1))] = i;
+    nh += __popc(hm);
+  }
+  __syncwarp();
+  // M in 3 x 3 blocks: m00, m01 (m10 = m01^T), m11
+  double m00[3][3], m01[3][3], m11[3][3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) m00[a][c] = m01[a][c] = m11[a][c] = 0.0;
+  // x = B_a Sig_ab B_b^T of a pair of runs by 3 x 3 blocks hh (00, 11, 01, 10), one block per iteration; the unordered
+  // pair adds its transpose too
+  for (int idx = lane; idx < 4 * nh * nh; idx += LANES) {
+    const int pr = idx >> 2, hh = idx & 3, ia = pr / nh, ib = pr % nh;
+    const bool same = ia == ib;
+    if (ib < ia || (same && hh == 3)) continue;
+    const int pa = hpos[b + ia], pb = hpos[b + ib];
+    const int ha = hh == 1 || hh == 3 ? 1 : 0, hb = hh == 1 || hh == 2 ? 1 : 0;
+    double x[3][3];
+    cov_pair_gather<P>(Bs + ((size_t)pa * 6 + 3 * ha) * P, Bs + ((size_t)pb * 6 + 3 * hb) * P, P, Sig, nP,
+                       obs_cam[rows[pa]], obs_cam[rows[pb]], x);
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const double d = same ? x[a][c] : x[a][c] + x[c][a];
+        m00[a][c] += hh == 0 ? d : 0.0;
+        m11[a][c] += hh == 1 ? d : 0.0;
+        m01[a][c] += hh == 2 ? x[a][c] : hh == 3 ? x[c][a] : 0.0;
+      }
+  }
+  double m[21];
+#pragma unroll
+  for (int a = 0; a < 6; ++a)
+#pragma unroll
+    for (int c = a; c < 6; ++c)
+      m[ut<6>(a, c)] = a < 3 ? (c < 3 ? m00[a][c] : m01[a][c - 3]) : m11[a - 3][c - 3];
+  group_sum<LANES>(m);
+  if (!live || lane != 0) return;
+#pragma unroll
+  for (int a = 0; a < 21; ++a) Mout[21 * (size_t)g + a] = m[a];
+}
+
+// Per group with status 0, 3 or 4 (NaN otherwise), at the refined pose q*:
+//   Sigma_q = s2 H^-1 + H^-1 M H^-1,  H = sum over the consensus rows of J_q^T J_q,  M = rig_camterm_kernel's camera term
+//   (nullptr: M = 0).
+template <int LANES>
+__global__ void __launch_bounds__(TRI_THREADS)
+rig_cov_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
+               const int* __restrict__ rows, const int* __restrict__ obs_cam, const int* __restrict__ obs_pt,
+               const double* __restrict__ obs_px, const double* __restrict__ model, int n_groups,
+               const double* __restrict__ pose, const int* __restrict__ status, const double* __restrict__ Mg,
+               double s2, double* __restrict__ cov) {
+  extern __shared__ double s_cam[];
+  int stride;
+  const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
+  const int lane = threadIdx.x & (LANES - 1);
+  const long long g = (blockIdx.x * (long long)blockDim.x + threadIdx.x) / LANES;
+  const bool live = g < n_groups;
+  const int st = live ? status[g] : TRI_FEW_ROWS;
+  const bool on = st == TRI_OK || st == TRI_MAX_ITER || st == TRI_BEHIND;
+  const int b = on ? start[g] : 0, e = on ? start[g + 1] : 0;
+  double q[6], B[CT_JR + 9];
+  rig_cov_pose(pose, g, on, q, B);
+  double h[21];
+#pragma unroll
+  for (int a = 0; a < 21; ++a) h[a] = 0.0;
+  for (int i = b + lane; i < e; i += LANES) {
+    const int r = rows[i];
+    double J[12], rr[2];
+    rig_row_jac(cams + (size_t)stride * obs_cam[r], B, q + 3, model + 3 * (size_t)obs_pt[r],
+                reinterpret_cast<const double2*>(obs_px)[r], rr, J);
+#pragma unroll
+    for (int a = 0; a < 6; ++a)
+#pragma unroll
+      for (int c = a; c < 6; ++c) h[ut<6>(a, c)] = fma(J[a], J[c], fma(J[6 + a], J[6 + c], h[ut<6>(a, c)]));
+  }
+  group_sum<LANES>(h);
+  if (!live || lane != 0) return;
+  double* out = cov + 36 * (size_t)g;
+  if (!on) {
+    for (int a = 0; a < 36; ++a) out[a] = res_nan();
+    return;
+  }
+  double m[21];
+#pragma unroll
+  for (int a = 0; a < 21; ++a) m[a] = Mg ? Mg[21 * (size_t)g + a] : 0.0;
+  // H^-1 column by column, then out = s2 H^-1 + H^-1 M H^-1 (symmetrised), res_cov_kernel's tail
+  double L[6][6], Hi[6][6];
+  res_chol<6>(h, 0.0, L);
+#pragma unroll
+  for (int c = 0; c < 6; ++c) {
+    double v[6];
+#pragma unroll
+    for (int a = 0; a < 6; ++a) v[a] = a == c ? 1.0 : 0.0;
+    res_chol_solve<6>(L, v);
+#pragma unroll
+    for (int a = 0; a < 6; ++a) Hi[a][c] = v[a];
+  }
+  double T[6][6];  // M H^-1
+#pragma unroll
+  for (int a = 0; a < 6; ++a)
+#pragma unroll
+    for (int c = 0; c < 6; ++c) {
+      double v = 0.0;
+#pragma unroll
+      for (int j = 0; j < 6; ++j) v += m[a <= j ? ut<6>(a, j) : ut<6>(j, a)] * Hi[j][c];
+      T[a][c] = v;
+    }
+#pragma unroll
+  for (int a = 0; a < 6; ++a)
+#pragma unroll
+    for (int c = a; c < 6; ++c) {
+      double v1 = s2 * Hi[a][c], v2 = s2 * Hi[c][a];
+#pragma unroll
+      for (int j = 0; j < 6; ++j) {
+        v1 += Hi[a][j] * T[j][c];
+        v2 += Hi[c][j] * T[j][a];
+      }
+      out[6 * a + c] = out[6 * c + a] = 0.5 * (v1 + v2);
+    }
+}
+
+}  // namespace cb

@@ -74,8 +74,10 @@ def default_gauge(x, cam_offsets, observed, has_constraints: bool) -> np.ndarray
 
 @dataclass
 class PoseUncertainty:
-    """One camera's pose uncertainty relative to the gauge.  position_cov: world-frame covariance of the centre
-    C = -R^T t; orientation_cov: covariance of the body-frame rotation error (R_true = R exp([e]x)), rad^2."""
+    """A pose's uncertainty, in one of two conventions.  A camera's (``pose_from_extrinsics``, X_cam = R X_w + t,
+    relative to the gauge): position_cov is the world-frame covariance of the centre C = -R^T t.  A rigid body's
+    (``pose_from_body``, X_w = R M + t): position_cov is the world-frame covariance of the body origin t.  In both,
+    orientation_cov is the covariance of the rotation error on the right (R_true = R exp([e]x)), rad^2."""
 
     position_cov: np.ndarray
     orientation_cov: np.ndarray
@@ -101,6 +103,16 @@ def pose_from_extrinsics(rvec, tvec, cov6) -> PoseUncertainty:
     Jr = so3_right_jacobian(r)
     cov6 = np.asarray(cov6, dtype=np.float64)
     return PoseUncertainty(position_cov=G @ cov6 @ G.T, orientation_cov=Jr @ cov6[:3, :3] @ Jr.T)
+
+
+def pose_from_body(rvec, tvec, cov6) -> PoseUncertainty:
+    """First-order uncertainty of a rigid body's pose X_w = R(r) M + t from its 6x6 (r, t) covariance: the body origin
+    is t, so position_cov = cov[3:, 3:]; the rotation error e = Jr(r) dr.  ``tvec`` is unused and kept for the
+    signature of ``pose_from_extrinsics``."""
+    del tvec
+    Jr = so3_right_jacobian(np.asarray(rvec, dtype=np.float64))
+    cov6 = np.asarray(cov6, dtype=np.float64)
+    return PoseUncertainty(position_cov=cov6[3:, 3:].copy(), orientation_cov=Jr @ cov6[:3, :3] @ Jr.T)
 
 
 def camera_poses(x, cam_offsets, cam_cov) -> list[PoseUncertainty | None]:

@@ -490,6 +490,66 @@ int cb_resect_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam
                      int32_t* n_inliers_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
                      CbResectStats* stats, int device, void* stream);
 
+typedef struct CbRigidStats {
+  double group_ms;      /* upload + validation + undistortion + radix sort + group boundaries */
+  double points_ms;     /* the (group, point) sort, the point consensus, the qualified points and the prior lookup */
+  double consensus_ms;  /* Horn hypotheses, MSAC scoring, selection and the compaction of the consensus rows */
+  double refine_ms;     /* the Levenberg-Marquardt kernel on the consensus rows */
+  double cov_ms;        /* the camera sort, the camera-term and covariance kernels (0 without cov_out) */
+  double total_ms;
+  int32_t kernel_launches;
+  int32_t pad_;
+} CbRigidStats;
+
+/* Robust pose of a rigid body seen by a calibrated rig (DESIGN.md section 4.14): X_w = R(r) M + t for the body's own
+ * model points M.  Cameras in the bundle-adjustment layout as cb_triangulate_refine, cam_cov (nullable) the
+ * n_camera_params^2 camera covariance (BAProblem.covariance's cameras).  model_xyz[n_model][3] is a host array in the
+ * body's frame; obs_pt[n_obs] (the model point of a row) indexes it.  Observations (raw pixels) are host arrays or, with
+ * obs_on_device, device pointers (obs_cam, obs_key, obs_pt, obs_px).  A group is the rows of one obs_key: one body at
+ * one moment (key = frame, or (body, frame); several bodies share the model table through disjoint point ranges), k rows
+ * key-sorted and in caller order within a key.  Optional priors: prior_key[n_prior] (strictly ascending) and
+ * prior_pose[n_prior][6] (finite), host arrays; a group's prior is the entry of its key.
+ *   1. k < 4: status 1.  A row whose model point is not finite is unusable: it scores tau^2 and is never an inlier.
+ *   2. point hypotheses: each model point p with rows in the group gets cb_triangulate_robust's consensus on those rows
+ *      (the same tau, min_inliers 2, max_pairs): the DLT point of the best view pair, or none (a point whose rows all
+ *      come from one camera, or whose views do not agree; its rows still take part in scoring and refinement).  The
+ *      qualified points are the points with a point hypothesis, positions 0..n_q-1 in ascending model index.
+ *   3. samples, T = C(n_q, 3): every triple in lexicographic order when T <= max_samples, else cb_resect_robust's
+ *      splitmix64 draw.
+ *   4. pose hypothesis of a sample: Horn's closed-form absolute orientation (JOSA A 4(4), 1987) without scale of the
+ *      three model points against their point hypotheses: q the eigenvector of the largest eigenvalue of Horn's 4 x 4 N,
+ *      R = R(q), t = mean(X) - R mean(M).  None when the model triangle is degenerate,
+ *      |(M_j - M_i) x (M_l - M_i)| <= 1e-9 |M_j - M_i| |M_l - M_i|, or R or t is not finite.  The group's prior, if it
+ *      has one, is slot 0; sample m is slot 1 + m.
+ *   5. score (MSAC): sum over all k rows of min(e_r^2, tau^2), e_r = |pi(R M_r + t; c_r) - u_r| in raw pixels with the
+ *      engine's projection and the row's own camera; a row behind its camera, with a non-finite error or an unusable
+ *      point adds tau^2.  The lowest score wins, the lowest slot on a tie.
+ *   6. consensus set: the usable rows in front of their camera with e_r^2 <= tau^2 at the winner.  No hypothesis, or
+ *      fewer than min_inliers such rows: status 5 (pose, cov, rmse NaN, n_inliers 0, no row inlier).  One round.
+ *   7. Levenberg-Marquardt over q = (r, t) on the consensus rows from the winner's R as a rotation vector with theta in
+ *      [0, pi]: cb_resect_robust's loop (lambda0 1e-3, / 10, * 10, |d| <= xtol (|q| + xtol), max_iter) with
+ *      J_q = J_X [d(R(r) M)/dr | I] per row.
+ *   8. cov = pixel_sigma^2 H^-1 + H^-1 G cam_cov G^T H^-1, G = sum over the consensus rows of J_q^T J_c (6 x
+ *      n_camera_params, pixels); without cam_cov the first term alone.  It assumes the body's observations are
+ *      independent of those that calibrated the rig, and takes the model as exact.
+ *   9. status, first match wins: 1;  5;  2 H not positive definite at the start or at the solution (a Cholesky pivot
+ *      <= 1e-12 of the Jacobi-scaled D^-1/2 H D^-1/2, e.g. every consensus row on one marker; pose = the hypothesis, cov
+ *      NaN);  3 max_iter reached;  4 a consensus row is behind its camera at q*;  0 none.
+ * Arguments: threshold_px tau finite > 0, min_inliers >= 4, max_pairs >= 1, 1 <= max_samples <= 4096, max_iter >= 1,
+ * finite pixel_sigma >= 0 and xtol >= 0; obs_pt in [0, n_model).
+ * Outputs per group in ascending key order (host, room for max_groups): pose[6] = (r, t), cov[36] (nullable), rmse_px
+ * over the consensus rows, count, n_inliers, n_points (qualified points), rep_row, status; inlier[n_obs] (caller
+ * order).  No floating-point atomics: repeated calls return bit-identical outputs. */
+int cb_rigid_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                         const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs,
+                         const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px,
+                         int obs_on_device, double threshold_px, int32_t min_inliers, int32_t max_pairs,
+                         int32_t max_samples, int32_t n_prior, const int64_t* prior_key, const double* prior_pose,
+                         double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups, int32_t* n_groups_out,
+                         double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
+                         int32_t* n_inliers_out, int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out,
+                         uint8_t* inlier_out, CbRigidStats* stats, int device, void* stream);
+
 typedef struct CbRelPoseStats {
   double group_ms;      /* upload + undistortion + grouping by key, the correspondence slots and their sort by pair */
   double consensus_ms;  /* five-point hypotheses, MSAC scoring, selection and the compaction of the consensus sets */

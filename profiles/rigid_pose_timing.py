@@ -1,0 +1,162 @@
+"""Stage times and accuracy of cb_rigid_pose_robust (DESIGN.md 4.14), one JSON line per workload.
+
+    python profiles/rigid_pose_timing.py [track] [board64] [--steps 5] [--warmup 2]
+
+track: section 4.9's scene (resect_robust_timing.make("track")) keyed by frame: a 0.2 m cluster of 12 markers seen by 8
+pinhole cameras 3 m away over 50 000 frames, 50 000 groups of 96 rows, 5 % of the rows moved by up to +-200 px, no
+prior.  The same input keyed by (camera, frame) goes through resect_robust, and each camera's pose of the cluster is
+turned into a body pose (X_w = R_c^T (X_cam - t_c)) for the per-camera error beside the rig's.  board64: 64 pinhole
+cameras on a ring of 3 m around a 10 x 7 ChArUco-like board (0.04 m squares, 70 corners) at 2 000 random poses, a
+corner seen by the cameras on its front side (about 2 200 rows per frame), 5 % outliers, with the camera covariance
+term (a block-diagonal 1 mrad / 1 mm camera covariance, the cameras perturbed by one draw of it).  Stage times are the
+CUDA events recorded inside the call (CbRigidStats), the median over --steps timed calls after --warmup.  Pose errors
+are over the groups with status 0: the angle of R_true^T R and the distance of the body origins; chi2 is the mean of
+e^T Sigma^-1 e over those groups (6 when the covariance is calibrated).  The card's name and power limit are printed with
+the numbers.
+"""
+import argparse
+import json
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+HERE = Path(__file__).resolve().parent
+sys.path.insert(0, str(HERE.parent))
+sys.path.insert(0, str(HERE))
+from caliscope_b200.resection import resect_robust  # noqa: E402
+from caliscope_b200.rigid import RigidStats, pose_rigid_robust  # noqa: E402
+from resect_robust_timing import _outliers, card, make, rodrigues  # noqa: E402
+from scipy.spatial.transform import Rotation  # noqa: E402
+
+TAU = 4.0
+
+
+def _rotvec(R):
+    """rotation vectors of (n, 3, 3) matrices, NaN where R is not finite"""
+    R = np.asarray(R, np.float64)
+    ok = np.isfinite(R).all(axis=(-2, -1))
+    out = np.full(R.shape[:-1], np.nan)
+    out[ok] = Rotation.from_matrix(R[ok]).as_rotvec()
+    return out
+
+
+def _ring(centers, target=(0.0, 0.0, 1.0)):
+    """(R, t) of cameras at `centers` looking at `target` (z forward, y down)"""
+    Rc = []
+    for c in centers:
+        z = np.asarray(target) - c
+        z /= np.linalg.norm(z)
+        x = np.cross([0.0, 0.0, -1.0], z)
+        x /= np.linalg.norm(x)
+        Rc.append(np.stack([x, np.cross(z, x), z]))
+    Rc = np.array(Rc)
+    return Rc, -np.einsum("cij,cj->ci", Rc, centers)
+
+
+def _errors(pose, truth, m):
+    if not m.any():
+        return {}
+    dR = np.einsum("nji,njk->nik", rodrigues(pose[m, :3]), rodrigues(truth[m, :3]))
+    ang = np.degrees(np.arccos(np.clip((np.trace(dR, axis1=1, axis2=2) - 1) / 2, -1, 1)))
+    d = np.linalg.norm(pose[m, 3:] - truth[m, 3:], axis=1) * 1e3
+    return {"pos_median_mm": float(np.median(d)), "pos_p99_mm": float(np.percentile(d, 99)),
+            "angle_median_deg": float(np.median(ang)), "angle_p99_deg": float(np.percentile(ang, 99))}  # fmt: skip
+
+
+def _chi2(pose, cov, truth, m):
+    e = pose[m] - truth[m]
+    return float(np.mean(np.einsum("gi,gi->g", e, np.linalg.solve(cov[m], e[:, :, None])[:, :, 0])))
+
+
+def track():
+    """(rigid inputs, body truth per frame, moved rows, kwargs, per-camera body errors from resect_robust)"""
+    (flags, const, cam_x, mk, obs_cam, key, obs_pt, px), truth_g, moved, _ = make("track")
+    n_cams = len(flags)
+    n_frames = len(truth_g) // n_cams
+    # the scene's cameras (make's look-at ring), with rotation vectors that hold near theta = pi too
+    ang = 2 * np.pi * np.arange(n_cams) / n_cams
+    Rc, tc = _ring(np.stack([3 * np.cos(ang), 3 * np.sin(ang), np.full(n_cams, 1.0)], axis=1))
+    cam_x = np.concatenate([_rotvec(Rc), tc], axis=1).ravel()
+    # body pose from camera 0's camera-from-cluster truth: R_b = R_c^T R_g, t_b = R_c^T (t_g - t_c)
+    Rb = np.einsum("ji,fjk->fik", Rc[0], rodrigues(truth_g[:n_frames, :3]))
+    tb = np.einsum("ji,fj->fi", Rc[0], truth_g[:n_frames, 3:] - tc[0])
+    truth = np.concatenate([_rotvec(Rb), tb], axis=1)
+    frame = key % n_frames
+    t0 = time.perf_counter()
+    r = resect_robust(flags, const, cam_x, mk, obs_cam, key, obs_pt, px, threshold_px=TAU, use_prior=False)
+    res_s = time.perf_counter() - t0
+    g = np.arange(len(r.pose))
+    c, f = g // n_frames, g % n_frames
+    Rw = np.einsum("gji,gjk->gik", Rc[c], rodrigues(r.pose[:, :3]))
+    tw = np.einsum("gji,gj->gi", Rc[c], r.pose[:, 3:] - tc[c])
+    per_cam = _errors(np.concatenate([_rotvec(Rw), tw], axis=1), truth[f], r.status == 0)
+    per_cam["wall_s"] = res_s
+    return (flags, const, cam_x, mk, obs_cam, frame.astype(np.int64), obs_pt, px), truth, moved, {}, per_cam
+
+
+def board64(n_frames=2000):
+    rng = np.random.default_rng(11)
+    n_cams = 64
+    ang = 2 * np.pi * np.arange(n_cams) / n_cams
+    centers = np.stack([3 * np.cos(ang), 3 * np.sin(ang), 1.0 + 0.3 * np.sin(3 * ang)], axis=1)
+    Rc, tc = _ring(centers)
+    gx, gy = np.meshgrid(np.arange(10) * 0.04, np.arange(7) * 0.04)
+    model = np.stack([gx.ravel() - 0.18, gy.ravel() - 0.12, np.zeros(70)], axis=1)
+    rv = rng.normal(size=(n_frames, 3))
+    rv *= (rng.uniform(0, 0.8 * np.pi, n_frames) / np.linalg.norm(rv, axis=1))[:, None]
+    truth = np.concatenate([rv, rng.uniform(-0.3, 0.3, (n_frames, 3)) + [0.0, 0.0, 1.0]], axis=1)
+    Rb = rodrigues(rv)
+    Xw = np.einsum("fij,mj->fmi", Rb, model) + truth[:, None, 3:]  # (f, m, 3)
+    normal = Rb[:, :, 2]  # board z in the world
+    Xc = np.einsum("cij,fmj->cfmi", Rc, Xw) + tc[:, None, None]
+    facing = np.einsum("fi,cfi->cf", normal, centers[:, None] - truth[None, :, 3:]) > 0
+    vis = facing[:, :, None] & (Xc[..., 2] > 0.1)
+    uv = Xc[..., :2] / Xc[..., 2:] * 1000.0 + [640.0, 360.0]
+    c, f, m = np.nonzero(vis)
+    order = np.lexsort((c, m, f))
+    c, f, m = c[order], f[order], m[order]
+    px = uv[c, f, m] + rng.normal(0, 0.5, (len(c), 2))
+    px, moved = _outliers(rng, px)
+    flags = np.zeros(n_cams, np.int32)
+    const = np.zeros((n_cams, 9))
+    const[:, :4] = [1000.0, 1000.0, 640.0, 360.0]
+    cam_x = np.concatenate([_rotvec(Rc), tc], axis=1).ravel()
+    cc = np.diag(np.tile([1e-3**2] * 3 + [1e-3**2] * 3, n_cams))
+    x_cal = cam_x + np.sqrt(np.diag(cc)) * rng.normal(size=len(cam_x))
+    args = (flags, const, x_cal, model, c.astype(np.int32), f.astype(np.int64), m.astype(np.int32), px)
+    return args, truth, moved, {"camera_cov": cc}, None
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("workloads", nargs="*", default=["track", "board64"])
+    ap.add_argument("--steps", type=int, default=5)
+    ap.add_argument("--warmup", type=int, default=2)
+    a = ap.parse_args()
+    who = card()
+    for name in a.workloads:
+        args, truth, moved, kw, per_cam = {"track": track, "board64": board64}[name]()
+        runs = []
+        for i in range(a.warmup + a.steps):
+            st = RigidStats()
+            r = pose_rigid_robust(*args, threshold_px=TAU, pixel_sigma=0.5, stats=st, **kw)
+            if i >= a.warmup:
+                runs.append(st)
+        med = lambda f: float(np.median([getattr(s, f) for s in runs]))  # noqa: E731
+        ok = r.status == 0
+        out = {"workload": name, "card": who, "groups": int(len(r.status)), "rows": int(len(args[4])),
+               "stage_ms": {f: med(f) for f in ("group_ms", "points_ms", "consensus_ms", "refine_ms", "cov_ms",
+                                                "total_ms")},
+               "kernel_launches": runs[-1].kernel_launches, "status0": float(ok.mean()),
+               "moved_rows": int(moved.sum()), "moved_rejected": float((~r.inlier[moved]).mean()),
+               "clean_kept": float(r.inlier[~moved].mean()), "rig": _errors(r.pose, truth, ok),
+               "chi2_mean": _chi2(r.pose, r.cov, truth, ok)}  # fmt: skip
+        if per_cam is not None:
+            out["per_camera_resect"] = per_cam
+        print(json.dumps(out), flush=True)
+
+
+if __name__ == "__main__":
+    main()
