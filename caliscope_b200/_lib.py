@@ -278,6 +278,12 @@ SYMBOLS = {
          C.c_int32, C.c_int32, _P, _P, C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P,
          _P, _P, _P, _P, _P, _P, C.POINTER(RigidStats), C.c_int, _P],
     ),
+    "cb_rigid_pose_robust_gp3p": (
+        C.c_int,
+        [C.c_int32, _P, _P, _P, _P, C.c_int32, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32,
+         C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32),
+         _P, _P, _P, _P, _P, _P, _P, _P, _P, C.POINTER(RigidStats), C.c_int, _P],
+    ),
     "cb_relative_pose_robust": (
         C.c_int,
         [C.c_int32, _P, _P, _P, C.c_int64, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32, C.c_double, C.c_int32,

@@ -3995,8 +3995,8 @@ int rigid_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const
                const double* prior_pose, double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups,
                int32_t* n_groups_out, double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
                int32_t* n_inliers_out, int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out,
-               uint8_t* inlier_out, CbRigidStats* stats, int device, void* stream) {
-  const char* who = "cb_rigid_pose_robust";
+               uint8_t* inlier_out, CbRigidStats* stats, int device, void* stream, int32_t gp3p_samples,
+               const char* who) {
   TriCams cams;
   CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, who, &cams));
   CB_TRY(select_device(device));
@@ -4092,16 +4092,24 @@ int rigid_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[3], st));
 
-  // pose consensus: winner, count, rep_row, n_inliers, n_points, status 0 / 1 / 5, flags
+  // pose consensus: winner, count, rep_row, n_inliers, n_points, status 0 / 1 / 5, flags; the gP3P variant only when
+  // gP3P samples are asked for
   Consensus cs;
   int* d_npts = nullptr;
   CB_TRY(consensus_alloc(n_groups, n, cb::RES_HYP, false, sf, st, &cs));
   CB_TRY(sf.alloc(&d_npts, (size_t)n_groups));
   CB_CUDA(cudaEventRecord(ev[4], st));
   with_lanes(lanes, [&](auto L) {
-    CB_LAUNCH(cb::rig_consensus_kernel<L.value>, blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
-              cam_in_smem, g.start, g.rows, g.cam, d_pt, d_px, d_model, d_qstart, d_qX, d_qM, d_pidx, d_ppose, n_groups,
-              tau, min_inliers, max_samples, cs.hyp, cs.count, cs.rep, cs.nin, d_npts, cs.status, cs.flag, cs.inl);
+    if (gp3p_samples > 0)
+      CB_LAUNCH((cb::rig_consensus_kernel<L.value, true>), blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
+                cam_in_smem, g.start, g.rows, g.cam, d_pt, d_px, d_model, d_qstart, d_qX, d_qM, d_pidx, d_ppose,
+                n_groups, tau, min_inliers, max_samples, cs.hyp, cs.count, cs.rep, cs.nin, d_npts, cs.status, cs.flag,
+                cs.inl, g.xy, gp3p_samples);
+    else
+      CB_LAUNCH((cb::rig_consensus_kernel<L.value, false>), blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
+                cam_in_smem, g.start, g.rows, g.cam, d_pt, d_px, d_model, d_qstart, d_qX, d_qM, d_pidx, d_ppose,
+                n_groups, tau, min_inliers, max_samples, cs.hyp, cs.count, cs.rep, cs.nin, d_npts, cs.status, cs.flag,
+                cs.inl, nullptr, 0);
   });
   CB_CUDA(cudaGetLastError());
   CB_TRY(consensus_compact(g.rows, n, n_groups, sf, st, &cs));
@@ -4193,9 +4201,66 @@ int rigid_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const
   return CB_OK;
 }
 
+// The argument checks of cb_rigid_pose_robust(_gp3p) (`who` names the call in the errors), then rigid_impl
+int rigid_checked(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                  const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs,
+                  const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px,
+                  int obs_on_device, double threshold_px, int32_t min_inliers, int32_t max_pairs, int32_t max_samples,
+                  int32_t gp3p_samples, int32_t n_prior, const int64_t* prior_key, const double* prior_pose,
+                  double pixel_sigma, int32_t max_iter, double xtol, int32_t max_groups, int32_t* n_groups_out,
+                  double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out, int32_t* n_inliers_out,
+                  int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
+                  CbRigidStats* stats, int device, void* stream, const char* who) {
+  if (n_cams <= 0 || !cam_flags || !cam_const || !cam_x || n_model < 0 || (n_model > 0 && !model_xyz) || n_obs < 0 ||
+      n_obs > 0x7fffffffLL || !n_groups_out || max_groups < 0 ||
+      (n_obs > 0 && (!obs_cam || !obs_key || !obs_pt || !obs_px || !inlier_out || n_model == 0)) ||
+      (max_groups > 0 && (!pose_out || !rmse_px_out || !count_out || !n_inliers_out || !n_points_out || !rep_row_out ||
+                          !status_out)) ||
+      !(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma)) || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol)) ||
+      !(threshold_px > 0.0 && std::isfinite(threshold_px)) || min_inliers < 4 || max_pairs < 1 || max_samples < 1 ||
+      max_samples > 4096 || gp3p_samples < 0 || gp3p_samples > 4096 || n_prior < 0 ||
+      (n_prior > 0 && (!prior_key || !prior_pose))) {
+    g_last_error = std::string(who) + ": bad argument";
+    return CB_E_INVALID;
+  }
+  for (int i = 0; i < n_prior; ++i) {
+    if (i > 0 && !(prior_key[i] > prior_key[i - 1])) {
+      g_last_error = std::string(who) + ": prior keys must be strictly ascending";
+      return CB_E_INVALID;
+    }
+    for (int k = 0; k < 6; ++k)
+      if (!std::isfinite(prior_pose[6 * (size_t)i + k])) {
+        g_last_error = std::string(who) + ": prior pose " + std::to_string(i) + " is not finite";
+        return CB_E_INVALID;
+      }
+  }
+  return rigid_impl(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_model, model_xyz, n_obs, obs_cam, obs_key, obs_pt,
+                    obs_px, obs_on_device, threshold_px, min_inliers, max_pairs, max_samples, n_prior, prior_key,
+                    prior_pose, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, pose_out, cov_out, rmse_px_out,
+                    count_out, n_inliers_out, n_points_out, rep_row_out, status_out, inlier_out, stats, device, stream,
+                    gp3p_samples, who);
+}
+
 }  // namespace
 
 extern "C" {
+
+int cb_rigid_pose_robust_gp3p(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                              const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs,
+                              const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt,
+                              const double* obs_px, int obs_on_device, double threshold_px, int32_t min_inliers,
+                              int32_t max_pairs, int32_t max_samples, int32_t gp3p_samples, int32_t n_prior,
+                              const int64_t* prior_key, const double* prior_pose, double pixel_sigma, int32_t max_iter,
+                              double xtol, int32_t max_groups, int32_t* n_groups_out, double* pose_out,
+                              double* cov_out, double* rmse_px_out, int32_t* count_out, int32_t* n_inliers_out,
+                              int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
+                              CbRigidStats* stats, int device, void* stream) {
+  return rigid_checked(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_model, model_xyz, n_obs, obs_cam, obs_key,
+                       obs_pt, obs_px, obs_on_device, threshold_px, min_inliers, max_pairs, max_samples, gp3p_samples,
+                       n_prior, prior_key, prior_pose, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, pose_out,
+                       cov_out, rmse_px_out, count_out, n_inliers_out, n_points_out, rep_row_out, status_out,
+                       inlier_out, stats, device, stream, "cb_rigid_pose_robust_gp3p");
+}
 
 int cb_rigid_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
                          const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs,
@@ -4206,32 +4271,11 @@ int cb_rigid_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double*
                          double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
                          int32_t* n_inliers_out, int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out,
                          uint8_t* inlier_out, CbRigidStats* stats, int device, void* stream) {
-  if (n_cams <= 0 || !cam_flags || !cam_const || !cam_x || n_model < 0 || (n_model > 0 && !model_xyz) || n_obs < 0 ||
-      n_obs > 0x7fffffffLL || !n_groups_out || max_groups < 0 ||
-      (n_obs > 0 && (!obs_cam || !obs_key || !obs_pt || !obs_px || !inlier_out || n_model == 0)) ||
-      (max_groups > 0 && (!pose_out || !rmse_px_out || !count_out || !n_inliers_out || !n_points_out || !rep_row_out ||
-                          !status_out)) ||
-      !(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma)) || max_iter < 1 || !(xtol >= 0.0 && std::isfinite(xtol)) ||
-      !(threshold_px > 0.0 && std::isfinite(threshold_px)) || min_inliers < 4 || max_pairs < 1 || max_samples < 1 ||
-      max_samples > 4096 || n_prior < 0 || (n_prior > 0 && (!prior_key || !prior_pose))) {
-    g_last_error = "cb_rigid_pose_robust: bad argument";
-    return CB_E_INVALID;
-  }
-  for (int i = 0; i < n_prior; ++i) {
-    if (i > 0 && !(prior_key[i] > prior_key[i - 1])) {
-      g_last_error = "cb_rigid_pose_robust: prior keys must be strictly ascending";
-      return CB_E_INVALID;
-    }
-    for (int k = 0; k < 6; ++k)
-      if (!std::isfinite(prior_pose[6 * (size_t)i + k])) {
-        g_last_error = "cb_rigid_pose_robust: prior pose " + std::to_string(i) + " is not finite";
-        return CB_E_INVALID;
-      }
-  }
-  return rigid_impl(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_model, model_xyz, n_obs, obs_cam, obs_key, obs_pt,
-                    obs_px, obs_on_device, threshold_px, min_inliers, max_pairs, max_samples, n_prior, prior_key,
-                    prior_pose, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, pose_out, cov_out, rmse_px_out,
-                    count_out, n_inliers_out, n_points_out, rep_row_out, status_out, inlier_out, stats, device, stream);
+  return rigid_checked(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_model, model_xyz, n_obs, obs_cam, obs_key,
+                       obs_pt, obs_px, obs_on_device, threshold_px, min_inliers, max_pairs, max_samples, 0, n_prior,
+                       prior_key, prior_pose, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, pose_out, cov_out,
+                       rmse_px_out, count_out, n_inliers_out, n_points_out, rep_row_out, status_out, inlier_out, stats,
+                       device, stream, "cb_rigid_pose_robust");
 }
 
 }  // extern "C"

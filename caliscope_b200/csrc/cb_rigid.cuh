@@ -1,7 +1,8 @@
 // Robust pose of a rigid body seen by a calibrated rig (cb_rigid_pose_robust, DESIGN.md section 4.14): per group (the
 // rows of one body at one moment, every camera's), Horn poses of triples of triangulated model points scored by MSAC
 // over all rows, the consensus rows, then Levenberg-Marquardt over the body pose (r, t) with X_w = R(r) M + t and its
-// first-order covariance with the rig's camera term.  oracle/rigid_pose_robust.py states the rule.
+// first-order covariance with the rig's camera term.  oracle/rigid_pose_robust.py states the rule and
+// oracle/rigid_pose_gp3p.py its gP3P hypotheses.
 //
 // The point hypotheses come from tri_consensus_kernel run unchanged on the (group, model point) sub-groups; the kernels
 // here take the qualified points of each group (qX, qM: ascending model index) and follow the short shape of
@@ -90,6 +91,332 @@ __device__ __forceinline__ double rig_row_err2(const double* cams, int stride, c
   return tri_row_err2(cams + (size_t)stride * obs_cam[r], X, reinterpret_cast<const double2*>(obs_px)[r], front);
 }
 
+// ---- generalized three-point pose (gP3P) -------------------------------------------------------------------------------
+// The body poses that put three model points M_i on three rays X_i = c_i + lambda_i d_i from different cameras (one
+// camera: P3P).  oracle/gp3p.py states the rule; the constants are its own.
+constexpr double GP3P_PARALLEL = 1e-12;  // det(sum (I - d d^T)) at or below this: the rays are parallel
+constexpr double GP3P_CLAMP = 1e-8;      // Delta_j >= -GP3P_CLAMP (1 + p_j^2) is clamped to 0, below it: no hypothesis
+constexpr double GP3P_UMAX = 1e9;        // roots beyond |u_1| = GP3P_UMAX are not sought
+constexpr int GP3P_NEWTON = 3;           // Newton steps of the polish at most
+constexpr int GP3P_MAX = 8;              // roots of the octic, so hypotheses of one sample: slot 1 + 8 m + c
+constexpr int GP3P_ITERS = 100;          // safeguarded Newton steps per root at most
+
+// the normalised system of one sample (oracle/gp3p.py steps 1-2): lh the depths of the feet of X^ on the lines, cp the
+// feet relative to X^ over s, D2 the squared model sides over s^2 (12, 13, 23), p_j and Delta_j (j = 2, 3) in u_1, and
+// the octic F, lowest degree first
+struct GP3PSys {
+  double Xh[3], lh[3], cp[3][3], s, D2[3];
+  double p[2][2], dl[2][3];
+  double f[9];
+};
+
+template <int NA, int NB>
+__device__ __forceinline__ void gp_mul(const double (&a)[NA], const double (&b)[NB], double (&o)[NA + NB - 1]) {
+#pragma unroll
+  for (int i = 0; i < NA + NB - 1; ++i) o[i] = 0.0;
+#pragma unroll
+  for (int i = 0; i < NA; ++i)
+#pragma unroll
+    for (int j = 0; j < NB; ++j) o[i + j] = fma(a[i], b[j], o[i + j]);
+}
+
+__device__ __forceinline__ double gp_dot(const double* a, const double* b) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
+
+// Steps 0-2 on camera centres c, unit rays d and model points M: false for a degenerate model triangle or parallel rays
+__device__ __forceinline__ bool rig_gp3p_system(const double c[3][3], const double d[3][3], const double M[3][3],
+                                                GP3PSys& S) {
+  double u[3], v[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    u[a] = M[1][a] - M[0][a];
+    v[a] = M[2][a] - M[0][a];
+  }
+  const double x0 = u[1] * v[2] - u[2] * v[1], x1 = u[2] * v[0] - u[0] * v[2], x2 = u[0] * v[1] - u[1] * v[0];
+  const double nu2 = gp_dot(u, u), nv2 = gp_dot(v, v);
+  if (!(sqrt(x0 * x0 + x1 * x1 + x2 * x2) > RIG_DEGENERATE * sqrt(nu2) * sqrt(nv2))) return false;
+  // A = sum (I - d d^T), b = sum (I - d d^T) c, X^ = A^-1 b by the adjugate
+  double A[3][3], bb[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    bb[a] = 0.0;
+#pragma unroll
+    for (int e = 0; e < 3; ++e) A[a][e] = 0.0;
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double dc = gp_dot(d[i], c[i]);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      bb[a] += c[i][a] - d[i][a] * dc;
+#pragma unroll
+      for (int e = 0; e < 3; ++e) A[a][e] += (a == e ? 1.0 : 0.0) - d[i][a] * d[i][e];
+    }
+  }
+  const double C00 = A[1][1] * A[2][2] - A[1][2] * A[2][1], C01 = A[1][2] * A[2][0] - A[1][0] * A[2][2],
+               C02 = A[1][0] * A[2][1] - A[1][1] * A[2][0];
+  const double det = A[0][0] * C00 + A[0][1] * C01 + A[0][2] * C02;
+  if (!(det > GP3P_PARALLEL)) return false;
+  const double C11 = A[0][0] * A[2][2] - A[0][2] * A[2][0], C12 = A[0][1] * A[2][0] - A[0][0] * A[2][1],
+               C22 = A[0][0] * A[1][1] - A[0][1] * A[1][0];
+  const double id = 1.0 / det;
+  double* Xh = S.Xh;  // A is symmetric: its adjugate is the cofactor matrix
+  Xh[0] = (C00 * bb[0] + C01 * bb[1] + C02 * bb[2]) * id;
+  Xh[1] = (C01 * bb[0] + C11 * bb[1] + C12 * bb[2]) * id;
+  Xh[2] = (C02 * bb[0] + C12 * bb[1] + C22 * bb[2]) * id;
+  const double D01 = sqrt(nu2), D02 = sqrt(nv2);
+  double w[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) w[a] = M[2][a] - M[1][a];
+  const double D12 = sqrt(gp_dot(w, w));
+  S.s = fmax(fmax(D01, D02), D12);
+  const double is = 1.0 / S.s;
+  S.D2[0] = (D01 * is) * (D01 * is);
+  S.D2[1] = (D02 * is) * (D02 * is);
+  S.D2[2] = (D12 * is) * (D12 * is);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    double xc[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) xc[a] = Xh[a] - c[i][a];
+    S.lh[i] = gp_dot(d[i], xc);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) S.cp[i][a] = (c[i][a] + S.lh[i] * d[i][a] - Xh[a]) / S.s;
+  }
+  // p_j, Delta_j for j = 2, 3 (index 0, 1 here)
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    double wj[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) wj[a] = S.cp[0][a] - S.cp[1 + j][a];
+    const double dw = gp_dot(d[1 + j], wj), a1 = gp_dot(d[0], d[1 + j]);
+    S.p[j][0] = dw;
+    S.p[j][1] = a1;
+    S.dl[j][0] = dw * dw - (gp_dot(wj, wj) - S.D2[j]);
+    S.dl[j][1] = 2.0 * dw * a1 - 2.0 * gp_dot(d[0], wj);
+    S.dl[j][2] = a1 * a1 - 1.0;
+  }
+#pragma unroll
+  for (int a = 0; a < 3; ++a) w[a] = S.cp[1][a] - S.cp[2][a];
+  const double a23 = gp_dot(d[1], d[2]), e2 = gp_dot(d[1], w), e3 = gp_dot(d[2], w);
+  const double(&p2)[2] = S.p[0];
+  const double(&p3)[2] = S.p[1];
+  double p22[3], p33[3], p23[3];
+  gp_mul(p2, p2, p22);
+  gp_mul(p3, p3, p33);
+  gp_mul(p2, p3, p23);
+  double P0[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) P0[i] = p22[i] + S.dl[0][i] + p33[i] + S.dl[1][i] - 2.0 * a23 * p23[i];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) P0[i] += 2.0 * e2 * p2[i] - 2.0 * e3 * p3[i];
+  P0[0] += gp_dot(w, w) - S.D2[2];
+  double P2[2], P3[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    P2[i] = 2.0 * p2[i] - 2.0 * a23 * p3[i];
+    P3[i] = 2.0 * p3[i] - 2.0 * a23 * p2[i];
+  }
+  P2[0] += 2.0 * e2;
+  P3[0] -= 2.0 * e3;
+  const double P23 = -2.0 * a23;
+  double d23[5], P00[5], P22[3], P33[3], P22d[5], P33d[5], P2P3[3];
+  gp_mul(S.dl[0], S.dl[1], d23);
+  gp_mul(P0, P0, P00);
+  gp_mul(P2, P2, P22);
+  gp_mul(P3, P3, P33);
+  gp_mul(P22, S.dl[0], P22d);
+  gp_mul(P33, S.dl[1], P33d);
+  gp_mul(P2, P3, P2P3);
+  double Q0[5], Q1[3];
+#pragma unroll
+  for (int i = 0; i < 5; ++i) Q0[i] = P00[i] + P23 * P23 * d23[i] - (P22d[i] + P33d[i]);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) Q1[i] = 2.0 * (P23 * P0[i] - P2P3[i]);
+  double Q00[9], Q11[5], Q11d[9];
+  gp_mul(Q0, Q0, Q00);
+  gp_mul(Q1, Q1, Q11);
+  gp_mul(Q11, d23, Q11d);
+#pragma unroll
+  for (int i = 0; i < 9; ++i) S.f[i] = Q00[i] - Q11d[i];
+  return true;
+}
+
+// G_J = F^(J) (degree 8 - J) at x and its derivative
+template <int J>
+__device__ __forceinline__ void gp_deriv_eval(const double (&f)[9], double x, double& g, double& dg) {
+  constexpr int N = 8 - J;
+  double c[N + 1];
+#pragma unroll
+  for (int i = 0; i <= N; ++i) {
+    double k = 1.0;
+#pragma unroll
+    for (int q = 1; q <= J; ++q) k *= (double)(i + q);  // (i + J)! / i!
+    c[i] = f[i + J] * k;
+  }
+  g = c[N];
+  dg = 0.0;
+#pragma unroll
+  for (int i = N - 1; i >= 0; --i) {
+    dg = fma(dg, x, g);
+    g = fma(g, x, c[i]);
+  }
+}
+
+// The root of G_J in (lo, hi] where G_J is monotone (glo = G_J(lo), ghi = G_J(hi)), NaN without a sign change there:
+// Newton steps safeguarded by the bracket, bisection when a step leaves it
+template <int J>
+__device__ __forceinline__ double gp_bracket(const double (&f)[9], double lo, double hi, double glo, double ghi) {
+  if (!((glo < 0.0 && ghi >= 0.0) || (glo > 0.0 && ghi <= 0.0))) return res_nan();
+  if (ghi == 0.0) return hi;
+  double a = glo < 0.0 ? lo : hi, b = glo < 0.0 ? hi : lo;  // G(a) < 0 < G(b)
+  double x = 0.5 * (lo + hi);
+#pragma unroll 1
+  for (int it = 0; it < GP3P_ITERS; ++it) {
+    double g, dg;
+    gp_deriv_eval<J>(f, x, g, dg);
+    if (g == 0.0) break;
+    if (g < 0.0) a = x;
+    else b = x;
+    double xn = x - g / dg;
+    if (!(xn > fmin(a, b) && xn < fmax(a, b))) xn = 0.5 * (a + b);
+    const bool done = fabs(xn - x) <= 1e-15 * fmax(1.0, fabs(x));
+    x = xn;
+    if (done) break;
+  }
+  return x;
+}
+
+// The roots of G_J, ascending in slots 0..7-J (NaN: none in that slot), from those of G_{J+1} (slots 0..6-J): G_J is
+// monotone between consecutive real roots of its derivative, so each such interval of [-B, B] holds at most one root
+template <int J>
+__device__ __forceinline__ void gp_level(const double (&f)[9], double B, double (&r)[GP3P_MAX]) {
+  double lo = -B, g, dg;
+  gp_deriv_eval<J>(f, lo, g, dg);
+  double glo = g;
+#pragma unroll
+  for (int i = 0; i < 8 - J; ++i) {
+    const double hi = i < 7 - J ? r[i] : B;  // r[i] is G_{J+1}'s slot i and becomes G_J's
+    if (i < 7 - J && isnan(hi)) continue;
+    gp_deriv_eval<J>(f, hi, g, dg);
+    r[i] = gp_bracket<J>(f, lo, hi, glo, g);
+    lo = hi;
+    glo = g;
+  }
+}
+
+// The real roots of the octic F in [-B, B], B = Fujiwara's bound 2 max |f_{8-i} / f_8|^(1/i) clamped to [1, GP3P_UMAX],
+// ascending in r (NaN: none), through the derivative chain F^(7), ..., F (Gauss-Lucas: the derivatives' real roots lie
+// within F's bound too).  Only the coefficients and the eight slots stay in registers.
+__device__ __forceinline__ void rig_gp3p_roots(const double (&f)[9], double (&r)[GP3P_MAX]) {
+  double B = 0.0;
+#pragma unroll
+  for (int i = 1; i <= 8; ++i) B = fmax(B, pow(fabs(f[8 - i] / f[8]), 1.0 / i));
+  B = 2.0 * B;
+  B = isnan(B) ? GP3P_UMAX : fmin(fmax(B, 1.0), GP3P_UMAX);
+#pragma unroll
+  for (int i = 0; i < GP3P_MAX; ++i) r[i] = res_nan();
+  // F^(8) is a constant: F^(7) has its one slot in [-B, B]
+  gp_level<7>(f, B, r);
+  gp_level<6>(f, B, r);
+  gp_level<5>(f, B, r);
+  gp_level<4>(f, B, r);
+  gp_level<3>(f, B, r);
+  gp_level<2>(f, B, r);
+  gp_level<1>(f, B, r);
+  gp_level<0>(f, B, r);
+}
+
+// f_12, f_13, f_23 at u and the points Y_i = c'_i + u_i d_i
+__device__ __forceinline__ void gp_resid(const GP3PSys& S, const double d[3][3], const double* u, double* fr,
+                                         double Y[3][3]) {
+#pragma unroll
+  for (int i = 0; i < 3; ++i)
+#pragma unroll
+    for (int a = 0; a < 3; ++a) Y[i][a] = fma(u[i], d[i][a], S.cp[i][a]);
+#pragma unroll
+  for (int q = 0; q < 3; ++q) {
+    const int i = q == 2 ? 1 : 0, j = q == 0 ? 1 : 2;
+    double e[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) e[a] = Y[i][a] - Y[j][a];
+    fr[q] = gp_dot(e, e) - S.D2[q];
+  }
+}
+
+// Step 3 for root u1: the world points X_i = X^ + s (c'_i + u_i d_i) = c_i + lambda_i d_i (false: no hypothesis).
+// Not inlined: the system S then stays in the lane's local memory, which keeps rig_consensus_kernel<LANES, true> free
+// of spills (inlined, the root loop needs more than 255 registers).
+__device__ __noinline__ bool rig_gp3p_points(const GP3PSys& S, const double d[3][3], double u1, double X[3][3]) {
+  double pv[2], sq[2];
+  bool ok = true;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    pv[j] = fma(S.p[j][1], u1, S.p[j][0]);
+    const double dv = fma(fma(S.dl[j][2], u1, S.dl[j][1]), u1, S.dl[j][0]);
+    ok = ok && !(dv < -GP3P_CLAMP * (1.0 + pv[j] * pv[j]));
+    sq[j] = sqrt(fmax(dv, 0.0));
+  }
+  if (!ok) return false;
+  double u[3] = {u1, 0.0, 0.0}, best = __longlong_as_double(0x7ff0000000000000LL);
+  bool any = false;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const double t[3] = {u1, pv[0] + (q < 2 ? sq[0] : -sq[0]), pv[1] + ((q & 1) == 0 ? sq[1] : -sq[1])};
+    double fr[3], Y[3][3];
+    gp_resid(S, d, t, fr, Y);
+    if (fabs(fr[2]) < best) {
+      best = fabs(fr[2]);
+      u[1] = t[1];
+      u[2] = t[2];
+      any = true;
+    }
+  }
+  if (!any) return false;
+  double fr[3], Y[3][3];
+  gp_resid(S, d, u, fr, Y);
+  double ss = fr[0] * fr[0] + fr[1] * fr[1] + fr[2] * fr[2];
+#pragma unroll 1
+  for (int it = 0; it < GP3P_NEWTON; ++it) {
+    // J rows (f_12, f_13, f_23): d f_ij / d u_i = 2 e . d_i, d f_ij / d u_j = -2 e . d_j, e = Y_i - Y_j
+    double e[3][3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      e[0][a] = Y[0][a] - Y[1][a];
+      e[1][a] = Y[0][a] - Y[2][a];
+      e[2][a] = Y[1][a] - Y[2][a];
+    }
+    const double J00 = 2.0 * gp_dot(e[0], d[0]), J01 = -2.0 * gp_dot(e[0], d[1]);
+    const double J10 = 2.0 * gp_dot(e[1], d[0]), J12 = -2.0 * gp_dot(e[1], d[2]);
+    const double J21 = 2.0 * gp_dot(e[2], d[1]), J22 = -2.0 * gp_dot(e[2], d[2]);
+    // [[J00 J01 0] [J10 0 J12] [0 J21 J22]] x = f by Cramer
+    const double det = J00 * (-J12 * J21) - J01 * (J10 * J22);
+    const double x0 = (fr[0] * (-J12 * J21) - J01 * (fr[1] * J22 - J12 * fr[2])) / det;
+    const double x1 = (J00 * (fr[1] * J22 - J12 * fr[2]) - fr[0] * (J10 * J22)) / det;
+    const double x2 = (fr[0] * (J10 * J21) - J00 * (J21 * fr[1]) - J01 * (J10 * fr[2])) / det;
+    const double un[3] = {u[0] - x0, u[1] - x1, u[2] - x2};
+    double fn[3], Yn[3][3];
+    gp_resid(S, d, un, fn, Yn);
+    const double sn = fn[0] * fn[0] + fn[1] * fn[1] + fn[2] * fn[2];
+    if (!(sn < ss)) break;
+    ss = sn;
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+      u[q] = un[q];
+      fr[q] = fn[q];
+#pragma unroll
+      for (int a = 0; a < 3; ++a) Y[q][a] = Yn[q][a];
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    const double lam = fma(S.s, u[i], S.lh[i]);
+    ok = ok && isfinite(lam) && lam > 0.0;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) X[i][a] = fma(S.s, Y[i][a], S.Xh[a]);
+  }
+  return ok;
+}
+
 // Per group, the first qualified point qstart[g] (qG: the group of each qualified point, ascending; qstart[n_groups] =
 // n_q) and the prior row of the group's key (-1: none) by binary searches
 __global__ void rig_group_kernel(const int* __restrict__ start, const int* __restrict__ rows,
@@ -140,12 +467,84 @@ __global__ void rig_qual_kernel(const int* __restrict__ sstart, const unsigned l
   qG[j] = (int)(k >> pt_bits);
 }
 
+// The gP3P hypotheses of sample m (row positions p of the group starting at b) scored over the group's rows [b, e):
+// the best of them replaces (best, best_s, bR, bt) when its score is lower, at slot 1 + GP3P_MAX m + c
+__device__ __forceinline__ void rig_gp3p_task(const double* cams, int stride, const int* __restrict__ rows,
+                                              const int* __restrict__ obs_cam, const int* __restrict__ obs_pt,
+                                              const double* __restrict__ obs_px, const double* __restrict__ obs_xy,
+                                              const double* __restrict__ model, int b, int e, const int (&p)[3],
+                                              long long m, double tau2, double& best, long long& best_s, double* bR,
+                                              double* bt) {
+  double c[3][3], d[3][3], M[3][3];
+  int pt[3];
+  bool ok = true;
+#pragma unroll
+  for (int s = 0; s < 3; ++s) {
+    const int r = rows[b + p[s]];
+    pt[s] = obs_pt[r];
+    const double* cam = cams + (size_t)stride * obs_cam[r];
+    const double* mp = model + 3 * (size_t)pt[s];
+    const double2 n = reinterpret_cast<const double2*>(obs_xy)[r];
+    const bool fish = (((int)cam[CT_FLAGS]) & 2) != 0;
+    ok = ok && isfinite(n.x) && isfinite(n.y) && !(fish && n.x == -1000000.0 && n.y == -1000000.0);
+    const double in = 1.0 / sqrt(n.x * n.x + n.y * n.y + 1.0);
+    const double y[3] = {n.x * in, n.y * in, in};
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      M[s][a] = mp[a];
+      ok = ok && isfinite(mp[a]);
+      // c = -R^T t, d = R^T y
+      c[s][a] = -(cam[CT_R + a] * cam[CT_T] + cam[CT_R + 3 + a] * cam[CT_T + 1] + cam[CT_R + 6 + a] * cam[CT_T + 2]);
+      d[s][a] = cam[CT_R + a] * y[0] + cam[CT_R + 3 + a] * y[1] + cam[CT_R + 6 + a] * y[2];
+    }
+  }
+  ok = ok && pt[0] != pt[1] && pt[0] != pt[2] && pt[1] != pt[2];
+  GP3PSys S;
+  if (!ok || !rig_gp3p_system(c, d, M, S)) return;
+  double roots[GP3P_MAX];
+  rig_gp3p_roots(S.f, roots);
+  int h = 0;
+#pragma unroll 1
+  for (int q = 0; q < GP3P_MAX; ++q) {
+    double u1 = roots[0];
+#pragma unroll
+    for (int j = 1; j < GP3P_MAX; ++j) u1 = q == j ? roots[j] : u1;  // selects, so the slots stay in registers
+    double X[3][3], R[9], t[3];
+    if (isnan(u1) || !rig_gp3p_points(S, d, u1, X)) continue;
+    double Mq[3][3];  // the model points again from memory: fewer registers live across the root loop
+#pragma unroll
+    for (int s = 0; s < 3; ++s)
+#pragma unroll
+      for (int a = 0; a < 3; ++a) Mq[s][a] = model[3 * (size_t)pt[s] + a];
+    if (!rig_horn(Mq, X, R, t)) continue;
+    double sc = 0.0;
+    for (int i = b; i < e; ++i) {
+      bool front;
+      const double e2 = rig_row_err2(cams, stride, R, t, rows[i], obs_cam, obs_pt, obs_px, model, front);
+      sc += msac_term(front, e2, tau2);
+    }
+    if (sc < best) {
+      best = sc;
+      best_s = 1 + GP3P_MAX * m + h;
+#pragma unroll
+      for (int a = 0; a < 9; ++a) bR[a] = R[a];
+#pragma unroll
+      for (int a = 0; a < 3; ++a) bt[a] = t[a];
+    }
+    ++h;
+  }
+}
+
 // One group per LANES lanes.  Task 0 is the group's prior pose (prior_idx >= 0), task 1 + m sample m of the group's
 // n_q qualified points (res_sample<3>); the lanes stride over the tasks, each builds its task's Horn pose and scores it
 // over all k rows (slots increase along a lane's tasks, so the first of equal scores stays).  group_argmin picks the
 // winner, which reaches the group's lanes from the lane that owns its task; then consensus_classify.  Writes hyp
 // (R row-major, t; NaN without consensus), count, rep_row, n_inliers, n_points (n_q), status (1, 5 or 0) and the flags.
-template <int LANES>
+// GP3P (launched when gp3p_samples > 0): in a group with k >= 4 rows and n_q < 3, task 1 + m is instead gP3P sample m
+// of the group's k rows (res_sample<3> with gp3p_samples, rig_gp3p_task on the undistorted coordinates obs_xy), whose
+// hypotheses take slots 1 + 8 m + c; the slot's task, not the slot, names the owning lane.  Every other group runs the
+// Horn path as it is.  GP3P = false ignores obs_xy and gp3p_samples.
+template <int LANES, bool GP3P>
 __global__ void __launch_bounds__(TRI_THREADS)
 rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
                      const int* __restrict__ rows, const int* __restrict__ obs_cam, const int* __restrict__ obs_pt,
@@ -154,7 +553,8 @@ rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_s
                      const double* __restrict__ prior_pose, int n_groups, double tau, int min_inliers, int max_samples,
                      double* __restrict__ hyp, int* __restrict__ count, int* __restrict__ rep_row,
                      int* __restrict__ n_inliers, int* __restrict__ n_points, int* __restrict__ status,
-                     unsigned char* __restrict__ pos_flag, unsigned char* __restrict__ inlier) {
+                     unsigned char* __restrict__ pos_flag, unsigned char* __restrict__ inlier,
+                     const double* __restrict__ obs_xy, int gp3p_samples) {
   extern __shared__ double s_cam[];
   int stride;
   const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
@@ -167,8 +567,10 @@ rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_s
   const int st = k < 4 ? TRI_FEW_ROWS : TRI_OK;
   const double tau2 = tau * tau;
   const double inf = __longlong_as_double(0x7ff0000000000000LL);
-  const long long T = res_triples(nq);
-  const long long ntask = (live && st == TRI_OK) ? 1 + (T < max_samples ? T : (long long)max_samples) : 0;
+  const bool gp = GP3P && nq < 3;  // this group's samples are gP3P samples of its rows
+  const long long T = gp ? res_triples(k) : res_triples(nq);
+  const int cap = gp ? gp3p_samples : max_samples;
+  const long long ntask = (live && st == TRI_OK) ? 1 + (T < cap ? T : (long long)cap) : 0;
   double best = inf, bR[9], bt[3];
 #pragma unroll
   for (int a = 0; a < 9; ++a) bR[a] = 0.0;
@@ -176,6 +578,15 @@ rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_s
   for (int a = 0; a < 3; ++a) bt[a] = 0.0;
   long long best_s = 0x7fffffffffffffffLL;
   for (long long task = lane; task < ntask; task += LANES) {
+    if constexpr (GP3P) {
+      if (gp && task > 0) {
+        int p[3];
+        if (res_sample<3>(task - 1, T, cap, k, p))
+          rig_gp3p_task(cams, stride, rows, obs_cam, obs_pt, obs_px, obs_xy, model, b, e, p, task - 1, tau2, best,
+                        best_s, bR, bt);
+        continue;
+      }
+    }
     double R[9], t[3];
     if (task == 0) {
       if (pi < 0) continue;
@@ -219,7 +630,8 @@ rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_s
   }
   group_argmin<LANES>(best, best_s);
   const bool found = best < inf;
-  const int owner = found ? (int)(best_s % LANES) : 0;
+  const long long wtask = gp && best_s > 0 ? 1 + (best_s - 1) / GP3P_MAX : best_s;  // the winner's task
+  const int owner = found ? (int)(wtask % LANES) : 0;
   group_bcast<LANES>(bR, owner);
   group_bcast<LANES>(bt, owner);
   int nin;

@@ -51,7 +51,8 @@ class RigidStats:
 def pose_rigid_robust(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, obs_pt, obs_px, *, threshold_px: float,
                       min_inliers: int = 6, max_pairs: int = 16, max_samples: int = 64, prior=None,
                       pixel_sigma: float = 1.0, camera_cov=None, max_iter: int = 20, xtol: float = 1e-12,
-                      device: int = 0, stream: int = 0, stats: RigidStats | None = None) -> RigidPoses:
+                      gp3p_samples: int = 0, device: int = 0, stream: int = 0,
+                      stats: RigidStats | None = None) -> RigidPoses:
     """Robust pose of a rigid body seen by several calibrated cameras at once (``cb_rigid_pose_robust``, DESIGN.md
     section 4.14).
 
@@ -69,7 +70,12 @@ def pose_rigid_robust(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, 
     pose is refined on them and ``cov = pixel_sigma^2 H^-1 + H^-1 G camera_cov G^T H^-1``.
 
     ``prior`` is ``(keys, poses)``: a pose (n, 6) per key, e.g. the previous frame's ``RigidPoses.key`` and ``pose``.
-    Rows that are not finite are dropped, so a tracking loop can pass the last output unchanged."""
+    Rows that are not finite are dropped, so a tracking loop can pass the last output unchanged.
+
+    ``gp3p_samples`` (0: off, else 1..4096) poses groups with fewer than three triangulated markers, e.g. markers each
+    seen by one camera, without a prior: up to that many triples of the group's rows from any cameras go through a
+    generalized-camera three-point solver (gP3P), whose poses join the prior in the same consensus.  Groups with three
+    or more triangulated markers give the same outputs, bit for bit, as with ``gp3p_samples=0``."""
     if not (np.isfinite(threshold_px) and threshold_px > 0):
         raise ValueError(f"threshold_px must be finite and > 0, got {threshold_px}")
     if int(min_inliers) < 4:
@@ -78,6 +84,8 @@ def pose_rigid_robust(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, 
         raise ValueError(f"max_pairs must be >= 1, got {max_pairs}")
     if not 1 <= int(max_samples) <= 4096:
         raise ValueError(f"max_samples must be in 1..4096, got {max_samples}")
+    if not 0 <= int(gp3p_samples) <= 4096:
+        raise ValueError(f"gp3p_samples must be in 0..4096, got {gp3p_samples}")
     if not (np.isfinite(pixel_sigma) and pixel_sigma >= 0):
         raise ValueError(f"pixel_sigma must be finite and >= 0, got {pixel_sigma}")
     if int(max_iter) < 1:
@@ -108,12 +116,13 @@ def pose_rigid_robust(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, 
     ng = C.c_int32(0)
     st = L.RigidStats()
     L.check(
-        lib.cb_rigid_pose_robust(nc, _ptr(flags), _ptr(const), _ptr(cx), None if ccov is None else _ptr(ccov),
-                                 len(model), _ptr(model), n, cam_p, key_p, pt_p, px_p, 1 if on_dev else 0,
-                                 float(threshold_px), int(min_inliers), int(max_pairs), int(max_samples), len(pkey),
-                                 _ptr(pkey), _ptr(ppose), float(pixel_sigma), int(max_iter), float(xtol), n,
-                                 C.byref(ng), _ptr(pose), _ptr(cov), _ptr(rmse), _ptr(count), _ptr(nin), _ptr(npts),
-                                 _ptr(rep), _ptr(status), _ptr(inlier), C.byref(st), int(device), C.c_void_p(stream)),
+        lib.cb_rigid_pose_robust_gp3p(nc, _ptr(flags), _ptr(const), _ptr(cx), None if ccov is None else _ptr(ccov),
+                                      len(model), _ptr(model), n, cam_p, key_p, pt_p, px_p, 1 if on_dev else 0,
+                                      float(threshold_px), int(min_inliers), int(max_pairs), int(max_samples),
+                                      int(gp3p_samples), len(pkey), _ptr(pkey), _ptr(ppose), float(pixel_sigma),
+                                      int(max_iter), float(xtol), n, C.byref(ng), _ptr(pose), _ptr(cov), _ptr(rmse),
+                                      _ptr(count), _ptr(nin), _ptr(npts), _ptr(rep), _ptr(status), _ptr(inlier),
+                                      C.byref(st), int(device), C.c_void_p(stream)),
         "pose_rigid_robust",
     )  # fmt: skip
     g = ng.value

@@ -521,6 +521,16 @@ typedef struct CbRigidStats {
  *      R = R(q), t = mean(X) - R mean(M).  None when the model triangle is degenerate,
  *      |(M_j - M_i) x (M_l - M_i)| <= 1e-9 |M_j - M_i| |M_l - M_i|, or R or t is not finite.  The group's prior, if it
  *      has one, is slot 0; sample m is slot 1 + m.
+ *   3-4 with gp3p_samples > 0 (1..4096), in a group with k >= 4 rows and n_q < 3 (every other group as above):
+ *      samples of three row positions 0..k-1, every triple in lexicographic order when C(k, 3) <= gp3p_samples, else
+ *      section 4.9's splitmix64 draw of gp3p_samples.  A sample gives no hypothesis when two of its rows share a model
+ *      point, a row is unusable (model point not finite, or undistorted coordinate not finite or the fisheye failure
+ *      sentinel), the model triangle is degenerate or the rays are parallel; else oracle/gp3p.py's gp3p on the rows'
+ *      camera centres c_i = -R_i^T t_i, unit rays d_i = R_i^T (x_i, y_i, 1) / |.| of the undistorted normalised
+ *      coordinates and model points: the real roots of the octic in the first depth, each back-substituted, polished by
+ *      Newton on the three distance equations and posed by Horn.  Hypothesis c of sample m is slot 1 + 8 m + c.
+ *      Constants: rays parallel when det(sum (I - d_i d_i^T)) <= 1e-12; Delta_j >= -1e-8 (1 + p_j^2) clamped to 0,
+ *      below it no hypothesis; roots with |u_1| <= 1e9; at most 3 Newton steps.
  *   5. score (MSAC): sum over all k rows of min(e_r^2, tau^2), e_r = |pi(R M_r + t; c_r) - u_r| in raw pixels with the
  *      engine's projection and the row's own camera; a row behind its camera, with a non-finite error or an unusable
  *      point adds tau^2.  The lowest score wins, the lowest slot on a tie.
@@ -549,6 +559,20 @@ int cb_rigid_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double*
                          double* pose_out, double* cov_out, double* rmse_px_out, int32_t* count_out,
                          int32_t* n_inliers_out, int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out,
                          uint8_t* inlier_out, CbRigidStats* stats, int device, void* stream);
+
+/* cb_rigid_pose_robust with gP3P hypotheses (steps 3-4 with gp3p_samples above): gp3p_samples 0 is
+ * cb_rigid_pose_robust itself, 1..4096 the most gP3P samples a group draws, anything else CB_E_INVALID.  Groups with
+ * three or more qualified points give the outputs of gp3p_samples = 0 bit for bit. */
+int cb_rigid_pose_robust_gp3p(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                              const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs,
+                              const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt,
+                              const double* obs_px, int obs_on_device, double threshold_px, int32_t min_inliers,
+                              int32_t max_pairs, int32_t max_samples, int32_t gp3p_samples, int32_t n_prior,
+                              const int64_t* prior_key, const double* prior_pose, double pixel_sigma, int32_t max_iter,
+                              double xtol, int32_t max_groups, int32_t* n_groups_out, double* pose_out,
+                              double* cov_out, double* rmse_px_out, int32_t* count_out, int32_t* n_inliers_out,
+                              int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
+                              CbRigidStats* stats, int device, void* stream);
 
 typedef struct CbRelPoseStats {
   double group_ms;      /* upload + undistortion + grouping by key, the correspondence slots and their sort by pair */

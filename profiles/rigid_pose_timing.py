@@ -1,6 +1,6 @@
 """Stage times and accuracy of cb_rigid_pose_robust (DESIGN.md 4.14), one JSON line per workload.
 
-    python profiles/rigid_pose_timing.py [track] [board64] [--steps 5] [--warmup 2]
+    python profiles/rigid_pose_timing.py [track] [board64] [sparse] [--steps 5] [--warmup 2] [--gp3p-samples G]
 
 track: section 4.9's scene (resect_robust_timing.make("track")) keyed by frame: a 0.2 m cluster of 12 markers seen by 8
 pinhole cameras 3 m away over 50 000 frames, 50 000 groups of 96 rows, 5 % of the rows moved by up to +-200 px, no
@@ -13,6 +13,12 @@ CUDA events recorded inside the call (CbRigidStats), the median over --steps tim
 are over the groups with status 0: the angle of R_true^T R and the distance of the body origins; chi2 is the mean of
 e^T Sigma^-1 e over those groups (6 when the covariance is calibrated).  The card's name and power limit are printed with
 the numbers.
+
+sparse: 6 pinhole cameras on a ring of 3 m around a 0.2 m cluster of 8 markers, each (marker,
+camera) row kept with probability 0.25 (about a fifth of the frames have fewer than three markers seen by two cameras),
+0.5 px noise, 3 % of the rows moved by up to 200 px, no prior, 20 000 frames.  --gp3p-samples G (default 0: off) is passed to every
+workload; with G > 0 the line also holds the same call with gP3P off: the share of groups with status 0 both ways, and
+the pose errors and chi2 of the groups only gP3P poses.
 """
 import argparse
 import json
@@ -129,24 +135,42 @@ def board64(n_frames=2000):
     return args, truth, moved, {"camera_cov": cc}, None
 
 
+def sparse(n_frames=20000):
+    """make_bodies' ring scene thinned to visibility 0.25 (tests/_rigid_cases.py), with outliers"""
+    from tests._rigid_cases import make_bodies, plant_outliers
+
+    b = make_bodies(51, n_cams=6, n_frames=n_frames, n_model=8, noise=0.5, visible=0.25)
+    b.obs_px, moved = plant_outliers(52, b.obs_px, 0.03, lo=10.0, hi=200.0)
+    args = (b.flags, b.const, b.cam_x, b.model, b.obs_cam, b.obs_key, b.obs_pt, b.obs_px)
+    return args, b.truth, moved, {}, None
+
+
+def _timed(args, kw, steps, warmup):
+    runs = []
+    for i in range(warmup + steps):
+        st = RigidStats()
+        r = pose_rigid_robust(*args, threshold_px=TAU, pixel_sigma=0.5, stats=st, **kw)
+        if i >= warmup:
+            runs.append(st)
+    return r, runs
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("workloads", nargs="*", default=["track", "board64"])
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
+    ap.add_argument("--gp3p-samples", type=int, default=0)
     a = ap.parse_args()
     who = card()
     for name in a.workloads:
-        args, truth, moved, kw, per_cam = {"track": track, "board64": board64}[name]()
-        runs = []
-        for i in range(a.warmup + a.steps):
-            st = RigidStats()
-            r = pose_rigid_robust(*args, threshold_px=TAU, pixel_sigma=0.5, stats=st, **kw)
-            if i >= a.warmup:
-                runs.append(st)
+        args, truth, moved, kw, per_cam = {"track": track, "board64": board64, "sparse": sparse}[name]()
+        kw = dict(kw, gp3p_samples=a.gp3p_samples)
+        r, runs = _timed(args, kw, a.steps, a.warmup)
         med = lambda f: float(np.median([getattr(s, f) for s in runs]))  # noqa: E731
         ok = r.status == 0
-        out = {"workload": name, "card": who, "groups": int(len(r.status)), "rows": int(len(args[4])),
+        out = {"workload": name, "card": who, "gp3p_samples": a.gp3p_samples, "groups": int(len(r.status)),
+               "rows": int(len(args[4])), "n_points_below_3": float((r.n_points < 3).mean()),
                "stage_ms": {f: med(f) for f in ("group_ms", "points_ms", "consensus_ms", "refine_ms", "cov_ms",
                                                 "total_ms")},
                "kernel_launches": runs[-1].kernel_launches, "status0": float(ok.mean()),
@@ -155,6 +179,16 @@ def main():
                "chi2_mean": _chi2(r.pose, r.cov, truth, ok)}  # fmt: skip
         if per_cam is not None:
             out["per_camera_resect"] = per_cam
+        if a.gp3p_samples > 0:
+            r0, runs0 = _timed(args, dict(kw, gp3p_samples=0), a.steps, a.warmup)
+            new = (r0.status != 0) & ok
+            out["gp3p_off"] = {"status0": float((r0.status == 0).mean()),
+                               "consensus_ms": float(np.median([s.consensus_ms for s in runs0])),
+                               "total_ms": float(np.median([s.total_ms for s in runs0])),
+                               "rig": _errors(r0.pose, truth, r0.status == 0),
+                               "chi2_mean": _chi2(r0.pose, r0.cov, truth, r0.status == 0)}  # fmt: skip
+            out["newly_posed"] = {"groups": int(new.sum()), "rig": _errors(r.pose, truth, new),
+                                  "chi2_mean": _chi2(r.pose, r.cov, truth, new) if new.any() else None}  # fmt: skip
         print(json.dumps(out), flush=True)
 
 
