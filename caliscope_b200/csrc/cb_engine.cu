@@ -4096,26 +4096,28 @@ int rigid_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const
   // gP3P samples are asked for
   Consensus cs;
   int* d_npts = nullptr;
+  unsigned char* d_amb = nullptr;  // the groups of status 6 (gP3P only)
   CB_TRY(consensus_alloc(n_groups, n, cb::RES_HYP, false, sf, st, &cs));
   CB_TRY(sf.alloc(&d_npts, (size_t)n_groups));
+  if (gp3p_samples > 0) CB_TRY(sf.alloc(&d_amb, (size_t)n_groups));
   CB_CUDA(cudaEventRecord(ev[4], st));
   with_lanes(lanes, [&](auto L) {
     if (gp3p_samples > 0)
       CB_LAUNCH((cb::rig_consensus_kernel<L.value, true>), blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
                 cam_in_smem, g.start, g.rows, g.cam, d_pt, d_px, d_model, d_qstart, d_qX, d_qM, d_pidx, d_ppose,
                 n_groups, tau, min_inliers, max_samples, cs.hyp, cs.count, cs.rep, cs.nin, d_npts, cs.status, cs.flag,
-                cs.inl, g.xy, gp3p_samples);
+                cs.inl, g.xy, gp3p_samples, d_amb);
     else
       CB_LAUNCH((cb::rig_consensus_kernel<L.value, false>), blocks, cb::TRI_THREADS, cam_smem, st, cams.camtab, n_cams,
                 cam_in_smem, g.start, g.rows, g.cam, d_pt, d_px, d_model, d_qstart, d_qX, d_qM, d_pidx, d_ppose,
                 n_groups, tau, min_inliers, max_samples, cs.hyp, cs.count, cs.rep, cs.nin, d_npts, cs.status, cs.flag,
-                cs.inl, nullptr, 0);
+                cs.inl, nullptr, 0, nullptr);
   });
   CB_CUDA(cudaGetLastError());
   CB_TRY(consensus_compact(g.rows, n, n_groups, sf, st, &cs));
   CB_CUDA(cudaEventRecord(ev[5], st));
 
-  // refinement on the consensus rows from the winners
+  // refinement on the consensus rows from the winners, then status 6 for the ambiguous gP3P groups
   double *d_pose = nullptr, *d_rmse = nullptr;
   int* d_status = nullptr;
   CB_TRY(sf.alloc(&d_pose, 6 * (size_t)n_groups));
@@ -4127,6 +4129,7 @@ int rigid_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const
               cs.start, cs.rows, g.cam, d_pt, d_px, d_model, n_groups, cs.status, cs.hyp, max_iter, xtol, d_pose,
               d_rmse, d_status);
   });
+  if (d_amb) CB_LAUNCH(cb::rig_ambiguous_kernel, cdiv(n_groups, 256), 256, 0, st, d_amb, n_groups, d_status);
   CB_CUDA(cudaGetLastError());
   CB_CUDA(cudaEventRecord(ev[7], st));
 

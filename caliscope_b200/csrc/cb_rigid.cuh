@@ -19,6 +19,7 @@
 namespace cb {
 
 constexpr double RIG_DEGENERATE = 1e-9;  // |u x v| <= this |u| |v|: a model triangle without a rotation
+constexpr int RIG_AMBIGUOUS = 6;  // status: a gP3P winner whose consensus rows hold fewer than four model points
 
 // Horn's closed-form absolute orientation (JOSA A 4(4), 1987) without scale of three model points M against their
 // world points X: q the eigenvector of the largest eigenvalue of Horn's N (sym4_min_eigvec of -N), R = R(q),
@@ -543,7 +544,10 @@ __device__ __forceinline__ void rig_gp3p_task(const double* cams, int stride, co
 // GP3P (launched when gp3p_samples > 0): in a group with k >= 4 rows and n_q < 3, task 1 + m is instead gP3P sample m
 // of the group's k rows (res_sample<3> with gp3p_samples, rig_gp3p_task on the undistorted coordinates obs_xy), whose
 // hypotheses take slots 1 + 8 m + c; the slot's task, not the slot, names the owning lane.  Every other group runs the
-// Horn path as it is.  GP3P = false ignores obs_xy and gp3p_samples.
+// Horn path as it is.  GP3P also writes ambiguous[g] = 1 for a group with consensus whose winner is a gP3P hypothesis
+// and whose consensus rows hold fewer than four distinct model points (lane 0 scans the flags in order and stops at the
+// fourth), else 0; rig_ambiguous_kernel turns it into status 6 after the refinement.  GP3P = false ignores obs_xy,
+// gp3p_samples and ambiguous.
 template <int LANES, bool GP3P>
 __global__ void __launch_bounds__(TRI_THREADS)
 rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_smem, const int* __restrict__ start,
@@ -554,7 +558,7 @@ rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_s
                      double* __restrict__ hyp, int* __restrict__ count, int* __restrict__ rep_row,
                      int* __restrict__ n_inliers, int* __restrict__ n_points, int* __restrict__ status,
                      unsigned char* __restrict__ pos_flag, unsigned char* __restrict__ inlier,
-                     const double* __restrict__ obs_xy, int gp3p_samples) {
+                     const double* __restrict__ obs_xy, int gp3p_samples, unsigned char* __restrict__ ambiguous) {
   extern __shared__ double s_cam[];
   int stride;
   const double* cams = tri_stage_camtab(camtab, n_cams, cam_in_smem, s_cam, stride);
@@ -639,7 +643,24 @@ rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_s
       found && st == TRI_OK, rows, b, e, lane, tau2, min_inliers,
       [&](int r, bool& front) { return rig_row_err2(cams, stride, bR, bt, r, obs_cam, obs_pt, obs_px, model, front); },
       pos_flag, inlier, nin);
+  if constexpr (GP3P) __syncwarp();  // every lane's pos_flag from consensus_classify is visible to lane 0
   if (!live || lane != 0) return;
+  if constexpr (GP3P) {
+    int ns = 0;  // distinct model points of the consensus rows, up to 4
+    if (ok && gp && best_s > 0) {
+      int p0 = -1, p1 = -1, p2 = -1;
+      for (int i = b; i < e && ns < 4; ++i) {
+        if (!pos_flag[i]) continue;
+        const int pt = obs_pt[rows[i]];
+        if (pt == p0 || pt == p1 || pt == p2) continue;
+        p2 = ns == 2 ? pt : p2;
+        p1 = ns == 1 ? pt : p1;
+        p0 = ns == 0 ? pt : p0;
+        ++ns;
+      }
+    }
+    ambiguous[g] = ns > 0 && ns < 4 ? 1 : 0;
+  }
   count[g] = k;
   rep_row[g] = rows[b];
   n_inliers[g] = ok ? nin : 0;
@@ -649,6 +670,13 @@ rig_consensus_kernel(const double* __restrict__ camtab, int n_cams, int cam_in_s
   for (int a = 0; a < 9; ++a) hyp[RES_HYP * g + a] = ok ? bR[a] : res_nan();
 #pragma unroll
   for (int a = 0; a < 3; ++a) hyp[RES_HYP * g + 9 + a] = ok ? bt[a] : res_nan();
+}
+
+// Status 6 for the groups rig_consensus_kernel<LANES, true> flagged ambiguous: it comes before 2, 3 and 4, so it replaces
+// whatever the refinement wrote (every flagged group had consensus).  The covariance kernels then leave cov NaN.
+__global__ void rig_ambiguous_kernel(const unsigned char* __restrict__ ambiguous, int n_groups, int* __restrict__ status) {
+  const int g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n_groups && ambiguous[g]) status[g] = RIG_AMBIGUOUS;
 }
 
 // J = d pi / d (r, t) of the body pose (2 x 6, pixels) from the row's J_X (normalised, 2 x 3) at B (R(r) and its right

@@ -17,7 +17,9 @@ from .uncertainty import PoseUncertainty, pose_from_body
 class RigidPoses:
     """Per group in ascending key order.  pose = (r, t) with X_w = R(r) M + t for the model points M.  status: 0 ok,
     1 fewer than 4 rows, 2 not positive definite (pose is the winning hypothesis, cov NaN), 3 iteration limit, 4 a
-    consensus row behind its camera at the solution, 5 no consensus (pose, cov, rmse NaN)."""
+    consensus row behind its camera at the solution, 5 no consensus (pose, cov, rmse NaN), 6 (gP3P only) ambiguous: a
+    gP3P winner whose consensus rows hold fewer than four distinct markers, which can fit two poses exactly (pose and
+    rmse of the refined winner, cov NaN)."""
 
     pose: np.ndarray  # (G, 6)
     cov: np.ndarray  # (G, 6, 6)
@@ -75,7 +77,9 @@ def pose_rigid_robust(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, 
     ``gp3p_samples`` (0: off, else 1..4096) poses groups with fewer than three triangulated markers, e.g. markers each
     seen by one camera, without a prior: up to that many triples of the group's rows from any cameras go through a
     generalized-camera three-point solver (gP3P), whose poses join the prior in the same consensus.  Groups with three
-    or more triangulated markers give the same outputs, bit for bit, as with ``gp3p_samples=0``."""
+    or more triangulated markers give the same outputs, bit for bit, as with ``gp3p_samples=0``.  A group that gP3P
+    poses from fewer than four distinct markers is status 6 (no covariance): with two triangulated markers and a third
+    seen by one camera, two poses can fit every row."""
     if not (np.isfinite(threshold_px) and threshold_px > 0):
         raise ValueError(f"threshold_px must be finite and > 0, got {threshold_px}")
     if int(min_inliers) < 4:

@@ -562,7 +562,13 @@ int cb_rigid_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double*
 
 /* cb_rigid_pose_robust with gP3P hypotheses (steps 3-4 with gp3p_samples above): gp3p_samples 0 is
  * cb_rigid_pose_robust itself, 1..4096 the most gP3P samples a group draws, anything else CB_E_INVALID.  Groups with
- * three or more qualified points give the outputs of gp3p_samples = 0 bit for bit. */
+ * three or more qualified points give the outputs of gp3p_samples = 0 bit for bit.
+ *   9 in a group that gP3P reaches, with status 6 added: a group whose consensus winner is a gP3P hypothesis (slot >= 1
+ *      in a group with n_q < 3) and whose consensus rows hold fewer than four distinct model points is ambiguous,
+ *      status 6: refinement runs as for status 0, pose and rmse are reported, cov is NaN.  First match wins: 1, 5, 6,
+ *      2, 3, 4, 0.  Two triangulated markers leave the body free to turn about their axis; a third marker seen by one
+ *      camera lies on a circle about that axis, which its ray can meet twice, and both poses fit every row.  A group
+ *      won by its prior (slot 0) keeps step 9's statuses: the prior chooses the branch. */
 int cb_rigid_pose_robust_gp3p(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
                               const double* cam_cov, int32_t n_model, const double* model_xyz, int64_t n_obs,
                               const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt,

@@ -15,6 +15,12 @@ Steps 1-2 and 5-9 are ``oracle/rigid_pose_robust.py``'s.  Steps 3-4 there, and i
      Newton on the three distance equations and posed by Horn.  Hypothesis c of sample m is slot 1 + 8 m + c.
      Constants: rays parallel when det(sum (I - d_i d_i^T)) <= 1e-12; Delta_j >= -1e-8 (1 + p_j^2) clamped to 0,
      below it no hypothesis; roots with |u_1| <= 1e9; at most 3 Newton steps.
+  9 in a group that gP3P reaches, with status 6 added: a group whose consensus winner is a gP3P hypothesis (slot >= 1)
+     and whose consensus rows hold fewer than four distinct model points is ambiguous, status 6: refinement runs as
+     for status 0, pose and rmse are reported, cov is NaN.  First match wins: 1, 5, 6, 2, 3, 4, 0.  Three markers of
+     which fewer than three are triangulated fix the pose only up to a branch: two triangulated markers leave a
+     rotation about their axis, the third marker lies on a circle and its ray meets that circle twice, and both poses
+     fit the rows exactly.  A group won by its prior (slot 0) keeps step 9's statuses: the prior chooses the branch.
 
 A group with n_q >= 3 (or k < 4) has no gP3P sample, so its outputs are ``rigid_pose_robust``'s own: this oracle takes
 them from there and restates steps 3-9 only for the groups that gP3P reaches.
@@ -30,7 +36,8 @@ from oracle.rigid_pose_robust import (STATUS_FEW_ROWS, STATUS_NOT_PD, RigidResul
 from oracle.triangulation_refine import group_rows
 from oracle.triangulation_robust import row_errors
 
-__all__ = ["rigid_pose_gp3p", "rays"]
+STATUS_AMBIGUOUS = 6
+__all__ = ["STATUS_AMBIGUOUS", "rigid_pose_gp3p", "rays"]
 
 
 def rays(cam_flags, cam_const, cam_x, obs_cam, obs_px):
@@ -126,7 +133,9 @@ def rigid_pose_gp3p(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, ob
         q0 = np.concatenate([rot_log(Rs[w]), ts[w]])
         Mc = model[obs_pt[crow]]
         q, rmse, st = refine_body(*cams, obs_cam[crow], obs_px[crow], Mc, q0, max_iter=max_iter, xtol=xtol)
+        if slots[w] >= 1 and len(np.unique(obs_pt[crow])) < 4:
+            st = STATUS_AMBIGUOUS
         res.pose[g], res.rmse_px[g], res.status[g] = q, rmse, st
-        if st != STATUS_NOT_PD:
+        if st not in (STATUS_NOT_PD, STATUS_AMBIGUOUS):
             res.cov[g] = body_covariance(*cams, obs_cam[crow], obs_px[crow], Mc, q, pixel_sigma, camera_cov)
     return res

@@ -71,9 +71,19 @@ def _errors(pose, truth, m):
             "angle_median_deg": float(np.median(ang)), "angle_p99_deg": float(np.percentile(ang, 99))}  # fmt: skip
 
 
-def _chi2(pose, cov, truth, m):
+def _chi2_each(pose, cov, truth, m):
     e = pose[m] - truth[m]
-    return float(np.mean(np.einsum("gi,gi->g", e, np.linalg.solve(cov[m], e[:, :, None])[:, :, 0])))
+    return np.einsum("gi,gi->g", e, np.linalg.solve(cov[m], e[:, :, None])[:, :, 0])
+
+
+def _chi2(pose, cov, truth, m):
+    return float(np.mean(_chi2_each(pose, cov, truth, m)))
+
+
+def _distinct_markers(r, obs_key, obs_pt, groups):
+    """the distinct model points of each group's consensus rows"""
+    g_of_row = np.searchsorted(r.key, obs_key)
+    return [int(len(np.unique(obs_pt[(g_of_row == g) & r.inlier]))) for g in groups]
 
 
 def track():
@@ -187,8 +197,16 @@ def main():
                                "total_ms": float(np.median([s.total_ms for s in runs0])),
                                "rig": _errors(r0.pose, truth, r0.status == 0),
                                "chi2_mean": _chi2(r0.pose, r0.cov, truth, r0.status == 0)}  # fmt: skip
+            d = _chi2_each(r.pose, r.cov, truth, new)
+            far = np.flatnonzero(new)[d > 22.46]  # beyond chi-square(6)'s 0.999 quantile
+            amb = (r0.status != 0) & (r.status == 6)
             out["newly_posed"] = {"groups": int(new.sum()), "rig": _errors(r.pose, truth, new),
-                                  "chi2_mean": _chi2(r.pose, r.cov, truth, new) if new.any() else None}  # fmt: skip
+                                  "chi2_mean": float(d.mean()) if new.any() else None,
+                                  "chi2_median": float(np.median(d)) if new.any() else None,
+                                  "chi2_above_22_46": int(len(far)), "status6_groups": int(amb.sum()),
+                                  "above_22_46": [{"key": int(r.key[g]), "chi2": float(x),
+                                                   "distinct_markers": n} for g, x, n in
+                                                  zip(far, d[d > 22.46], _distinct_markers(r, args[5], args[6], far))]}  # fmt: skip
         print(json.dumps(out), flush=True)
 
 
