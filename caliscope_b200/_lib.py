@@ -170,6 +170,17 @@ class RigidStats(C.Structure):
     ]
 
 
+class RigidModelStats(C.Structure):
+    _fields_ = [
+        ("group_ms", C.c_double),
+        ("solve_ms", C.c_double),
+        ("cov_ms", C.c_double),
+        ("total_ms", C.c_double),
+        ("kernel_launches", C.c_int32),
+        ("pad_", C.c_int32),
+    ]
+
+
 class RelPoseStats(C.Structure):
     _fields_ = [
         ("group_ms", C.c_double),
@@ -283,6 +294,12 @@ SYMBOLS = {
         [C.c_int32, _P, _P, _P, _P, C.c_int32, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_double, C.c_int32, C.c_int32,
          C.c_int32, C.c_int32, C.c_int32, _P, _P, C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32),
          _P, _P, _P, _P, _P, _P, _P, _P, _P, C.POINTER(RigidStats), C.c_int, _P],
+    ),
+    "cb_rigid_model_refine": (
+        C.c_int,
+        [C.c_int32, _P, _P, _P, _P, C.c_int32, _P, C.c_int32, _P, C.c_int64, _P, _P, _P, _P, C.c_int, C.c_int32, _P, _P,
+         C.c_double, C.c_int32, C.c_double, C.c_int32, C.POINTER(C.c_int32), _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+         _P, _P, C.POINTER(RigidModelStats), C.c_int, _P],
     ),
     "cb_relative_pose_robust": (
         C.c_int,

@@ -42,6 +42,7 @@
 #include "cb_bootstrap.cuh"
 #include "cb_relpose.cuh"
 #include "cb_intrinsics.cuh"
+#include "cb_rigid_model.cuh"
 #include "cb_peer.cuh"
 
 namespace {
@@ -4279,6 +4280,423 @@ int cb_rigid_pose_robust(int32_t n_cams, const int32_t* cam_flags, const double*
                        prior_key, prior_pose, pixel_sigma, max_iter, xtol, max_groups, n_groups_out, pose_out, cov_out,
                        rmse_px_out, count_out, n_inliers_out, n_points_out, rep_row_out, status_out, inlier_out, stats,
                        device, stream, "cb_rigid_pose_robust");
+}
+
+}  // extern "C"
+
+namespace {
+
+// An orthonormal basis (3K x (3K - 6), row-major) of the null space of C^T, C = [I_3 | [M0_k - mean M0]x] per marker:
+// the last 3K - 6 columns of Q of C's Householder QR
+std::vector<double> rmod_gauge_basis(const double* M0, int K) {
+  const int n = 3 * K;
+  double mb[3] = {0, 0, 0};
+  for (int k = 0; k < K; ++k)
+    for (int a = 0; a < 3; ++a) mb[a] += M0[3 * k + a] / K;
+  std::vector<double> Cm((size_t)n * 6, 0.0), Q((size_t)n * n, 0.0), v(n);
+  for (int k = 0; k < K; ++k) {
+    const double d[3] = {M0[3 * k] - mb[0], M0[3 * k + 1] - mb[1], M0[3 * k + 2] - mb[2]};
+    const double sk[3][3] = {{0, -d[2], d[1]}, {d[2], 0, -d[0]}, {-d[1], d[0], 0}};
+    for (int a = 0; a < 3; ++a) {
+      Cm[(3 * k + a) * 6 + a] = 1.0;
+      for (int c = 0; c < 3; ++c) Cm[(3 * k + a) * 6 + 3 + c] = sk[a][c];
+    }
+  }
+  for (int i = 0; i < n; ++i) Q[(size_t)i * n + i] = 1.0;
+  std::vector<std::vector<double>> hv;
+  for (int j = 0; j < 6; ++j) {  // Householder vectors
+    double nrm = 0.0;
+    for (int i = j; i < n; ++i) nrm += Cm[i * 6 + j] * Cm[i * 6 + j];
+    nrm = std::sqrt(nrm);
+    const double alpha = Cm[j * 6 + j] > 0 ? -nrm : nrm;
+    std::fill(v.begin(), v.end(), 0.0);
+    for (int i = j; i < n; ++i) v[i] = Cm[i * 6 + j];
+    v[j] -= alpha;
+    double vn = 0.0;
+    for (int i = j; i < n; ++i) vn += v[i] * v[i];
+    if (vn > 0)
+      for (int c = j; c < 6; ++c) {
+        double s = 0.0;
+        for (int i = j; i < n; ++i) s += v[i] * Cm[i * 6 + c];
+        s = 2.0 * s / vn;
+        for (int i = j; i < n; ++i) Cm[i * 6 + c] -= s * v[i];
+      }
+    for (double& x : v) x = vn > 0 ? x / std::sqrt(vn) : 0.0;
+    hv.push_back(v);
+  }
+  // Q = H_0 ... H_5 applied to the identity's columns 6 .. n-1
+  std::vector<double> N((size_t)n * (n - 6));
+  for (int c = 6; c < n; ++c) {
+    std::vector<double> x(n, 0.0);
+    x[c] = 1.0;
+    for (int j = 5; j >= 0; --j) {
+      double s = 0.0;
+      for (int i = 0; i < n; ++i) s += hv[j][i] * x[i];
+      for (int i = 0; i < n; ++i) x[i] -= 2.0 * s * hv[j][i];
+    }
+    for (int i = 0; i < n; ++i) N[(size_t)i * (n - 6) + (c - 6)] = x[i];
+  }
+  return N;
+}
+
+// The camera term of the covariance (cb_rigid_model.cuh): the used rows sorted by (frame, camera) (stable) into runs,
+// each run's D, the bodies' G^ and cov += P G^ Sigma_c G^^T P
+int rmod_camterm(int32_t n_cams, const TriCams& cams, const double* cam_cov, const cb::RmodArgs& A, const ObsGroups& g,
+                 int F, const std::vector<int>& fused, const std::vector<int>& uf_start, const std::vector<int>& uf_list,
+                 const std::vector<int>& active, const int32_t* body_start, ScopedFree& sf, cudaStream_t st) {
+  const int P = cams.P;
+  int n_rows = 0;
+  CB_CUDA(cudaMemcpyAsync(&n_rows, g.start + F, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  double* d_sig = nullptr;
+  CB_TRY(tri_cam_cov_upload(n_cams, cams, cam_cov, sf, st, &d_sig));
+  std::vector<int> fslot(F, -1);
+  for (int j = 0; j < uf_start.back(); ++j) fslot[uf_list[j]] = j;
+  const int* d_fslot = nullptr;
+  CB_TRY(to_device(fslot.data(), (size_t)F, 0, &d_fslot, sf, st));
+  int* d_fbody = nullptr;  // the body of every frame, from the frame table's order
+  {
+    std::vector<int> fb(F, 0);
+    for (size_t b = 0; b + 1 < uf_start.size(); ++b)
+      for (int j = uf_start[b]; j < uf_start[b + 1]; ++j) fb[uf_list[j]] = (int)b;
+    CB_TRY(to_device(fb.data(), (size_t)F, 0, (const int**)&d_fbody, sf, st));
+  }
+  const int cam_bits = std::max(1, bits_for((unsigned long long)(n_cams - 1)));
+  const int key_bits = std::min(64, cam_bits + bits_for((unsigned long long)F));
+  unsigned long long *d_k = nullptr, *d_ks = nullptr;
+  int *d_crow = nullptr, *d_rstart = nullptr, n_runs = 0;
+  CB_TRY(sf.alloc(&d_k, (size_t)n_rows));
+  CB_TRY(sf.alloc(&d_ks, (size_t)n_rows));
+  CB_TRY(sf.alloc(&d_crow, (size_t)n_rows));
+  CB_LAUNCH(cb::res_pt_key_kernel<32>, cdiv((long long)F * 32, 256), 256, 0, st, g.start, g.rows, g.cam, F, cam_bits,
+            d_k);
+  CB_CUB(sf, cub::DeviceRadixSort::SortPairs, d_k, d_ks, g.rows, d_crow, n_rows, 0, key_bits, st);
+  g_launches.fetch_add(2 * ((key_bits + 7) / 8));
+  CB_TRY(sorted_key_bounds(d_ks, n_rows, st, sf, &d_rstart, &n_runs));
+  int *d_rframe, *d_rcam, *d_frun0, *d_frun1;
+  long long *d_rsize, *d_roff;
+  CB_TRY(sf.alloc(&d_rframe, (size_t)n_runs));
+  CB_TRY(sf.alloc(&d_rcam, (size_t)n_runs));
+  CB_TRY(sf.alloc(&d_rsize, (size_t)n_runs + 1));
+  CB_TRY(sf.alloc(&d_roff, (size_t)n_runs + 1));
+  CB_TRY(sf.alloc(&d_frun0, (size_t)F));
+  CB_TRY(sf.alloc(&d_frun1, (size_t)F));
+  CB_CUDA(cudaMemsetAsync(d_frun0, 0, sizeof(int) * F, st));
+  CB_CUDA(cudaMemsetAsync(d_frun1, 0, sizeof(int) * F, st));
+  CB_LAUNCH(cb::rmod_runs_kernel, cdiv(n_runs + 1, 256), 256, 0, st, d_rstart, d_ks, cam_bits, n_runs, d_fslot,
+            A.fmask, d_fbody, A.status, P, d_rframe, d_rcam, d_rsize, d_frun0, d_frun1);
+  CB_CUB(sf, cub::DeviceScan::ExclusiveSum, d_rsize, d_roff, n_runs + 1, st);
+  g_launches.fetch_add(2);
+  long long nD = 0;
+  CB_CUDA(cudaMemcpyAsync(&nD, d_roff + n_runs, sizeof(long long), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  double* d_D = nullptr;
+  CB_TRY(sf.alloc(&d_D, (size_t)std::max(nD, 1LL)));
+  const int nP = n_cams * P;
+  std::vector<long long> gofs(active.size() + 1, 0);
+  for (size_t j = 0; j < active.size(); ++j)
+    gofs[j + 1] = gofs[j] + 3LL * (body_start[active[j] + 1] - body_start[active[j]]) * nP;
+  const long long* d_gofs = nullptr;
+  CB_TRY(to_device(gofs.data(), gofs.size(), 0, &d_gofs, sf, st));
+  double *d_G, *d_GS, *d_Y, *d_T2;
+  long long ncov = 0;
+  CB_CUDA(cudaMemcpyAsync(&ncov, A.coff + (uf_start.size() - 1), sizeof(long long), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  CB_TRY(sf.alloc(&d_G, (size_t)std::max(gofs.back(), 1LL)));
+  CB_TRY(sf.alloc(&d_GS, (size_t)std::max(gofs.back(), 1LL)));
+  CB_TRY(sf.alloc(&d_Y, (size_t)std::max(ncov, 1LL)));
+  CB_TRY(sf.alloc(&d_T2, (size_t)std::max(ncov, 1LL)));
+  const auto launch_runs = [&](auto kern, size_t smem) -> int {
+    CB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CB_LAUNCH(kern, cdiv(n_runs, cb::RMOD_RUN_WARPS), 32 * cb::RMOD_RUN_WARPS, smem, st, A, d_rstart, d_crow, d_rframe,
+              d_roff, d_fslot, d_fbody, n_runs, d_D);
+    return CB_OK;
+  };
+  if (P == 9) CB_TRY(launch_runs(cb::rmod_run_kernel<9>, cb::RMOD_RUN_WARPS * sizeof(cb::RmodRunWarp<9>)));
+  else CB_TRY(launch_runs(cb::rmod_run_kernel<6>, cb::RMOD_RUN_WARPS * sizeof(cb::RmodRunWarp<6>)));
+  CB_LAUNCH(cb::rmod_gsum_kernel, cdiv(gofs.back(), 256), 256, 0, st, A, (int)active.size(), n_cams, P, d_gofs,
+            d_frun0, d_frun1, d_rcam, d_roff, d_D, d_G);
+  CB_LAUNCH(cb::rmod_camterm_kernel, (int)active.size(), 256, 0, st, A, nP, d_gofs, d_G, d_sig, d_GS, d_Y, d_T2);
+  CB_CUDA(cudaGetLastError());
+  return CB_OK;
+}
+
+// cb_rigid_model_refine after its argument checks: upload, grouping by key, the frame table, the per-body frame lists
+// and gauge bases on the host, the Levenberg-Marquardt and covariance cluster kernels
+int rmod_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+              const double* cam_cov, int32_t n_model,
+              const double* model_xyz, int32_t n_bodies, const int32_t* body_start, int64_t n_obs,
+              const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt, const double* obs_px,
+              int obs_on_device, int32_t n_start, const int64_t* start_key, const double* start_pose,
+              double pixel_sigma, int32_t max_iter, double xtol, int32_t max_frames, int32_t* n_frames_out,
+              double* model_out, double* cov_out, int32_t* status_out, int32_t* iterations_out, double* rmse_px_out,
+              int32_t* body_frames_out, int32_t* body_rows_out, int64_t* key_out, double* pose_out,
+              double* frame_rmse_px_out, int32_t* count_out, int32_t* frame_status_out, CbRigidModelStats* stats,
+              int device, void* stream) {
+  const char* who = "cb_rigid_model_refine";
+  const double nan = std::numeric_limits<double>::quiet_NaN();
+  TriCams cams;
+  CB_TRY(tri_cams_prepare(n_cams, cam_flags, cam_const, cam_x, who, &cams));
+  CB_TRY(select_device(device));
+  *n_frames_out = 0;
+  if (stats) std::memset(stats, 0, sizeof(*stats));
+  std::memcpy(model_out, model_xyz, sizeof(double) * 3 * (size_t)n_model);
+  std::vector<long long> coff(n_bodies + 1, 0);
+  for (int b = 0; b < n_bodies; ++b) {
+    const long long n3 = 3LL * (body_start[b + 1] - body_start[b]);
+    coff[b + 1] = coff[b] + n3 * n3;
+    status_out[b] = cb::RM_UNUSED;
+    iterations_out[b] = body_frames_out[b] = body_rows_out[b] = 0;
+    rmse_px_out[b] = nan;
+  }
+  if (cov_out) std::fill(cov_out, cov_out + coff[n_bodies], nan);
+  if (n_obs == 0) return CB_OK;
+  const long long launches0 = g_launches.load();
+  cudaStream_t st = (cudaStream_t)stream;
+  ScopedFree sf(st);
+  const int n = (int)n_obs;
+  StageEvents<6> ev;
+  CB_TRY(ev.create());
+  CB_CUDA(cudaEventRecord(ev[0], st));
+  const int *d_cam = nullptr, *d_pt = nullptr, *d_bs = nullptr;
+  const long long *d_key = nullptr, *d_skey = nullptr;
+  const double *d_px = nullptr, *d_spose = nullptr;
+  CB_TRY(to_device(obs_cam, (size_t)n, obs_on_device, &d_cam, sf, st));
+  CB_TRY(to_device((const long long*)obs_key, (size_t)n, obs_on_device, &d_key, sf, st));
+  CB_TRY(to_device(obs_pt, (size_t)n, obs_on_device, &d_pt, sf, st));
+  CB_TRY(to_device(obs_px, 2 * (size_t)n, obs_on_device, &d_px, sf, st));
+  CB_TRY(to_device(body_start, (size_t)n_bodies + 1, 0, &d_bs, sf, st));
+  if (n_start > 0) {
+    CB_TRY(to_device((const long long*)start_key, (size_t)n_start, 0, &d_skey, sf, st));
+    CB_TRY(to_device(start_pose, 6 * (size_t)n_start, 0, &d_spose, sf, st));
+  }
+  int* d_bad = nullptr;
+  CB_TRY(sf.alloc(&d_bad, 1));
+  CB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+  CB_LAUNCH(cb::tri_validate_kernel, cdiv(n, 256), 256, 0, st, d_pt, nullptr, (long long)n, n_model, d_bad);
+  int bad = 0;
+  CB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (bad) {
+    g_last_error = std::string(who) + ": model point index out of range in " + std::to_string(bad) + " rows";
+    return CB_E_INVALID;
+  }
+  ObsGroups g;
+  CB_TRY(obs_group_stage(n_cams, nullptr, n, d_cam, (const int64_t*)d_key, d_px, 1, max_frames, n_frames_out, who,
+                         ev[1], sf, st, &g));
+  CB_TRY(tri_cams_upload(n_cams, cam_flags, cam_const, cam_x, &cams, sf, st));
+  const int F = g.n_groups;
+  int *d_fbody = nullptr, *d_fused = nullptr, *d_rep = nullptr;
+  unsigned* d_fmask = nullptr;
+  double* d_pose = nullptr;
+  CB_TRY(sf.alloc(&d_fbody, (size_t)F));
+  CB_TRY(sf.alloc(&d_fused, (size_t)F));
+  CB_TRY(sf.alloc(&d_fmask, (size_t)F));
+  CB_TRY(sf.alloc(&d_pose, 6 * (size_t)F));
+  CB_CUDA(cudaMemsetAsync(d_bad, 0, sizeof(int), st));
+  CB_LAUNCH(cb::rmod_frame_kernel, cdiv(F, 128), 128, 0, st, g.start, g.rows, d_pt, d_key, d_bs, n_bodies, d_skey,
+            d_spose, n_start, F, d_fbody, d_fmask, d_fused, d_pose, d_bad);
+  CB_CUDA(cudaGetLastError());
+  std::vector<int> fbody(F), fused(F), fstart(F + 1), rows(n);
+  std::vector<unsigned> fmask(F);
+  std::vector<double> pose0(6 * (size_t)F);
+  CB_CUDA(cudaMemcpyAsync(&bad, d_bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(fbody.data(), d_fbody, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(fused.data(), d_fused, sizeof(int) * F, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(fmask.data(), d_fmask, sizeof(unsigned) * F, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(fstart.data(), g.start, sizeof(int) * (F + 1), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(rows.data(), g.rows, sizeof(int) * n, cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaMemcpyAsync(pose0.data(), d_pose, sizeof(double) * pose0.size(), cudaMemcpyDeviceToHost, st));
+  CB_CUDA(cudaStreamSynchronize(st));
+  if (bad) {
+    g_last_error = std::string(who) + ": " + std::to_string(bad) + " keys have rows in two bodies";
+    return CB_E_INVALID;
+  }
+  // per body, its used frames in key order (CSR), the bodies to solve, their gauge bases and scratch offsets
+  std::vector<int> uf_start(n_bodies + 1, 0), uf_list, active;
+  std::vector<unsigned> seen(n_bodies, 0);
+  for (int f = 0; f < F; ++f)
+    if (fused[f]) {
+      ++uf_start[fbody[f] + 1];
+      seen[fbody[f]] |= fmask[f];
+      body_rows_out[fbody[f]] += fstart[f + 1] - fstart[f];
+    }
+  for (int b = 0; b < n_bodies; ++b) uf_start[b + 1] += uf_start[b];
+  uf_list.assign(std::max(uf_start[n_bodies], 1), 0);
+  std::vector<long long> goff(uf_list.size() + 1, 0);
+  {
+    std::vector<int> fill(uf_start.begin(), uf_start.end() - 1);
+    for (int f = 0; f < F; ++f)
+      if (fused[f]) uf_list[fill[fbody[f]]++] = f;
+  }
+  for (int j = 0; j < uf_start[n_bodies]; ++j)
+    goff[j + 1] = goff[j] + cb::RMOD_FRAME + cb::RMOD_MARK * (long long)__builtin_popcount(fmask[uf_list[j]]);
+  std::vector<long long> noff(n_bodies + 1, 0), toff(n_bodies + 1, 0);
+  std::vector<double> Nall;
+  int max_nf = 0;
+  for (int b = 0; b < n_bodies; ++b) {
+    const int K = body_start[b + 1] - body_start[b], nf = uf_start[b + 1] - uf_start[b];
+    const long long n3 = 3LL * K;
+    body_frames_out[b] = nf;
+    noff[b + 1] = noff[b];
+    toff[b + 1] = toff[b];
+    const unsigned full = K == 32 ? 0xffffffffu : (1u << K) - 1;
+    if (nf == 0 || seen[b] != full) continue;
+    active.push_back(b);
+    max_nf = std::max(max_nf, nf);
+    const std::vector<double> N = rmod_gauge_basis(model_xyz + 3 * (size_t)body_start[b], K);
+    Nall.insert(Nall.end(), N.begin(), N.end());
+    noff[b + 1] += (long long)N.size();
+    toff[b + 1] += 2 * n3 * (n3 - 6) + n3 * (n3 + 1) / 2 + 2 * n3 + 1;
+  }
+  CB_CUDA(cudaEventRecord(ev[2], st));
+  const int n_active = (int)active.size();
+  std::vector<int> bstatus(n_bodies, cb::RM_UNUSED), biters(n_bodies, 0);
+  std::vector<double> fcost(F, nan), pose(pose0);
+  if (n_active > 0) {
+    const int *d_act, *d_ufs, *d_ufl;
+    const long long *d_goff, *d_noff, *d_toff, *d_coff;
+    const double* d_N;
+    CB_TRY(to_device(active.data(), active.size(), 0, &d_act, sf, st));
+    CB_TRY(to_device(uf_start.data(), uf_start.size(), 0, &d_ufs, sf, st));
+    CB_TRY(to_device(uf_list.data(), uf_list.size(), 0, &d_ufl, sf, st));
+    CB_TRY(to_device(goff.data(), goff.size(), 0, &d_goff, sf, st));
+    CB_TRY(to_device(noff.data(), noff.size(), 0, &d_noff, sf, st));
+    CB_TRY(to_device(toff.data(), toff.size(), 0, &d_toff, sf, st));
+    CB_TRY(to_device(coff.data(), coff.size(), 0, &d_coff, sf, st));
+    CB_TRY(to_device(Nall.data(), Nall.size(), 0, &d_N, sf, st));
+    double *d_model, *d_gram, *d_trial, *d_tot, *d_fcost, *d_cov = nullptr, *d_pmat = nullptr;
+    const bool camterm = cam_cov && cov_out;
+    int *d_status, *d_iters;
+    CB_TRY(to_device(model_xyz, 3 * (size_t)n_model, 0, (const double**)&d_model, sf, st));
+    CB_TRY(sf.alloc(&d_gram, (size_t)goff.back()));
+    CB_TRY(sf.alloc(&d_trial, 6 * uf_list.size()));
+    CB_TRY(sf.alloc(&d_tot, (size_t)toff[n_bodies]));
+    CB_TRY(sf.alloc(&d_fcost, (size_t)F));
+    CB_TRY(sf.alloc(&d_status, (size_t)n_bodies));
+    CB_TRY(sf.alloc(&d_iters, (size_t)n_bodies));
+    if (cov_out) CB_TRY(sf.alloc(&d_cov, (size_t)coff[n_bodies]));
+    if (camterm) CB_TRY(sf.alloc(&d_pmat, (size_t)coff[n_bodies]));
+    CB_CUDA(cudaMemcpyAsync(d_fcost, fcost.data(), sizeof(double) * F, cudaMemcpyHostToDevice, st));
+    cb::RmodArgs A{cams.camtab, cb::CT_SIZE, g.start, g.rows, g.cam, d_pt, d_px, d_act, d_bs, d_ufs, d_ufl, d_goff,
+                   d_fmask, d_N, d_noff, d_model, d_pose, d_gram, d_trial, d_tot, d_toff, d_status, d_iters, d_fcost,
+                   d_cov, d_pmat, d_coff, pixel_sigma * pixel_sigma, (int)max_iter, xtol};
+    // a cluster of cs CTAs per body: intr_lm_kernel's rule, about four frames per warp up to 8 CTAs
+    const int cs = std::max(1, std::min(cb::INTR_MAX_CLUSTER, cdiv(max_nf, 4 * cb::RMOD_WARPS)));
+    const ClusterConfig cfg(n_active * cs, cb::RMOD_THREADS, cs, cb::RMOD_SMEM, st);
+    CB_CUDA(cudaFuncSetAttribute(cb::rmod_lm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb::RMOD_SMEM));
+    CB_CUDA(cudaFuncSetAttribute(cb::rmod_cov_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)cb::RMOD_SMEM));
+    CB_CUDA(cudaEventRecord(ev[3], st));
+    CB_CUDA(cudaLaunchKernelEx(&cfg.cfg, cb::rmod_lm_kernel, A));
+    g_launches.fetch_add(1);
+    CB_CUDA(cudaEventRecord(ev[4], st));
+    CB_CUDA(cudaLaunchKernelEx(&cfg.cfg, cb::rmod_cov_kernel, A));
+    g_launches.fetch_add(1);
+    if (camterm) CB_TRY(rmod_camterm(n_cams, cams, cam_cov, A, g, F, fused, uf_start, uf_list, active, body_start, sf, st));
+    CB_CUDA(cudaEventRecord(ev[5], st));
+    std::vector<double> cov(cov_out ? (size_t)coff[n_bodies] : 0);
+    CB_CUDA(cudaMemcpyAsync(model_out, d_model, sizeof(double) * 3 * (size_t)n_model, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(pose.data(), d_pose, sizeof(double) * pose.size(), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(fcost.data(), d_fcost, sizeof(double) * F, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(bstatus.data(), d_status, sizeof(int) * n_bodies, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaMemcpyAsync(biters.data(), d_iters, sizeof(int) * n_bodies, cudaMemcpyDeviceToHost, st));
+    if (cov_out) CB_CUDA(cudaMemcpyAsync(cov.data(), d_cov, sizeof(double) * cov.size(), cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaStreamSynchronize(st));
+    for (int b : active) {
+      const int lo = body_start[b], K = body_start[b + 1] - lo;
+      status_out[b] = bstatus[b];
+      iterations_out[b] = biters[b];
+      if (bstatus[b] == cb::RM_NOT_PD) {  // the start layout and poses, cov and rmse NaN
+        std::memcpy(model_out + 3 * (size_t)lo, model_xyz + 3 * (size_t)lo, sizeof(double) * 3 * K);
+        for (int j = uf_start[b]; j < uf_start[b + 1]; ++j) {
+          const int f = uf_list[j];
+          std::memcpy(&pose[6 * (size_t)f], &pose0[6 * (size_t)f], sizeof(double) * 6);
+          fcost[f] = nan;
+        }
+        continue;
+      }
+      double c = 0.0;
+      for (int j = uf_start[b]; j < uf_start[b + 1]; ++j) c += fcost[uf_list[j]];
+      rmse_px_out[b] = std::sqrt(c / body_rows_out[b]);
+      if (cov_out) std::memcpy(cov_out + coff[b], cov.data() + coff[b], sizeof(double) * (coff[b + 1] - coff[b]));
+    }
+  } else {
+    CB_CUDA(cudaEventRecord(ev[3], st));
+    CB_CUDA(cudaEventRecord(ev[4], st));
+    CB_CUDA(cudaEventRecord(ev[5], st));
+  }
+  for (int f = 0; f < F; ++f) {
+    const int c = fstart[f + 1] - fstart[f], bs = status_out[fbody[f]];
+    key_out[f] = obs_on_device ? 0 : obs_key[rows[fstart[f]]];
+    count_out[f] = c;
+    frame_status_out[f] = fused[f] ? bs : cb::RM_UNUSED;
+    frame_rmse_px_out[f] = fused[f] ? std::sqrt(fcost[f] / c) : nan;
+    std::memcpy(pose_out + 6 * (size_t)f, &pose[6 * (size_t)f], sizeof(double) * 6);
+  }
+  if (obs_on_device) {  // the keys from the device rows
+    std::vector<long long> all(n);
+    CB_CUDA(cudaMemcpyAsync(all.data(), d_key, sizeof(long long) * n, cudaMemcpyDeviceToHost, st));
+    CB_CUDA(cudaStreamSynchronize(st));
+    for (int f = 0; f < F; ++f) key_out[f] = all[rows[fstart[f]]];
+  }
+  if (stats) {
+    stats->group_ms = ev.ms(0, 2);
+    stats->solve_ms = ev.ms(3, 4);
+    stats->cov_ms = ev.ms(4, 5);
+    stats->total_ms = ev.ms(0, 5);
+    stats->kernel_launches = (int)(g_launches.load() - launches0);
+  }
+  return CB_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cb_rigid_model_refine(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                          const double* cam_cov, int32_t n_model, const double* model_xyz, int32_t n_bodies, const int32_t* body_start,
+                          int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt,
+                          const double* obs_px, int obs_on_device, int32_t n_start, const int64_t* start_key,
+                          const double* start_pose, double pixel_sigma, int32_t max_iter, double xtol,
+                          int32_t max_frames, int32_t* n_frames_out, double* model_out, double* cov_out,
+                          int32_t* status_out, int32_t* iterations_out, double* rmse_px_out, int32_t* body_frames_out,
+                          int32_t* body_rows_out, int64_t* key_out, double* pose_out, double* frame_rmse_px_out,
+                          int32_t* count_out, int32_t* frame_status_out, CbRigidModelStats* stats, int device,
+                          void* stream) {
+  const char* who = "cb_rigid_model_refine";
+  auto refuse = [&](const std::string& why) {
+    g_last_error = std::string(who) + ": " + why;
+    return CB_E_INVALID;
+  };
+  if (n_cams <= 0 || !cam_flags || !cam_const || !cam_x || n_model <= 0 || !model_xyz || n_bodies <= 0 ||
+      !body_start || n_obs < 0 || n_obs > 0x7fffffffLL || !n_frames_out || max_frames < 0 || n_start < 0 ||
+      (n_start > 0 && (!start_key || !start_pose)) ||
+      (n_obs > 0 && (!obs_cam || !obs_key || !obs_pt || !obs_px)) || !model_out || !status_out || !iterations_out ||
+      !rmse_px_out || !body_frames_out || !body_rows_out ||
+      (max_frames > 0 && (!key_out || !pose_out || !frame_rmse_px_out || !count_out || !frame_status_out)))
+    return refuse("bad argument");
+  if (!(pixel_sigma >= 0.0 && std::isfinite(pixel_sigma))) return refuse("pixel_sigma must be finite and >= 0");
+  if (!(xtol >= 0.0 && std::isfinite(xtol))) return refuse("xtol must be finite and >= 0");
+  if (max_iter < 1) return refuse("max_iter must be >= 1");
+  if (body_start[0] != 0 || body_start[n_bodies] != n_model) return refuse("body_start must run from 0 to n_model");
+  for (int b = 0; b < n_bodies; ++b) {
+    const int K = body_start[b + 1] - body_start[b];
+    if (K < 3 || K > cb::RMOD_KMAX)
+      return refuse("body " + std::to_string(b) + " has " + std::to_string(K) + " markers, outside 3..32");
+  }
+  for (int k = 0; k < 3 * n_model; ++k)
+    if (!std::isfinite(model_xyz[k])) return refuse("model_xyz is not finite");
+  for (int i = 0; i < n_start; ++i) {
+    if (i > 0 && !(start_key[i] > start_key[i - 1])) return refuse("start keys must be strictly ascending");
+    for (int k = 0; k < 6; ++k)
+      if (!std::isfinite(start_pose[6 * (size_t)i + k]))
+        return refuse("start pose " + std::to_string(i) + " is not finite");
+  }
+  return rmod_impl(n_cams, cam_flags, cam_const, cam_x, cam_cov, n_model, model_xyz, n_bodies, body_start, n_obs, obs_cam,
+                   obs_key, obs_pt, obs_px, obs_on_device, n_start, start_key, start_pose, pixel_sigma, max_iter, xtol,
+                   max_frames, n_frames_out, model_out, cov_out, status_out, iterations_out, rmse_px_out,
+                   body_frames_out, body_rows_out, key_out, pose_out, frame_rmse_px_out, count_out, frame_status_out,
+                   stats, device, stream);
 }
 
 }  // extern "C"

@@ -144,3 +144,94 @@ def pose_rigid_robust(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, 
     return RigidPoses(pose=pose[:g], cov=cov[:g], rmse_px=rmse[:g], count=count[:g], n_inliers=nin[:g],
                       n_points=npts[:g], rep_row=rep, status=status[:g], inlier=inlier[:n].astype(bool),
                       key=np.asarray(keys, np.int64))  # fmt: skip
+
+
+@dataclass
+class RigidModel:
+    """Refined marker layouts (``refine_rigid_model``).  Per body: status 0 ok, 1 not solved (no used frame, or a marker
+    without a row in a used frame: layout and poses are the start, cov NaN), 2 not positive definite at the start or
+    at the solution (layout and poses are the start, cov and rmse NaN), 3 iteration limit, 4 a row behind its camera at
+    the solution.  Per frame in ascending key order; a frame's status is 1 when it takes no part (no finite start pose,
+    fewer than 4 rows or fewer than 3 markers) or its body has status 1, else its body's status."""
+
+    model: np.ndarray  # (n_model, 3)
+    cov: list  # per body, (3K, 3K)
+    status: np.ndarray  # (n_bodies,) int32
+    iterations: np.ndarray
+    rmse_px: np.ndarray  # over the body's rows in used frames
+    n_frames: np.ndarray  # used frames
+    n_rows: np.ndarray
+    key: np.ndarray  # (F,) int64
+    pose: np.ndarray  # (F, 6) refined (r, t), X_w = R(r) M + t
+    frame_rmse_px: np.ndarray
+    count: np.ndarray  # every row of the key
+    frame_status: np.ndarray
+
+
+@dataclass
+class RigidModelStats:
+    group_ms: float = 0.0
+    solve_ms: float = 0.0
+    cov_ms: float = 0.0
+    total_ms: float = 0.0
+    kernel_launches: int = 0
+
+
+def refine_rigid_model(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key, obs_pt, obs_px, start, *, bodies=None,
+                       pixel_sigma: float = 1.0, camera_cov=None, max_iter: int = 100, xtol: float = 1e-12,
+                       device: int = 0, stream: int = 0, stats: RigidModelStats | None = None) -> RigidModel:  # fmt: skip
+    """Refine rigid-body marker layouts from tracked frames (``cb_rigid_model_refine``, DESIGN.md section 4.15).
+
+    The rig, ``model_xyz`` (the start layout, e.g. a nominal CAD layout) and the observations follow
+    ``pose_rigid_robust``; pass the rows to use, typically those ``RigidPoses.inlier`` marks.  ``start`` is
+    ``(keys, poses)``, one start pose per key (e.g. ``RigidPoses.key`` and ``pose``); non-finite rows are dropped.
+    ``bodies`` is ``body_start`` (n_bodies + 1, from 0 to n_model): model points body_start[b] .. body_start[b+1]-1 are
+    body b, with 3 to 32 markers; None is one body.  Every frame's rows must belong to one body.
+
+    One Levenberg-Marquardt per body over its layout and every frame pose, the frames eliminated, with the gauge held
+    by inner constraints on the start layout: the result keeps the start's centroid and has no net rotation against
+    it.  ``cov`` is ``pixel_sigma^2 P + P G camera_cov G^T P`` with ``P = N (N^T S N)^-1 N^T``: the pixel term, which
+    shrinks as frames are added, and the rig's term through the Schur-reduced cross term G to the camera parameters,
+    which does not.  ``camera_cov`` is ``Covariance.cameras`` of the rig (None: the pixel term alone)."""
+    model = np.ascontiguousarray(model_xyz, dtype=np.float64)
+    if model.ndim != 2 or model.shape[1] != 3 or len(model) == 0:
+        raise ValueError(f"model_xyz must be (n_model, 3) with n_model >= 1, got {model.shape}")
+    bs = np.ascontiguousarray([0, len(model)] if bodies is None else np.asarray(bodies).ravel(), dtype=np.int32)
+    skey = np.asarray(start[0], dtype=np.int64).ravel()
+    spose = np.asarray(start[1], dtype=np.float64).reshape(-1, 6)
+    if len(skey) != len(spose):
+        raise ValueError(f"start keys and poses differ in length: {len(skey)} and {len(spose)}")
+    keep = np.isfinite(spose).all(axis=1)
+    skey, spose = np.ascontiguousarray(skey[keep]), np.ascontiguousarray(spose[keep])
+    lib = L.load()
+    nc, flags, const, cx, ccov, n, on_dev, (cam_p, key_p, px_p, pt_p), _keep = _calibrated_inputs(
+        cam_flags, cam_const, cam_x, camera_cov, obs_cam, obs_key, obs_px, device, obs_pt=obs_pt)
+    nb = len(bs) - 1
+    m = max(n, 1)
+    sizes = 3 * np.diff(bs.astype(np.int64)) if nb > 0 else np.zeros(0, np.int64)
+    out_model = np.empty_like(model)
+    cov = np.empty(max(int((sizes * sizes).sum()), 1))
+    status, iters, nfr, nrows = (np.zeros(max(nb, 1), np.int32) for _ in range(4))
+    rmse = np.empty(max(nb, 1))
+    key, pose, frmse = np.empty(m, np.int64), np.empty((m, 6)), np.empty(m)
+    count, fstatus = np.empty(m, np.int32), np.empty(m, np.int32)
+    nf = C.c_int32(0)
+    st = L.RigidModelStats()
+    L.check(
+        lib.cb_rigid_model_refine(nc, _ptr(flags), _ptr(const), _ptr(cx), None if ccov is None else _ptr(ccov), len(model), _ptr(model), nb, _ptr(bs), n,
+                                  cam_p, key_p, pt_p, px_p, 1 if on_dev else 0, len(skey), _ptr(skey), _ptr(spose),
+                                  float(pixel_sigma), int(max_iter), float(xtol), n, C.byref(nf), _ptr(out_model),
+                                  _ptr(cov), _ptr(status), _ptr(iters), _ptr(rmse), _ptr(nfr), _ptr(nrows), _ptr(key),
+                                  _ptr(pose), _ptr(frmse), _ptr(count), _ptr(fstatus), C.byref(st), int(device),
+                                  C.c_void_p(stream)),
+        "refine_rigid_model",
+    )  # fmt: skip
+    if stats is not None:
+        stats.group_ms, stats.solve_ms, stats.cov_ms = st.group_ms, st.solve_ms, st.cov_ms
+        stats.total_ms, stats.kernel_launches = st.total_ms, st.kernel_launches
+    offs = np.concatenate([[0], np.cumsum(sizes * sizes)])
+    covs = [cov[offs[b] : offs[b + 1]].reshape(sizes[b], sizes[b]).copy() for b in range(nb)]
+    f = nf.value
+    return RigidModel(model=out_model, cov=covs, status=status[:nb], iterations=iters[:nb], rmse_px=rmse[:nb],
+                      n_frames=nfr[:nb], n_rows=nrows[:nb], key=key[:f], pose=pose[:f], frame_rmse_px=frmse[:f],
+                      count=count[:f], frame_status=fstatus[:f])  # fmt: skip

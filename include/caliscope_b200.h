@@ -580,6 +580,63 @@ int cb_rigid_pose_robust_gp3p(int32_t n_cams, const int32_t* cam_flags, const do
                               int32_t* n_points_out, int32_t* rep_row_out, int32_t* status_out, uint8_t* inlier_out,
                               CbRigidStats* stats, int device, void* stream);
 
+typedef struct CbRigidModelStats {
+  double group_ms;  /* upload + validation + grouping by key, the frame table and the per-body frame lists */
+  double solve_ms;  /* the Levenberg-Marquardt cluster kernel */
+  double cov_ms;    /* the covariance cluster kernel (status 2 / 4, rmse, cov) */
+  double total_ms;
+  int32_t kernel_launches;
+  int32_t pad_;
+} CbRigidModelStats;
+
+/* Refinement of rigid-body marker layouts from tracked frames (DESIGN.md section 4.15): one Levenberg-Marquardt per body
+ * over its layout and every frame pose, with the frames eliminated, and the layout's covariance.  Cameras in the
+ * bundle-adjustment layout as cb_triangulate_refine, cam_cov (nullable) the n_camera_params^2 camera covariance
+ * (BAProblem.covariance's cameras).  model_xyz[n_model][3] (host) is the start layout M0;
+ * body_start[n_bodies + 1] (host, ascending from 0 to n_model): model points body_start[b] .. body_start[b+1]-1 are body
+ * b, with 3 <= K <= 32 markers.  Observations (raw pixels) are host arrays or, with obs_on_device, device pointers
+ * (obs_cam, obs_key, obs_pt, obs_px); rows with equal obs_key are one frame of one body (all its rows in one body's
+ * range).  start_key[n_start] (strictly ascending) and start_pose[n_start][6] (finite) are the start pose (r, t) per key,
+ * host arrays; X_w = R(r_f) M_k + t_f.
+ *   1. frames: a frame is used when it has a start pose, at least 4 rows and at least 3 distinct markers among them;
+ *      otherwise its status is 1 and its rows take no part.  A body's status is 1 when it has no used frame, or when
+ *      one of its markers has no row in a used frame; its layout is then the start, its cov NaN and its frames' poses
+ *      the start.
+ *   2. residuals over body b's rows in used frames: the projection of R(r_f) M_k + t_f with the row's own camera (the
+ *      engine's projection), minus the raw pixel, in pixels.
+ *   3. gauge: inner constraints on the start layout, sum_k (M_k - M0_k) = 0 and
+ *      sum_k (M0_k - mean M0) x (M_k - M0_k) = 0: steps dM lie in null(C^T), C (3K x 6) = [I_3 | [M0_k - mean M0]x] per
+ *      marker.  The result keeps the start's centroid and has no net rotation against it.
+ *   4. step: H_MM + lam diag(H_MM) and H_ff + lam diag(H_ff) per frame; the frames eliminated into
+ *      S_lam = H_MM,lam - sum_f H_Mf H_ff,lam^-1 H_fM; dM = -N (N^T S_lam N)^-1 N^T b for an orthonormal basis N of
+ *      null(C^T); each frame's step by back-substitution.  lambda0 1e-3, / 10 on a lower cost, * 10 otherwise; stop
+ *      when |d| <= xtol (|x| + xtol), d and x over the layout and every frame pose of the body; max_iter steps at most;
+ *      a damped block that is not positive definite is a rejected step.
+ *   5. covariance at the solution (lam = 0), P = N (N^T S N)^-1 N^T, (3K)^2 per body:
+ *      cov = pixel_sigma^2 P + P G Sigma_c G^T P, G = sum_f (G_M,f - H_Mf H_ff^-1 G_f) the Schur-reduced cross term to
+ *      the camera parameters, G_.,f = sum over the frame's rows of J_.^T J_c in pixels; without cam_cov the first term
+ *      alone.  Cross-body correlation through the cameras is not given.
+ *   6. status per body, first match wins: 1;  2 N^T S N not positive definite at the start or at the solution (a
+ *      Cholesky pivot <= 1e-12 of its Jacobi scaling; layout and poses are the start, cov and rmse NaN);  3 max_iter
+ *      reached;  4 a row behind its camera at the solution;  0 none.
+ * Arguments: finite pixel_sigma >= 0 and xtol >= 0, max_iter >= 1, obs_pt in [0, n_model); CB_E_INVALID otherwise, and
+ * for a frame whose rows span two bodies.  cam_cov is read only with cov_out.
+ * Outputs: model_out[n_model][3]; cov_out (nullable) the per-body (3K)^2 blocks end to end in body order; per body
+ * status, iterations, rmse_px (over its rows in used frames), n_frames (used frames), n_rows; per frame in ascending key
+ * order (room for max_frames): key, pose[6], rmse_px (NaN for a frame that takes no part), count (every row of the key),
+ * status (1 for a frame that takes no part or whose body has status 1, else its body's status).  No floating-point
+ * atomics: repeated calls return bit-identical outputs. */
+int cb_rigid_model_refine(int32_t n_cams, const int32_t* cam_flags, const double* cam_const, const double* cam_x,
+                          const double* cam_cov, int32_t n_model, const double* model_xyz, int32_t n_bodies, const int32_t* body_start,
+                          int64_t n_obs, const int32_t* obs_cam, const int64_t* obs_key, const int32_t* obs_pt,
+                          const double* obs_px, int obs_on_device, int32_t n_start, const int64_t* start_key,
+                          const double* start_pose, double pixel_sigma, int32_t max_iter, double xtol,
+                          int32_t max_frames, int32_t* n_frames_out, double* model_out, double* cov_out,
+                          int32_t* status_out, int32_t* iterations_out, double* rmse_px_out, int32_t* body_frames_out,
+                          int32_t* body_rows_out, int64_t* key_out, double* pose_out, double* frame_rmse_px_out,
+                          int32_t* count_out, int32_t* frame_status_out, CbRigidModelStats* stats, int device,
+                          void* stream);
+
 typedef struct CbRelPoseStats {
   double group_ms;      /* upload + undistortion + grouping by key, the correspondence slots and their sort by pair */
   double consensus_ms;  /* five-point hypotheses, MSAC scoring, selection and the compaction of the consensus sets */
