@@ -4575,6 +4575,9 @@ int rmod_impl(int32_t n_cams, const int32_t* cam_flags, const double* cam_const,
     CB_TRY(sf.alloc(&d_fcost, (size_t)F));
     CB_TRY(sf.alloc(&d_status, (size_t)n_bodies));
     CB_TRY(sf.alloc(&d_iters, (size_t)n_bodies));
+    // every body starts unsolved: rmod_lm_kernel writes only the active bodies' statuses, and the camera term's run
+    // sizes read the status of every used frame's body
+    CB_CUDA(cudaMemcpyAsync(d_status, bstatus.data(), sizeof(int) * n_bodies, cudaMemcpyHostToDevice, st));
     if (cov_out) CB_TRY(sf.alloc(&d_cov, (size_t)coff[n_bodies]));
     if (camterm) CB_TRY(sf.alloc(&d_pmat, (size_t)coff[n_bodies]));
     CB_CUDA(cudaMemcpyAsync(d_fcost, fcost.data(), sizeof(double) * F, cudaMemcpyHostToDevice, st));

@@ -186,7 +186,8 @@ def refine_rigid_model(cam_flags, cam_const, cam_x, model_xyz, obs_cam, obs_key,
     ``pose_rigid_robust``; pass the rows to use, typically those ``RigidPoses.inlier`` marks.  ``start`` is
     ``(keys, poses)``, one start pose per key (e.g. ``RigidPoses.key`` and ``pose``); non-finite rows are dropped.
     ``bodies`` is ``body_start`` (n_bodies + 1, from 0 to n_model): model points body_start[b] .. body_start[b+1]-1 are
-    body b, with 3 to 32 markers; None is one body.  Every frame's rows must belong to one body.
+    body b, with 3 to 32 markers; None is one body.  Every frame's rows must belong to one body, and every
+    ``obs_key`` must be non-negative (``EngineError`` otherwise).
 
     One Levenberg-Marquardt per body over its layout and every frame pose, the frames eliminated, with the gauge held
     by inner constraints on the start layout: the result keeps the start's centroid and has no net rotation against

@@ -619,8 +619,8 @@ typedef struct CbRigidModelStats {
  *   6. status per body, first match wins: 1;  2 N^T S N not positive definite at the start or at the solution (a
  *      Cholesky pivot <= 1e-12 of its Jacobi scaling; layout and poses are the start, cov and rmse NaN);  3 max_iter
  *      reached;  4 a row behind its camera at the solution;  0 none.
- * Arguments: finite pixel_sigma >= 0 and xtol >= 0, max_iter >= 1, obs_pt in [0, n_model); CB_E_INVALID otherwise, and
- * for a frame whose rows span two bodies.  cam_cov is read only with cov_out.
+ * Arguments: finite pixel_sigma >= 0 and xtol >= 0, max_iter >= 1, obs_cam in [0, n_cams), obs_key >= 0, obs_pt in
+ * [0, n_model); CB_E_INVALID otherwise, and for a frame whose rows span two bodies.  cam_cov is read only with cov_out.
  * Outputs: model_out[n_model][3]; cov_out (nullable) the per-body (3K)^2 blocks end to end in body order; per body
  * status, iterations, rmse_px (over its rows in used frames), n_frames (used frames), n_rows; per frame in ascending key
  * order (room for max_frames): key, pose[6], rmse_px (NaN for a frame that takes no part), count (every row of the key),

@@ -6,9 +6,10 @@ TEST INFRASTRUCTURE ONLY — the product (caliscope_b200/) never imports this mo
 
 Cameras in the bundle-adjustment layout (cam_flags, cam_const, the camera section of x), an optional camera_cov
 (n_camera_params^2); the start layout model_xyz (n_model, 3), X_w = R(r_f) M_k + t_f; observations obs_cam, obs_key,
-obs_pt (the model point of the row), obs_px (raw pixels); start poses (keys strictly ascending, poses (n, 6) finite);
-body_start (n_bodies + 1): model points body_start[b] .. body_start[b+1]-1 are body b, 3 <= K <= 32.  A frame is the
-rows of one obs_key; all its rows belong to one body.
+obs_pt (the model point of the row), obs_px (raw pixels); keys are non-negative (the engine refuses a negative
+obs_key, as every call that groups rows by key does; this oracle does not check it); start poses (keys strictly
+ascending, poses (n, 6) finite); body_start (n_bodies + 1): model points body_start[b] .. body_start[b+1]-1 are
+body b, 3 <= K <= 32.  A frame is the rows of one obs_key; all its rows belong to one body.
   1. Frames.  A frame is used when it has a finite start pose, at least 4 rows and at least 3 distinct markers among
      them; otherwise its status is 1 and its rows take no part.  A body's status is 1 when it has no used frame, or
      when one of its markers has no row in a used frame; its layout is then the start, its cov NaN and its frames'

@@ -10,7 +10,7 @@ from oracle.ba_oracle import rodrigues
 from oracle.resection_robust import rot_log
 from tests._rigid_cases import Bodies, make_bodies
 
-__all__ = ["Scene", "make_scene", "multi_body", "kabsch_error", "one_camera_marker_scene", "behind_scene"]
+__all__ = ["Scene", "make_scene", "multi_body", "kabsch_error", "one_camera_marker_scene", "behind_scene", "check"]
 
 
 @dataclass
@@ -21,6 +21,7 @@ class Scene:
     start_key: np.ndarray
     start_pose: np.ndarray
     body_start: np.ndarray
+    frame_keys: np.ndarray | None = None  # the key of each row of bodies.truth
 
     def args(self):
         b = self.bodies
@@ -44,7 +45,8 @@ def make_scene(seed, *, n_model=8, n_frames=20, n_cams=8, noise=0.3, model_off=2
     keys = np.unique(b.obs_key)
     idx = np.searchsorted(np.asarray(kw.get("frame_keys", np.arange(n_frames))), keys)
     start = np.array([perturb_pose(rng, b.truth[i], rot_deg, trans) for i in idx])
-    return Scene(b, b.model.copy(), nominal, keys, start, np.array([0, n_model]))
+    return Scene(b, b.model.copy(), nominal, keys, start, np.array([0, n_model]),
+                 np.asarray(kw.get("frame_keys", np.arange(n_frames)), np.int64))  # fmt: skip
 
 
 def multi_body(seed, sizes=(4, 6, 3), n_frames=12, **kw) -> Scene:
@@ -138,3 +140,27 @@ def behind_scene(seed) -> Scene:
     b.obs_px = np.vstack([b.obs_px, np.zeros((len(extra), 2))])
     b.obs_px = _reproject(b, b.truth, 0.0, seed)
     return sc
+
+
+def check(d, o):
+    """A device result d against the oracle's o: statuses, the frame table and counts exactly, iterations at the limit,
+    layout, poses, rmse and cov to rounding-level tolerances (NaN where the oracle has NaN)."""
+    assert (d.status == o.status).all()
+    assert (d.frame_status == o.frame_status).all() and (d.key == o.key).all() and (d.count == o.count).all()
+    assert (d.n_frames == o.n_frames).all() and (d.n_rows == o.n_rows).all()
+    # iteration counts agree at the limit; below it the last steps compare costs at rounding level
+    assert (d.iterations[d.status == 3] == o.iterations[o.status == 3]).all()
+    ok = np.isin(d.status, (0, 3, 4))
+    scale = max(1.0, np.abs(o.model).max())
+    assert np.abs(d.model - o.model).max() <= 1e-7 * scale
+    fin = np.isfinite(o.pose).all(axis=1)
+    assert (np.isfinite(d.pose).all(axis=1) == fin).all()
+    if fin.any():
+        assert np.abs(d.pose[fin] - o.pose[fin]).max() <= 1e-7 * max(1.0, np.abs(o.pose[fin]).max())
+    np.testing.assert_allclose(d.rmse_px, o.rmse_px, rtol=1e-7, atol=1e-9)  # NaN where the oracle has NaN
+    np.testing.assert_allclose(d.frame_rmse_px, o.frame_rmse_px, rtol=1e-7, atol=1e-9)
+    for b in range(len(d.status)):
+        if ok[b]:
+            assert np.abs(d.cov[b] - o.cov[b]).max() <= 1e-6 * np.abs(o.cov[b]).max()
+        else:
+            assert np.isnan(d.cov[b]).all()
